@@ -7,7 +7,7 @@
 //   entropy/ANSRangeCodec.go:171-270  updateFrequencies / encodeHeader + EntropyUtils.go:38-67 EncodeAlphabet
 //   entropy/ANSRangeCodec.go:446-468  encSymbol.reset        -> packed 8-byte table entries
 //   entropy/ANSRangeCodec.go:313-405  encodeSymbol / encodeChunk -> ans0_encode_kernel
-//   entropy/ANSRangeCodec.go:605-710  decodeHeader           -> ans_walk_kernel (skim) + ans0_decode_kernel (full)
+//   entropy/ANSRangeCodec.go:605-710  decodeHeader           -> ans0_walk_kernel (skim) + ans0_tables_kernel (full)
 //   entropy/ANSRangeCodec.go:846-957  decodeSymbol / decodeChunkV2 -> ans0_decode_kernel
 //
 // Parallel decomposition (the wire format pins it): the unit of independent work is one 16 KiB chunk whose four
@@ -604,22 +604,24 @@ __global__ void __launch_bounds__(32) ans0_walk_kernel(const uint32_t* __restric
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// decode (v3): FOUR lanes per chunk (lane k owns rANS state k), 8 chunks per warp, 16 chunks per 64-thread CTA.
-//
-// History: v1 = one thread per chunk with ILP over the 4 states: one warp per scheduler, 198 instructions
-// per step, stalled every step on some lane's stream refill. v2 = 4 lanes per chunk, 32 chunks per CTA: correct but
-// 72 KiB of shared memory per CTA -> 444 resident CTAs for the 512 of the 256 MiB workload (two waves of an
-// indivisible 4096-step chain) and a scoreboard wait at the warp-convergence point after the conditional refill.
-// v3 keeps the 4-lane layout and
-//   * shrinks the per-chunk tables to 1964 bytes (24-slot start-of-symbol buckets: bits 8..31 = start flags, low
-//     byte = rank-1; 256 symbol entries sym | freq << 8 | cum << 20; 256-byte payload ring) so that 7 CTAs x 16
-//     chunks = 112 chunks fit per SM: a single wave for the 16384 chunks of 64 x 4 MiB needs 147 SMs (H100: 132, so a short second wave);
-//   * resolves the shared byte cursor with one __ballot_sync per step (order st3, st2, st1, st0,
-//     ANSRangeCodec.go:904-917) and reads the renormalisation word with one ld.shared.u16, branch free;
-//   * issues the ring refill loads unconditionally every 4 steps (clamped address) and consumes them one iteration
-//     later, so no step waits on a load issued in the same iteration;
-//   * transposes the decoded bytes across the 4 lanes with two shuffles per 4 steps and stores 16 bytes per chunk.
-// Table word w of chunk g lives at (w * 8 + g): the 8 chunks of a warp own disjoint groups of 4 banks.
+// decode: ans0_walk_kernel locates the chunk headers, ans0_tables_kernel turns each header into a table record, and
+// ans0_decode_kernel runs the rANS chains. FOUR lanes per chunk (lane k owns rANS state k), 8 chunks per warp, 16 chunks
+// per 64-thread CTA, 7 CTAs x 16 = 112 chunks per SM: the 16384 chunks of 64 x 4 MiB need 147 SMs for a single wave
+// (H100: 132, so a short second wave).
+//   * bucket word = start flags of 24 slots in bits 0..23 | (symbols started before the bucket - 1) << 24, bucket 0
+//     stores its flags without slot 0: symbol index = (b >> 24) + popc(b & ((2 << r) - 1)) needs no masking and the
+//     byte address of the symbol entry is one IMAD after the POPC; the bucket index is one IMAD.HI
+//     (slot / 24 = umulhi(slot, ceil(2^32 / 24)));
+//   * symbol entry = freq << 20 | cum << 8 | sym: the frequency is one shift away from the multiply;
+//   * table word w of chunk g lives at (w * 8 + g): the 8 chunks of a warp own disjoint groups of 4 banks;
+//   * every chunk's 256-byte payload ring is 256-byte aligned in the shared window: ring addresses are one LOP3
+//     ((pos & 0xFE) | base);
+//   * the shared byte cursor is resolved with one __ballot_sync per step (order st3, st2, st1, st0,
+//     ANSRangeCodec.go:904-917) and the renormalisation word is read with two ld.shared.u16, branch free;
+//   * the ring is refilled with cp.async (no register destination) and a round is consumed one iteration after it was
+//     issued, so no step waits on a load issued in the same iteration;
+//   * the decoded bytes are transposed across the 4 lanes with two shuffles per 4 steps, 16 bytes stored per chunk.
+// Warp region (bytes): 8 rings x 256 | 171 x 8 bucket words | 256 x 8 symbol words | pad to a multiple of 256.
 // ------------------------------------------------------------------------------------------------------------
 static const int RING_WORDS = 64;  // 32-bit words per chunk ring (256 bytes)
 
@@ -632,271 +634,8 @@ struct DecLane {
 // The ring holds RAW stream bytes (filled with cp.async, no register staging); the payload starts s16 bits into the
 // 16-bit unit at ring byte 0 + cur2, so a renormalisation word is the 16 bits at bit offset s16 of the 4 bytes at cur2.
 template <bool ALL_ACTIVE>
-KZ_D void dec_step(DecLane& L, const uint32_t* bm, const uint32_t* symtab, uint32_t ring_base, uint32_t mask, uint32_t lr, uint32_t rsh,
-                   uint32_t hi_mask, uint32_t grp_mask, bool active) {
-    const uint32_t slot = L.st & mask;
-    const uint32_t w = (slot * 2731u) >> 16;  // slot / 24 (exact for slot < 4096)
-    const uint32_t b = bm[w * 8];
-    const uint32_t m = (0x200u << (slot - 24u * w)) - 0x100u;
-    const uint32_t idx = (b + __popc(b & m)) & 0xFFu;
-    const uint32_t e = symtab[idx * 8];
-    const uint32_t nst = ((e >> 8) & 0xFFFu) * (L.st >> lr) + slot - (e >> 20);  // D(x) (ANSRangeCodec.go:849)
-    bool need = nst < (uint32_t)ANS_TOP;
-    if (!ALL_ACTIVE) need = need && active;
-    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, need);
-    const uint32_t t2 = L.cur2 + 2u * __popc(bal & hi_mask);
-    uint32_t va, vb;
-    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(va) : "r"(ring_base + (t2 & (4 * RING_WORDS - 2))));
-    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(vb) : "r"(ring_base + ((t2 + 2) & (4 * RING_WORDS - 2))));
-    const uint32_t x = __byte_perm(va, vb, 0x0145) >> rsh;  // big-endian 32 bits at t2, shifted so that the word sits in the low 16 bits
-    const uint32_t nst2 = __byte_perm(x, nst, 0x5410);      // (nst << 16) | (x & 0xFFFF)
-    if (ALL_ACTIVE || active) {
-        L.st = need ? nst2 : nst;
-        L.cur2 += 2u * __popc(bal & grp_mask);
-    }
-    L.acc = __byte_perm(L.acc, e, 0x4321);  // acc = (acc >> 8) | (sym << 24)
-}
-
-__global__ void __launch_bounds__(64, 7) ans0_decode_kernel(const uint32_t* __restrict__ words, uint64_t words_len /*in 32-bit words*/,
-                                                            const DecChunk* __restrict__ chunks, int nchunks,
-                                                            const uint64_t* __restrict__ chunk_hdr_bit, uint8_t* __restrict__ out,
-                                                            int32_t* __restrict__ status) {
-    extern __shared__ uint32_t s_dec[];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, k = lane & 3;  // chunk slot inside the warp, state index
-    uint32_t* wbase = s_dec + warp * DEC_WARP_WORDS;
-    uint32_t* bm = wbase + g;                                   // bucket w at bm[w*8]
-    uint32_t* symtab = wbase + DEC_BM_WORDS * 8 + g;            // entry i at symtab[i*8]
-    uint32_t* ring = wbase + (DEC_BM_WORDS + 256) * 8 + g * RING_WORDS;
-    const int c = blockIdx.x * DEC_CTA_CHUNKS + warp * 8 + g;
-    const uint32_t grp_mask = 0xFu << (lane & ~3);
-    const uint32_t hi_mask = grp_mask & ~((2u << lane) - 1u);  // lanes of my group with a higher state index (they read first)
-
-    // ---- per-chunk set-up by the group leader (k == 0): header parse, tables, chunk prologue
-    uint32_t lr = 12, nsteps = 0, tail = 0;
-    uint64_t pb = 0, pe = 0;
-    uint8_t* dst = nullptr;
-    int mode = 0;  // 0 = nothing to do, 1 = rANS decode
-    if (k == 0 && c < nchunks) {
-        const DecChunk ck = chunks[c];
-        dst = out + ck.out_off;
-        if (status[ck.block] == 0) {
-            BitReader br(words, chunk_hdr_bit[c], ck.end_bit);
-            lr = 8 + br.read(3);
-            const uint32_t scale = 1u << lr;
-            uint32_t llr = 3;
-            while ((1u << llr) <= lr) llr++;
-            int asz = 0;
-            if (br.read(1) == 0) {
-                if (br.read(1) == 0) {
-                    asz = 256;
-                    for (int i = 0; i < 256; i++) symtab[i * 8] = (uint32_t)i;
-                }
-            } else {
-                uint32_t last = br.read(5);
-                for (uint32_t i = 0; i <= last; i++) {
-                    uint32_t m = br.read(8);
-                    while (m) {
-                        int j = __ffs((int)m) - 1;
-                        m &= m - 1;
-                        symtab[asz * 8] = 8 * i + (uint32_t)j;
-                        asz++;
-                    }
-                }
-            }
-            if (asz == 0 || lr > 12) {
-                atomicCAS(&status[ck.block], 0, asz == 0 ? -KZ_E_PROCESS_BLOCK : -KZ_E_INVALID_CODEC);
-            } else if (asz == 1) {  // Read :737-741
-                const uint8_t v = (uint8_t)symtab[0];
-                for (uint32_t i = 0; i < ck.out_len; i++) dst[i] = v;
-            } else {
-                const int gs = asz < 64 ? 6 : 8;
-                uint32_t sum = 0;
-                bool bad = false;
-                for (int i = 1; i < asz; i += gs) {
-                    uint32_t log_max = br.read(llr);
-                    if ((1u << log_max) > scale) bad = true;
-                    int endj = i + gs < asz ? i + gs : asz;
-                    for (int j = i; j < endj; j++) {
-                        uint32_t freq = 1;
-                        if (log_max > 0) {
-                            freq = 1 + br.read(log_max);
-                            if (freq >= scale) bad = true;
-                        }
-                        symtab[j * 8] |= freq << 8;
-                        sum += freq;
-                    }
-                }
-                if (scale <= sum) bad = true;
-                if (!bad) {
-                    symtab[0] |= (scale - sum) << 8;
-                    const uint32_t nb = (scale + 23) / 24;
-                    for (uint32_t w = 0; w < nb; w++) bm[w * 8] = 0;
-                    uint32_t cum = 0;
-                    for (int i = 0; i < asz; i++) {
-                        const uint32_t e = symtab[i * 8];
-                        const uint32_t f = (e >> 8) & 0xFFFu;  // every frequency is <= scale - 1 <= 4095 when asz >= 2 (decSymbol.reset :973-978)
-                        const uint32_t w = cum / 24;
-                        bm[w * 8] |= 0x100u << (cum - 24 * w);
-                        symtab[i * 8] = e | (cum << 20);
-                        cum += f;
-                    }
-                    uint32_t running = 0;
-                    for (uint32_t w = 0; w < nb; w++) {
-                        const uint32_t b = bm[w * 8];
-                        bm[w * 8] = b | ((running - 1u) & 0xFFu);
-                        running += __popc(b >> 8);
-                    }
-                    const uint32_t sz = br.read_varint();
-                    const uint32_t s0 = br.read(32), s1 = br.read(32), s2 = br.read(32), s3 = br.read(32);
-                    if (sz >= (uint32_t)ANS_MAX_CHUNK || br.overrun || br.pos + 8ull * sz > ck.end_bit) bad = true;
-                    if (!bad) {
-                        pb = br.pos;
-                        pe = pb + 8ull * sz;
-                        nsteps = ck.out_len >> 2;
-                        tail = ck.out_len & 3;
-                        mode = 1;
-                        ring[0] = s0;  // park the initial states where the other lanes can fetch them
-                        ring[1] = s1;
-                        ring[2] = s2;
-                        ring[3] = s3;
-                    }
-                }
-                if (bad || br.overrun) atomicCAS(&status[ck.block], 0, -KZ_E_PROCESS_BLOCK);
-            }
-        }
-    }
-    __syncwarp();
-    const int leader = lane & ~3;
-    mode = __shfl_sync(0xFFFFFFFFu, mode, leader);
-    lr = __shfl_sync(0xFFFFFFFFu, lr, leader);
-    nsteps = __shfl_sync(0xFFFFFFFFu, nsteps, leader);
-    pb = __shfl_sync(0xFFFFFFFFu, pb, leader);
-    pe = __shfl_sync(0xFFFFFFFFu, pe, leader);
-    dst = (uint8_t*)(uintptr_t)__shfl_sync(0xFFFFFFFFu, (uint64_t)(uintptr_t)dst, leader);
-    DecLane L;
-    L.st = mode ? ring[k] : 0u;
-    L.acc = 0;
-    if (!mode) nsteps = 0;
-    __syncwarp();
-    uint32_t max_steps = nsteps, min_steps = nsteps;
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        max_steps = max(max_steps, __shfl_xor_sync(0xFFFFFFFFu, max_steps, d));
-        min_steps = min(min_steps, __shfl_xor_sync(0xFFFFFFFFu, min_steps, d));
-    }
-    if (max_steps == 0) return;
-
-    // ---- payload ring: raw copy of the stream starting at the 16-byte aligned block that holds the first payload bit.
-    // Ring byte r <-> source byte base_b + r. The 4 lanes of a group fetch 4 x 16 bytes per refill round with cp.async
-    // (no register destination: nothing in the decode loop waits on a global load it issued itself).
-    const uint64_t base_b = (pb >> 3) & ~15ull;            // source byte of ring byte 0
-    const uint32_t rel = (uint32_t)(pb - 8 * base_b);      // payload bit offset inside the ring, 0..134
-    const uint32_t rsh = 16u - (rel & 15u);                // see dec_step
-    const uint64_t end_b = (pe + 7) >> 3;                  // first source byte past the payload
-    const uint64_t lim_b = words_len * 4;
-    uint32_t fill = 0;                                     // ring byte offset (unwrapped, multiple of 64) of the next refill round
-    L.cur2 = 2u * (rel >> 4);
-    const uint32_t ring_base = smem_u32(ring);
-    auto issue = [&](bool want) {  // lane k copies source bytes [base_b + fill + 16k, +16) into the ring
-        const uint64_t sb = base_b + fill + 16u * k;
-        const bool ok = want && sb < end_b && sb + 16 <= lim_b;
-        const uint32_t dst_addr = ring_base + ((fill + 16u * k) & (4 * RING_WORDS - 1));
-        const uint8_t* src = reinterpret_cast<const uint8_t*>(words) + (ok ? sb : 0);
-        const uint32_t src_size = ok ? 16u : 0u;  // src-size 0 zero-fills: the guard past the payload (:888-893)
-        if (want) asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_addr), "l"(src), "r"(src_size) : "memory");
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll 1
-    for (int r = 0; r < 4; r++) {  // initial fill: the whole ring
-        issue(mode != 0);
-        fill += 64;
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
-    bool pending = false;
-    const uint32_t mask = (1u << lr) - 1u;
-
-    // 4x4 byte transpose    // 4x4 byte transpose inside the group: after 4 steps lane k holds [a_k0 a_k1 a_k2 a_k3] (a_kj = symbol of state k in
-    // step j, output position 4j + 3 - k); lane j stores the word of step j: [a_3j a_2j a_1j a_0j].
-    auto transpose = [&](uint32_t acc) -> uint32_t {
-        const uint32_t o2 = __shfl_xor_sync(0xFFFFFFFFu, acc, 2);
-        const uint32_t t1 = (k & 2) ? __byte_perm(acc, o2, 0x3276) : __byte_perm(acc, o2, 0x5410);
-        const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, t1, 1);
-        return (k & 1) ? __byte_perm(t1, o1, 0x5173) : __byte_perm(t1, o1, 0x0426);
-    };
-    auto maintain = [&]() {  // every 4 steps, uniform for the warp
-        asm volatile("cp.async.wait_group 0;" ::: "memory");  // the round issued one iteration ago has landed
-        fill += pending ? 64u : 0u;
-        __syncwarp();
-        // refill when at most 160 bytes are buffered ahead of the cursor: the new 64-byte round then only overwrites
-        // consumed bytes, and 4 steps consume at most 32 bytes
-        pending = mode && (int32_t)(fill - L.cur2) <= (4 * RING_WORDS - 64 - 32);
-        issue(pending);
-    };
-
-    const uint32_t fast_iters = min_steps >> 2;  // iterations in which every group of the warp is active
-    uint32_t it = 0;
-    uint8_t* dptr = dst + 4 * k;
-    for (; it < fast_iters; it++) {
-        dec_step<true>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec_step<true>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec_step<true>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec_step<true>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        *reinterpret_cast<uint32_t*>(dptr + (size_t)it * 16) = transpose(L.acc);
-        maintain();
-    }
-    const uint32_t all_iters = max_steps >> 2;
-    for (; it < all_iters; it++) {  // groups with fewer steps idle here
-        const bool active = (it * 4 + 3) < nsteps;
-        dec_step<false>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec_step<false>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec_step<false>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec_step<false>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        const uint32_t w = transpose(L.acc);
-        if (active) *reinterpret_cast<uint32_t*>(dptr + (size_t)it * 16) = w;
-        maintain();
-    }
-    {  // remaining 0..3 steps of a group (only the last chunk of a block can have nsteps % 4 != 0)
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncwarp();
-        const uint32_t done = nsteps & ~3u;
-        uint32_t rem_max = nsteps - done;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) rem_max = max(rem_max, __shfl_xor_sync(0xFFFFFFFFu, rem_max, d));
-        for (uint32_t r = 0; r < rem_max; r++) {
-            const bool active = done + r < nsteps;
-            dec_step<false>(L, bm, symtab, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-            if (active) dst[(size_t)(done + r) * 4 + (3 - k)] = (uint8_t)(L.acc >> 24);
-        }
-    }
-    // tail bytes follow the consumed words (:951-954)
-    if (mode && k == 0 && tail) {
-        uint64_t pos = 8 * (base_b + L.cur2) + (rel & 15u);  // bit position of the cursor in the stream
-        for (uint32_t j = 0; j < tail; j++, pos += 8) dst[(size_t)nsteps * 4 + j] = pos + 8 <= pe ? (uint8_t)bits_at(words, pos, 8) : 0;
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// decode (v4): same decomposition as v3 (4 lanes per chunk, 8 chunks per warp, 16 chunks per 64-thread CTA, 112
-// chunks per SM), shorter per-step dependent chain. A profile of v3: 58.6 instructions
-// per warp per step, almost all of them on one serial chain ("wait" 2.2 + "short_scoreboard" 1.8 cycles per issue,
-// issue slots 52 % used) -> the step time is (instructions on the chain) x (dependent-issue latency). v4
-//   * bucket word = start flags of 24 slots in bits 0..23 | (symbols started before the bucket - 1) << 24, bucket 0
-//     stores its flags without slot 0: symbol index = (b >> 24) + popc(b & ((2 << r) - 1)) needs no masking and the
-//     byte address of the symbol entry is one IMAD after the POPC;
-//   * bucket index with one IMAD.HI (slot / 24 = umulhi(slot, ceil(2^32 / 24)));
-//   * symbol entry = freq << 20 | cum << 8 | sym: the frequency is one shift away from the multiply;
-//   * every chunk's 256-byte ring is 256-byte aligned in the shared window: ring addresses are one LOP3
-//     ((pos & 0xFE) | base);
-//   * the refill bookkeeping is a per-lane countdown of valid 16-byte units and a running source pointer instead of
-//     64-bit range checks per round.
-// Warp region (bytes): 8 rings x 256 | 171 x 8 bucket words | 256 x 8 symbol words | pad to a multiple of 256.
-// ------------------------------------------------------------------------------------------------------------
-template <bool ALL_ACTIVE>
-KZ_D void dec4_step(DecLane& L, uint32_t bm_base, uint32_t sym_base, uint32_t ring_base, uint32_t mask, uint32_t lr, uint32_t rsh, uint32_t hi_mask,
-                    uint32_t grp_mask, bool active) {
+KZ_D void dec_step(DecLane& L, uint32_t bm_base, uint32_t sym_base, uint32_t ring_base, uint32_t mask, uint32_t lr, uint32_t rsh, uint32_t hi_mask,
+                   uint32_t grp_mask, bool active) {
     const uint32_t st = L.st;
     const uint32_t slot = st & mask;
     const uint32_t w = __umulhi(slot, 178956971u);  // slot / 24, exact for slot < 2^16
@@ -923,247 +662,11 @@ KZ_D void dec4_step(DecLane& L, uint32_t bm_base, uint32_t sym_base, uint32_t ri
     L.acc = __byte_perm(L.acc, e, 0x4321);  // acc = (acc >> 8) | (sym << 24)
 }
 
-__global__ void __launch_bounds__(64, 7) ans0_decode4_kernel(const uint32_t* __restrict__ words, uint64_t words_len /*in 32-bit words*/,
-                                                             const DecChunk* __restrict__ chunks, int nchunks,
-                                                             const uint64_t* __restrict__ chunk_hdr_bit, uint8_t* __restrict__ out,
-                                                             int32_t* __restrict__ status) {
-    extern __shared__ __align__(256) uint32_t s_dec4[];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, k = lane & 3;  // chunk slot inside the warp, state index
-    // the rings must be 256-byte aligned in the shared window (DEC4_SMEM carries 256 bytes of slack for this)
-    uint32_t* s_al = s_dec4 + (((0u - smem_u32(s_dec4)) & 255u) >> 2);
-    uint32_t* wbase = s_al + warp * DEC4_WARP_WORDS;
-    uint32_t* ring = wbase + g * RING_WORDS;
-    uint32_t* bm = wbase + 8 * RING_WORDS + g;                       // bucket w at bm[w*8]
-    uint32_t* symtab = wbase + 8 * RING_WORDS + DEC_BM_WORDS * 8 + g;  // entry i at symtab[i*8]
-    const int c = blockIdx.x * DEC_CTA_CHUNKS + warp * 8 + g;
-    const uint32_t grp_mask = 0xFu << (lane & ~3);
-    const uint32_t hi_mask = grp_mask & ~((2u << lane) - 1u);  // lanes of my group with a higher state index (they read first)
-
-    // ---- per-chunk set-up by the group leader (k == 0): header parse, tables, chunk prologue (decodeHeader :605-710)
-    uint32_t lr = 12, nsteps = 0, tail = 0;
-    uint64_t pb = 0, pe = 0;
-    uint8_t* dst = nullptr;
-    int mode = 0;  // 0 = nothing to do, 1 = rANS decode
-    if (k == 0 && c < nchunks) {
-        const DecChunk ck = chunks[c];
-        dst = out + ck.out_off;
-        if (status[ck.block] == 0) {
-            BitReader br(words, chunk_hdr_bit[c], ck.end_bit);
-            lr = 8 + br.read(3);
-            const uint32_t scale = 1u << lr;
-            uint32_t llr = 3;
-            while ((1u << llr) <= lr) llr++;
-            int asz = 0;
-            if (br.read(1) == 0) {
-                if (br.read(1) == 0) {
-                    asz = 256;
-                    for (int i = 0; i < 256; i++) symtab[i * 8] = (uint32_t)i;
-                }
-            } else {
-                uint32_t last = br.read(5);
-                for (uint32_t i = 0; i <= last; i++) {
-                    uint32_t m = br.read(8);
-                    while (m) {
-                        int j = __ffs((int)m) - 1;
-                        m &= m - 1;
-                        symtab[asz * 8] = 8 * i + (uint32_t)j;
-                        asz++;
-                    }
-                }
-            }
-            if (asz == 0 || lr > 12) {
-                atomicCAS(&status[ck.block], 0, asz == 0 ? -KZ_E_PROCESS_BLOCK : -KZ_E_INVALID_CODEC);
-            } else if (asz == 1) {  // Read :737-741
-                const uint8_t v = (uint8_t)symtab[0];
-                for (uint32_t i = 0; i < ck.out_len; i++) dst[i] = v;
-            } else {
-                const int gs = asz < 64 ? 6 : 8;
-                uint32_t sum = 0;
-                bool bad = false;
-                for (int i = 1; i < asz; i += gs) {
-                    uint32_t log_max = br.read(llr);
-                    if ((1u << log_max) > scale) bad = true;
-                    int endj = i + gs < asz ? i + gs : asz;
-                    for (int j = i; j < endj; j++) {
-                        uint32_t freq = 1;
-                        if (log_max > 0) {
-                            freq = 1 + br.read(log_max);
-                            if (freq >= scale) bad = true;
-                        }
-                        symtab[j * 8] |= freq << 20;
-                        sum += freq;
-                    }
-                }
-                if (scale <= sum) bad = true;
-                if (!bad) {
-                    symtab[0] |= (scale - sum) << 20;
-                    const uint32_t nb = (scale + 23) / 24;
-                    for (uint32_t w = 0; w < nb; w++) bm[w * 8] = 0;
-                    uint32_t cum = 0;
-                    for (int i = 0; i < asz; i++) {
-                        const uint32_t e = symtab[i * 8];
-                        const uint32_t f = e >> 20;  // every frequency is <= scale - 1 <= 4095 when asz >= 2 (decSymbol.reset :973-978)
-                        const uint32_t w = cum / 24;
-                        if (cum) bm[w * 8] |= 1u << (cum - 24 * w);  // slot 0 always starts symbol 0: its flag is implied
-                        symtab[i * 8] = e | (cum << 8);
-                        cum += f;
-                    }
-                    uint32_t running = 0;  // symbols started before the bucket, minus 1 (bucket 0: the implied start)
-                    for (uint32_t w = 0; w < nb; w++) {
-                        const uint32_t b = bm[w * 8];
-                        bm[w * 8] = b | (running << 24);
-                        running += __popc(b);
-                    }
-                    const uint32_t sz = br.read_varint();
-                    const uint32_t s0 = br.read(32), s1 = br.read(32), s2 = br.read(32), s3 = br.read(32);
-                    if (sz >= (uint32_t)ANS_MAX_CHUNK || br.overrun || br.pos + 8ull * sz > ck.end_bit) bad = true;
-                    if (!bad) {
-                        pb = br.pos;
-                        pe = pb + 8ull * sz;
-                        nsteps = ck.out_len >> 2;
-                        tail = ck.out_len & 3;
-                        mode = 1;
-                        ring[0] = s0;  // park the initial states where the other lanes can fetch them
-                        ring[1] = s1;
-                        ring[2] = s2;
-                        ring[3] = s3;
-                    }
-                }
-                if (bad || br.overrun) atomicCAS(&status[ck.block], 0, -KZ_E_PROCESS_BLOCK);
-            }
-        }
-    }
-    __syncwarp();
-    const int leader = lane & ~3;
-    mode = __shfl_sync(0xFFFFFFFFu, mode, leader);
-    lr = __shfl_sync(0xFFFFFFFFu, lr, leader);
-    nsteps = __shfl_sync(0xFFFFFFFFu, nsteps, leader);
-    pb = __shfl_sync(0xFFFFFFFFu, pb, leader);
-    pe = __shfl_sync(0xFFFFFFFFu, pe, leader);
-    dst = (uint8_t*)(uintptr_t)__shfl_sync(0xFFFFFFFFu, (uint64_t)(uintptr_t)dst, leader);
-    DecLane L;
-    L.st = mode ? ring[k] : 0u;
-    L.acc = 0;
-    if (!mode) nsteps = 0;
-    __syncwarp();
-    uint32_t max_steps = nsteps, min_steps = nsteps;
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        max_steps = max(max_steps, __shfl_xor_sync(0xFFFFFFFFu, max_steps, d));
-        min_steps = min(min_steps, __shfl_xor_sync(0xFFFFFFFFu, min_steps, d));
-    }
-    if (max_steps == 0) return;
-
-    // ---- payload ring: raw copy of the stream starting at the 16-byte aligned block that holds the first payload bit.
-    // Ring byte r <-> source byte base_b + r. Round n copies source bytes [base_b + 64 n, +64): lane k its 16-byte unit.
-    // A unit is copied when it starts before the end of the payload and lies inside the stream buffer, otherwise it is
-    // zero filled (the guard past the payload, :888-893): the first `left` rounds of this lane copy, the others fill.
-    const uint8_t* bytes = reinterpret_cast<const uint8_t*>(words);
-    const uint64_t base_b = (pb >> 3) & ~15ull;            // source byte of ring byte 0
-    const uint32_t rel = (uint32_t)(pb - 8 * base_b);      // payload bit offset inside the ring, 0..134
-    const uint32_t rsh = 16u - (rel & 15u);                // see dec4_step
-    const uint64_t end_b = (pe + 7) >> 3;                  // first source byte past the payload
-    const uint64_t lim_b = words_len * 4;
-    const uint64_t lim_u = lim_b >= 15 ? lim_b - 15 : 0;   // units must start below this to be entirely readable
-    const uint64_t stop_b = end_b < lim_u ? end_b : lim_u;
-    const uint64_t first_u = base_b + 16u * k;
-    int32_t left = (mode && stop_b > first_u) ? (int32_t)((stop_b - first_u + 63) >> 6) : 0;
-    const uint8_t* src = bytes + first_u;
-    const uint32_t ring_base = smem_u32(ring);
-    const uint32_t unit_base = ring_base | (16u * k);
-    uint32_t fill = 0;  // ring byte offset (unwrapped, multiple of 64) of the next refill round
-    L.cur2 = 2u * (rel >> 4);
-    auto issue = [&]() {
-        const bool ok = left > 0;
-        const uint8_t* s = ok ? src : bytes;
-        const uint32_t src_size = ok ? 16u : 0u;  // src-size 0 zero-fills
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(unit_base | (fill & 0xC0u)), "l"(s), "r"(src_size) : "memory");
-        src += 64;
-        fill += 64;
-        left--;
-    };
-    if (mode) {
-#pragma unroll 1
-        for (int r = 0; r < 4; r++) issue();  // initial fill: the whole ring
-    } else {
-        fill = 0x40000000u;  // never refills
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
-    const uint32_t mask = (1u << lr) - 1u;
-    const uint32_t bm_base = smem_u32(bm), sym_base = smem_u32(symtab);
-
-    // 4x4 byte transpose inside the group: after 4 steps lane k holds [a_k0 a_k1 a_k2 a_k3] (a_kj = symbol of state k in
-    // step j, output position 4j + 3 - k); lane j stores the word of step j: [a_3j a_2j a_1j a_0j].
-    auto transpose = [&](uint32_t acc) -> uint32_t {
-        const uint32_t o2 = __shfl_xor_sync(0xFFFFFFFFu, acc, 2);
-        const uint32_t t1 = (k & 2) ? __byte_perm(acc, o2, 0x3276) : __byte_perm(acc, o2, 0x5410);
-        const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, t1, 1);
-        return (k & 1) ? __byte_perm(t1, o1, 0x5173) : __byte_perm(t1, o1, 0x0426);
-    };
-    auto maintain = [&]() {  // every 4 steps, uniform for the warp
-        asm volatile("cp.async.wait_group 0;" ::: "memory");  // the round issued one iteration ago has landed
-        __syncwarp();
-        // refill when at most 160 bytes are buffered ahead of the cursor: the new 64-byte round then only overwrites
-        // consumed bytes (4 steps consume at most 32 bytes) and at least 128 buffered bytes remain while it is in flight
-        if ((int32_t)(fill - L.cur2) <= (4 * RING_WORDS - 64 - 32)) issue();
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-
-    const uint32_t fast_iters = min_steps >> 2;  // iterations in which every group of the warp is active
-    uint32_t it = 0;
-    uint8_t* dptr = dst + 4 * k;
-    for (; it < fast_iters; it++) {
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        *reinterpret_cast<uint32_t*>(dptr) = transpose(L.acc);
-        dptr += 16;
-        maintain();
-    }
-    const uint32_t all_iters = max_steps >> 2;
-    for (; it < all_iters; it++) {  // groups with fewer steps idle here
-        const bool active = (it * 4 + 3) < nsteps;
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        const uint32_t w = transpose(L.acc);
-        if (active) *reinterpret_cast<uint32_t*>(dptr) = w;
-        dptr += 16;
-        maintain();
-    }
-    {  // remaining 0..3 steps of a group (only the last chunk of a block can have nsteps % 4 != 0)
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncwarp();
-        const uint32_t done = nsteps & ~3u;
-        uint32_t rem_max = nsteps - done;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) rem_max = max(rem_max, __shfl_xor_sync(0xFFFFFFFFu, rem_max, d));
-        for (uint32_t r = 0; r < rem_max; r++) {
-            const bool active = done + r < nsteps;
-            dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-            if (active) dst[(size_t)(done + r) * 4 + (3 - k)] = (uint8_t)(L.acc >> 24);
-        }
-    }
-    // tail bytes follow the consumed words (:951-954)
-    if (mode && k == 0 && tail) {
-        uint64_t pos = 8 * (base_b + L.cur2) + (rel & 15u);  // bit position of the cursor in the stream
-        for (uint32_t j = 0; j < tail; j++, pos += 8) dst[(size_t)nsteps * 4 + j] = pos + 8 <= pe ? (uint8_t)bits_at(words, pos, 8) : 0;
-    }
-}
-
-
 // ------------------------------------------------------------------------------------------------------------
-// decode tables (v5): the header parse and table construction of decode v3/v4 ran on ONE lane per chunk (a serial
-// walk of ~300 bit-field reads through global memory, ~7 % of the kernel) while the other 31 lanes waited. Here one WARP
-// per chunk parses the header from a shared-memory window (alphabet by popc/prefix sums, group lengths chased by lane 0,
-// frequencies extracted group-parallel, cumulative frequencies by a warp scan, start flags by shared-memory atomics) and
-// writes a DEC_TAB_WORDS record per chunk: 171 bucket words | 256 symbol entries | lr, mode, steps, tail, payload begin /
-// end bit, 4 states. ans0_decode5_kernel only copies the records (cp.async) into its interleaved layout.
+// decode tables: one WARP per chunk parses the header from a shared-memory window (alphabet by popc/prefix sums, group
+// lengths chased by lane 0, frequencies extracted group-parallel, cumulative frequencies by a warp scan, start flags by
+// shared-memory atomics) and writes a DEC_TAB_WORDS record per chunk: 171 bucket words | 256 symbol entries | lr, mode, steps, tail, payload begin /
+// end bit, 4 states. ans0_decode_kernel only copies the records (cp.async) into its interleaved layout.
 // Chunks whose alphabet has a single symbol are filled here (Read :737-741) and need no decode.
 // ------------------------------------------------------------------------------------------------------------
 static const int TAB_WIN_WORDS = 160;  // 3 + 6 + 256 + 32 x 124 bits of header + 40 bits varint + 128 bits states + slack
@@ -1371,16 +874,16 @@ __global__ void __launch_bounds__(128) ans0_tables_kernel(const uint32_t* __rest
     }
 }
 
-__global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __restrict__ words, uint64_t words_len /*in 32-bit words*/, const uint32_t* __restrict__ tabs,
+__global__ void __launch_bounds__(64, 7) ans0_decode_kernel(const uint32_t* __restrict__ words, uint64_t words_len /*in 32-bit words*/, const uint32_t* __restrict__ tabs,
                                                              const DecChunk* __restrict__ chunks, int nchunks,
                                                              const uint64_t* __restrict__ chunk_hdr_bit, uint8_t* __restrict__ out,
                                                              int32_t* __restrict__ status) {
-    extern __shared__ __align__(256) uint32_t s_dec5[];
+    extern __shared__ __align__(256) uint32_t s_dec[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, k = lane & 3;  // chunk slot inside the warp, state index
-    // the rings must be 256-byte aligned in the shared window (DEC4_SMEM carries 256 bytes of slack for this)
-    uint32_t* s_al = s_dec5 + (((0u - smem_u32(s_dec5)) & 255u) >> 2);
-    uint32_t* wbase = s_al + warp * DEC4_WARP_WORDS;
+    // the rings must be 256-byte aligned in the shared window (DEC_SMEM carries 256 bytes of slack for this)
+    uint32_t* s_al = s_dec + (((0u - smem_u32(s_dec)) & 255u) >> 2);
+    uint32_t* wbase = s_al + warp * DEC_WARP_WORDS;
     uint32_t* ring = wbase + g * RING_WORDS;
     uint32_t* bm = wbase + 8 * RING_WORDS + g;                       // bucket w at bm[w*8]
     uint32_t* symtab = wbase + 8 * RING_WORDS + DEC_BM_WORDS * 8 + g;  // entry i at symtab[i*8]
@@ -1437,7 +940,7 @@ __global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __r
     const uint8_t* bytes = reinterpret_cast<const uint8_t*>(words);
     const uint64_t base_b = (pb >> 3) & ~15ull;            // source byte of ring byte 0
     const uint32_t rel = (uint32_t)(pb - 8 * base_b);      // payload bit offset inside the ring, 0..134
-    const uint32_t rsh = 16u - (rel & 15u);                // see dec4_step
+    const uint32_t rsh = 16u - (rel & 15u);                // see dec_step
     const uint64_t end_b = (pe + 7) >> 3;                  // first source byte past the payload
     const uint64_t lim_b = words_len * 4;
     const uint64_t lim_u = lim_b >= 15 ? lim_b - 15 : 0;   // units must start below this to be entirely readable
@@ -1494,15 +997,15 @@ __global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __r
     // it starts at >= 240, drops by at most 64 per check while above 128, and never drops once it is refilled every time.
     // 8 steps consume at most 64 bytes and a consuming lane reads at most 4 bytes past its word: always inside landed data.
     for (; it + 2 <= fast_iters; it += 2) {
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
         *reinterpret_cast<uint32_t*>(dptr) = transpose(L.acc);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
         *reinterpret_cast<uint32_t*>(dptr + 16) = transpose(L.acc);
         dptr += 32;
         asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -1511,10 +1014,10 @@ __global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __r
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     for (; it < fast_iters; it++) {
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
-        dec4_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
+        dec_step<true>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, true);
         *reinterpret_cast<uint32_t*>(dptr) = transpose(L.acc);
         dptr += 16;
         maintain();
@@ -1522,10 +1025,10 @@ __global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __r
     const uint32_t all_iters = max_steps >> 2;
     for (; it < all_iters; it++) {  // groups with fewer steps idle here
         const bool active = (it * 4 + 3) < nsteps;
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
-        dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
+        dec_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
+        dec_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
+        dec_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
+        dec_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
         const uint32_t w = transpose(L.acc);
         if (active) *reinterpret_cast<uint32_t*>(dptr) = w;
         dptr += 16;
@@ -1540,173 +1043,13 @@ __global__ void __launch_bounds__(64, 7) ans0_decode5_kernel(const uint32_t* __r
         for (int d = 16; d > 0; d >>= 1) rem_max = max(rem_max, __shfl_xor_sync(0xFFFFFFFFu, rem_max, d));
         for (uint32_t r = 0; r < rem_max; r++) {
             const bool active = done + r < nsteps;
-            dec4_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
+            dec_step<false>(L, bm_base, sym_base, ring_base, mask, lr, rsh, hi_mask, grp_mask, active);
             if (active) dst[(size_t)(done + r) * 4 + (3 - k)] = (uint8_t)(L.acc >> 24);
         }
     }
     // tail bytes follow the consumed words (:951-954)
     if (mode && k == 0 && tail) {
         uint64_t pos = 8 * (base_b + L.cur2) + (rel & 15u);  // bit position of the cursor in the stream
-        for (uint32_t j = 0; j < tail; j++, pos += 8) dst[(size_t)nsteps * 4 + j] = pos + 8 <= pe ? (uint8_t)bits_at(words, pos, 8) : 0;
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// decode (v6): ONE THREAD per chunk. v3..v5 put the four states of a chunk on four lanes: every warp instruction then
-// sits on one serial chain (ncu: 47 instructions per step at ~7 cycles each, issue slots half empty) and the shared
-// cursor costs a ballot + popc + two ring loads per symbol. Here a thread owns all four states of its chunk:
-//   * the four table look-ups of a step are independent -> the in-order issue of the warp always has other work while a
-//     shared-memory load or a dependent ALU result is in flight (4-way ILP instead of none);
-//   * the byte cursor is a private 64-bit shift register refilled 32 bits at a time from the thread's ring: a
-//     renormalisation is "take the top 16 bits, shift" (no ballot, no popc, no address arithmetic), and the arbitrary bit
-//     alignment of the payload is absorbed once per refill by a funnel shift;
-//   * tables are lane-private columns (word i of thread t at i * 112 + t): at most 2-way bank conflicts (t vs t + 16);
-//   * a step yields one complete output word [s3 s2 s1 s0]; four steps are stored with one 16-byte store.
-// 112 chunk slots per CTA, one CTA per SM (219,968 bytes of shared memory), 147 CTAs for 64 x 4 MiB: one wave on 147 SMs, two on the H100's 132.
-// No barrier of any kind is needed: a thread only touches its own column, its own ring and its own cp.async groups.
-// ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) ans0_decode6_kernel(const uint32_t* __restrict__ words, uint64_t words_len /*in 32-bit words*/,
-                                                              const uint32_t* __restrict__ tabs, const DecChunk* __restrict__ chunks, int nchunks,
-                                                              uint8_t* __restrict__ out) {
-    extern __shared__ __align__(16) uint32_t s_dec6[];
-    const int t = threadIdx.x;
-    const int c = blockIdx.x * DEC6_CHUNKS + t;
-    if (t >= DEC6_CHUNKS || c >= nchunks) return;
-    const uint32_t* rec = tabs + (size_t)c * DEC_TAB_WORDS;
-    const uint32_t* meta = rec + DEC_BM_WORDS + 256;
-    if (__ldg(meta + 1) == 0) return;  // nothing to decode (single symbol chunk, or the block failed)
-    constexpr int NT = DEC_BM_WORDS + 256;
-    constexpr uint32_t COL = 4u * DEC6_CHUNKS;  // byte stride between two words of a column
-    uint32_t* col = s_dec6 + t;
-    {  // my column: 427 words of the record
-        const uint4* r4 = reinterpret_cast<const uint4*>(rec);
-#pragma unroll 4
-        for (int i = 0; i < NT / 4; i++) {
-            const uint4 v = __ldg(r4 + i);
-            col[(4 * i) * DEC6_CHUNKS] = v.x;
-            col[(4 * i + 1) * DEC6_CHUNKS] = v.y;
-            col[(4 * i + 2) * DEC6_CHUNKS] = v.z;
-            col[(4 * i + 3) * DEC6_CHUNKS] = v.w;
-        }
-        for (int i = NT & ~3; i < NT; i++) col[i * DEC6_CHUNKS] = __ldg(rec + i);
-    }
-    const uint32_t lr = __ldg(meta);
-    const uint32_t nsteps = __ldg(meta + 2), tail = __ldg(meta + 3);
-    const uint64_t pb = (uint64_t)__ldg(meta + 4) | ((uint64_t)__ldg(meta + 5) << 32);
-    const uint64_t pe = (uint64_t)__ldg(meta + 6) | ((uint64_t)__ldg(meta + 7) << 32);
-    uint32_t st0 = __ldg(meta + 8), st1 = __ldg(meta + 9), st2 = __ldg(meta + 10), st3 = __ldg(meta + 11);
-    uint8_t* dst = out + chunks[c].out_off;
-
-    // ---- payload ring (256 bytes, private): raw copy of the stream from the 16-byte aligned unit that holds the first
-    // payload bit; units that start at or after the end of the payload (or would leave the buffer) are zero filled
-    const uint8_t* bytes = reinterpret_cast<const uint8_t*>(words);
-    const uint64_t base_b = (pb >> 3) & ~15ull;
-    const uint32_t rel = (uint32_t)(pb - 8 * base_b);  // 0..135
-    const uint64_t end_b = (pe + 7) >> 3;
-    const uint64_t lim_b = words_len * 4;
-    const uint64_t lim_u = lim_b >= 15 ? lim_b - 15 : 0;
-    const uint64_t stop_b = end_b < lim_u ? end_b : lim_u;
-    int32_t left = stop_b > base_b ? (int32_t)((stop_b - base_b + 15) >> 4) : 0;  // valid 16-byte units still to copy
-    const uint8_t* src = bytes + base_b;
-    const uint32_t ring_base = smem_u32(s_dec6 + NT * DEC6_CHUNKS + t * 64);
-    uint32_t fill = 0;  // bytes copied into the ring so far (unwrapped, multiple of 64)
-    auto issue_round = [&]() {
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const bool ok = left > 0;
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(ring_base + ((fill + 16u * u) & 255u)), "l"(ok ? src : bytes),
-                         "r"(ok ? 16u : 0u)
-                         : "memory");
-            src += 16;
-            left--;
-        }
-        fill += 64;
-    };
-#pragma unroll 1
-    for (int r = 0; r < 4; r++) issue_round();
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-
-    // ---- bit reader: `head` holds the next nbits (multiple of 16) bits of the payload, most significant first
-    const uint32_t sh = rel & 31u;
-    uint32_t rp = (rel >> 5) * 4u;  // ring byte offset (unwrapped) of the next word to pull
-    auto ring_be32 = [&](uint32_t off) -> uint32_t {
-        uint32_t v;
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(ring_base + (off & 252u)));
-        return bswap32(v);
-    };
-    uint64_t head;
-    uint32_t prev;
-    {
-        const uint32_t w0 = ring_be32(rp), w1 = ring_be32(rp + 4), w2 = ring_be32(rp + 8);
-        head = ((uint64_t)__funnelshift_l(w1, w0, sh) << 32) | __funnelshift_l(w2, w1, sh);
-        prev = w2;
-        rp += 12;
-    }
-    const uint32_t rp0 = rp;
-    uint32_t nbits = 64;
-    auto refill = [&]() {  // nbits in {0, 16, 32} here
-        const uint32_t w = ring_be32(rp);
-        const uint32_t x = __funnelshift_l(w, prev, sh);
-        prev = w;
-        rp += 4;
-        head |= (uint64_t)x << (32u - nbits);
-        nbits += 32;
-    };
-    const uint32_t mask = (1u << lr) - 1u;
-    const uint32_t bm_base = smem_u32(col), sym_base = smem_u32(col + DEC_BM_WORDS * DEC6_CHUNKS);
-    uint32_t acc = 0;
-    auto decode = [&](uint32_t& st) {
-        const uint32_t slot = st & mask;
-        const uint32_t w = __umulhi(slot, 178956971u);  // slot / 24
-        uint32_t b, e;
-        asm("ld.shared.u32 %0, [%1];" : "=r"(b) : "r"(bm_base + w * COL));
-        const uint32_t r = slot - 24u * w;
-        const uint32_t p = (uint32_t)__popc(b & ((2u << r) - 1u));
-        asm("ld.shared.u32 %0, [%1];" : "=r"(e) : "r"(sym_base + (b >> 24) * COL + p * COL));
-        uint32_t nst = (e >> 20) * (st >> lr) + (slot - ((e >> 8) & 0xFFFu));  // D(x) (ANSRangeCodec.go:849)
-        if (nst < (uint32_t)ANS_TOP) {  // renormalise: 16 bits, big endian (:851-856)
-            nst = (nst << 16) | (uint32_t)(head >> 48);
-            head <<= 16;
-            nbits -= 16;
-        }
-        st = nst;
-        acc = __byte_perm(acc, e, 0x4321);  // acc = (acc >> 8) | (sym << 24)
-    };
-    auto step = [&]() -> uint32_t {  // one symbol per state in the order st3, st2, st1, st0 (:904-917); returns [s3 s2 s1 s0]
-        if (nbits <= 32) refill();
-        decode(st3);
-        decode(st2);
-        if (nbits <= 32) refill();
-        decode(st1);
-        decode(st0);
-        return acc;
-    };
-    const uint32_t iters = nsteps >> 2;
-    uint4* d4 = reinterpret_cast<uint4*>(dst);
-    for (uint32_t it = 0; it < iters; it++) {
-        uint4 o;
-        o.x = step();
-        o.y = step();
-        o.z = step();
-        o.w = step();
-        d4[it] = o;
-        asm volatile("cp.async.wait_group 0;" ::: "memory");  // the round issued one iteration ago has landed
-        // refill when at most 160 bytes are buffered ahead of the reader: the new round only overwrites consumed bytes
-        if ((int32_t)(fill - rp) <= 160) issue_round();
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    for (uint32_t s = iters << 2; s < nsteps; s++) {  // only the last chunk of a block has nsteps % 4 != 0
-        const uint32_t w = step();
-        dst[4 * s] = (uint8_t)w;
-        dst[4 * s + 1] = (uint8_t)(w >> 8);
-        dst[4 * s + 2] = (uint8_t)(w >> 16);
-        dst[4 * s + 3] = (uint8_t)(w >> 24);
-    }
-    if (tail) {  // the tail bytes follow the consumed words (:951-954)
-        uint64_t pos = pb + 64ull + 8ull * (rp - rp0) - nbits;
         for (uint32_t j = 0; j < tail; j++, pos += 8) dst[(size_t)nsteps * 4 + j] = pos + 8 <= pe ? (uint8_t)bits_at(words, pos, 8) : 0;
     }
 }

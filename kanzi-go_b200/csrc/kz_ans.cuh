@@ -37,14 +37,12 @@ static const int ENC_OUT_RING_WORDS = 64;
 static const int ENC_WARP_WORDS = 256 * 8 + 8 * ENC_OUT_RING_WORDS + 8 * 16;
 static const int ENC_CTA_CHUNKS = 64;
 static const size_t ENC_SMEM = (4096 + 8 * ENC_WARP_WORDS) * sizeof(uint32_t);
-// decode: per warp (8 chunks): 171x8 bitmap buckets (24 slots each) + 256x8 symbol entries + 8 rings of 64 words; 2 warps per CTA
+// decode: per warp (8 chunks) 8 rings of 64 words (each 256-byte aligned) + 171x8 bucket words + 256x8 symbol words, padded
+// to 256 bytes; 2 warps per CTA, plus 256 bytes of slack to align the rings
 static const int DEC_BM_WORDS = 171;
-static const int DEC_WARP_WORDS = (DEC_BM_WORDS + 256) * 8 + 8 * 64;
 static const int DEC_CTA_CHUNKS = 16;
-static const size_t DEC_SMEM = 2 * DEC_WARP_WORDS * sizeof(uint32_t);
-// decode v4: per warp 8 rings of 64 words (each 256-byte aligned) + 171x8 bucket words + 256x8 symbol words, padded to 256 bytes
-static const int DEC4_WARP_WORDS = ((8 * 64 + (DEC_BM_WORDS + 256) * 8) + 63) & ~63;
-static const size_t DEC4_SMEM = 2 * DEC4_WARP_WORDS * sizeof(uint32_t) + 256;
+static const int DEC_WARP_WORDS = ((8 * 64 + (DEC_BM_WORDS + 256) * 8) + 63) & ~63;
+static const size_t DEC_SMEM = 2 * DEC_WARP_WORDS * sizeof(uint32_t) + 256;
 
 // expands the per-block descriptors into per-chunk ones on the device (grid: (ceil(max chunks per block / 256), blocks))
 __global__ void expand_chunks_kernel(const DecBlock* blocks, int nblocks, DecChunk* chunks);
@@ -58,20 +56,12 @@ __global__ void ans_walk_kernel(const uint32_t* words, const DecBlock* blocks, i
                                 int32_t* status);
 __global__ void ans0_walk_kernel(const uint32_t* words, uint64_t words_len, const DecBlock* blocks, int nblocks, uint64_t* chunk_hdr_bit,
                                  uint64_t* blk_end, int32_t* status);
-__global__ void ans0_decode_kernel(const uint32_t* words, uint64_t words_len, const DecChunk* chunks, int nchunks, const uint64_t* chunk_hdr_bit,
-                                   uint8_t* out, int32_t* status);
-// decode v5: per chunk record written by ans0_tables_kernel: 171 bucket words | 256 symbol entries | 12 words of chunk state
+// per chunk record written by ans0_tables_kernel: 171 bucket words | 256 symbol entries | 12 words of chunk state
 static const int DEC_TAB_WORDS = 440;
 __global__ void ans0_tables_kernel(const uint32_t* words, uint64_t words_len, const DecChunk* chunks, int nchunks, const uint64_t* chunk_hdr_bit,
                                    uint32_t* tabs, uint8_t* out, int32_t* status);
-__global__ void ans0_decode5_kernel(const uint32_t* words, uint64_t words_len, const uint32_t* tabs, const DecChunk* chunks, int nchunks,
-                                    const uint64_t* chunk_hdr_bit, uint8_t* out, int32_t* status);
-// decode v6: one thread per chunk, 112 chunks per CTA: 427 table words + 64 ring words per chunk
-static const int DEC6_CHUNKS = 112;
-static const size_t DEC6_SMEM = (size_t)DEC6_CHUNKS * (DEC_BM_WORDS + 256 + 64) * sizeof(uint32_t);
-__global__ void ans0_decode6_kernel(const uint32_t* words, uint64_t words_len, const uint32_t* tabs, const DecChunk* chunks, int nchunks, uint8_t* out);
-__global__ void ans0_decode4_kernel(const uint32_t* words, uint64_t words_len, const DecChunk* chunks, int nchunks, const uint64_t* chunk_hdr_bit,
-                                    uint8_t* out, int32_t* status);
+__global__ void ans0_decode_kernel(const uint32_t* words, uint64_t words_len, const uint32_t* tabs, const DecChunk* chunks, int nchunks,
+                                   const uint64_t* chunk_hdr_bit, uint8_t* out, int32_t* status);
 
 // ---- bit-granular concatenation (kz_concat.cu)
 // seg_dst[i] = absolute destination bit of segment i; copies seg_bits[i] bits from seg_src[i] (byte address, any alignment)

@@ -129,33 +129,24 @@ struct CtxLzHook : LzHook {
         cur = nullptr;
     }
 };
-// KZ_LZ_PARSE=serial selects the round-1 parse (one lane per block replays the reference loop); default: the data-parallel path
-bool lz_serial_parse() {
-    static const bool v = [] {
-        const char* e = getenv("KZ_LZ_PARSE");
-        return e && e[0] == 's';
-    }();
-    return v;
-}
-
 // LZ / LZX forward of a batch: the data-parallel path (kz_lz_par.cu); blocks it hands back (status 3: no fixed point of the table
-// membership within its round limit) and everything under KZ_LZ_PARSE=serial go through the serial parse of kz_lz.cu.
+// membership within its round limit) go through the serial parse of kz_lz.cu.
 int upload(kz_ctx* ctx, Packer& pk);
 int lz_forward_batch(kz_ctx* ctx, const uint8_t* d_in, uint8_t* d_out, std::vector<LzBlock>& lb, bool extra, std::vector<LzResult>& hres) {
     const uint32_t nblocks = (uint32_t)lb.size();
     hres.assign(nblocks, LzResult{1, 0, 0, 0, 0, 0, 0});
-    bool serial = lz_serial_parse();
-    if (!serial) {
+    {
         CtxLzWorkspace W(ctx);
         CtxLzHook H(ctx);
         CK(lz_forward_parallel(d_in, d_out, lb, extra, W, ctx->stream, hres, &H));
+        bool serial = false;
         for (uint32_t b = 0; b < nblocks; b++) serial = serial || hres[b].status == 3;
         if (!serial) return 0;
     }
     uint32_t max_len = 0;
     std::vector<LzBlock> sb(lb);
     for (uint32_t b = 0; b < nblocks; b++) {
-        if (!lz_serial_parse() && hres[b].status != 3) sb[b].len = 0;  // done by the parallel path
+        if (hres[b].status != 3) sb[b].len = 0;  // done by the parallel path
         max_len = std::max(max_len, sb[b].len);
     }
     const uint64_t sstride = (lz_scratch_bytes(max_len) + 255) & ~size_t(255);
@@ -185,7 +176,7 @@ int lz_forward_batch(kz_ctx* ctx, const uint8_t* d_in, uint8_t* d_out, std::vect
     CK(cudaMemcpyAsync(sres.data(), d_res, (size_t)nblocks * sizeof(LzResult), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     for (uint32_t b = 0; b < nblocks; b++)
-        if (lz_serial_parse() || hres[b].status == 3) hres[b] = sres[b];
+        if (hres[b].status == 3) hres[b] = sres[b];
     return 0;
 }
 
@@ -737,25 +728,15 @@ int decode_batch(kz_ctx* ctx, uint32_t etype, const uint32_t* d_words, uint64_t 
             ans0_walk_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_words, words_len, (DecBlock*)(T + o_blocks), nblocks, (uint64_t*)(T + o_hbit),
                                                               (uint64_t*)(T + o_end), d_status);
         }
-        if (ctx->ans0_dec_version >= 5) {
+        {
             CK(ctx->d_enc_tab.ensure((size_t)nchunks * DEC_TAB_WORDS * sizeof(uint32_t) + 256));
             LaunchScope ls(ctx, "ans0_tables");
             ans0_tables_kernel<<<(nchunks + 3) / 4, 128, 0, ctx->stream>>>(d_words, words_len, d_dchunks, nchunks, (uint64_t*)(T + o_hbit),
                                                                         ctx->d_enc_tab.as<uint32_t>(), d_out, d_status);
         }
         LaunchScope ls(ctx, "ans0_decode");
-        if (ctx->ans0_dec_version >= 6)
-            ans0_decode6_kernel<<<(nchunks + DEC6_CHUNKS - 1) / DEC6_CHUNKS, 128, DEC6_SMEM, ctx->stream>>>(
-                d_words, words_len, ctx->d_enc_tab.as<uint32_t>(), d_dchunks, nchunks, d_out);
-        else if (ctx->ans0_dec_version >= 5)
-            ans0_decode5_kernel<<<(nchunks + DEC_CTA_CHUNKS - 1) / DEC_CTA_CHUNKS, 64, DEC4_SMEM, ctx->stream>>>(
-                d_words, words_len, ctx->d_enc_tab.as<uint32_t>(), d_dchunks, nchunks, (uint64_t*)(T + o_hbit), d_out, d_status);
-        else if (ctx->ans0_dec_version == 3)
-            ans0_decode_kernel<<<(nchunks + DEC_CTA_CHUNKS - 1) / DEC_CTA_CHUNKS, 64, DEC_SMEM, ctx->stream>>>(d_words, words_len, d_dchunks,
-                                                                                                   nchunks, (uint64_t*)(T + o_hbit), d_out, d_status);
-        else
-            ans0_decode4_kernel<<<(nchunks + DEC_CTA_CHUNKS - 1) / DEC_CTA_CHUNKS, 64, DEC4_SMEM, ctx->stream>>>(d_words, words_len, d_dchunks,
-                                                                                                     nchunks, (uint64_t*)(T + o_hbit), d_out, d_status);
+        ans0_decode_kernel<<<(nchunks + DEC_CTA_CHUNKS - 1) / DEC_CTA_CHUNKS, 64, DEC_SMEM, ctx->stream>>>(
+            d_words, words_len, ctx->d_enc_tab.as<uint32_t>(), d_dchunks, nchunks, (uint64_t*)(T + o_hbit), d_out, d_status);
     }
     if (!xjobs.empty()) {
         LaunchScope ls(ctx, "extract");
@@ -921,13 +902,6 @@ struct TransformPlan {
     }
 };
 
-// The stages added last (PACK / DNA / MM, LZ / LZX inside sequences, the magic-number data type, TEXT) can be switched off with
-// KZ_EXPERIMENTAL=0: the library then answers "not available" for them, as it did before they existed.
-bool experimental_stages() {
-    const char* e = getenv("KZ_EXPERIMENTAL");
-    return !(e && e[0] == '0');
-}
-
 // etype: the entropy codec of the stream. The reference picks the TEXT encoding from it (transform/Factory.go:99-119): encoding 2 for NONE /
 // ANS0 / HUFFMAN / RANGE, encoding 1 otherwise; only encoding 2 (textCodec2) exists here, so TEXT with any other codec is refused
 // rather than written in a form the reference could not read.
@@ -936,13 +910,6 @@ int plan_transforms(kz_ctx* ctx, uint64_t t48, uint32_t etype, TransformPlan& p,
     for (int i = 0; i < p.nt; i++)
         if (p.ids[i] == KZ_T_TEXT && !(etype == KZ_E_NONE || etype == KZ_E_ANS0 || etype == KZ_E_HUFFMAN || etype == KZ_E_RANGE))
             return ctx->fail(err_code, "TEXT with this entropy codec selects the reference's text encoding 1, which the GPU path does not implement (NONE / ANS0 / HUFFMAN / RANGE select encoding 2)");
-    if (!experimental_stages()) {
-        for (int i = 0; i < p.nt; i++) {
-            const uint64_t t = p.ids[i];
-            const bool newer = t == KZ_T_PACK || t == KZ_T_DNA || t == KZ_T_MM || t == KZ_T_TEXT || t == KZ_T_UTF || t == KZ_T_EXE || ((t == KZ_T_LZ || t == KZ_T_LZX) && p.nt > 1);
-            if (newer) return ctx->fail(err_code, "transform stage switched off by KZ_EXPERIMENTAL=0: PACK / DNA / MM / TEXT, LZ / LZX inside a sequence");
-        }
-    }
     for (int i = 0; i < p.nt; i++)
         if (p.ids[i] == KZ_T_TEXT && !text_available())
             return ctx->fail(err_code, "TEXT: the library was built without the static dictionary (kanzi-go_b200/gen_text_dict.py)");
@@ -965,54 +932,36 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
     if (t == KZ_T_BWT) {
         CK(ctx->d_lens.ensure((size_t)nblocks * 4 + 64));
         uint32_t* d_post = ctx->d_lens.as<uint32_t>();
-        static const bool one_by_one = [] {  // KZ_BWT_FWD=single: one suffix sort per block (round 1)
-            const char* e = getenv("KZ_BWT_FWD");
-            return e && e[0] == 's' && e[1] == 'i';
-        }();
-        if (one_by_one) {
-            uint32_t max_len = 0;
-            for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, len[b]);
-            CK(ctx->d_ws.ensure(bwt_forward_workspace(max_len)));
-            for (uint32_t b = 0; b < nblocks; b++) {
+        // all blocks of a sub-batch are suffix-sorted together (kz_bwt.cu: bwt_forward_batch)
+        for (uint32_t b0 = 0; b0 < nblocks;) {
+            std::vector<uint64_t> so, dof;
+            std::vector<uint32_t> nn, num;
+            uint64_t total = 0;
+            uint32_t b = b0;
+            for (; b < nblocks; b++) {
                 if (!active[b] || len[b] < 2) continue;
-                LaunchScope ls(ctx, "bwt_forward");
-                cudaError_t e = bwt_forward_device(d_in + b * istride, len[b], d_out + b * ostride, d_post + b, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream,
-                                                   &ctx->launches);
-                if (e == cudaSuccess) applied[b] = 1;
-                else if (e != cudaErrorInvalidValue) return ctx->cuda_fail(e, "bwt_forward");
-            }
-        } else {
-            // all blocks of a sub-batch are suffix-sorted together (kz_bwt.cu: bwt_forward_batch)
-            for (uint32_t b0 = 0; b0 < nblocks;) {
-                std::vector<uint64_t> so, dof;
-                std::vector<uint32_t> nn, num;
-                uint64_t total = 0;
-                uint32_t b = b0;
-                for (; b < nblocks; b++) {
-                    if (!active[b] || len[b] < 2) continue;
-                    if (len[b] > bwt_forward_batch_max_total()) {  // a block the batch's key layout cannot hold (1 GiB): its own suffix sort
-                        if (!nn.empty()) break;                    // flush what has been collected first
-                        CK(ctx->d_ws.ensure(bwt_forward_workspace(len[b])));
-                        LaunchScope ls(ctx, "bwt_forward");
-                        cudaError_t e = bwt_forward_device(d_in + b * istride, len[b], d_out + b * ostride, d_post + b, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                           ctx->stream, &ctx->launches);
-                        if (e == cudaSuccess) applied[b] = 1;
-                        else if (e != cudaErrorInvalidValue) return ctx->cuda_fail(e, "bwt_forward");
-                        continue;
-                    }
-                    if (!nn.empty() && (total + len[b] > bwt_forward_batch_max_total() || nn.size() >= bwt_forward_batch_max_blocks())) break;
-                    so.push_back(b * istride), dof.push_back(b * ostride), nn.push_back(len[b]), num.push_back(b);
-                    total += len[b];
+                if (len[b] > bwt_forward_batch_max_total()) {  // a block the batch's key layout cannot hold (1 GiB): its own suffix sort
+                    if (!nn.empty()) break;                    // flush what has been collected first
+                    CK(ctx->d_ws.ensure(bwt_forward_workspace(len[b])));
+                    LaunchScope ls(ctx, "bwt_forward");
+                    cudaError_t e = bwt_forward_device(d_in + b * istride, len[b], d_out + b * ostride, d_post + b, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
+                                                       ctx->stream, &ctx->launches);
+                    if (e == cudaSuccess) applied[b] = 1;
+                    else if (e != cudaErrorInvalidValue) return ctx->cuda_fail(e, "bwt_forward");
+                    continue;
                 }
-                b0 = b;
-                if (nn.empty()) continue;
-                CK(ctx->d_ws.ensure(bwt_forward_batch_workspace(total, (uint32_t)nn.size())));
-                LaunchScope ls(ctx, "bwt_forward");
-                cudaError_t e = bwt_forward_batch(d_in, d_out, so.data(), dof.data(), nn.data(), num.data(), (uint32_t)nn.size(), d_post, ctx->d_ws.as<uint8_t>(),
-                                                  ctx->d_ws.cap, ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_forward");
-                for (uint32_t k : num) applied[k] = 1;
+                if (!nn.empty() && (total + len[b] > bwt_forward_batch_max_total() || nn.size() >= bwt_forward_batch_max_blocks())) break;
+                so.push_back(b * istride), dof.push_back(b * ostride), nn.push_back(len[b]), num.push_back(b);
+                total += len[b];
             }
+            b0 = b;
+            if (nn.empty()) continue;
+            CK(ctx->d_ws.ensure(bwt_forward_batch_workspace(total, (uint32_t)nn.size())));
+            LaunchScope ls(ctx, "bwt_forward");
+            cudaError_t e = bwt_forward_batch(d_in, d_out, so.data(), dof.data(), nn.data(), num.data(), (uint32_t)nn.size(), d_post, ctx->d_ws.as<uint8_t>(),
+                                              ctx->d_ws.cap, ctx->stream, &ctx->launches);
+            if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_forward");
+            for (uint32_t k : num) applied[k] = 1;
         }
         std::vector<uint32_t> post(nblocks);
         CK(cudaMemcpyAsync(post.data(), d_post, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1438,49 +1387,29 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         std::vector<uint8_t> heads((size_t)nblocks * 64, 0);
         CK(cudaMemcpy2DAsync(heads.data(), 64, d_in, stride, 33, nblocks, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        static const bool one_by_one = [] {  // KZ_BWT_INV=single: one set of launches per block (round 1)
-            const char* e = getenv("KZ_BWT_INV");
-            return e && e[0] == 's';
-        }();
-        if (one_by_one) {
-            uint32_t max_len = 0;
-            for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, len[b]);
-            CK(ctx->d_ws.ensure(bwt_inverse_workspace(max_len)));
-            for (uint32_t b = 0; b < nblocks; b++) {
+        for (uint32_t b0 = 0; b0 < nblocks;) {
+            std::vector<uint64_t> so, dof;
+            std::vector<uint32_t> ll, num;
+            std::vector<uint8_t> hh;
+            uint64_t total = 0;
+            uint32_t b = b0;
+            for (; b < nblocks; b++) {
                 if (!active[b]) continue;
-                uint32_t produced = 0;
-                LaunchScope ls(ctx, "bwt_inverse");
-                cudaError_t e = bwt_inverse_device(d_in + b * stride, &heads[(size_t)b * 64], len[b], d_out + b * stride, cap, &produced, ctx->d_ws.as<uint8_t>(),
-                                                   ctx->d_ws.cap, ctx->stream, &ctx->launches);
-                if (e == cudaErrorInvalidValue) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header");
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
-                len[b] = produced;
+                if (!ll.empty() && (total + len[b] > bwt_inverse_batch_max_total() || ll.size() >= bwt_inverse_batch_max_blocks())) break;
+                so.push_back(b * stride), dof.push_back(b * stride), ll.push_back(len[b]), num.push_back(b);
+                hh.insert(hh.end(), heads.begin() + (size_t)b * 64, heads.begin() + (size_t)(b + 1) * 64);
+                total += len[b];
             }
-        } else {
-            for (uint32_t b0 = 0; b0 < nblocks;) {
-                std::vector<uint64_t> so, dof;
-                std::vector<uint32_t> ll, num;
-                std::vector<uint8_t> hh;
-                uint64_t total = 0;
-                uint32_t b = b0;
-                for (; b < nblocks; b++) {
-                    if (!active[b]) continue;
-                    if (!ll.empty() && (total + len[b] > bwt_inverse_batch_max_total() || ll.size() >= bwt_inverse_batch_max_blocks())) break;
-                    so.push_back(b * stride), dof.push_back(b * stride), ll.push_back(len[b]), num.push_back(b);
-                    hh.insert(hh.end(), heads.begin() + (size_t)b * 64, heads.begin() + (size_t)(b + 1) * 64);
-                    total += len[b];
-                }
-                b0 = b;
-                if (ll.empty()) continue;
-                CK(ctx->d_ws.ensure(bwt_inverse_batch_workspace(total, (uint32_t)ll.size())));
-                std::vector<uint32_t> produced(ll.size(), 0);
-                LaunchScope ls(ctx, "bwt_inverse");
-                cudaError_t e = bwt_inverse_batch(d_in, d_out, so.data(), dof.data(), ll.data(), hh.data(), (uint32_t)ll.size(), cap, produced.data(),
-                                                  ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
-                if (e == cudaErrorInvalidValue) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header or data");
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
-                for (size_t k = 0; k < num.size(); k++) len[num[k]] = produced[k];
-            }
+            b0 = b;
+            if (ll.empty()) continue;
+            CK(ctx->d_ws.ensure(bwt_inverse_batch_workspace(total, (uint32_t)ll.size())));
+            std::vector<uint32_t> produced(ll.size(), 0);
+            LaunchScope ls(ctx, "bwt_inverse");
+            cudaError_t e = bwt_inverse_batch(d_in, d_out, so.data(), dof.data(), ll.data(), hh.data(), (uint32_t)ll.size(), cap, produced.data(),
+                                              ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
+            if (e == cudaErrorInvalidValue) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header or data");
+            if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
+            for (size_t k = 0; k < num.size(); k++) len[num[k]] = produced[k];
         }
     } else if (t == KZ_T_BWTS) {
         uint32_t max_len = 0;
@@ -1539,31 +1468,11 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         }
         std::vector<uint32_t> hl(nblocks);
         std::vector<int32_t> hs(nblocks);
-        static const bool serial_inverse = [] {  // KZ_LZ_INV=serial: the round-1 kernel (one warp per block copies match by match)
-            const char* e = getenv("KZ_LZ_INV");
-            return e && e[0] == 's';
-        }();
-        if (!serial_inverse) {
+        {
             CtxLzWorkspace W(ctx);
             CtxLzHook H(ctx);
             cudaError_t e = lz_inverse_parallel(d_in, d_out, lb, W, ctx->stream, hl, hs, &H, &ctx->launches);
             if (e != cudaSuccess) return ctx->cuda_fail(e, "lz_inverse");
-        } else {
-            Packer pk;
-            const size_t o_lb = pk.add(lb.data(), lb.size() * sizeof(LzBlock));
-            const size_t o_len = pk.reserve((size_t)nblocks * 4);
-            const size_t o_st = pk.reserve((size_t)nblocks * 4);
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "lz_inverse");
-                lz_inverse_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_in, (LzBlock*)(T + o_lb), (int)nblocks, d_out, (uint32_t*)(T + o_len), (int32_t*)(T + o_st));
-            }
-            CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(hl.data(), T + o_len, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaMemcpyAsync(hs.data(), T + o_st, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
         }
         for (uint32_t b = 0; b < nblocks; b++) {
             if (!active[b] || len[b] == 0) continue;
@@ -1695,26 +1604,17 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
             fb[b].pad = 0;
         }
         Packer pk;
-        const size_t o_fb = pk.add(fb.data(), fb.size() * sizeof(FsdBlock));
         const size_t o_res = pk.reserve((size_t)nblocks * sizeof(FsdResult));
         int rc = upload(ctx, pk);
         if (rc) return rc;
         uint8_t* T = ctx->d_tables.as<uint8_t>();
         {
-            static const bool warp_per_block = [] {  // KZ_MM_INV=warp: one warp per block walks the rounds (first data-parallel version)
-                const char* e = getenv("KZ_MM_INV");
-                return e && e[0] == 'w';
-            }();
             LaunchScope ls(ctx, "fsd_inverse");
-            cudaError_t e;
-            if (warp_per_block) {
-                e = fsd_inverse_batch(d_in, d_out, (const FsdBlock*)(T + o_fb), nblocks, (FsdResult*)(T + o_res), ctx->stream, &ctx->launches);
-            } else {
-                uint64_t total_len = 0;
-                for (uint32_t b = 0; b < nblocks; b++) total_len += fb[b].len;
-                CK(ctx->d_ws.ensure(fsd_inverse_workspace(nblocks, total_len)));
-                e = fsd_inverse_tiles(d_in, d_out, fb.data(), nblocks, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, (FsdResult*)(T + o_res), ctx->stream, &ctx->launches);
-            }
+            uint64_t total_len = 0;
+            for (uint32_t b = 0; b < nblocks; b++) total_len += fb[b].len;
+            CK(ctx->d_ws.ensure(fsd_inverse_workspace(nblocks, total_len)));
+            cudaError_t e = fsd_inverse_tiles(d_in, d_out, fb.data(), nblocks, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, (FsdResult*)(T + o_res), ctx->stream,
+                                              &ctx->launches);
             if (e != cudaSuccess) return ctx->cuda_fail(e, "fsd_inverse");
         }
         std::vector<FsdResult> hr(nblocks);
@@ -2025,30 +1925,11 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
         }
         std::vector<uint32_t> hl(nblocks);
         std::vector<int32_t> hs(nblocks);
-        static const bool serial_inverse = [] {  // KZ_LZ_INV=serial: the round-1 kernel (one warp per block copies match by match)
-            const char* e = getenv("KZ_LZ_INV");
-            return e && e[0] == 's';
-        }();
-        if (!serial_inverse) {  // the stream's only stage is LZ / LZX (kanzi -l 1): the same data-parallel inverse as inside a sequence
+        {  // the stream's only stage is LZ / LZX (kanzi -l 1): the same data-parallel inverse as inside a sequence
             CtxLzWorkspace W(ctx);
             CtxLzHook H(ctx);
             cudaError_t e = lz_inverse_parallel(d_pre, d_dst, lb, W, ctx->stream, hl, hs, &H, &ctx->launches);
             if (e != cudaSuccess) return ctx->cuda_fail(e, "lz_inverse");
-        } else {
-            Packer pk;
-            const size_t o_lb = pk.add(lb.data(), lb.size() * sizeof(LzBlock));
-            const size_t o_len = pk.reserve((size_t)nblocks * 4);
-            const size_t o_st = pk.reserve((size_t)nblocks * 4);
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "lz_inverse");
-                lz_inverse_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_pre, (LzBlock*)(T + o_lb), (int)nblocks, d_dst, (uint32_t*)(T + o_len), (int32_t*)(T + o_st));
-            }
-            CK(cudaMemcpyAsync(hl.data(), T + o_len, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaMemcpyAsync(hs.data(), T + o_st, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
         }
         uint64_t off = 0;
         for (uint32_t b = 0; b < nblocks; b++) {
@@ -2162,10 +2043,6 @@ int kz_init(int device, kz_ctx** out) {
     }
     cudaFuncSetAttribute(ans0_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENC_SMEM);
     cudaFuncSetAttribute(ans0_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DEC_SMEM);
-    cudaFuncSetAttribute(ans0_decode4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DEC4_SMEM);
-    cudaFuncSetAttribute(ans0_decode5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DEC4_SMEM);
-    cudaFuncSetAttribute(ans0_decode6_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DEC6_SMEM);
-    if (const char* v = getenv("KZ_ANS0_DEC")) ctx->ans0_dec_version = atoi(v);  // 3 = previous kernel generation (A/B measurements)
     cudaFuncSetAttribute(huf_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HUF_DEC_SMEM);
     *out = ctx;
     return 0;
@@ -2301,7 +2178,7 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     if (rc) return rc;
     const uint8_t* d_data = nullptr;
     std::vector<int32_t> init_dt;
-    if (plan.uses_magic() && nblocks && experimental_stages()) {  // the first four bytes of every block decide its initial data type
+    if (plan.uses_magic() && nblocks) {  // the first four bytes of every block decide its initial data type
         std::vector<uint8_t> heads((size_t)nblocks * 4, 0);
         const size_t last = n - (size_t)(nblocks - 1) * block_size;
         if (nblocks > 1) CK(cudaMemcpy2DAsync(heads.data(), 4, d_src, block_size, 4, nblocks - 1, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2640,8 +2517,7 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     if (rc) return rc;
     const uint8_t* d_data = nullptr;
     std::vector<int32_t> init_dt(nblocks, 0);
-    if (experimental_stages())
-        for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(slab + b * block_stride, block_len[b]);
+    for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(slab + b * block_stride, block_len[b]);
     rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), 0, 0, dstride, block_len, nblocks, &d_data, jobs, &init_dt);
     if (rc) return rc;
     if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
@@ -2819,8 +2695,6 @@ int kz_entropy_decode(kz_ctx* ctx, uint32_t type, const uint8_t* src, size_t src
 }
 
 int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
-    if ((type == KZ_T_PACK || type == KZ_T_DNA || type == KZ_T_MM || type == KZ_T_TEXT || type == KZ_T_UTF || type == KZ_T_EXE) && ctx && !experimental_stages())
-        return ctx->fail(KZ_ERR_CREATE_CODEC, "transform switched off by KZ_EXPERIMENTAL=0: PACK / DNA / MM / TEXT");
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     ctx->stream_bs = ctx->user_stream_bs;
@@ -2894,8 +2768,6 @@ int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8
 }
 
 int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
-    if ((type == KZ_T_PACK || type == KZ_T_DNA || type == KZ_T_MM || type == KZ_T_TEXT || type == KZ_T_UTF || type == KZ_T_EXE) && ctx && !experimental_stages())
-        return ctx->fail(KZ_ERR_CREATE_CODEC, "transform switched off by KZ_EXPERIMENTAL=0: PACK / DNA / MM / TEXT");
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     ctx->stream_bs = ctx->user_stream_bs;

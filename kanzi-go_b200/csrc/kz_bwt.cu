@@ -522,29 +522,6 @@ __global__ void __launch_bounds__(256) bwtu_apply_kernel(uint32_t* __restrict__ 
     sa[cpos[u]] = v;
     rank[v] = g;
 }
-// segmented variant of a later round: the compacted members are already grouped (a group = a contiguous range), so each group is a segment
-// sorted by the 32-bit second key alone
-__global__ void __launch_bounds__(256) bwtu_keys32_kernel(const uint32_t* __restrict__ rank, const uint32_t* __restrict__ cval, uint32_t m,
-                                                           const BwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t h, uint32_t* __restrict__ lo_keys,
-                                                           uint8_t* __restrict__ segflag) {
-    __shared__ uint32_t s_base[BWT_BATCH_MAX];
-    __shared__ uint32_t s_n[BWT_BATCH_MAX];
-    for (uint32_t k = threadIdx.x; k < nb; k += 256) s_base[k] = blocks[k].base, s_n[k] = blocks[k].n;
-    __syncthreads();
-    const uint32_t u = blockIdx.x * 256 + threadIdx.x;
-    if (u >= m) return;
-    const uint32_t i = cval[u];
-    const uint32_t b = bwtb_find(s_base, nb, i);
-    const uint64_t end = (uint64_t)s_base[b] + s_n[b];
-    lo_keys[u] = (uint64_t)i + h < end ? rank[i + h] + 1 : 0;
-    segflag[u] = (u == 0 || rank[cval[u - 1]] != rank[i]) ? 1 : 0;
-}
-__global__ void __launch_bounds__(256) bwtu_heads32_kernel(const uint32_t* __restrict__ lo_sorted, const uint8_t* __restrict__ segflag, const uint32_t* __restrict__ cpos,
-                                                            uint32_t m, uint32_t* __restrict__ f) {
-    const uint32_t u = blockIdx.x * 256 + threadIdx.x;
-    if (u >= m) return;
-    f[u] = (segflag[u] || lo_sorted[u] != lo_sorted[u - 1]) ? cpos[u] : 0u;
-}
 }  // namespace
 
 size_t bwt_forward_batch_workspace(uint64_t total, uint32_t nblocks) {
@@ -554,7 +531,7 @@ size_t bwt_forward_batch_workspace(uint64_t total, uint32_t nblocks) {
     cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int64_t)total, 0, 64);
     size_t temp2 = 0;
     cub::DeviceSelect::Flagged(nullptr, temp2, (const uint32_t*)nullptr, (const uint8_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)total);
-    size_t temp3 = 0;
+    size_t temp3 = 0;  // no round runs a segmented sort, but its scratch size is still part of the workspace bound
     cub::DeviceSegmentedSort::SortPairs(nullptr, temp3, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)total,
                                         (int64_t)total, (const uint32_t*)nullptr, (const uint32_t*)nullptr);
     return (size_t)total * (8 * 2 + 4 * 2 + 4 + 4 + 4 * 4 + 1) + 4 * ((size_t)total / 2048 + 16) + (size_t)nblocks * sizeof(BwtBatchBlock) + 16 * 256 +
@@ -617,13 +594,9 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
     int end_bit = 64;
     uint32_t max_n = 0;
     for (uint32_t k = 0; k < nb; k++) max_n = std::max(max_n, hb[k].n);
-    static const bool full_rounds = [] {  // KZ_BWT_FWD=full: every round sorts the whole batch (first batched version)
-        const char* ev = getenv("KZ_BWT_FWD");
-        return ev && ev[0] == 'f';
-    }();
+    // round 0: the whole batch
     uint32_t* sa = nullptr;
-    // round 0 (and every round under KZ_BWT_FWD=full): the whole batch
-    for (int round = 0; round < 40; round++) {
+    {
         cub::DoubleBuffer<uint64_t> k(keys_a, keys_b);
         cub::DoubleBuffer<uint32_t> v(idx_a, idx_b);
         size_t tb = temp_bytes;
@@ -649,13 +622,7 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
             (*launches) += 2;
             return cudaGetLastError();
         }
-        if (!full_rounds) break;
-        bwtb_double_keys_kernel<<<G, T, 0, stream>>>(rank, d_blocks, nb, total, h, lg, keys_a, idx_a);
-        (*launches)++;
-        h *= 2;
-        end_bit = 2 * (int)lg;
     }
-    if (full_rounds) return cudaErrorUnknown;
     // later rounds: the members of groups with more than one suffix only
     uint32_t m = 0;
     {
@@ -674,47 +641,18 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
     }
     end_bit = 2 * (int)lg;
     uint32_t* nhead = head;  // reused: new group heads of the compacted members
-    // later rounds: 64-bit radix sorts of (group head, second key) over the compacted members. KZ_BWT_FWD=segmented: one segment per group
-    // sorted by the 32-bit second key (cub::DeviceSegmentedSort) — measured no faster on the metric's slab
-    static const bool radix_rounds = [] {
-        const char* ev = getenv("KZ_BWT_FWD");
-        return !(ev && ev[0] == 's' && ev[1] == 'e');
-    }();
-    uint32_t* lo_in = reinterpret_cast<uint32_t*>(keys_a);
-    uint32_t* lo_out = reinterpret_cast<uint32_t*>(keys_b);
-    uint32_t* seg_off = reinterpret_cast<uint32_t*>(keys_b) + total;  // second half of keys_b: at most m + 1 offsets
+    // later rounds: 64-bit radix sorts of (group head, second key) over the compacted members
     for (int round = 1; round < 48 && m > 0; round++) {
         const uint32_t GM = (m + T - 1) / T, nscan_m = (m + 2047) / 2048;
-        const uint32_t* sorted_val = nullptr;
-        uint32_t* other = nullptr;
-        if (radix_rounds) {
-            bwtu_keys_kernel<<<GM, T, 0, stream>>>(rank, cval_a, m, d_blocks, nb, h, lg, keys_a);
-            cub::DoubleBuffer<uint64_t> k(keys_a, keys_b);
-            cub::DoubleBuffer<uint32_t> v(cval_a, cval_b);
-            size_t tb = temp_bytes;
-            e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)m, 0, end_bit, stream);
-            if (e != cudaSuccess) return e;
-            bwtu_heads_kernel<<<GM, T, 0, stream>>>(k.Current(), cpos_a, m, nhead);
-            sorted_val = v.Current();
-            other = v.Current() == cval_a ? cval_b : cval_a;
-        } else {
-            // the groups are contiguous ranges of the compacted order: one segment each, sorted by the second key alone
-            bwtu_keys32_kernel<<<GM, T, 0, stream>>>(rank, cval_a, m, d_blocks, nb, h, lo_in, uflags);
-            size_t tb = temp_bytes;
-            e = cub::DeviceSelect::Flagged(temp, tb, cub::CountingInputIterator<uint32_t>(0), uflags, seg_off, d_count, (int64_t)m, stream);
-            if (e != cudaSuccess) return e;
-            uint32_t nseg = 0;
-            if ((e = cudaMemcpyAsync(&nseg, d_count, 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
-            if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
-            if ((e = cudaMemcpyAsync(seg_off + nseg, &m, 4, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-            tb = temp_bytes;
-            e = cub::DeviceSegmentedSort::SortPairs(temp, tb, (const uint32_t*)lo_in, lo_out, (const uint32_t*)cval_a, cval_b, (int64_t)m, (int64_t)nseg, seg_off,
-                                                    seg_off + 1, stream);
-            if (e != cudaSuccess) return e;
-            bwtu_heads32_kernel<<<GM, T, 0, stream>>>(lo_out, uflags, cpos_a, m, nhead);
-            sorted_val = cval_b;
-            other = cval_a;
-        }
+        bwtu_keys_kernel<<<GM, T, 0, stream>>>(rank, cval_a, m, d_blocks, nb, h, lg, keys_a);
+        cub::DoubleBuffer<uint64_t> k(keys_a, keys_b);
+        cub::DoubleBuffer<uint32_t> v(cval_a, cval_b);
+        size_t tb = temp_bytes;
+        e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)m, 0, end_bit, stream);
+        if (e != cudaSuccess) return e;
+        bwtu_heads_kernel<<<GM, T, 0, stream>>>(k.Current(), cpos_a, m, nhead);
+        const uint32_t* sorted_val = v.Current();
+        uint32_t* other = v.Current() == cval_a ? cval_b : cval_a;
         scan_max_local_kernel<<<nscan_m, 256, 0, stream>>>(nhead, m, block_max);
         scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(block_max, nscan_m);
         bwtu_apply_kernel<<<GM, T, 0, stream>>>(nhead, block_max, cpos_a, sorted_val, m, sa, rank);
@@ -722,7 +660,7 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
         h *= 2;
         if (h >= 2 * (uint64_t)max_n) break;  // every suffix pair has been compared past the end of its block
         bwtu_flags_kernel<<<GM, T, 0, stream>>>(nhead, cpos_a, m, uflags);
-        size_t tb = temp_bytes;
+        tb = temp_bytes;
         e = cub::DeviceSelect::Flagged(temp, tb, (const uint32_t*)cpos_a, uflags, cpos_b, d_count, (int64_t)m, stream);
         if (e != cudaSuccess) return e;
         tb = temp_bytes;

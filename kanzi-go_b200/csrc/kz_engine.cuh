@@ -127,7 +127,6 @@ struct kz_ctx {
     std::string err;
     uint64_t launches = 0;
     bool profile = false;
-    int ans0_dec_version = 5;  // 6 = thread-per-chunk kernel (correct, measured slower), 4 / 3 = older generations
     kz::EncPlan enc_plan;
     bool fragment = false;        // encode_batch: LAYOUT_STREAM without the end marker (kz_compress_fragment_device)
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points

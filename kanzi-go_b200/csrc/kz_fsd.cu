@@ -357,134 +357,6 @@ __global__ void __launch_bounds__(32) fsd_final_kernel(const FsdBlock* __restric
     res[b] = r;
 }
 
-// ---- inverse: one warp per block, 32 source bytes per round (FSDCodec.go:317-401) ----
-// out[o] = f(out[o - dist]) is `dist` interleaved chains; along a chain the delta tokens are a prefix sum (mod 256) and the rare escape
-// tokens (0xFF + payload: out = payload ^ previous) cut it. A round takes 32 source bytes, one per lane:
-//   * which 0xFF bytes are escape markers is a parity question inside runs of 0xFF (a marker's successor is a payload, whatever its value),
-//     answered with one ballot and a clz per lane; the marker state is carried into the next round;
-//   * every byte that is not a marker is one output token; the k-th token moves to lane k (through 64 bytes of shared memory);
-//   * token values: inclusive shuffle scan with stride `dist` over the deltas (escape tokens count as 0) on top of the chain's last value
-//     of earlier rounds (the last 16 outputs live in the registers of lanes 0..15), then one correction per escape token of the round, in
-//     order: E = payload ^ value before it; every later token of its chain moves by E - tentative value;
-//   * one coalesced store. XOR coding is the same scan with xor and no escapes.
-// ~250 cycles per 32 bytes instead of ~140 per byte for the one-thread walk this replaces.
-__global__ void __launch_bounds__(32) fsd_inverse_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, int nblocks, uint8_t* __restrict__ out,
-                                                          FsdResult* __restrict__ res) {
-    __shared__ uint16_t s_tok[32];
-    const int b = blockIdx.x, lane = threadIdx.x;
-    if (b >= nblocks) return;
-    const FsdBlock blk = blocks[b];
-    FsdResult r;
-    r.status = 0;
-    r.out_len = 0;
-    r.data_type = 0;
-    r.mode = 0;
-    const uint32_t src_end = blk.len, dst_end = blk.cap;
-    const uint8_t* src = in + blk.src_off;
-    uint8_t* dst = out + blk.dst_off;
-    if (src_end == 0 || dst_end == 0) {
-        if (lane == 0) res[b] = r;
-        return;
-    }
-    bool bad = src_end < 2;
-    uint32_t mode = 0, dist = 0;
-    if (!bad) {
-        mode = src[0];
-        dist = src[1];
-        if (dist < 1 || (dist > 4 && dist != 8 && dist != 16)) bad = true;          // :337-339
-        if (!bad && (src_end - 2 < dist || dst_end < dist || mode > 1)) bad = true;  // :346-352, :392-394
-    }
-    if (bad) {
-        r.status = -KZ_E_PROCESS_BLOCK;
-        if (lane == 0) res[b] = r;
-        return;
-    }
-    // the first `dist` bytes are copied; tail = the last 16 outputs so far, out[di - 16 + lane] in lanes 0..15
-    uint32_t si = 2 + dist, di = dist;
-    uint32_t tail = 0;
-    if (lane < 16 && (uint32_t)lane + dist >= 16u) tail = src[2 + lane + dist - 16];
-    if ((uint32_t)lane < dist) dst[lane] = src[2 + lane];
-    uint32_t pending = 0;  // the previous round ended with an escape marker: this round's first byte is its payload
-    const uint32_t below = (1u << lane) - 1u;
-    // source bytes four rounds ahead (a round is ~500 cycles of shuffles and ballots, an HBM load ~800)
-    uint32_t n0 = si + lane < src_end ? src[si + lane] : 0u, n1 = si + 32 + lane < src_end ? src[si + 32 + lane] : 0u;
-    uint32_t n2 = si + 64 + lane < src_end ? src[si + 64 + lane] : 0u, n3 = si + 96 + lane < src_end ? src[si + 96 + lane] : 0u;
-    while (si < src_end && di < dst_end) {
-        const uint32_t t = n0;
-        const uint32_t cnt = min(32u, src_end - si);
-        const uint32_t valid = cnt == 32 ? 0xFFFFFFFFu : ((1u << cnt) - 1u);
-        n0 = n1, n1 = n2, n2 = n3;
-        n3 = si + 128 + lane < src_end ? src[si + 128 + lane] : 0u;
-        uint32_t marker = 0;
-        if (mode == 0) {
-            const uint32_t ff = __ballot_sync(0xFFFFFFFFu, t == 0xFFu) & valid;
-            const uint32_t nz = ~ff & below;                                   // bytes below this lane that are not 0xFF
-            const uint32_t s = nz ? 32u - (uint32_t)__clz((int)nz) : 0u;        // first lane of the run of 0xFF this lane is in
-            const uint32_t par = (s == 0 && pending) ? 1u : 0u;                 // a run that starts with a payload
-            const bool is_marker = ((ff >> lane) & 1u) && ((((uint32_t)lane - s) & 1u) == par);
-            marker = __ballot_sync(0xFFFFFFFFu, is_marker);
-        }
-        const uint32_t payload = ((marker << 1) | pending) & valid;  // bytes that follow a marker
-        const uint32_t tokens = valid & ~marker;                     // bytes that produce an output byte
-        const uint32_t m = (uint32_t)__popc(tokens);
-        if (di + m > dst_end) {  // the reference stops at dst_end with source bytes left: an error (:398-400)
-            bad = true;
-            break;
-        }
-        // token k -> lane k (through shared memory: every token lane knows its output index by a popc)
-        if ((tokens >> lane) & 1u) s_tok[__popc(tokens & below)] = (uint16_t)(t | (((payload >> lane) & 1u) << 8));
-        __syncwarp();
-        const uint32_t tw = (uint32_t)lane < m ? s_tok[lane] : 0u;
-        __syncwarp();
-        const uint32_t tk = tw & 0xFFu;
-        const bool is_esc = (tw >> 8) != 0;
-        uint32_t v;  // value to combine along the chain: the delta, or 0 for an escape token
-        if (mode == 0) v = is_esc ? 0u : ((tk & 1u) ? (0u - ((tk + 1u) >> 1)) : (tk >> 1));  // _FSD_ZIGZAG2
-        else v = tk;
-        if ((uint32_t)lane >= m) v = 0;
-        for (uint32_t d = dist; d < 32; d <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, v, d);
-            if ((uint32_t)lane >= d) v = mode == 0 ? v + y : v ^ y;
-        }
-        // the chain's last value of earlier rounds: out[di + (lane % dist) - dist] = tail lane 16 + (lane % dist) - dist
-        const uint32_t head = (uint32_t)lane % dist;
-        const uint32_t base = __shfl_sync(0xFFFFFFFFu, tail, (int)(16u + head - dist));
-        v = (mode == 0 ? v + base : v ^ base) & 0xFFu;
-        if (mode == 0) {
-            uint32_t esc = __ballot_sync(0xFFFFFFFFu, is_esc);
-            while (esc) {  // escapes of the round in order: every earlier token already has its final value
-                const int e = __ffs((int)esc) - 1;
-                esc &= esc - 1;
-                const uint32_t prev_in = __shfl_sync(0xFFFFFFFFu, v, e >= (int)dist ? e - (int)dist : 0);
-                const uint32_t prev_old = __shfl_sync(0xFFFFFFFFu, tail, (int)(16u + (uint32_t)e - dist) & 31);
-                const uint32_t prev = e >= (int)dist ? prev_in : prev_old;
-                const uint32_t tent = __shfl_sync(0xFFFFFFFFu, v, e);
-                const uint32_t pay = __shfl_sync(0xFFFFFFFFu, tk, e);
-                const uint32_t delta = ((pay ^ prev) - tent) & 0xFFu;
-                if (lane >= e && ((uint32_t)(lane - e) % dist) == 0) v = (v + delta) & 0xFFu;
-            }
-        }
-        if ((uint32_t)lane < m) dst[di + lane] = (uint8_t)v;
-        // new tail: out[di + m - 16 + j] for j = 0..15
-        {
-            const int j = lane & 15;
-            const int pos = (int)m - 16 + j;  // index into this round's outputs (negative: still in the old tail)
-            const uint32_t from_new = __shfl_sync(0xFFFFFFFFu, v, pos >= 0 ? pos : 0);
-            const uint32_t from_old = __shfl_sync(0xFFFFFFFFu, tail, pos >= 0 ? 0 : (pos + 16) & 15);
-            tail = pos >= 0 ? from_new : from_old;
-        }
-        pending = (marker >> 31) & 1u;
-        if (cnt < 32) pending = (marker >> (cnt - 1)) & 1u;
-        di += m;
-        si += cnt;
-    }
-    if (!bad && pending) bad = true;       // a marker was the last source byte (:380-383)
-    if (!bad && si != src_end) bad = true;  // :398-400
-    r.out_len = di;
-    if (bad) r.status = -KZ_E_PROCESS_BLOCK;
-    if (lane == 0) res[b] = r;
-}
-
 }  // namespace
 
 size_t fsd_workspace(uint32_t nblocks, uint32_t max_len) {
@@ -514,15 +386,23 @@ cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBloc
     return cudaGetLastError();
 }
 
-// ---- inverse over tiles of 32 source bytes, all tiles of all blocks at once (the default) ------------------------------------------------------
-// What a round of fsd_inverse_kernel carries into the next one is (a) whether its last byte was an escape marker, (b) the output offset,
-// (c) the last value of each of the `dist` chains. (a) and (b) are decided by a scan over tiles: a tile's marker pattern depends on the
+// ---- inverse over tiles of 32 source bytes, all tiles of all blocks at once (FSDCodec.go:317-401) ---------------------------------------------
+// out[o] = f(out[o - dist]) is `dist` interleaved chains; along a chain the delta tokens are a prefix sum (mod 256) and the rare escape
+// tokens (0xFF + payload: out = payload ^ previous) cut it. A round of 32 source bytes, one per lane:
+//   * which 0xFF bytes are escape markers is a parity question inside runs of 0xFF (a marker's successor is a payload, whatever its value),
+//     answered with one ballot and a clz per lane;
+//   * every byte that is not a marker is one output token; the k-th token moves to lane k;
+//   * token values: inclusive shuffle scan with stride `dist` over the deltas (escape tokens count as 0) on top of the chain's value when
+//     the round starts, then one correction per escape token of the round, in order: E = payload ^ value before it; every later token of
+//     its chain moves by E - tentative value. XOR coding is the same scan with xor and no escapes.
+// What a round carries into the next one is (a) whether its last byte was an escape marker, (b) the output offset, (c) the last value of
+// each of the `dist` chains. (a) and (b) are decided by a scan over tiles: a tile's marker pattern depends on the
 // incoming marker bit only through its leading run of 0xFF, so every tile is classified under both hypotheses (K1) and one warp per block
 // chains them (K2). (c): along a chain the deltas are a prefix sum and every escape replaces the value by payload ^ previous, which is not
 // a sum — but the escapes are few: each tile computes its chain totals and the list of its escapes with the delta sum in front of each
 // (K3); the chain totals are scanned over the tiles (K3b), the escapes are compacted into one list per block (K3c) and one warp per block (lane =
-// chain) walks that list only: corr = (payload ^ (linear value before + corr)) - linear value before (K4e). K5 is a round of fsd_inverse_kernel
-// with all three carries given.
+// chain) walks that list only: corr = (payload ^ (linear value before + corr)) - linear value before (K4e). K5 is the round above with all
+// three carries given.
 namespace {
 const int FSD_ESC_SLOTS = 17;  // escapes of a tile: marker + payload take two bytes, plus one whose marker ended the tile before
 struct FsdiBlock {
@@ -870,7 +750,7 @@ __global__ void __launch_bounds__(128) fsdi_k5_kernel(const uint8_t* __restrict_
     uint32_t v = (mode == 0 ? prefix + base : prefix ^ base) & 0xFFu;
     if (mode == 0) {
         uint32_t em = __ballot_sync(0xFFFFFFFFu, is_esc);
-        while (em) {  // escapes of the tile in order (as in fsd_inverse_kernel)
+        while (em) {  // escapes of the tile in order
             const int e = __ffs((int)em) - 1;
             em &= em - 1;
             const uint32_t prev_in = __shfl_sync(0xFFFFFFFFu, v, e >= (int)dist ? e - (int)dist : 0);
@@ -902,7 +782,7 @@ size_t fsd_inverse_workspace(uint32_t nblocks, uint64_t total_len) {
     return tiles * (4 + 4 + 16 + 16 + 1 + 4 * FSD_ESC_SLOTS + 1 + 4 + (8 + 16) * FSD_ESC_SLOTS) + (size_t)nblocks * (sizeof(FsdiBlock) + sizeof(FsdiState) + 4) + 24 * 256 + 4096;
 }
 
-// FSDCodec.Inverse of a batch over tiles (kernels above); h_blocks: the descriptors on the host. KZ_MM_INV=warp: fsd_inverse_kernel (one warp per block).
+// FSDCodec.Inverse of a batch over tiles (kernels above); h_blocks: the descriptors on the host.
 cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, FsdResult* d_res,
                               cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
@@ -953,14 +833,6 @@ cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const FsdBloc
     fsdi_result_kernel<<<(nblocks + 127) / 128, 128, 0, stream>>>(d_b, (int)nblocks, d_st, d_res);
     if (launches) *launches += 8;
     if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;  // hb / blk_of_group go out of scope
-    return cudaGetLastError();
-}
-
-cudaError_t fsd_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* d_blocks, uint32_t nblocks, FsdResult* d_res, cudaStream_t stream,
-                              uint64_t* launches) {
-    if (nblocks == 0) return cudaSuccess;
-    fsd_inverse_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, d_out, d_res);
-    if (launches) *launches += 1;
     return cudaGetLastError();
 }
 

@@ -31,7 +31,5 @@ cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBloc
 size_t fsd_inverse_workspace(uint32_t nblocks, uint64_t total_len);
 cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, FsdResult* d_res,
                               cudaStream_t stream, uint64_t* launches);
-cudaError_t fsd_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* d_blocks, uint32_t nblocks, FsdResult* d_res, cudaStream_t stream,
-                              uint64_t* launches);
 
 }  // namespace kz

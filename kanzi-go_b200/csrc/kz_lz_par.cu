@@ -398,7 +398,7 @@ __global__ void __launch_bounds__(128) lzp_junction_kernel(const uint8_t* __rest
 // packed junction record of the walk: n (9 bits) | END_BLOCK << 9 | status << 10 | fix_n << 12 | idx << 19; second word: joined segment
 __global__ void __launch_bounds__(256) lzp_walk_kernel(const PBlock* __restrict__ blocks, const uint32_t* __restrict__ act_blocks, const SegDesc* __restrict__ desc_all,
                                                         const Junction* __restrict__ junc_all, Piece* __restrict__ pieces, uint32_t* __restrict__ piece_start,
-                                                        PState* __restrict__ pst, int skip_small) {
+                                                        PState* __restrict__ pst) {
     __shared__ uint32_t s_w0[WALK_WIN], s_w1[WALK_WIN];
     __shared__ int s_k, s_stop;
     const uint32_t b = act_blocks[blockIdx.x];
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(256) lzp_walk_kernel(const PBlock* __restrict_
         }
         return;
     }
-    if (skip_small && B.nsegs <= (uint32_t)WALKP_MAX_SERIAL_FROM) return;  // lzp_walk_par_kernel does these
+    if (B.nsegs <= (uint32_t)WALKP_MAX_SERIAL_FROM) return;  // lzp_walk_par_kernel does these
     const SegDesc* desc = desc_all + B.seg_base;
     const Junction* junc = junc_all + B.seg_base;
     Piece* pc = pieces + B.piece_off;
@@ -1033,12 +1033,8 @@ cudaError_t lz_forward_parallel_sub(const uint8_t* d_in, uint8_t* d_out, const L
         {
             LzHookScope hs(hook, round == 0 ? "lz_stitch_r0" : (round == 1 ? "lz_stitch_r1" : "lz_stitch"));
             lzp_junction_kernel<<<(NS + 3) / 4, 128, 0, stream>>>(d_in, d_pb, d_bos, extra ? 1 : 0, d_acts, NS, rec_r, d_logs, d_desc, d_jfix, d_junc, d_dirty, round == 0 ? 1 : 0);
-            static const bool serial_walk = [] {  // KZ_LZ_WALK=serial: the one-thread walk for every block
-                const char* ev = getenv("KZ_LZ_WALK");
-                return ev && ev[0] == 's';
-            }();
-            if (!serial_walk) lzp_walk_par_kernel<<<NB, 256, 0, stream>>>(d_pb, d_actb, d_desc, d_junc, d_pieces, d_pstart, d_pst);
-            lzp_walk_kernel<<<NB, 256, 0, stream>>>(d_pb, d_actb, d_desc, d_junc, d_pieces, d_pstart, d_pst, serial_walk ? 0 : 1);
+            lzp_walk_par_kernel<<<NB, 256, 0, stream>>>(d_pb, d_actb, d_desc, d_junc, d_pieces, d_pstart, d_pst);
+            lzp_walk_kernel<<<NB, 256, 0, stream>>>(d_pb, d_actb, d_desc, d_junc, d_pieces, d_pstart, d_pst);
             lzp_stitch_kernel<<<NB, 32, 0, stream>>>(d_in, d_pb, d_actb, extra ? 1 : 0, rec_r, d_logs, d_desc, d_fix, d_pieces, d_pstart, d_pst);
         }
         {

@@ -17,7 +17,7 @@
 //   3. sbrt_rank_kernel    per segment, one warp: lane l owns the keys of symbols l, l+32, ...; per byte the owner of c
 //                          broadcasts key(c), every lane counts its larger keys, one REDUX gives r.
 // Inverse: the list itself is the decoder state (r -> c needs the list, which needs all earlier symbols), so a block is
-// one serial chain: one thread per block walks it with the list in shared memory (blocks run concurrently).
+// one serial chain: one CTA per block walks it with the list in registers (blocks run concurrently).
 #include "kz_sbrt.cuh"
 
 namespace kz {
@@ -162,149 +162,7 @@ __global__ void __launch_bounds__(128) sbrt_rank_kernel(const uint8_t* __restric
     }
 }
 
-// ---- inverse: one warp per block, lane 0 walks the chain (SBRT.go:177-226)
-// The list is the decoder state, so the chain is serial. v1 kept symbol -> q and rank -> symbol in shared memory: two
-// dependent loads per bubble step (280 cycles per byte measured). Now
-//   * the list is stored by RANK as 64-bit entries (q << 32 | symbol): moving an entry is one load + one store and the next
-//     four entries are loaded together before they are compared (their addresses do not depend on the comparisons);
-//   * the first four entries (symbol, q, p) live in registers: after a BWT most ranks are 0..3 and cost a few compares;
-//   * p (last position) stays a table by symbol for the entries that are not in registers.
-template <bool PACKED>
-__global__ void __launch_bounds__(32) sbrt_inverse_kernel_t(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks, int mode,
-                                                            uint8_t* __restrict__ out) {
-    __shared__ uint64_t s_ent[256 + 8];  // entry of rank r at s_ent[r + 4]; four sentinels (q = "infinite") below rank 0
-    __shared__ int32_t s_p[256];
-    const int b = blockIdx.x, lane = threadIdx.x;
-    if (b >= nblocks) return;
-    const SbrtBlock blk = blocks[b];
-    if (!blk.active) return;
-    for (int i = lane; i < 256; i += 32) {
-        s_ent[i + 4] = (uint64_t)i;  // q = 0, symbol i
-        s_p[i] = 0;
-    }
-    if (lane < 4) s_ent[lane] = ~0ull >> 1;
-    if (lane < 4) s_ent[260 + lane] = 0;
-    __syncwarp();
-    if (lane != 0) return;
-    const uint8_t* src = data + blk.src_off;
-    uint8_t* dst = out + blk.dst_off;
-    const uint32_t n = blk.len;
-    uint64_t* ent = s_ent + 4;
-    // register copies of list ranks 0..3 (the shared entries of these ranks are stale and never read)
-    uint32_t y0 = 0, y1 = 1, y2 = 2, y3 = 3;
-    int32_t q0 = 0, q1 = 0, q2 = 0, q3 = 0;
-    int32_t p0 = 0, p1 = 0, p2 = 0, p3 = 0;
-    auto step = [&](uint32_t i, uint32_t r) -> uint32_t {
-        uint32_t c;
-        int32_t pc;
-        if (r < 4) {
-            if (r == 0) {
-                c = y0, pc = p0;
-            } else if (r == 1) {
-                c = y1, pc = p1;
-            } else if (r == 2) {
-                c = y2, pc = p2;
-            } else {
-                c = y3, pc = p3;
-            }
-        } else if (PACKED) {  // blocks < 128 MiB: q (27 bits) | p (27 bits) | symbol in one entry, no second look-up
-            const uint64_t e = ent[r];
-            c = (uint32_t)e & 0xFF;
-            pc = (int32_t)((e >> 8) & 0x7FFFFFFu);
-        } else {
-            c = (uint32_t)ent[r] & 0xFF;
-            pc = s_p[c];
-        }
-        const int32_t qc = mode == 1 ? (int32_t)i : ((int32_t)i + pc) >> 1;
-        if (r >= 4) {  // bubble up inside shared memory down to rank 4 (SBRT.go:214-220), four entries per round
-            const uint64_t lim = PACKED ? (((uint64_t)(uint32_t)qc << 35) | 0x7FFFFFFFFull) : (((uint64_t)(uint32_t)qc << 32) | 0xFFFFFFFFull);  // entry <= lim  <=>  q <= qc
-            while (r > 4) {
-                const uint64_t e1 = ent[r - 1], e2 = ent[(int)r - 2], e3 = ent[(int)r - 3], e4 = ent[(int)r - 4];  // ranks < 4 are stale: guarded by r > 4
-                if (e1 > lim) break;
-                ent[r] = e1;
-                r--;
-                if (r <= 4 || e2 > lim) break;
-                ent[r] = e2;
-                r--;
-                if (r <= 4 || e3 > lim) break;
-                ent[r] = e3;
-                r--;
-                if (r <= 4 || e4 > lim) break;
-                ent[r] = e4;
-                r--;
-            }
-            if (r > 4 || q3 > qc) {  // stays behind the register entries (r == 4: the entry of rank 3 is in a register)
-                if (PACKED) {
-                    ent[r] = ((uint64_t)(uint32_t)qc << 35) | ((uint64_t)i << 8) | c;
-                } else {
-                    ent[r] = ((uint64_t)(uint32_t)qc << 32) | c;
-                    s_p[c] = (int32_t)i;
-                }
-                return c;
-            }
-            // entry 3 drops to rank 4, c enters the registers at rank 3
-            if (PACKED) {
-                ent[4] = ((uint64_t)(uint32_t)q3 << 35) | ((uint64_t)(uint32_t)p3 << 8) | y3;
-            } else {
-                ent[4] = ((uint64_t)(uint32_t)q3 << 32) | y3;
-                s_p[y3] = p3;
-            }
-            r = 3;
-        }
-        // c belongs at some rank <= r <= 3: the entries with q <= qc right above it move down by one
-        if (r == 3) {
-            if (q2 <= qc) {
-                y3 = y2, q3 = q2, p3 = p2;
-                r = 2;
-            } else {
-                y3 = c, q3 = qc, p3 = (int32_t)i;
-                return c;
-            }
-        }
-        if (r == 2) {
-            if (q1 <= qc) {
-                y2 = y1, q2 = q1, p2 = p1;
-                r = 1;
-            } else {
-                y2 = c, q2 = qc, p2 = (int32_t)i;
-                return c;
-            }
-        }
-        if (r == 1) {
-            if (q0 <= qc) {
-                y1 = y0, q1 = q0, p1 = p0;
-                r = 0;
-            } else {
-                y1 = c, q1 = qc, p1 = (int32_t)i;
-                return c;
-            }
-        }
-        y0 = c, q0 = qc, p0 = (int32_t)i;
-        return c;
-    };
-    const uint32_t n16 = n >> 4;
-    const uint4* s4 = reinterpret_cast<const uint4*>(src);
-    uint4* d4 = reinterpret_cast<uint4*>(dst);
-    uint4 x = n16 ? __ldg(&s4[0]) : make_uint4(0, 0, 0, 0);
-    for (uint32_t v = 0; v < n16; v++) {
-        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
-        if (v + 1 < n16) x = __ldg(&s4[v + 1]);  // next 16 ranks in flight while these are decoded
-        uint32_t o[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const uint32_t i = 16 * v + 4 * k;
-            uint32_t y = step(i, w[k] & 0xFF);
-            y |= step(i + 1, (w[k] >> 8) & 0xFF) << 8;
-            y |= step(i + 2, (w[k] >> 16) & 0xFF) << 16;
-            y |= step(i + 3, w[k] >> 24) << 24;
-            o[k] = y;
-        }
-        d4[v] = make_uint4(o[0], o[1], o[2], o[3]);
-    }
-    for (uint32_t i = n16 << 4; i < n; i++) dst[i] = (uint8_t)step(i, src[i]);
-}
-
-// ---- inverse, warp-resident (default): the 256-entry list lives in the registers of one warp, lane l holds ranks 8 l .. 8 l + 7
+// ---- inverse for blocks > 16 MiB, warp-resident: the 256-entry list lives in the registers of one warp, lane l holds ranks 8 l .. 8 l + 7
 // as (q, p << 8 | symbol). The list is always sorted by q (descending; SBRT.go:214-220 only ever moves the accessed symbol up, and its
 // new q is never below its old one), so the move-up is a LOCAL decision per list position j <= r:
 //     q[j] >  qc                 -> stays
@@ -429,216 +287,17 @@ __global__ void __launch_bounds__(32) sbrt_inverse_warp_kernel(const uint8_t* __
     }
 }
 
-// ---- inverse, branch-free variant of the warp-resident list (default for blocks <= 16 MiB) ------------------------------------------------
-// The source-level profile of the kernel above showed one warp issuing ~77 instructions per rank at an IPC of
-// 0.33: a quarter of the stall samples sit on the loop / path branches and their targets, a tenth on an S2R + shared-memory address per
-// stored byte, the rest is the dependent issue latency of a single warp. This variant has no branch inside a round of 32 ranks: the round is
-// fully unrolled (the next rank is a shuffle from a constant lane), every rank — zero included — takes the same predicated move-up over the
-// 8 entries of every lane, and the decoded byte of step j is kept in a register of lane j. ~55 instructions per rank, no S2R, no LDC.
-template <bool RANK_MODE>
-__global__ void __launch_bounds__(32) sbrt_inverse_flat_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
-                                                                uint8_t* __restrict__ out) {
-    const int b = blockIdx.x, lane = threadIdx.x;
-    if (b >= nblocks) return;
-    const SbrtBlock blk = blocks[b];
-    if (!blk.active) return;
-    const uint8_t* src = data + blk.src_off;
-    uint8_t* dst = out + blk.dst_off;
-    const uint32_t n = blk.len;
-    uint32_t Q[8], X[8];  // lane l holds ranks 8 l .. 8 l + 7: q and (p << 8 | symbol)
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        Q[k] = 0;
-        X[k] = (uint32_t)(8 * lane + k);
-    }
-    const uint32_t base = 8u * (uint32_t)lane;
-    auto step = [&](uint32_t r, uint32_t i) -> uint32_t {
-        // the entry of rank r: a select tree over the three low bits of r in every lane, one shuffle from the owner lane
-        const uint32_t up_q = __shfl_up_sync(0xFFFFFFFFu, Q[7], 1), up_x = __shfl_up_sync(0xFFFFFFFFu, X[7], 1);
-        const bool b0 = r & 1u, b1 = r & 2u, b2 = r & 4u;
-        const uint32_t a0 = b0 ? X[1] : X[0], a1 = b0 ? X[3] : X[2], a2 = b0 ? X[5] : X[4], a3 = b0 ? X[7] : X[6];
-        const uint32_t c0 = b1 ? a1 : a0, c1 = b1 ? a3 : a2;
-        const uint32_t x = __shfl_sync(0xFFFFFFFFu, b2 ? c1 : c0, (int)(r >> 3));
-        const uint32_t sym = x & 0xFFu;
-        const uint32_t qc = RANK_MODE ? (i + (x >> 8)) >> 1 : i;  // i, p < 2^24
-        const uint32_t fresh = (i << 8) | sym;
-        // local move-up rule (see above): position j <= r with q[j] <= qc takes the accessed symbol if q[j - 1] > qc, else the entry of j - 1
-        // d = r - base: slot k of this lane is at or below the accessed rank when k <= d
-        const int d = (int)r - (int)base;
-        bool gk = Q[7] > qc;
-#pragma unroll
-        for (int k = 7; k >= 1; k--) {
-            const bool gk1 = Q[k - 1] > qc;
-            const bool mv = k <= d && !gk;
-            const uint32_t xin = gk1 ? fresh : X[k - 1];
-            Q[k] = mv ? min(Q[k - 1], qc) : Q[k];  // g[k - 1] ? qc : Q[k - 1]
-            X[k] = mv ? xin : X[k];
-            gk = gk1;
-        }
-        {
-            const bool g_up = lane == 0 ? true : up_q > qc;
-            const bool mv = 0 <= d && !gk;
-            Q[0] = mv ? (g_up ? qc : up_q) : Q[0];
-            X[0] = mv ? (g_up ? fresh : up_x) : X[0];
-        }
-        return sym;
-    };
-    uint32_t nxt = (uint32_t)lane < n ? src[lane] : 0u;
-    uint32_t i0 = 0;
-    for (; i0 + 32 <= n; i0 += 32) {
-        const uint32_t mine = nxt;
-        nxt = i0 + 32 + lane < n ? src[i0 + 32 + lane] : 0u;  // next round's ranks in flight
-        uint32_t ob = 0;
-#pragma unroll
-        for (int j = 0; j < 32; j++) {
-            const uint32_t sym = step(__shfl_sync(0xFFFFFFFFu, mine, j), i0 + (uint32_t)j);
-            ob = lane == j ? sym : ob;
-        }
-        dst[i0 + lane] = (uint8_t)ob;
-    }
-    if (i0 < n) {  // last, partial round
-        const uint32_t mine = nxt;
-        uint32_t ob = 0;
-        for (uint32_t j = 0; i0 + j < n; j++) {
-            const uint32_t sym = step(__shfl_sync(0xFFFFFFFFu, mine, (int)j), i0 + j);
-            ob = (uint32_t)lane == j ? sym : ob;
-        }
-        if (i0 + lane < n) dst[i0 + lane] = (uint8_t)ob;
-    }
-}
-
-// ---- inverse, the list mirrored in shared memory so that the NEXT rank's entry is known before the move-up is done ---------------------------
-// In the flat kernel every instruction of a step sits on the dependent chain: select tree + shuffle for the entry of rank r -> qc -> 40
-// instructions of move-up -> next step's select tree (177 cycles per rank measured, 70 instructions at IPC 0.4). Here the registers keep the
-// list for the move-up, and a copy in shared memory (2 KiB) serves the look-ups: after step j - 1 has stored its lanes' entries, the
-// candidates for the rank r2 of step j + 1 are loaded from the state BEFORE step j — entry r2 and entry r2 - 1 — and step j decides with two
-// compares which one (or its own fresh entry) stands at rank r2 afterwards (the move-up rule applied to that one position). The chain per
-// rank is qc -> 2 compares -> 2 selects -> next qc; the move-up, the stores and the loads for the step after next overlap it.
-template <bool RANK_MODE>
-__global__ void __launch_bounds__(32) sbrt_inverse_mirror_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
-                                                                  uint8_t* __restrict__ out) {
-    __shared__ __align__(16) uint32_t s_q[256];
-    __shared__ __align__(16) uint32_t s_x[256];
-    const int b = blockIdx.x, lane = threadIdx.x;
-    if (b >= nblocks) return;
-    const SbrtBlock blk = blocks[b];
-    if (!blk.active) return;
-    const uint8_t* src = data + blk.src_off;
-    uint8_t* dst = out + blk.dst_off;
-    const uint32_t n = blk.len;
-    uint32_t Q[8], X[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        Q[k] = 0;
-        X[k] = (uint32_t)(8 * lane + k);
-        s_q[8 * lane + k] = 0;
-        s_x[8 * lane + k] = (uint32_t)(8 * lane + k);
-    }
-    __syncwarp();
-    const uint32_t base = 8u * (uint32_t)lane;
-    uint4* sq4 = reinterpret_cast<uint4*>(s_q) + 2 * lane;
-    uint4* sx4 = reinterpret_cast<uint4*>(s_x) + 2 * lane;
-    // candidates for the next rank, from the state before the current step
-    uint32_t a_q, a_x, b_q, b_x;
-    auto load_candidates = [&](uint32_t r2) {
-        const uint32_t r1 = r2 ? r2 - 1 : 0;
-        a_q = s_q[r2], a_x = s_x[r2], b_q = s_q[r1], b_x = s_x[r1];
-    };
-    // one rank: x = the entry at rank r (known to every lane), r2 = the next rank; returns the symbol, leaves the next entry in x.
-    // Instruction order matters (one warp, in-order issue): the decision about the next entry reads the candidates loaded at the end of the
-    // previous step, so it stands in the middle of the move-up — far enough behind those loads, early enough for the next step's qc.
-    auto step = [&](uint32_t r, uint32_t r2, uint32_t i, uint32_t& x) -> uint32_t {
-        const uint32_t up_q = __shfl_up_sync(0xFFFFFFFFu, Q[7], 1), up_x = __shfl_up_sync(0xFFFFFFFFu, X[7], 1);
-        const uint32_t sym = x & 0xFFu;
-        const uint32_t qc = RANK_MODE ? (i + (x >> 8)) >> 1 : i;  // i, p < 2^24
-        const uint32_t fresh = (i << 8) | sym;
-        const int d = (int)r - (int)base;
-        bool gk = Q[7] > qc;
-#pragma unroll
-        for (int k = 7; k >= 4; k--) {  // predicated moves (alu pipe: 2 compares + 1 min per slot; the moves can go to the fma pipe)
-            const bool gk1 = Q[k - 1] > qc;
-            uint32_t xin = X[k - 1];
-            if (gk1) xin = fresh;
-            if (k <= d && !gk) {
-                Q[k] = min(Q[k - 1], qc);
-                X[k] = xin;
-            }
-            gk = gk1;
-        }
-        {  // the entry at rank r2 after this step: the move-up rule for that one position
-            const bool mv = r2 <= r && !(a_q > qc);
-            const bool gb = r2 == 0 || b_q > qc;
-            x = mv ? (gb ? fresh : b_x) : a_x;
-        }
-#pragma unroll
-        for (int k = 3; k >= 1; k--) {
-            const bool gk1 = Q[k - 1] > qc;
-            uint32_t xin = X[k - 1];
-            if (gk1) xin = fresh;
-            if (k <= d && !gk) {
-                Q[k] = min(Q[k - 1], qc);
-                X[k] = xin;
-            }
-            gk = gk1;
-        }
-        {
-            const bool g_up = lane == 0 ? true : up_q > qc;
-            uint32_t qin = up_q, xin = up_x;
-            if (g_up) qin = qc, xin = fresh;
-            if (0 <= d && !gk) {
-                Q[0] = qin;
-                X[0] = xin;
-            }
-        }
-        sq4[0] = make_uint4(Q[0], Q[1], Q[2], Q[3]);
-        sq4[1] = make_uint4(Q[4], Q[5], Q[6], Q[7]);
-        sx4[0] = make_uint4(X[0], X[1], X[2], X[3]);
-        sx4[1] = make_uint4(X[4], X[5], X[6], X[7]);
-        __syncwarp();
-        return sym;
-    };
-    if (n == 0) return;
-    uint32_t mine = (uint32_t)lane < n ? src[lane] : 0u;
-    uint32_t nxt = 32u + lane < n ? src[32 + lane] : 0u;
-    uint32_t x = s_x[__shfl_sync(0xFFFFFFFFu, mine, 0)];  // entry of the first rank in the initial list
-    load_candidates(__shfl_sync(0xFFFFFFFFu, mine, 1));   // (rank 1 of a 1-byte block: lane 1 holds 0)
-    uint32_t i0 = 0;
-    for (; i0 + 32 <= n; i0 += 32) {
-        const uint32_t nn = i0 + 64 + lane < n ? src[i0 + 64 + lane] : 0u;  // the round after next in flight
-        uint32_t ob = 0;
-#pragma unroll
-        for (int j = 0; j < 32; j++) {
-            const uint32_t r = __shfl_sync(0xFFFFFFFFu, mine, j);
-            const uint32_t r2 = j < 31 ? __shfl_sync(0xFFFFFFFFu, mine, (j + 1) & 31) : __shfl_sync(0xFFFFFFFFu, nxt, 0);
-            const uint32_t r3 = j < 30 ? __shfl_sync(0xFFFFFFFFu, mine, (j + 2) & 31) : __shfl_sync(0xFFFFFFFFu, nxt, (j + 2) & 31);
-            const uint32_t sym = step(r, r2, i0 + (uint32_t)j, x);
-            load_candidates(r3);  // for the step after this one's successor: the state now is the state before step j + 1
-            ob = lane == j ? sym : ob;
-        }
-        dst[i0 + lane] = (uint8_t)ob;
-        mine = nxt;
-        nxt = nn;
-    }
-    if (i0 < n) {  // last, partial round (ranks past the end read as 0: harmless look-ups)
-        uint32_t ob = 0;
-        for (uint32_t j = 0; i0 + j < n; j++) {
-            const uint32_t r = __shfl_sync(0xFFFFFFFFu, mine, (int)j);
-            const uint32_t r2 = j < 31 ? __shfl_sync(0xFFFFFFFFu, mine, (int)((j + 1) & 31)) : 0u;
-            const uint32_t r3 = j < 30 ? __shfl_sync(0xFFFFFFFFu, mine, (int)((j + 2) & 31)) : 0u;
-            const uint32_t sym = step(r, r2, i0 + j, x);
-            load_candidates(r3);
-            ob = (uint32_t)lane == j ? sym : ob;
-        }
-        if (i0 + lane < n) dst[i0 + lane] = (uint8_t)ob;
-    }
-}
-
-// ---- inverse, the mirrored list spread over W warps (default W = 4) ------------------------------------------------------------------------------
-// The mirror kernel is bound by the ALU pipe of its one scheduler: ~50 integer / predicate instructions per rank at 2 cycles each (16 lanes
-// per cycle), 145 cycles per rank measured. With the list in shared memory for every look-up, nothing but the lane boundary ties the lanes
-// together, so the 256 entries are spread over W warps (8 / W entries per lane) that sit on different schedulers: every warp takes the same
-// decision about the next entry from the same shared-memory candidates, moves its own part of the list, stores it, and one CTA barrier per
-// rank publishes the stores; the entry that crosses a warp boundary is read from the mirror instead of a shuffle.
+// ---- inverse for blocks <= 16 MiB: the list in the registers of W = 4 warps, mirrored in shared memory ---------------------------------------
+// With the list only in registers, every instruction of a step sits on the dependent chain: look-up of the entry of rank r -> qc -> move-up
+// -> next step's look-up. Here the registers keep the list for the move-up, and a copy in shared memory serves the look-ups: after step j - 1
+// has stored its entries, the candidates for the rank r2 of step j + 1 are loaded from the state BEFORE step j — entry r2 and entry r2 - 1 —
+// and step j decides with two compares which one (or its own fresh entry) stands at rank r2 afterwards (the move-up rule applied to that one
+// position). The chain per rank is qc -> 2 compares -> 2 selects -> next qc; the move-up, the stores and the loads for the step after next
+// overlap it. On one warp this is bound by the ALU pipe of its scheduler (~50 integer / predicate instructions per rank), and with every
+// look-up served by the mirror nothing but the lane boundary ties the lanes together, so the 256 entries are spread over W warps (8 / W
+// entries per lane) that sit on different schedulers: every warp takes the same decision about the next entry from the same shared-memory
+// candidates, moves its own part of the list, stores it, and one CTA barrier per rank publishes the stores; the entry that crosses a warp
+// boundary is read from the mirror instead of a shuffle.
 template <bool RANK_MODE, int W>
 __global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
                                                                      uint8_t* __restrict__ out) {
@@ -747,24 +406,9 @@ __global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_
     }
 }
 
-// host entry. KZ_SBRT_INV=lane selects the round-1 kernel (lane 0 walks the chain; kept for comparison); packed = every block < 128 MiB
-void sbrt_inverse_launch(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, bool packed, cudaStream_t stream) {
-    static const bool old_kernel = [] {
-        const char* e = getenv("KZ_SBRT_INV");
-        return e && e[0] == 'l';
-    }();
-    if (!old_kernel) {  // the block lengths are not known here: 64-bit entries (sbrt_inverse_launch_len picks 32-bit ones for blocks <= 16 MiB)
-        sbrt_inverse_warp_kernel<uint64_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-        return;
-    }
-    if (packed) sbrt_inverse_kernel_t<true><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-    else sbrt_inverse_kernel_t<false><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-}
-
 // A chain is serial and latency-bound: a CTA that shares its SM with another chain's CTA runs at a fraction of its speed for the whole launch, and
 // the block scheduler does pack CTAs (six per SM were seen: 1.6 s instead of 0.26 s) when kernels of other streams occupy the GPU at launch time.
 // Dynamic shared memory that nobody touches caps the chains per SM at ceil(nblocks / SMs): the chains spread over the GPU whatever runs beside them.
-// KZ_SBRT_SMEM_KB overrides the amount for nblocks <= SMs (A/B measurements).
 template <typename K>
 static size_t spread_chains(K kernel, int nblocks) {
     int dev = 0, sms = 0;
@@ -772,15 +416,7 @@ static size_t spread_chains(K kernel, int nblocks) {
     const int per = (nblocks + sms - 1) / sms;
     if (per > 5) return 0;  // small blocks in large numbers: several chains per SM overlap their latencies, no cap
     const size_t sm_bytes = 228 * 1024;
-    size_t dyn = sm_bytes / (size_t)(per + 1);
-    if (per == 1) {
-        static const int kb = [] {
-            const char* e = getenv("KZ_SBRT_SMEM_KB");
-            return e ? atoi(e) : -1;
-        }();
-        if (kb >= 0) dyn = (size_t)kb * 1024;
-    }
-    if (dyn == 0) return 0;
+    const size_t dyn = sm_bytes / (size_t)(per + 1);
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess) {
         cudaGetLastError();
         return 0;
@@ -789,47 +425,9 @@ static size_t spread_chains(K kernel, int nblocks) {
 }
 
 void sbrt_inverse_launch_len(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, uint32_t max_len, cudaStream_t stream) {
-    static const bool old_kernel = [] {
-        const char* e = getenv("KZ_SBRT_INV");
-        return e && e[0] == 'l';
-    }();
-    if (old_kernel) {
-        sbrt_inverse_launch(data, d_blocks, nblocks, mode, out, max_len < (1u << 27), stream);
-        return;
-    }
-    static const bool branchy = [] {  // KZ_SBRT_INV=warp: the first warp-resident kernel (run skipping, separate paths for ranks < 8)
-        const char* e = getenv("KZ_SBRT_INV");
-        return e && e[0] == 'w';
-    }();
-    static const bool flat = [] {  // KZ_SBRT_INV=flat: the branch-free kernel without the shared-memory mirror
-        const char* e = getenv("KZ_SBRT_INV");
-        return e && e[0] == 'f';
-    }();
-    if (max_len <= (1u << 24) && !branchy && (mode == 1 || mode == 2)) {
-        if (flat) {
-            if (mode == 2) sbrt_inverse_flat_kernel<true><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, out);
-            else sbrt_inverse_flat_kernel<false><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, out);
-        } else {
-            static const int warps = [] {  // KZ_SBRT_WARPS = 1 (mirror kernel), 2, 4 (default) or 8
-                const char* e = getenv("KZ_SBRT_WARPS");
-                return e ? atoi(e) : 4;
-            }();
-            if (warps == 8) {
-                if (mode == 2) sbrt_inverse_multi_kernel<true, 8><<<nblocks, 256, spread_chains(sbrt_inverse_multi_kernel<true, 8>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-                else sbrt_inverse_multi_kernel<false, 8><<<nblocks, 256, spread_chains(sbrt_inverse_multi_kernel<false, 8>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-            } else if (warps == 4) {
-                if (mode == 2) sbrt_inverse_multi_kernel<true, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<true, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-                else sbrt_inverse_multi_kernel<false, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<false, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-            } else if (warps == 2) {
-                if (mode == 2) sbrt_inverse_multi_kernel<true, 2><<<nblocks, 64, spread_chains(sbrt_inverse_multi_kernel<true, 2>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-                else sbrt_inverse_multi_kernel<false, 2><<<nblocks, 64, spread_chains(sbrt_inverse_multi_kernel<false, 2>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-            } else {
-                if (mode == 2) sbrt_inverse_mirror_kernel<true><<<nblocks, 32, spread_chains(sbrt_inverse_mirror_kernel<true>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-                else sbrt_inverse_mirror_kernel<false><<<nblocks, 32, spread_chains(sbrt_inverse_mirror_kernel<false>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-            }
-        }
-    } else if (max_len <= (1u << 24)) sbrt_inverse_warp_kernel<uint32_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-    else sbrt_inverse_warp_kernel<uint64_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
+    if (max_len > (1u << 24)) sbrt_inverse_warp_kernel<uint64_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
+    else if (mode == 2) sbrt_inverse_multi_kernel<true, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<true, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
+    else sbrt_inverse_multi_kernel<false, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<false, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
 }
 
 }  // namespace kz

@@ -19,9 +19,7 @@ __global__ void sbrt_last2_kernel(const uint8_t* data, const SbrtBlock* blocks, 
 __global__ void sbrt_carry_kernel(const SbrtBlock* blocks, int32_t* table);
 __global__ void sbrt_rank_kernel(const uint8_t* data, const SbrtBlock* blocks, int nblocks, int mode, const uint32_t* seg_block, uint32_t nsegs_total,
                                  const int32_t* table, uint8_t* out);
-// packed = every block of the batch is shorter than 128 MiB (64-bit list entries then carry q, p and the symbol)
-void sbrt_inverse_launch(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, bool packed, cudaStream_t stream);
-// default entry: warp-resident list kernel (32-bit entries for blocks up to 16 MiB, 64-bit above); max_len = longest block of the batch
+// mode: 1 = MTFT, 2 = RANK; max_len = longest block of the batch (blocks up to 16 MiB take the 4-warp kernel, longer ones the one-warp kernel)
 void sbrt_inverse_launch_len(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, uint32_t max_len, cudaStream_t stream);
 
 }  // namespace kz

@@ -231,14 +231,6 @@ __global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __
 
 }  // namespace
 
-bool text_serial_walk() {  // KZ_TEXT_FORWARD=serial: the round-1 path (one thread per block walks the words)
-    static const bool v = [] {
-        const char* e = getenv("KZ_TEXT_FORWARD");
-        return e && e[0] == 's';
-    }();
-    return v;
-}
-
 size_t text_workspace_serial(uint32_t nblocks, uint64_t stream_block_size) {
     const uint32_t lg = log_hash_size(stream_block_size);
     return align256(sizeof(Entry) * STATIC_WORDS) + align256(SWORDS_BYTES) + align256((size_t)nblocks * 256 * 4) + align256((size_t)nblocks * 65536 * 4) +
@@ -268,26 +260,24 @@ cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
     if ((e = cudaMemsetAsync(w.hist1, 0, (size_t)nblocks * 65536 * 4, stream)) != cudaSuccess) return e;
     text_hist_kernel<<<dim3(HIST_SLICES, nblocks), 256, 0, stream>>>(d_in, d_blocks, w.hist0, w.hist1);
     text_plan_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, w.hist0, w.hist1, w.go, d_res);
-    if (!text_serial_walk() && h_blocks) {
-        // data-parallel path (kz_text_par.cu); blocks it does not cover come back in `fallback` and take the serial walk below
-        uint8_t* pws = ws + align256(text_workspace_serial(nblocks, stream_block_size));
-        const size_t pws_bytes = ws_bytes - align256(text_workspace_serial(nblocks, stream_block_size));
-        std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
-        std::vector<uint32_t> fallback;
-        if ((e = text_forward_parallel(d_in, d_out, tb, w.go, stream_block_size, w.sdict, w.swords, S.n, pws, pws_bytes, d_res, stream, fallback, launches)) != cudaSuccess)
-            return e;
-        bool any = false;
-        for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
-        if (!any) return cudaGetLastError();
-        std::vector<uint32_t> go(nblocks);
-        // on the context's own (non-blocking) stream: a plain cudaMemcpy would neither wait for it nor leave other contexts alone
-        if ((e = cudaMemcpyAsync(go.data(), w.go, nblocks * 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
-        if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
-        for (uint32_t b = 0; b < nblocks; b++)
-            if (!fallback[b]) go[b] = 0;
-        if ((e = cudaMemcpyAsync(w.go, go.data(), nblocks * 4, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-        if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;  // `go` is a local
-    }
+    // data-parallel path (kz_text_par.cu); blocks it does not cover come back in `fallback` and take the serial walk below
+    uint8_t* pws = ws + align256(text_workspace_serial(nblocks, stream_block_size));
+    const size_t pws_bytes = ws_bytes - align256(text_workspace_serial(nblocks, stream_block_size));
+    std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
+    std::vector<uint32_t> fallback;
+    if ((e = text_forward_parallel(d_in, d_out, tb, w.go, stream_block_size, w.sdict, w.swords, S.n, pws, pws_bytes, d_res, stream, fallback, launches)) != cudaSuccess)
+        return e;
+    bool any = false;
+    for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
+    if (!any) return cudaGetLastError();
+    std::vector<uint32_t> go(nblocks);
+    // on the context's own (non-blocking) stream: a plain cudaMemcpy would neither wait for it nor leave other contexts alone
+    if ((e = cudaMemcpyAsync(go.data(), w.go, nblocks * 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    for (uint32_t b = 0; b < nblocks; b++)
+        if (!fallback[b]) go[b] = 0;
+    if ((e = cudaMemcpyAsync(w.go, go.data(), nblocks * 4, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;  // `go` is a local
     text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(w.go, w.sdict, S.n, w.map, w.log, w.list);
     text_forward_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, w.go, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);
     if (launches) *launches += 4;
@@ -308,27 +298,23 @@ cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
     cudaError_t e;
     if ((e = cudaMemcpyAsync(w.sdict, S.entries.data(), sizeof(Entry) * STATIC_WORDS, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     if ((e = cudaMemcpyAsync(w.swords, S.words.data(), SWORDS_BYTES, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-    const TextBlock* walk_blocks = d_blocks;
-    if (!text_serial_walk() && h_blocks) {
-        // data-parallel path (kz_text_par.cu); trivial blocks and every anomaly come back in `fallback` and take the serial walk below
-        const size_t used = align256(text_workspace_serial(nblocks, stream_block_size));
-        std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
-        std::vector<uint32_t> fallback;
-        if ((e = text_inverse_parallel(d_in, d_out, tb, stream_block_size, w.sdict, w.swords, S.n, ws + used, ws_bytes - used, d_res, stream, fallback, launches)) != cudaSuccess)
-            return e;
-        bool any = false;
-        for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
-        if (!any) return cudaGetLastError();
-        // the serial kernel writes res[b] for every block: give it a descriptor list in which the finished blocks are marked
-        for (uint32_t b = 0; b < nblocks; b++)
-            if (!fallback[b]) tb[b].pad = 1;
-        TextBlock* d_tmp = reinterpret_cast<TextBlock*>(w.hist1);  // the forward-only histogram area is free here
-        if ((e = cudaMemcpyAsync(d_tmp, tb.data(), nblocks * sizeof(TextBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-        if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
-        walk_blocks = d_tmp;
-    }
+    // data-parallel path (kz_text_par.cu); trivial blocks and every anomaly come back in `fallback` and take the serial walk below
+    const size_t used = align256(text_workspace_serial(nblocks, stream_block_size));
+    std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
+    std::vector<uint32_t> fallback;
+    if ((e = text_inverse_parallel(d_in, d_out, tb, stream_block_size, w.sdict, w.swords, S.n, ws + used, ws_bytes - used, d_res, stream, fallback, launches)) != cudaSuccess)
+        return e;
+    bool any = false;
+    for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
+    if (!any) return cudaGetLastError();
+    // the serial kernel writes res[b] for every block: give it a descriptor list in which the finished blocks are marked
+    for (uint32_t b = 0; b < nblocks; b++)
+        if (!fallback[b]) tb[b].pad = 1;
+    TextBlock* d_tmp = reinterpret_cast<TextBlock*>(w.hist1);  // the forward-only histogram area is free here
+    if ((e = cudaMemcpyAsync(d_tmp, tb.data(), nblocks * sizeof(TextBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
     text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(nullptr, w.sdict, S.n, w.map, w.log, w.list);
-    text_inverse_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, walk_blocks, (int)nblocks, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);
+    text_inverse_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_tmp, (int)nblocks, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);
     if (launches) *launches += 2;
     return cudaGetLastError();
 #endif

@@ -26,7 +26,7 @@ size_t text_workspace(uint32_t nblocks, uint64_t stream_block_size, uint32_t max
 size_t text_workspace_serial(uint32_t nblocks, uint64_t stream_block_size);          // serial walk only
 size_t text_workspace_inverse(uint32_t nblocks, uint64_t stream_block_size, uint32_t max_len);  // inverse (serial + data-parallel scratch)
 
-// h_blocks: host copy of d_blocks (the data-parallel path builds its own descriptors from it); nullptr selects the serial walk
+// h_blocks: host copy of d_blocks (the data-parallel path builds its own descriptors from it)
 cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
                                uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream, uint64_t* launches);
 cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,

@@ -1,6 +1,5 @@
 """GPU parity tests for EXE (EXECodec, transform/EXECodec.go) and for the complete chain of kanzi -l 4
 (TEXT+UTF+EXE+PACK+MM+ROLZ & NONE). The per-block logic is kz_exe_core.cuh, checked on the CPU by tests/test_exe_core_host.py."""
-import os
 import sys
 
 import numpy as np
@@ -8,9 +7,7 @@ import pytest
 
 from test_oracle_pre import _synth_arm64, _synth_x86
 
-_VALIDATED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "VALIDATED")
-_ok = os.environ.get("KZ_TEST_UNVALIDATED") == "1" or (os.path.exists(_VALIDATED) and "test_gpu_exe.py" in open(_VALIDATED).read())
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not _ok, reason="EXE kernels not yet confirmed on a GPU (set KZ_TEST_UNVALIDATED=1)")]
+pytestmark = pytest.mark.gpu
 
 T_EXE = 9
 

@@ -4,15 +4,7 @@ the transform chain of kanzi -l 2) and for the data type a block's magic number 
 import numpy as np
 import pytest
 
-import os
-
-# These kernels were written at the very end of round 1, when the GPU pool had no free slot left: until a GPU run has confirmed
-# them (tests/VALIDATED lists this file) they only run on request, so that an unconfirmed test cannot hide the rest of the suite.
-_VALIDATED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "VALIDATED")
-_ok = os.environ.get("KZ_TEST_UNVALIDATED") == "1" or (os.path.exists(_VALIDATED) and "test_gpu_pack.py" in open(_VALIDATED).read())
-if _ok:
-    os.environ["KZ_EXPERIMENTAL"] = "1"  # read by the library at every plan_transforms call
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not _ok, reason="PACK / MM kernels not yet confirmed on a GPU (set KZ_TEST_UNVALIDATED=1)")]
+pytestmark = pytest.mark.gpu
 
 T_PACK, T_DNA, T_MM = 18, 19, 15
 

@@ -47,6 +47,18 @@ def test_single_transform_parity(gpu, oracle, synth, kz, name, n):
         assert np.array_equal(back, x), (name, cname, n)
 
 
+@pytest.mark.parametrize("name", ["RANK", "MTFT"])
+def test_single_transform_parity_above_16mib(gpu, oracle, synth, kz, name):
+    """a block longer than 16 MiB: the inverse takes the one-warp kernel with 64-bit list entries, the only one for such blocks"""
+    n = (16 << 20) + 4097
+    t = kz.TRANSFORM_IDS[name]
+    x = synth.markov_text(n, seed=n)
+    want, _ = oracle.transform_forward(t, x)
+    got, _ = gpu.transform_forward(t, x)
+    assert want is not None and got is not None and np.array_equal(got, want), (name, n)
+    assert np.array_equal(gpu.transform_inverse(t, want, n + 64), x), name
+
+
 BWTS_SIZES = [1, 2, 3, 7, 16, 100, 255, 256, 257, 1000, 4096, 65536, 100003, 1 << 20]
 
 

@@ -1,13 +1,10 @@
 """GPU parity tests for TEXT (TextCodec encoding 2, transform/TextCodec.go:1137-1724): statistics / dictionary set-up kernels around the
 one-thread-per-block walk of kz_text_core.cuh (whose logic tests/test_text_core_host.py already checks on the CPU)."""
-import os
 
 import numpy as np
 import pytest
 
-_VALIDATED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "VALIDATED")
-_ok = os.environ.get("KZ_TEST_UNVALIDATED") == "1" or (os.path.exists(_VALIDATED) and "test_gpu_text.py" in open(_VALIDATED).read())
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not _ok, reason="TEXT kernels not yet confirmed on a GPU (set KZ_TEST_UNVALIDATED=1)")]
+pytestmark = pytest.mark.gpu
 
 T_TEXT = 10
 

@@ -1,14 +1,11 @@
 """GPU parity tests for UTF (UTFCodec, transform/UTFCodec.go:87-383) and for the complete transform chains of kanzi -l 3 and -l 5
 (TEXT+UTF+PACK+MM+LZX & HUFFMAN, TEXT+UTF+BWT+RANK+ZRLT & ANS0), which need every stage on the GPU. The per-block logic of UTF is
 kz_utf_core.cuh, already checked against the oracle on the CPU by tests/test_utf_core_host.py."""
-import os
 
 import numpy as np
 import pytest
 
-_VALIDATED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "VALIDATED")
-_ok = os.environ.get("KZ_TEST_UNVALIDATED") == "1" or (os.path.exists(_VALIDATED) and "test_gpu_utf.py" in open(_VALIDATED).read())
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not _ok, reason="UTF kernels not yet confirmed on a GPU (set KZ_TEST_UNVALIDATED=1)")]
+pytestmark = pytest.mark.gpu
 
 T_UTF = 17
 

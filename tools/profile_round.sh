@@ -10,7 +10,7 @@ echo "bench rc=$?"
 timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 20000 --csv --log-file $out/${tag}_launches_final.csv \
     python bench.py --steps 1 --warmup 1 --no-cpu-baseline --no-e2e > $out/${tag}_launch_bench.log 2>&1
 echo "launch list rc=$?"
-for k in sbrt_inverse_multi lzi_parse_kernel fsd_inverse_kernel sbrt_rank_kernel lzp_spec_kernel lzp_junction_kernel bwtu_keys_kernel lzp_derive_kernel tp_round_eval_kernel; do
+for k in sbrt_inverse_multi lzi_parse_kernel sbrt_rank_kernel lzp_spec_kernel lzp_junction_kernel bwtu_keys_kernel lzp_derive_kernel tp_round_eval_kernel; do
     timeout 400 ncu --set full --import-source on --clock-control none -k regex:$k -c 1 -f -o $out/${tag}_full_$k \
         python bench.py --steps 1 --warmup 1 --no-cpu-baseline --no-e2e > $out/${tag}_full_$k.log 2>&1
     echo "full $k rc=$?"
