@@ -134,10 +134,10 @@ namespace {
 // ------------------------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) alias_hist0_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, uint32_t* __restrict__ hist0) {
+__global__ void __launch_bounds__(256) alias_hist0_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, uint32_t* __restrict__ hist0) {
     __shared__ uint32_t h[256];
     const int b = blockIdx.y;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if (blk.len < 1024) return;
     h[threadIdx.x] = 0;
     __syncthreads();
@@ -160,14 +160,14 @@ __global__ void __launch_bounds__(256) alias_hist0_kernel(const uint8_t* __restr
 }
 
 // one warp per block, lane 0: AliasCodec.Forward :83-207 up to the choice of the coding mode
-__global__ void __launch_bounds__(32) alias_plan_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) alias_plan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                          const uint32_t* __restrict__ hist0, AliasInfo* __restrict__ infos, uint8_t* __restrict__ out,
-                                                         AliasResult* __restrict__ res) {
+                                                         StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     AliasInfo& I = infos[b];
-    AliasResult r;
+    StageResult r;
     r.status = 1;
     r.out_len = 0;
     r.data_type = blk.data_type;
@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(32) alias_plan_kernel(const uint8_t* __restric
     bool go = count >= 1024 && (uint64_t)blk.cap >= (uint64_t)count + 1024;  // _ALIAS_MIN_BLOCKSIZE :87, MaxEncodedLen :83
     int dt = blk.data_type;
     if (dt == DT_MULTIMEDIA || dt == DT_UTF8 || dt == DT_EXE || dt == DT_BIN) go = false;       // :98-104
-    if (blk.only_dna && dt != DT_UNDEFINED && dt != DT_DNA) go = false;                          // :106-108
+    if (blk.flags && dt != DT_UNDEFINED && dt != DT_DNA) go = false;                          // :106-108
     if (go) {
         const uint32_t* f = hist0 + (size_t)b * 256;
         uint32_t n0 = 0;
@@ -193,7 +193,7 @@ __global__ void __launch_bounds__(32) alias_plan_kernel(const uint8_t* __restric
         if (go && dt == DT_UNDEFINED) {  // :129-139
             dt = detect_simple_type_dev(count, f);
             if (dt != DT_UNDEFINED) r.data_type = dt;
-            if (dt != DT_DNA && blk.only_dna) go = false;
+            if (dt != DT_DNA && blk.flags) go = false;
         }
         if (go) {
             I.n0 = n0;
@@ -249,7 +249,7 @@ __global__ void __launch_bounds__(32) alias_plan_kernel(const uint8_t* __restric
 }
 
 // modes 2 / 3: every thread packs 4 (or 2) symbols into one byte
-__global__ void __launch_bounds__(256) alias_pack_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_pack_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                           uint8_t* __restrict__ out) {
     const int b = blockIdx.y;
     const AliasInfo& I = infos[b];
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256) alias_pack_kernel(const uint8_t* __restri
     __shared__ uint8_t m[256];
     m[threadIdx.x] = I.map8[threadIdx.x];
     __syncthreads();
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint8_t* src = in + blk.src_off;
     uint8_t* dst = out + blk.dst_off + I.hdr_len;
     const uint32_t count = blk.len;
@@ -277,11 +277,11 @@ __global__ void __launch_bounds__(256) alias_pack_kernel(const uint8_t* __restri
 }
 
 // mode 4: histogram of (previous byte, byte) pairs, previous = 0 for the first byte (ComputeHistogram order 1, internal/Global.go:305-341)
-__global__ void __launch_bounds__(256) alias_hist1_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_hist1_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                            uint32_t* __restrict__ hist1) {
     const int b = blockIdx.y;
     if (infos[b].mode != 4) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint8_t* src = in + blk.src_off;
     uint32_t* h = hist1 + (size_t)b * 65536;
     for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < blk.len; i += gridDim.x * 256) {
@@ -291,8 +291,8 @@ __global__ void __launch_bounds__(256) alias_hist1_kernel(const uint8_t* __restr
 }
 
 // mode 4: the n0 most frequent digrams, by decreasing (frequency, value) (:233-240), get the free byte values in increasing order
-__global__ void __launch_bounds__(1024) alias_select_kernel(const AliasBlock* __restrict__ blocks, AliasInfo* __restrict__ infos, const uint32_t* __restrict__ hist1,
-                                                             uint16_t* __restrict__ map16_all, uint8_t* __restrict__ out, AliasResult* __restrict__ res) {
+__global__ void __launch_bounds__(1024) alias_select_kernel(const StageBlock* __restrict__ blocks, AliasInfo* __restrict__ infos, const uint32_t* __restrict__ hist1,
+                                                             uint16_t* __restrict__ map16_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     AliasInfo& I = infos[b];
     if (I.mode != 4) return;
@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(1024) alias_select_kernel(const AliasBlock* __
     __shared__ unsigned long long s_best;
     __shared__ uint32_t s_cnt[32];
     __shared__ uint32_t s_n0;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t* h = hist1 + (size_t)b * 65536;
     uint16_t* map16 = map16_all + (size_t)b * 65536;
     uint8_t* dst = out + blk.dst_off;
@@ -394,11 +394,11 @@ __global__ void __launch_bounds__(1024) alias_select_kernel(const AliasBlock* __
     }
 }
 
-__global__ void __launch_bounds__(256) alias_dg_tiles_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_dg_tiles_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                               const uint16_t* __restrict__ map16_all, uint32_t* __restrict__ tile_fn, uint32_t ntiles) {
     const int b = blockIdx.y;
     if (infos[b].mode != 4) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if ((uint64_t)blockIdx.x * ALIAS_TILE >= blk.len) return;
     __shared__ uint32_t s_warp[8];
     uint32_t pm, nv;
@@ -410,14 +410,14 @@ __global__ void __launch_bounds__(256) alias_dg_tiles_kernel(const uint8_t* __re
 }
 
 // serial pass over the tile functions of a block: entering state and output offset of every tile, total size, final decision
-__global__ void __launch_bounds__(32) alias_dg_scan_kernel(const AliasBlock* __restrict__ blocks, int nblocks, AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(32) alias_dg_scan_kernel(const StageBlock* __restrict__ blocks, int nblocks, AliasInfo* __restrict__ infos,
                                                             const uint32_t* __restrict__ tile_fn, uint32_t* __restrict__ tile_in, uint32_t* __restrict__ tile_off,
-                                                            uint32_t ntiles, AliasResult* __restrict__ res) {
+                                                            uint32_t ntiles, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     AliasInfo& I = infos[b];
     if (I.mode != 4) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t nt = (blk.len + ALIAS_TILE - 1) / ALIAS_TILE;
     uint32_t state = 0, off = I.hdr_len;
     for (uint32_t t = 0; t < nt; t++) {
@@ -433,20 +433,20 @@ __global__ void __launch_bounds__(32) alias_dg_scan_kernel(const AliasBlock* __r
         return;  // mode stays 4: the emit kernel still runs, its output is ignored
     }
     I.status = 0;
-    AliasResult r = res[b];
+    StageResult r = res[b];
     r.status = 0;
     r.out_len = off;
     r.mode = 4;
     res[b] = r;
 }
 
-__global__ void __launch_bounds__(256) alias_dg_emit_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_dg_emit_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                              const uint16_t* __restrict__ map16_all, const uint32_t* __restrict__ tile_in,
                                                              const uint32_t* __restrict__ tile_off, uint32_t ntiles, uint8_t* __restrict__ out) {
     const int b = blockIdx.y;
     const AliasInfo& I = infos[b];
     if (I.mode != 4 || I.status != 0) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if ((uint64_t)blockIdx.x * ALIAS_TILE >= blk.len) return;
     __shared__ uint32_t s_warp[8];
     const uint16_t* map16 = map16_all + (size_t)b * 65536;
@@ -478,13 +478,13 @@ __global__ void __launch_bounds__(256) alias_dg_emit_kernel(const uint8_t* __res
 // ------------------------------------------------------------------------------------------------------------------
 // inverse
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(32) alias_inv_plan_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, int nblocks,
-                                                             AliasInfo* __restrict__ infos, AliasResult* __restrict__ res) {
+__global__ void __launch_bounds__(32) alias_inv_plan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
+                                                             AliasInfo* __restrict__ infos, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     AliasInfo& I = infos[b];
-    AliasResult r;
+    StageResult r;
     r.status = 0;
     r.out_len = 0;
     r.data_type = 0;
@@ -572,12 +572,12 @@ __global__ void __launch_bounds__(32) alias_inv_plan_kernel(const uint8_t* __res
     res[b] = r;
 }
 
-__global__ void __launch_bounds__(256) alias_inv_fill_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_inv_fill_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                               uint8_t* __restrict__ out) {
     const int b = blockIdx.y;
     const AliasInfo& I = infos[b];
     if (I.mode < 1 || I.mode > 3) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint8_t* src = in + blk.src_off;
     uint8_t* dst = out + blk.dst_off;
     __shared__ uint8_t sym[16];
@@ -610,7 +610,7 @@ __global__ void __launch_bounds__(256) alias_inv_fill_kernel(const uint8_t* __re
 }
 
 // mode 4: bytes of output produced by every tile of 4096 input bytes
-__global__ void __launch_bounds__(256) alias_inv_tiles_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_inv_tiles_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                                uint32_t* __restrict__ tile_fn, uint32_t ntiles) {
     const int b = blockIdx.y;
     const AliasInfo& I = infos[b];
@@ -634,14 +634,14 @@ __global__ void __launch_bounds__(256) alias_inv_tiles_kernel(const uint8_t* __r
     }
 }
 
-__global__ void __launch_bounds__(32) alias_inv_scan_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) alias_inv_scan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                              AliasInfo* __restrict__ infos, const uint32_t* __restrict__ tile_fn, uint32_t* __restrict__ tile_off,
-                                                             uint32_t ntiles, AliasResult* __restrict__ res) {
+                                                             uint32_t ntiles, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     AliasInfo& I = infos[b];
     if (I.mode != 4) return;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint8_t* src = in + blk.src_off;
     const uint32_t n = I.src_end - I.hdr_len;
     const uint32_t nt = (n + ALIAS_TILE - 1) / ALIAS_TILE;
@@ -660,7 +660,7 @@ __global__ void __launch_bounds__(32) alias_inv_scan_kernel(const uint8_t* __res
         if (I.src_end >= blk.len || off >= blk.cap) bad = true;
         off += 1;
     }
-    AliasResult r = res[b];
+    StageResult r = res[b];
     if (bad || off > 0xFFFFFFFFull) {
         I.status = -KZ_E_PROCESS_BLOCK;
         r.status = -KZ_E_PROCESS_BLOCK;
@@ -672,13 +672,13 @@ __global__ void __launch_bounds__(32) alias_inv_scan_kernel(const uint8_t* __res
     res[b] = r;
 }
 
-__global__ void __launch_bounds__(256) alias_inv_emit_kernel(const uint8_t* __restrict__ in, const AliasBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) alias_inv_emit_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const AliasInfo* __restrict__ infos,
                                                               const uint32_t* __restrict__ tile_off, uint32_t ntiles, uint8_t* __restrict__ out) {
     const int b = blockIdx.y;
     const AliasInfo& I = infos[b];
     if (I.mode != 4 || I.status != 0) return;
     const uint32_t n = I.src_end - I.hdr_len;
-    const AliasBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     uint8_t* dst = out + blk.dst_off;
     if (blockIdx.x == 0 && threadIdx.x == 0 && I.adjust != 0) dst[I.out_len - 1] = in[blk.src_off + I.src_end];
     if ((uint64_t)blockIdx.x * ALIAS_TILE >= n) return;
@@ -719,8 +719,8 @@ size_t alias_workspace(uint32_t nblocks, uint32_t max_len) {
            align256((size_t)nblocks * 65536 * 2) + 3 * align256((size_t)nblocks * ntiles * 4) + 256;
 }
 
-cudaError_t alias_forward_batch(const uint8_t* d_in, uint8_t* d_out, const AliasBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                                AliasResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t alias_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                                StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
     if (ws_bytes < alias_workspace(nblocks, max_len)) return cudaErrorInvalidValue;
     const Ws w = carve(ws, nblocks, max_len);
@@ -743,8 +743,8 @@ cudaError_t alias_forward_batch(const uint8_t* d_in, uint8_t* d_out, const Alias
     return cudaGetLastError();
 }
 
-cudaError_t alias_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const AliasBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                                AliasResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t alias_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                                StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
     if (ws_bytes < alias_workspace(nblocks, max_len)) return cudaErrorInvalidValue;
     const Ws w = carve(ws, nblocks, max_len);

@@ -5,31 +5,16 @@
 
 namespace kz {
 
-struct AliasBlock {
-    uint64_t src_off;   // byte offset of the block in the source buffer
-    uint64_t dst_off;   // byte offset of the block in the destination buffer
-    uint32_t len;       // input length (0 = inactive block)
-    uint32_t cap;       // destination capacity (inverse: len(dst) of the reference call)
-    int32_t data_type;  // forward: ctx["dataType"] before the call
-    uint32_t only_dna;  // forward: 1 for the DNA flavour (Factory.go:151-153 "packOnlyDNA")
-};
-struct AliasResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip; inverse: 0 = ok, negative = -(error code)
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call
-    uint32_t mode;      // 0 skip, 1 one symbol, 2 four symbols, 3 sixteen symbols, 4 digram aliases
-};
-
 static const uint32_t ALIAS_TILE = 4096;  // positions per tile of the digram parse / expansion scans
 
 // bytes of device workspace for a batch (forward and inverse)
 size_t alias_workspace(uint32_t nblocks, uint32_t max_len);
 
 // All blocks of a batch; d_blocks / d_res are device arrays of nblocks entries. No host synchronisation inside.
-cudaError_t alias_forward_batch(const uint8_t* d_in, uint8_t* d_out, const AliasBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                                AliasResult* d_res, cudaStream_t stream, uint64_t* launches);
-cudaError_t alias_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const AliasBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                                AliasResult* d_res, cudaStream_t stream, uint64_t* launches);
+cudaError_t alias_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                                StageResult* d_res, cudaStream_t stream, uint64_t* launches);
+cudaError_t alias_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                                StageResult* d_res, cudaStream_t stream, uint64_t* launches);
 
 // internal/Global.go:346-419 DetectSimpleType over a 256-bin histogram (device; header-only so that every kernel file can use it)
 static __device__ __forceinline__ int detect_simple_type_dev(uint32_t count, const uint32_t* f) {

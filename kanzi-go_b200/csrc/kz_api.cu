@@ -880,27 +880,19 @@ struct TransformPlan {
     int nt = 0;
     uint64_t ids[8];
     bool none() const { return nt == 1 && ids[0] == KZ_T_NONE; }
-    bool bwt() const { return nt == 1 && ids[0] == KZ_T_BWT; }
-    bool lz() const { return nt == 1 && (ids[0] == KZ_T_LZ || ids[0] == KZ_T_LZX); }
-    bool lzx() const { return nt == 1 && ids[0] == KZ_T_LZX; }
+    // the transforms that exist as GPU stages; every plan but NONE is a sequence of them
     static bool seq_id(uint64_t t) {
         return t == KZ_T_BWT || t == KZ_T_BWTS || t == KZ_T_RANK || t == KZ_T_MTFT || t == KZ_T_ZRLT || t == KZ_T_ROLZ || t == KZ_T_PACK || t == KZ_T_DNA || t == KZ_T_LZ ||
-               t == KZ_T_LZX || t == KZ_T_MM || t == KZ_T_TEXT || t == KZ_T_UTF || t == KZ_T_EXE || t == KZ_T_EXE;
+               t == KZ_T_LZX || t == KZ_T_MM || t == KZ_T_TEXT || t == KZ_T_UTF || t == KZ_T_EXE;
     }
-    // any sequence of BWT / BWTS / RANK / MTFT / ZRLT / ROLZ stages (e.g. "BWT+RANK+ZRLT", the transform chain of kanzi -l 5)
     // stages that read ctx["dataType"] in a way the block's magic number can change (LZ / LZX only look for DNA / small alphabets)
     bool uses_magic() const {
         for (int i = 0; i < nt; i++)
             if (ids[i] == KZ_T_ROLZ || ids[i] == KZ_T_PACK || ids[i] == KZ_T_DNA || ids[i] == KZ_T_MM || ids[i] == KZ_T_TEXT || ids[i] == KZ_T_UTF || ids[i] == KZ_T_EXE) return true;
         return false;
     }
-    bool generic() const {
-        if (bwt() || lz()) return false;  // single BWT / LZ / LZX keep their dedicated paths
-        for (int i = 0; i < nt; i++)
-            if (!seq_id(ids[i])) return false;
-        return true;
-    }
 };
+const char* const NO_GPU_TRANSFORM = "transform not available on the GPU path (BWT, BWTS, LZ, LZX, ROLZ, RANK, MTFT, ZRLT, PACK, DNA, MM, TEXT, UTF, EXE are)";
 
 // etype: the entropy codec of the stream. The reference picks the TEXT encoding from it (transform/Factory.go:99-119): encoding 2 for NONE /
 // ANS0 / HUFFMAN / RANGE, encoding 1 otherwise; only encoding 2 (textCodec2) exists here, so TEXT with any other codec is refused
@@ -913,22 +905,94 @@ int plan_transforms(kz_ctx* ctx, uint64_t t48, uint32_t etype, TransformPlan& p,
     for (int i = 0; i < p.nt; i++)
         if (p.ids[i] == KZ_T_TEXT && !text_available())
             return ctx->fail(err_code, "TEXT: the library was built without the static dictionary (kanzi-go_b200/gen_text_dict.py)");
-    if (!(p.none() || p.bwt() || p.lz() || p.generic()))
-        return ctx->fail(err_code, "transform sequence not available on the GPU path (sequences of BWT / BWTS / LZ / LZX / ROLZ / RANK / MTFT / ZRLT / PACK / DNA are)");
+    if (!p.none())
+        for (int i = 0; i < p.nt; i++)
+            if (!TransformPlan::seq_id(p.ids[i]))
+                return ctx->fail(err_code, "transform sequence not available on the GPU path (sequences of BWT / BWTS / LZ / LZX / ROLZ / RANK / MTFT / ZRLT / PACK / DNA / MM / TEXT / UTF / EXE are)");
     return 0;
 }
 
 
 // ------------------------------------------------------------------------------------------------------------
-// Generic transform sequences (ByteTransformSequence, transform/Sequence.go:64-186) over the stages that exist as
-// kernels: BWT, RANK, MTFT, ZRLT. Every stage processes all blocks of the batch; a stage that declines a block
-// ("skip", Sequence.go:100-105) leaves its skip bit set and the block moves on unchanged.
+// Transform sequences (ByteTransformSequence, transform/Sequence.go:64-186): every plan but NONE, one stage or several. Every stage
+// processes all blocks of the batch; a stage that declines a block ("skip", Sequence.go:100-105) leaves its skip bit set and the block
+// moves on unchanged.
 // ------------------------------------------------------------------------------------------------------------
+// The blocks of one stage call: block b is read at b * istride and written at b * ostride. A forward call passes `applied` (and `dts` when
+// the caller keeps ctx["dataType"]); an inverse call passes neither.
+struct StageIo {
+    uint64_t istride, ostride;
+    std::vector<uint32_t>& len;
+    const std::vector<uint8_t>& active;
+    std::vector<uint8_t>* applied;
+    std::vector<int32_t>* dts;
+};
+
+// A stage with one descriptor and one StageResult per block (ROLZ, TEXT, UTF, EXE, MM, PACK / DNA; Block is RolzBlock for ROLZ, which
+// carries a scratch offset, StageBlock otherwise). Every sub-batch of `sub` blocks (0: the whole batch) that holds an active block gets
+// its descriptors (offsets, len, data_type; `desc` sets cap and the stage's own fields), ws(nb, max_len) bytes of workspace, one upload
+// of the descriptors with room for the results, one `launch` (the stage's kernels) under a LaunchScope named `scope`, and the results
+// copied back. Forward: status 0 = transformed, anything else = declined, ctx["dataType"] after the call is kept for every active block;
+// a negative status fails with `bad` when one is given (EXE: a block the reference panics on). Inverse: any status but 0 fails with `bad`.
+template <class Block, class Desc, class Ws, class Launch>
+int run_desc_stage(kz_ctx* ctx, const StageIo& io, const char* scope, uint32_t sub, Desc desc, Ws ws, Launch launch, const char* bad = nullptr) {
+    const uint32_t nblocks = (uint32_t)io.len.size();
+    if (sub == 0) sub = nblocks;
+    for (uint32_t b0 = 0; b0 < nblocks; b0 += sub) {
+        const uint32_t nb = std::min(sub, nblocks - b0);
+        uint32_t max_len = 0;
+        for (uint32_t b = b0; b < b0 + nb; b++) max_len = std::max(max_len, io.active[b] ? io.len[b] : 0u);
+        if (max_len == 0) continue;
+        std::vector<Block> hb(nb);
+        for (uint32_t k = 0; k < nb; k++) {
+            const uint32_t b = b0 + k;
+            hb[k] = Block{};
+            hb[k].src_off = b * io.istride;
+            hb[k].dst_off = b * io.ostride;
+            hb[k].len = io.active[b] ? io.len[b] : 0;
+            hb[k].data_type = io.dts ? (*io.dts)[b] : 0;
+            desc(hb[k], b);
+        }
+        CK(ctx->d_ws.ensure(ws(nb, max_len)));
+        Packer pk;
+        const size_t o_blk = pk.add(hb.data(), hb.size() * sizeof(Block));
+        const size_t o_res = pk.reserve((size_t)nb * sizeof(StageResult));
+        int rc = upload(ctx, pk);
+        if (rc) return rc;
+        uint8_t* T = ctx->d_tables.as<uint8_t>();
+        {
+            LaunchScope ls(ctx, scope);
+            cudaError_t e = launch((const Block*)(T + o_blk), hb.data(), nb, max_len, (StageResult*)(T + o_res));
+            if (e != cudaSuccess) return ctx->cuda_fail(e, scope);
+        }
+        std::vector<StageResult> hr(nb);
+        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(StageResult), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t k = 0; k < nb; k++) {
+            const uint32_t b = b0 + k;
+            if (!io.active[b] || io.len[b] == 0) continue;
+            if (!io.applied) {
+                if (hr[k].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, bad);
+                io.len[b] = hr[k].out_len;
+                continue;
+            }
+            if (hr[k].status < 0 && bad) return ctx->fail(KZ_ERR_PROCESS_BLOCK, bad);
+            if (io.dts) (*io.dts)[b] = hr[k].data_type;
+            if (hr[k].status == 0) {
+                (*io.applied)[b] = 1;
+                io.len[b] = hr[k].out_len;
+            }
+        }
+    }
+    return 0;
+}
+
 // One forward stage. Block b: d_in + b*istride (len[b] bytes) -> d_out + b*ostride. applied[b] = 1 and len[b] updated on success.
 int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride, uint8_t* d_out, uint64_t ostride, std::vector<uint32_t>& len,
                   const std::vector<uint8_t>& active, std::vector<uint8_t>& applied, std::vector<int32_t>* dts = nullptr) {
     const uint32_t nblocks = (uint32_t)len.size();
     applied.assign(nblocks, 0);
+    const StageIo io{istride, ostride, len, active, &applied, dts};
     if (t == KZ_T_BWT) {
         CK(ctx->d_lens.ensure((size_t)nblocks * 4 + 64));
         uint32_t* d_post = ctx->d_lens.as<uint32_t>();
@@ -984,46 +1048,23 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
         uint32_t max_len = 0;
         for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, len[b]);
         const size_t sstride = rolz_scratch_bytes(max_len);
-        CK(ctx->d_ws.ensure(sstride * nblocks + 256));
-        std::vector<RolzBlock> rb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            rb[b].src_off = b * istride;
-            rb[b].dst_off = b * ostride;
-            rb[b].scratch_off = b * sstride;
-            rb[b].len = active[b] ? len[b] : 0;
-            rb[b].cap = (uint32_t)std::min<uint64_t>(ostride, 0xFFFFFFF0u);
-            rb[b].data_type = dts ? (*dts)[b] : 0;
-            rb[b].pad = 0;
-        }
-        Packer pk;
-        const size_t o_rb = pk.add(rb.data(), rb.size() * sizeof(RolzBlock));
-        const size_t o_res = pk.reserve((size_t)nblocks * sizeof(RolzResult));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        {
-            LaunchScope ls(ctx, "rolz_forward");
-            rolz_forward_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_in, (const RolzBlock*)(T + o_rb), (int)nblocks, ctx->d_ws.as<uint8_t>(), d_out,
-                                                                (RolzResult*)(T + o_res));
-        }
-        CK(cudaGetLastError());
-        std::vector<RolzResult> hr(nblocks);
-        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nblocks * sizeof(RolzResult), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (active[b] && len[b] && hr[b].status == 0) {
-                applied[b] = 1;
-                len[b] = hr[b].out_len;
-            }
-            if (dts && active[b] && len[b]) (*dts)[b] = hr[b].data_type;  // ctx["dataType"] after the call
-        }
+        return run_desc_stage<RolzBlock>(
+            ctx, io, "rolz_forward", 0,
+            [&](RolzBlock& d, uint32_t b) {
+                d.scratch_off = b * sstride;
+                d.cap = (uint32_t)std::min<uint64_t>(ostride, 0xFFFFFFF0u);
+            },
+            [&](uint32_t nb, uint32_t) { return sstride * nb + 256; },
+            [&](const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                rolz_forward_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, ctx->d_ws.as<uint8_t>(), d_out, res);
+                return cudaGetLastError();
+            });
     } else if (t == KZ_T_LZ || t == KZ_T_LZX) {  // LZCodec as a stage of a sequence (e.g. "DNA+LZ" = kanzi -l 2)
         const bool extra = t == KZ_T_LZX;
         uint32_t max_len = 0;
         for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, len[b]);
         if ((uint64_t)max_len + max_len / 64 + 128 > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for LZ");
         const uint64_t sstride = (lz_scratch_bytes(max_len) + 255) & ~size_t(255);
-        const size_t hbytes = ((size_t)nblocks << (extra ? 19 : 16)) * 4;
         std::vector<LzBlock> lb(nblocks);
         for (uint32_t b = 0; b < nblocks; b++) {
             lb[b].src_off = b * istride;
@@ -1046,215 +1087,55 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             }
     } else if (t == KZ_T_TEXT) {  // TextCodec (encoding 2): declines unless the block looks like text
         if (!text_available()) return ctx->fail(KZ_ERR_CREATE_CODEC, "TEXT: the library was built without the static dictionary");
-        const uint32_t SUB = 64;  // ~9 MB of dictionary per block
         const uint64_t sbs = ctx->stream_bs ? ctx->stream_bs : *std::max_element(len.begin(), len.end());
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            uint32_t max_len = 0;
-            for (uint32_t b = b0; b < b0 + nb; b++) max_len = std::max(max_len, active[b] ? len[b] : 0u);
-            if (max_len == 0) continue;
-            CK(ctx->d_ws.ensure(text_workspace(nb, sbs, max_len)));
-            std::vector<TextBlock> tb(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                tb[k].src_off = b * istride;
-                tb[k].dst_off = b * ostride;
-                tb[k].len = active[b] ? len[b] : 0;
-                tb[k].cap = len[b];  // MaxEncodedLen = srcLen (:1720-1724)
-                tb[k].data_type = dts ? (*dts)[b] : 0;
-                tb[k].pad = 0;
-            }
-            Packer pk;
-            const size_t o_tb = pk.add(tb.data(), tb.size() * sizeof(TextBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(TextResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "text_forward");
-                cudaError_t e = text_forward_batch(d_in, d_out, (const TextBlock*)(T + o_tb), tb.data(), nb, max_len, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                   (TextResult*)(T + o_res), ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "text_forward");
-            }
-            std::vector<TextResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(TextResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (dts) (*dts)[b] = hr[k].data_type;
-                if (hr[k].status == 0) {
-                    applied[b] = 1;
-                    len[b] = hr[k].out_len;
-                }
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "text_forward", 64,                          // ~9 MB of dictionary per block
+            [&](StageBlock& d, uint32_t b) { d.cap = len[b]; },  // MaxEncodedLen = srcLen (:1720-1724)
+            [&](uint32_t nb, uint32_t max_len) { return text_workspace(nb, sbs, max_len); },
+            [&](const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t max_len, StageResult* res) {
+                return text_forward_batch(d_in, d_out, db, hb, nb, max_len, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            });
     } else if (t == KZ_T_UTF) {  // UTFCodec.Forward: declines unless the block is UTF-8 with enough multi-byte sequences
-        const uint32_t SUB = 32;  // 16 MB of code point counters per block
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            bool any = false;
-            for (uint32_t b = b0; b < b0 + nb; b++) any = any || (active[b] && len[b]);
-            if (!any) continue;
-            CK(ctx->d_ws.ensure(utf_workspace(nb)));
-            std::vector<UtfBlock> ub(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                ub[k].src_off = b * istride;
-                ub[k].dst_off = b * ostride;
-                ub[k].len = active[b] ? len[b] : 0;
-                ub[k].cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 8192, 0xFFFFFFF0u);  // MaxEncodedLen (:386-388)
-                ub[k].data_type = dts ? (*dts)[b] : 0;
-                ub[k].pad = 0;
-            }
-            Packer pk;
-            const size_t o_ub = pk.add(ub.data(), ub.size() * sizeof(UtfBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(UtfResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "utf_forward");
-                cudaError_t e = utf_forward_batch(d_in, d_out, (const UtfBlock*)(T + o_ub), nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, (UtfResult*)(T + o_res),
-                                                  ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "utf_forward");
-            }
-            std::vector<UtfResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(UtfResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (dts) (*dts)[b] = hr[k].data_type;
-                if (hr[k].status == 0) {
-                    applied[b] = 1;
-                    len[b] = hr[k].out_len;
-                }
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "utf_forward", 32,  // 16 MB of code point counters per block
+            [&](StageBlock& d, uint32_t b) { d.cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 8192, 0xFFFFFFF0u); },  // MaxEncodedLen (:386-388)
+            [](uint32_t nb, uint32_t) { return utf_workspace(nb); },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                return utf_forward_batch(d_in, d_out, db, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            });
     } else if (t == KZ_T_EXE) {  // EXECodec.Forward: declines unless the block is x86 / ARM64 code
-        std::vector<ExeBlock> eb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            const uint64_t mel = len[b] <= 256 ? (uint64_t)len[b] + 32 : (uint64_t)len[b] + len[b] / 8;  // MaxEncodedLen (:701-708)
-            if (active[b] && mel > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for EXE");
-            eb[b].src_off = b * istride;
-            eb[b].dst_off = b * ostride;
-            eb[b].len = active[b] ? len[b] : 0;
-            eb[b].cap = (uint32_t)std::min<uint64_t>(mel, 0xFFFFFFF0u);
-            eb[b].data_type = dts ? (*dts)[b] : 0;
-            eb[b].pad = 0;
-        }
-        Packer pk;
-        const size_t o_eb = pk.add(eb.data(), eb.size() * sizeof(ExeBlock));
-        const size_t o_res = pk.reserve((size_t)nblocks * sizeof(ExeResult));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        {
-            LaunchScope ls(ctx, "exe_forward");
-            exe_forward_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_in, (const ExeBlock*)(T + o_eb), (int)nblocks, d_out, (ExeResult*)(T + o_res));
-            ctx->launches++;
-        }
-        CK(cudaGetLastError());
-        std::vector<ExeResult> hr(nblocks);
-        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nblocks * sizeof(ExeResult), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (!active[b] || len[b] == 0) continue;
-            if (hr[b].status < 0) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "EXE codec: malformed executable header (the reference panics on this block)");
-            if (dts) (*dts)[b] = hr[b].data_type;
-            if (hr[b].status == 0) {
-                applied[b] = 1;
-                len[b] = hr[b].out_len;
-            }
-        }
+        auto mel = [](uint32_t n) { return n <= 256 ? (uint64_t)n + 32 : (uint64_t)n + n / 8; };  // MaxEncodedLen (:701-708)
+        for (uint32_t b = 0; b < nblocks; b++)
+            if (active[b] && mel(len[b]) > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for EXE");
+        return run_desc_stage<StageBlock>(
+            ctx, io, "exe_forward", 0, [&](StageBlock& d, uint32_t b) { d.cap = (uint32_t)std::min<uint64_t>(mel(len[b]), 0xFFFFFFF0u); },
+            [](uint32_t, uint32_t) { return (size_t)0; },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                exe_forward_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, d_out, res);
+                return cudaGetLastError();
+            },
+            "EXE codec: malformed executable header (the reference panics on this block)");
     } else if (t == KZ_T_MM) {  // FSDCodec.Forward: declines unless a fixed-step delta lowers the sampled entropy
-        const uint32_t SUB = 1024;
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            uint32_t max_len = 0;
-            for (uint32_t b = b0; b < b0 + nb; b++) max_len = std::max(max_len, active[b] ? len[b] : 0u);
-            if (max_len == 0) continue;
-            if ((uint64_t)fsd_max_encoded_len(max_len) > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for MM");
-            CK(ctx->d_ws.ensure(fsd_workspace(nb, max_len)));
-            std::vector<FsdBlock> fb(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                fb[k].src_off = b * istride;
-                fb[k].dst_off = b * ostride;
-                fb[k].len = active[b] ? len[b] : 0;
-                fb[k].cap = fsd_max_encoded_len(len[b]);  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
-                fb[k].data_type = dts ? (*dts)[b] : 0;
-                fb[k].pad = 0;
-            }
-            Packer pk;
-            const size_t o_fb = pk.add(fb.data(), fb.size() * sizeof(FsdBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(FsdResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "fsd_forward");
-                cudaError_t e = fsd_forward_batch(d_in, d_out, (const FsdBlock*)(T + o_fb), nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                  (FsdResult*)(T + o_res), ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "fsd_forward");
-            }
-            std::vector<FsdResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(FsdResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (dts) (*dts)[b] = hr[k].data_type;
-                if (hr[k].status == 0) {
-                    applied[b] = 1;
-                    len[b] = hr[k].out_len;
-                }
-            }
-        }
+        for (uint32_t b = 0; b < nblocks; b++)
+            if (active[b] && fsd_max_encoded_len(len[b]) > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for MM");
+        return run_desc_stage<StageBlock>(
+            ctx, io, "fsd_forward", 1024,
+            [&](StageBlock& d, uint32_t b) { d.cap = fsd_max_encoded_len(len[b]); },  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
+            [](uint32_t nb, uint32_t max_len) { return fsd_workspace(nb, max_len); },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
+                return fsd_forward_batch(d_in, d_out, db, nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            });
     } else if (t == KZ_T_PACK || t == KZ_T_DNA) {  // AliasCodec.Forward: bit packing of small alphabets / digram aliases; often declines
-        const uint32_t SUB = 256;  // blocks per launch sequence (bounds the workspace: ~390 KB per block)
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            uint32_t max_len = 0;
-            for (uint32_t b = b0; b < b0 + nb; b++) max_len = std::max(max_len, active[b] ? len[b] : 0u);
-            if (max_len == 0) continue;
-            CK(ctx->d_ws.ensure(alias_workspace(nb, max_len)));
-            std::vector<AliasBlock> ab(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                ab[k].src_off = b * istride;
-                ab[k].dst_off = b * ostride;
-                ab[k].len = active[b] ? len[b] : 0;
-                ab[k].cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 1024, 0xFFFFFFF0u);  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
-                ab[k].data_type = dts ? (*dts)[b] : 0;
-                ab[k].only_dna = t == KZ_T_DNA ? 1u : 0u;
-            }
-            Packer pk;
-            const size_t o_ab = pk.add(ab.data(), ab.size() * sizeof(AliasBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(AliasResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "alias_forward");
-                cudaError_t e = alias_forward_batch(d_in, d_out, (const AliasBlock*)(T + o_ab), nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                    (AliasResult*)(T + o_res), ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "alias_forward");
-            }
-            std::vector<AliasResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(AliasResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (dts) (*dts)[b] = hr[k].data_type;
-                if (hr[k].status == 0) {
-                    applied[b] = 1;
-                    len[b] = hr[k].out_len;
-                }
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "alias_forward", 256,  // blocks per launch sequence (bounds the workspace: ~390 KB per block)
+            [&](StageBlock& d, uint32_t b) {
+                d.cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 1024, 0xFFFFFFF0u);  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
+                d.flags = t == KZ_T_DNA ? 1u : 0u;
+            },
+            [](uint32_t nb, uint32_t max_len) { return alias_workspace(nb, max_len); },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
+                return alias_forward_batch(d_in, d_out, db, nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            });
     } else if (t == KZ_T_RANK || t == KZ_T_MTFT) {  // SBRT.Forward never declines (buffers are sized for MaxEncodedLen)
         std::vector<SbrtBlock> sb(nblocks);
         std::vector<uint32_t> seg_block;
@@ -1338,51 +1219,12 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
     return 0;
 }
 
-// ByteTransformSequence.Forward for every block of a batch. jobs[] must be initialised (copy flags, lengths).
-int forward_generic(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, uint64_t stride, const std::vector<uint32_t>& blen, const uint8_t** d_data,
-                    std::vector<EncJob>& jobs, std::vector<int32_t>& dts) {
-    const uint32_t nblocks = (uint32_t)blen.size();
-    uint32_t max_len = 0;
-    for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, blen[b]);
-    // room for the largest stage output: +33 bytes per BWT / SBRT stage, n/64 + 128 for LZ, n/16 for MM, headers of PACK
-    const uint64_t gstride = ((uint64_t)max_len + max_len / 8 + 33ull * plan.nt + 8192 + 1024 + 256 + 15) & ~15ull;
-    CK(ctx->d_tmp.ensure(gstride * nblocks + 64));
-    CK(ctx->d_tmp2.ensure(gstride * nblocks + 64));
-    std::vector<uint32_t> len(blen);
-    std::vector<uint8_t> active(nblocks), applied;
-    std::vector<uint8_t> flags(nblocks, 0xFF);
-    for (uint32_t b = 0; b < nblocks; b++) active[b] = !jobs[b].copy && blen[b] > 0;
-    const uint8_t* cur = d_src;
-    uint64_t cur_stride = stride;
-    for (int i = 0; i < plan.nt; i++) {
-        uint8_t* outb = (i & 1) ? ctx->d_tmp2.as<uint8_t>() : ctx->d_tmp.as<uint8_t>();
-        uint64_t bytes_in = 0, bytes_out = 0;
-        for (uint32_t b = 0; b < nblocks; b++) bytes_in += active[b] ? len[b] : 0;
-        int rc = apply_forward(ctx, plan.ids[i], cur, cur_stride, outb, gstride, len, active, applied, &dts);
-        if (rc) return rc;
-        for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
-        note_stage_bytes(ctx, "fwd", plan.ids[i], bytes_in, bytes_out);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (applied[b]) flags[b] &= (uint8_t)~(1u << (7 - i));
-            else if (len[b]) CK(cudaMemcpyAsync(outb + b * gstride, cur + b * cur_stride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
-        }
-        cur = outb;
-        cur_stride = gstride;
-    }
-    for (uint32_t b = 0; b < nblocks; b++) {
-        EncJob& j = jobs[b];
-        j.data_off = b * gstride;
-        j.post_len = len[b];
-        if (!j.copy) j.skip_flags = flags[b];
-    }
-    *d_data = cur;
-    return 0;
-}
-
 // One inverse stage, mirror of apply_forward. cap = capacity of a destination block.
 int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, uint64_t stride, uint32_t cap, std::vector<uint32_t>& len,
                   const std::vector<uint8_t>& active) {
     const uint32_t nblocks = (uint32_t)len.size();
+    const StageIo io{stride, stride, len, active, nullptr, nullptr};
+    auto cap_all = [&](StageBlock& d, uint32_t) { d.cap = cap; };
     if (t == KZ_T_BWT) {
         std::vector<uint8_t> heads((size_t)nblocks * 64, 0);
         CK(cudaMemcpy2DAsync(heads.data(), 64, d_in, stride, 33, nblocks, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1424,37 +1266,18 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         }
     } else if (t == KZ_T_ROLZ) {
         const size_t sstride = rolz_scratch_bytes(cap);
-        CK(ctx->d_ws.ensure(sstride * nblocks + 256));
-        std::vector<RolzBlock> rb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            rb[b].src_off = b * stride;
-            rb[b].dst_off = b * stride;
-            rb[b].scratch_off = b * sstride;
-            rb[b].len = active[b] ? len[b] : 0;
-            rb[b].cap = cap;
-            rb[b].data_type = 0;
-            rb[b].pad = 0;
-        }
-        Packer pk;
-        const size_t o_rb = pk.add(rb.data(), rb.size() * sizeof(RolzBlock));
-        const size_t o_res = pk.reserve((size_t)nblocks * sizeof(RolzResult));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        {
-            LaunchScope ls(ctx, "rolz_inverse");
-            rolz_inverse_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_in, (const RolzBlock*)(T + o_rb), (int)nblocks, ctx->d_ws.as<uint8_t>(), d_out,
-                                                                (RolzResult*)(T + o_res));
-        }
-        CK(cudaGetLastError());
-        std::vector<RolzResult> hr(nblocks);
-        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nblocks * sizeof(RolzResult), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (!active[b] || len[b] == 0) continue;
-            if (hr[b].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "ROLZ codec inverse transform failed: invalid data");
-            len[b] = hr[b].out_len;
-        }
+        return run_desc_stage<RolzBlock>(
+            ctx, io, "rolz_inverse", 0,
+            [&](RolzBlock& d, uint32_t b) {
+                d.scratch_off = b * sstride;
+                d.cap = cap;
+            },
+            [&](uint32_t nb, uint32_t) { return sstride * nb + 256; },
+            [&](const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                rolz_inverse_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, ctx->d_ws.as<uint8_t>(), d_out, res);
+                return cudaGetLastError();
+            },
+            "ROLZ codec inverse transform failed: invalid data");
     } else if (t == KZ_T_LZ || t == KZ_T_LZX) {
         std::vector<LzBlock> lb(nblocks);
         for (uint32_t b = 0; b < nblocks; b++) {
@@ -1481,190 +1304,44 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         }
     } else if (t == KZ_T_TEXT) {
         if (!text_available()) return ctx->fail(KZ_ERR_CREATE_CODEC, "TEXT: the library was built without the static dictionary");
-        const uint32_t SUB = 64;
         const uint64_t sbs = ctx->stream_bs ? ctx->stream_bs : cap;
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            bool any = false;
-            for (uint32_t b = b0; b < b0 + nb; b++) any = any || (active[b] && len[b]);
-            if (!any) continue;
-            uint32_t longest = 0;
-            for (uint32_t b = b0; b < b0 + nb; b++) longest = std::max(longest, active[b] ? len[b] : 0u);
-            CK(ctx->d_ws.ensure(text_workspace_inverse(nb, sbs, longest)));
-            std::vector<TextBlock> tb(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                tb[k].src_off = b * stride;
-                tb[k].dst_off = b * stride;
-                tb[k].len = active[b] ? len[b] : 0;
-                tb[k].cap = cap;
-                tb[k].data_type = 0;
-                tb[k].pad = 0;
-            }
-            Packer pk;
-            const size_t o_tb = pk.add(tb.data(), tb.size() * sizeof(TextBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(TextResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "text_inverse");
-                cudaError_t e = text_inverse_batch(d_in, d_out, (const TextBlock*)(T + o_tb), tb.data(), nb, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                   (TextResult*)(T + o_res), ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "text_inverse");
-            }
-            std::vector<TextResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(TextResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (hr[k].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "Text transform failed: invalid data");
-                len[b] = hr[k].out_len;
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "text_inverse", 64, cap_all, [&](uint32_t nb, uint32_t max_len) { return text_workspace_inverse(nb, sbs, max_len); },
+            [&](const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
+                return text_inverse_batch(d_in, d_out, db, hb, nb, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            },
+            "Text transform failed: invalid data");
     } else if (t == KZ_T_UTF) {
-        const uint32_t SUB = 32;
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            bool any = false;
-            for (uint32_t b = b0; b < b0 + nb; b++) any = any || (active[b] && len[b]);
-            if (!any) continue;
-            CK(ctx->d_ws.ensure(utf_workspace(nb)));
-            std::vector<UtfBlock> ub(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                ub[k].src_off = b * stride;
-                ub[k].dst_off = b * stride;
-                ub[k].len = active[b] ? len[b] : 0;
-                ub[k].cap = cap;
-                ub[k].data_type = 0;
-                ub[k].pad = 0;
-            }
-            Packer pk;
-            const size_t o_ub = pk.add(ub.data(), ub.size() * sizeof(UtfBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(UtfResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "utf_inverse");
-                cudaError_t e = utf_inverse_batch(d_in, d_out, (const UtfBlock*)(T + o_ub), nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, (UtfResult*)(T + o_res),
-                                                  ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "utf_inverse");
-            }
-            std::vector<UtfResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(UtfResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (hr[k].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "UTF inverse transform failed: invalid data");
-                len[b] = hr[k].out_len;
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "utf_inverse", 32, cap_all, [](uint32_t nb, uint32_t) { return utf_workspace(nb); },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                return utf_inverse_batch(d_in, d_out, db, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            },
+            "UTF inverse transform failed: invalid data");
     } else if (t == KZ_T_EXE) {
-        std::vector<ExeBlock> eb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            eb[b].src_off = b * stride;
-            eb[b].dst_off = b * stride;
-            eb[b].len = active[b] ? len[b] : 0;
-            eb[b].cap = cap;
-            eb[b].data_type = 0;
-            eb[b].pad = 0;
-        }
-        Packer pk;
-        const size_t o_eb = pk.add(eb.data(), eb.size() * sizeof(ExeBlock));
-        const size_t o_res = pk.reserve((size_t)nblocks * sizeof(ExeResult));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        {
-            LaunchScope ls(ctx, "exe_inverse");
-            exe_inverse_kernel<<<nblocks, 32, 0, ctx->stream>>>(d_in, (const ExeBlock*)(T + o_eb), (int)nblocks, d_out, (ExeResult*)(T + o_res));
-            ctx->launches++;
-        }
-        CK(cudaGetLastError());
-        std::vector<ExeResult> hr(nblocks);
-        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nblocks * sizeof(ExeResult), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (!active[b] || len[b] == 0) continue;
-            if (hr[b].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "ExeCodec inverse transform failed: invalid data");
-            len[b] = hr[b].out_len;
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "exe_inverse", 0, cap_all, [](uint32_t, uint32_t) { return (size_t)0; },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                exe_inverse_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, d_out, res);
+                return cudaGetLastError();
+            },
+            "ExeCodec inverse transform failed: invalid data");
     } else if (t == KZ_T_MM) {
-        std::vector<FsdBlock> fb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            fb[b].src_off = b * stride;
-            fb[b].dst_off = b * stride;
-            fb[b].len = active[b] ? len[b] : 0;
-            fb[b].cap = cap;
-            fb[b].data_type = 0;
-            fb[b].pad = 0;
-        }
-        Packer pk;
-        const size_t o_res = pk.reserve((size_t)nblocks * sizeof(FsdResult));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        {
-            LaunchScope ls(ctx, "fsd_inverse");
-            uint64_t total_len = 0;
-            for (uint32_t b = 0; b < nblocks; b++) total_len += fb[b].len;
-            CK(ctx->d_ws.ensure(fsd_inverse_workspace(nblocks, total_len)));
-            cudaError_t e = fsd_inverse_tiles(d_in, d_out, fb.data(), nblocks, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, (FsdResult*)(T + o_res), ctx->stream,
-                                              &ctx->launches);
-            if (e != cudaSuccess) return ctx->cuda_fail(e, "fsd_inverse");
-        }
-        std::vector<FsdResult> hr(nblocks);
-        CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nblocks * sizeof(FsdResult), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (!active[b] || len[b] == 0) continue;
-            if (hr[b].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "FSD inverse transform failed: invalid data");
-            len[b] = hr[b].out_len;
-        }
+        uint64_t total_len = 0;
+        for (uint32_t b = 0; b < nblocks; b++) total_len += active[b] ? len[b] : 0;
+        return run_desc_stage<StageBlock>(
+            ctx, io, "fsd_inverse", 0, cap_all, [&](uint32_t nb, uint32_t) { return fsd_inverse_workspace(nb, total_len); },
+            [&](const StageBlock*, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
+                return fsd_inverse_tiles(d_in, d_out, hb, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            },
+            "FSD inverse transform failed: invalid data");
     } else if (t == KZ_T_PACK || t == KZ_T_DNA) {
-        const uint32_t SUB = 256;
-        for (uint32_t b0 = 0; b0 < nblocks; b0 += SUB) {
-            const uint32_t nb = std::min(SUB, nblocks - b0);
-            bool any = false;
-            for (uint32_t b = b0; b < b0 + nb; b++) any = any || (active[b] && len[b]);
-            if (!any) continue;
-            CK(ctx->d_ws.ensure(alias_workspace(nb, cap)));
-            std::vector<AliasBlock> ab(nb);
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                ab[k].src_off = b * stride;
-                ab[k].dst_off = b * stride;
-                ab[k].len = active[b] ? len[b] : 0;
-                ab[k].cap = cap;
-                ab[k].data_type = 0;
-                ab[k].only_dna = 0;
-            }
-            Packer pk;
-            const size_t o_ab = pk.add(ab.data(), ab.size() * sizeof(AliasBlock));
-            const size_t o_res = pk.reserve((size_t)nb * sizeof(AliasResult));
-            int rc = upload(ctx, pk);
-            if (rc) return rc;
-            uint8_t* T = ctx->d_tables.as<uint8_t>();
-            {
-                LaunchScope ls(ctx, "alias_inverse");
-                cudaError_t e = alias_inverse_batch(d_in, d_out, (const AliasBlock*)(T + o_ab), nb, cap, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                                    (AliasResult*)(T + o_res), ctx->stream, &ctx->launches);
-                if (e != cudaSuccess) return ctx->cuda_fail(e, "alias_inverse");
-            }
-            std::vector<AliasResult> hr(nb);
-            CK(cudaMemcpyAsync(hr.data(), T + o_res, (size_t)nb * sizeof(AliasResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t b = b0 + k;
-                if (!active[b] || len[b] == 0) continue;
-                if (hr[k].status) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "Alias codec inverse transform failed: invalid data");
-                len[b] = hr[k].out_len;
-            }
-        }
+        return run_desc_stage<StageBlock>(
+            ctx, io, "alias_inverse", 256, cap_all, [&](uint32_t nb, uint32_t) { return alias_workspace(nb, cap); },
+            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+                return alias_inverse_batch(d_in, d_out, db, nb, cap, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            },
+            "Alias codec inverse transform failed: invalid data");
     } else if (t == KZ_T_RANK || t == KZ_T_MTFT) {
         std::vector<SbrtBlock> sb(nblocks);
         for (uint32_t b = 0; b < nblocks; b++) {
@@ -1728,12 +1405,77 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
     return 0;
 }
 
-// ByteTransformSequence.Inverse for every block of a batch. Block b's pre_len bytes are at d_pre + b*pstride (a scratch
-// buffer of this context with room for blk_cap bytes per block); decoded blocks go to d_dst back to back (compact) or at
-// b * slot.
-int inverse_generic(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, uint32_t blk_cap, uint8_t* d_dst,
-                    size_t cap, std::vector<uint32_t>& out_len, uint64_t* total, uint64_t slot, bool compact) {
+// Forward transform stage (ByteTransformSequence.Forward, transform/Sequence.go:64-125) of every block of a batch.
+// Block b is d_src[b*stride : +len_b]. On return *d_data is the base of the post-transform data and jobs[] describes
+// every block for the entropy stage. NONE leaves the data in place; the stages alternate between ctx->d_tmp and ctx->d_tmp2.
+int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, size_t n, uint32_t block_size, uint64_t stride, const uint32_t* lens,
+                  uint32_t nblocks, const uint8_t** d_data, std::vector<EncJob>& jobs, const std::vector<int32_t>* init_dt = nullptr) {
+    jobs.resize(nblocks);
+    std::vector<uint32_t> len(nblocks);
+    uint32_t max_len = 0;
+    for (uint32_t b = 0; b < nblocks; b++) {
+        len[b] = lens ? lens[b] : (uint32_t)std::min<uint64_t>(block_size, n - (uint64_t)b * block_size);
+        max_len = std::max(max_len, len[b]);
+    }
+    *d_data = d_src;
+    for (uint32_t b = 0; b < nblocks; b++) {
+        EncJob& j = jobs[b];
+        j.data_off = (uint64_t)b * stride;
+        j.post_len = len[b];
+        j.ntransforms = (uint32_t)plan.nt;
+        j.skip_flags = 0x7F;  // NullTransform succeeds: bit 7 cleared (Sequence.go:65,107)
+        j.copy = len[b] <= SMALL_BLOCK;  // io/CompressedStream.go:773-776: transform and entropy forced to NONE
+        j.checksum = 0;
+    }
+    if (plan.none() || nblocks == 0) return 0;
+    // ctx["dataType"] of every block: the caller's value (from the block's magic number, encodingTask.encode :808-816), updated by the stages
+    std::vector<int32_t> dts(nblocks, 0);
+    if (init_dt) dts = *init_dt;
+    // room for the largest stage output: +33 bytes per BWT / SBRT stage, n/64 + 128 for LZ, n/16 for MM, headers of PACK
+    const uint64_t gstride = ((uint64_t)max_len + max_len / 8 + 33ull * plan.nt + 8192 + 1024 + 256 + 15) & ~15ull;
+    CK(ctx->d_tmp.ensure(gstride * nblocks + 64));
+    if (plan.nt > 1) CK(ctx->d_tmp2.ensure(gstride * nblocks + 64));  // stage i writes to d_tmp (i even) or d_tmp2 (i odd)
+    std::vector<uint8_t> active(nblocks), applied;
+    std::vector<uint8_t> flags(nblocks, 0xFF);
+    for (uint32_t b = 0; b < nblocks; b++) active[b] = !jobs[b].copy && len[b] > 0;
+    const uint8_t* cur = d_src;
+    uint64_t cur_stride = stride;
+    for (int i = 0; i < plan.nt; i++) {
+        uint8_t* outb = (i & 1) ? ctx->d_tmp2.as<uint8_t>() : ctx->d_tmp.as<uint8_t>();
+        uint64_t bytes_in = 0, bytes_out = 0;
+        for (uint32_t b = 0; b < nblocks; b++) bytes_in += active[b] ? len[b] : 0;
+        int rc = apply_forward(ctx, plan.ids[i], cur, cur_stride, outb, gstride, len, active, applied, &dts);
+        if (rc) return rc;
+        for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
+        note_stage_bytes(ctx, "fwd", plan.ids[i], bytes_in, bytes_out);
+        for (uint32_t b = 0; b < nblocks; b++) {
+            if (applied[b]) flags[b] &= (uint8_t)~(1u << (7 - i));
+            else if (len[b]) CK(cudaMemcpyAsync(outb + b * gstride, cur + b * cur_stride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+        cur = outb;
+        cur_stride = gstride;
+    }
+    for (uint32_t b = 0; b < nblocks; b++) {
+        EncJob& j = jobs[b];
+        j.data_off = b * gstride;
+        j.post_len = len[b];
+        if (!j.copy) j.skip_flags = flags[b];
+    }
+    *d_data = cur;
+    return 0;
+}
+
+// Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186) of every block of a batch. The entropy
+// stage left block b's pre_len bytes at d_pre + b*pstride, a scratch buffer of this context with room for pstride - 64 bytes per
+// block; the stages alternate between it and ctx->d_tmp2. Decoded blocks go to d_dst back to back (slot = 0) or at b * slot.
+// *total = bytes produced.
+int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, uint8_t* d_dst, size_t cap,
+                  std::vector<uint32_t>& out_len, uint64_t* total, uint64_t slot) {
     const uint32_t nblocks = (uint32_t)jobs.size();
+    out_len.assign(nblocks, 0);
+    *total = 0;
+    if (nblocks == 0) return 0;
+    const uint32_t blk_cap = (uint32_t)std::min<uint64_t>(pstride - 64, 0xFFFFFFF0u);
     std::vector<uint32_t> len(nblocks);
     for (uint32_t b = 0; b < nblocks; b++) len[b] = jobs[b].pre_len;
     CK(ctx->d_tmp2.ensure(pstride * nblocks + 64));
@@ -1760,7 +1502,7 @@ int inverse_generic(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>&
     }
     uint64_t off = 0;
     for (uint32_t b = 0; b < nblocks; b++) {
-        const uint64_t at = compact ? off : (uint64_t)b * slot;
+        const uint64_t at = slot ? (uint64_t)b * slot : off;
         if (at + len[b] > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
         if (len[b]) CK(cudaMemcpyAsync(d_dst + at, cur + b * pstride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
         out_len[b] = len[b];
@@ -1768,251 +1510,6 @@ int inverse_generic(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>&
     }
     *total = off;
     CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
-}
-
-// Forward transform stage (ByteTransformSequence.Forward, transform/Sequence.go:64-125) of every block of a batch.
-// Block b is d_src[b*stride : +len_b]. On return *d_data is the base of the post-transform data and jobs[] describes
-// every block for the entropy stage. NONE leaves the data in place; BWT writes header+BWT into ctx->d_tmp.
-int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, size_t n, uint32_t block_size, uint64_t stride, const uint32_t* lens,
-                  uint32_t nblocks, const uint8_t** d_data, std::vector<EncJob>& jobs, const std::vector<int32_t>* init_dt = nullptr, bool allow_copy = true) {
-    jobs.resize(nblocks);
-    std::vector<uint32_t> blen(nblocks);
-    uint32_t max_len = 0;
-    for (uint32_t b = 0; b < nblocks; b++) {
-        blen[b] = lens ? lens[b] : (uint32_t)std::min<uint64_t>(block_size, n - (uint64_t)b * block_size);
-        max_len = std::max(max_len, blen[b]);
-    }
-    *d_data = d_src;
-    for (uint32_t b = 0; b < nblocks; b++) {
-        EncJob& j = jobs[b];
-        j.data_off = (uint64_t)b * stride;
-        j.post_len = blen[b];
-        j.ntransforms = (uint32_t)plan.nt;
-        j.skip_flags = 0x7F;  // NullTransform succeeds: bit 7 cleared (Sequence.go:65,107)
-        j.copy = allow_copy && blen[b] <= SMALL_BLOCK;  // io/CompressedStream.go:773-776: transform and entropy forced to NONE
-        j.checksum = 0;
-    }
-    if (plan.none() || nblocks == 0) return 0;
-    // ctx["dataType"] of every block: the caller's value (from the block's magic number, encodingTask.encode :808-816), updated by the stages
-    std::vector<int32_t> dts(nblocks, 0);
-    if (init_dt) dts = *init_dt;
-    if (plan.generic()) return forward_generic(ctx, plan, d_src, stride, blen, d_data, jobs, dts);
-    if (plan.lz()) {
-        // ---- LZ / LZX (LZXCodec.Forward): one serial parse per block, all blocks of the batch in parallel
-        const bool extra = plan.lzx();
-        const uint64_t tstride = ((uint64_t)max_len + max_len / 64 + 64 + 64 + 15) & ~15ull;
-        const uint64_t sstride = (lz_scratch_bytes(max_len) + 255) & ~size_t(255);
-        const size_t hbytes = ((size_t)nblocks << (extra ? 19 : 16)) * 4;
-        CK(ctx->d_tmp.ensure(tstride * nblocks + 64));
-        std::vector<LzBlock> lb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            lb[b].src_off = (uint64_t)b * stride;
-            lb[b].dst_off = (uint64_t)b * tstride;
-            lb[b].scratch_off = (uint64_t)b * sstride;
-            lb[b].len = jobs[b].copy ? 0 : blen[b];  // COPY blocks: transform forced to NONE
-            lb[b].cap = 0;
-            lb[b].data_type = dts[b];
-            lb[b].pad = 0;
-        }
-        std::vector<LzResult> hres;
-        {
-            int rc = lz_forward_batch(ctx, d_src, ctx->d_tmp.as<uint8_t>(), lb, extra, hres);
-            if (rc) return rc;
-        }
-        for (uint32_t b = 0; b < nblocks; b++) {
-            EncJob& j = jobs[b];
-            j.data_off = (uint64_t)b * tstride;
-            if (!j.copy && hres[b].status == 0) {
-                j.post_len = hres[b].out_len;
-                j.skip_flags = 0x7F;
-            } else {
-                if (!j.copy) j.skip_flags = 0xFF;
-                if (blen[b]) CK(cudaMemcpyAsync(ctx->d_tmp.as<uint8_t>() + j.data_off, d_src + (uint64_t)b * stride, blen[b], cudaMemcpyDeviceToDevice, ctx->stream));
-            }
-        }
-        *d_data = ctx->d_tmp.as<uint8_t>();
-        return 0;
-    }
-    // ---- BWT (BWTBlockCodec.Forward): the blocks of the batch are suffix-sorted together (kz_bwt.cu: bwt_forward_batch)
-    const uint64_t tstride = ((uint64_t)max_len + 33 + 64 + 15) & ~15ull;
-    CK(ctx->d_tmp.ensure(tstride * nblocks + 64));
-    CK(ctx->d_lens.ensure((size_t)nblocks * 4 + 64));
-    uint8_t* tmp = ctx->d_tmp.as<uint8_t>();
-    uint32_t* d_post = ctx->d_lens.as<uint32_t>();
-    std::vector<uint8_t> ok(nblocks, 0);
-    for (uint32_t b0 = 0; b0 < nblocks;) {
-        std::vector<uint64_t> so, dof;
-        std::vector<uint32_t> nn, num;
-        uint64_t total = 0;
-        uint32_t b = b0;
-        for (; b < nblocks; b++) {
-            const uint8_t* src = d_src + (uint64_t)b * stride;
-            uint8_t* dst = tmp + (uint64_t)b * tstride;
-            if (jobs[b].copy || blen[b] < 2) {
-                if (blen[b]) CK(cudaMemcpyAsync(dst, src, blen[b], cudaMemcpyDeviceToDevice, ctx->stream));  // transform skipped: data unchanged
-                continue;
-            }
-            if (blen[b] > bwt_forward_batch_max_total()) {  // 1 GiB block: its own suffix sort
-                if (!nn.empty()) break;
-                CK(ctx->d_ws.ensure(bwt_forward_workspace(blen[b])));
-                LaunchScope ls(ctx, "bwt_forward");
-                cudaError_t e = bwt_forward_device(src, blen[b], dst, d_post + b, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
-                if (e == cudaSuccess) ok[b] = 1;
-                else if (e != cudaErrorInvalidValue) return ctx->cuda_fail(e, "bwt_forward");
-                else CK(cudaMemcpyAsync(dst, src, blen[b], cudaMemcpyDeviceToDevice, ctx->stream));
-                continue;
-            }
-            if (!nn.empty() && (total + blen[b] > bwt_forward_batch_max_total() || nn.size() >= bwt_forward_batch_max_blocks())) break;
-            so.push_back((uint64_t)b * stride), dof.push_back((uint64_t)b * tstride), nn.push_back(blen[b]), num.push_back(b);
-            total += blen[b];
-        }
-        b0 = b;
-        if (nn.empty()) continue;
-        CK(ctx->d_ws.ensure(bwt_forward_batch_workspace(total, (uint32_t)nn.size())));
-        LaunchScope ls(ctx, "bwt_forward");
-        cudaError_t e = bwt_forward_batch(d_src, tmp, so.data(), dof.data(), nn.data(), num.data(), (uint32_t)nn.size(), d_post, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap,
-                                          ctx->stream, &ctx->launches);
-        if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_forward");
-        for (uint32_t k : num) ok[k] = 1;
-    }
-    std::vector<uint32_t> post(nblocks);
-    CK(cudaMemcpyAsync(post.data(), d_post, (size_t)nblocks * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    for (uint32_t b = 0; b < nblocks; b++) {
-        EncJob& j = jobs[b];
-        j.data_off = (uint64_t)b * tstride;
-        if (ok[b]) {
-            j.post_len = post[b];
-            j.skip_flags = 0x7F;
-        } else if (!j.copy) {
-            j.skip_flags = 0xFF;  // the only transform failed -> all skip bits stay set (Sequence.go:100-105)
-        }
-    }
-    *d_data = tmp;
-    return 0;
-}
-
-// Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186). The entropy stage left block
-// b's pre_len bytes at d_pre + b*pstride; the decoded blocks are written back to back at d_dst. *total = bytes produced.
-// lz_slot / compact only matter for LZ: block b is decoded at d_dst + b * lz_slot; compact = the slots must tile the
-// output exactly (whole stream), otherwise the caller collects the slots itself (block batch).
-int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, const uint8_t* d_pre, uint64_t pstride, uint8_t* d_dst, size_t cap,
-                  std::vector<uint32_t>& out_len, uint64_t* total, uint64_t lz_slot = 0, bool compact = true) {
-    const uint32_t nblocks = (uint32_t)jobs.size();
-    out_len.assign(nblocks, 0);
-    *total = 0;
-    if (nblocks == 0) return 0;
-    if (plan.generic())
-        return inverse_generic(ctx, plan, jobs, const_cast<uint8_t*>(d_pre), pstride, (uint32_t)std::min<uint64_t>(pstride - 64, 0xFFFFFFF0u), d_dst, cap, out_len,
-                               total, lz_slot, compact);
-    if (plan.lz()) {
-        // every block decodes into its own slot (valid streams: all blocks but the last are block_size long)
-        uint32_t max_pre = 0;
-        for (auto& j : jobs) max_pre = std::max(max_pre, j.pre_len);
-        const uint64_t slot = lz_slot;
-        std::vector<LzBlock> lb(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            const bool skip = jobs[b].copy || (jobs[b].skip_flags & 0x80);
-            lb[b].src_off = (uint64_t)b * pstride;
-            lb[b].dst_off = (uint64_t)b * slot;
-            lb[b].scratch_off = 0;
-            lb[b].len = skip ? 0 : jobs[b].pre_len;
-            const uint64_t room = (uint64_t)b * slot < cap ? cap - (uint64_t)b * slot : 0;
-            lb[b].cap = (uint32_t)std::min<uint64_t>(room, slot);
-            lb[b].data_type = 0;
-            lb[b].pad = 0;
-        }
-        std::vector<uint32_t> hl(nblocks);
-        std::vector<int32_t> hs(nblocks);
-        {  // the stream's only stage is LZ / LZX (kanzi -l 1): the same data-parallel inverse as inside a sequence
-            CtxLzWorkspace W(ctx);
-            CtxLzHook H(ctx);
-            cudaError_t e = lz_inverse_parallel(d_pre, d_dst, lb, W, ctx->stream, hl, hs, &H, &ctx->launches);
-            if (e != cudaSuccess) return ctx->cuda_fail(e, "lz_inverse");
-        }
-        uint64_t off = 0;
-        for (uint32_t b = 0; b < nblocks; b++) {
-            const bool skip = jobs[b].copy || (jobs[b].skip_flags & 0x80);
-            if (skip) {
-                if ((uint64_t)b * slot + jobs[b].pre_len > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-                CK(cudaMemcpyAsync(d_dst + (uint64_t)b * slot, d_pre + (uint64_t)b * pstride, jobs[b].pre_len, cudaMemcpyDeviceToDevice, ctx->stream));
-                out_len[b] = jobs[b].pre_len;
-            } else {
-                if (hs[b]) {
-                    jobs[b].status = hs[b];
-                    return ctx->fail(KZ_ERR_PROCESS_BLOCK, "LZCodec inverse transform failed");
-                }
-                out_len[b] = hl[b];
-            }
-            if (b + 1 < nblocks && out_len[b] != slot && compact) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "unexpected decoded block length");
-            off += out_len[b];
-        }
-        *total = compact ? off : 0;
-        return 0;
-    }
-    // block headers of the BWT codec (<= 33 bytes) are needed on the host
-    std::vector<uint8_t> heads((size_t)nblocks * 64, 0);
-    CK(cudaMemcpy2DAsync(heads.data(), 64, d_pre, pstride, 33, nblocks, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    // output offsets follow from the block headers (decoded length = stream length - header), so all blocks can be inverted together
-    uint64_t off = 0;
-    std::vector<uint64_t> so, dof;
-    std::vector<uint32_t> ll, num;
-    std::vector<uint8_t> hh;
-    uint64_t batch_total = 0;
-    auto flush = [&]() -> int {
-        if (ll.empty()) return 0;
-        CK(ctx->d_ws.ensure(bwt_inverse_batch_workspace(batch_total, (uint32_t)ll.size())));
-        std::vector<uint32_t> produced(ll.size(), 0);
-        LaunchScope ls(ctx, "bwt_inverse");
-        cudaError_t e = bwt_inverse_batch(d_pre, d_dst, so.data(), dof.data(), ll.data(), hh.data(), (uint32_t)ll.size(), 0xFFFFFFFFu, produced.data(),
-                                          ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
-        if (e == cudaErrorInvalidValue) {
-            for (uint32_t k : num) jobs[k].status = -KZ_ERR_PROCESS_BLOCK;
-            return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header or data");
-        }
-        if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
-        so.clear(), dof.clear(), ll.clear(), num.clear(), hh.clear();
-        batch_total = 0;
-        return 0;
-    };
-    for (uint32_t b = 0; b < nblocks; b++) {
-        DecJob& j = jobs[b];
-        const uint8_t* src = d_pre + (uint64_t)b * pstride;
-        const bool skip = j.copy || (j.skip_flags & 0x80) || !plan.bwt();
-        if (skip) {
-            if (off + j.pre_len > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-            CK(cudaMemcpyAsync(d_dst + off, src, j.pre_len, cudaMemcpyDeviceToDevice, ctx->stream));
-            out_len[b] = j.pre_len;
-        } else {
-            const uint8_t* h = &heads[(size_t)b * 64];
-            const uint32_t header = (1u << ((h[0] >> 2) & 7)) * ((uint32_t)(h[0] & 3) + 1) + 1;
-            if (j.pre_len < 2 || j.pre_len < header) {
-                j.status = -KZ_ERR_PROCESS_BLOCK;
-                return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header");
-            }
-            const uint32_t produced = j.pre_len - header;
-            if (off + produced > cap) {
-                j.status = -KZ_ERR_PROCESS_BLOCK;
-                return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header");
-            }
-            if (!ll.empty() && (batch_total + j.pre_len > bwt_inverse_batch_max_total() || ll.size() >= bwt_inverse_batch_max_blocks())) {
-                int rc = flush();
-                if (rc) return rc;
-            }
-            so.push_back((uint64_t)b * pstride), dof.push_back(off), ll.push_back(j.pre_len), num.push_back(b);
-            hh.insert(hh.end(), h, h + 64);
-            batch_total += j.pre_len;
-            out_len[b] = produced;
-        }
-        off += out_len[b];
-    }
-    {
-        int rc = flush();
-        if (rc) return rc;
-    }
-    *total = off;
     return 0;
 }
 
@@ -2429,9 +1926,8 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
         if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid compressed block header");
         max_pre = std::max(max_pre, jobs[b].pre_len);
     }
-    uint64_t blk_room = max_pre;
-    if (plan.generic())  // Reader.processBlock :1649-1653: the task buffers hold blockSize + max(512, blockSize >> 4) bytes
-        blk_room = std::max<uint64_t>(blk_room, (uint64_t)sh.block_size + std::max<uint64_t>(512, sh.block_size >> 4));
+    // Reader.processBlock :1649-1653: the task buffers hold blockSize + max(512, blockSize >> 4) bytes
+    const uint64_t blk_room = std::max<uint64_t>(max_pre, (uint64_t)sh.block_size + std::max<uint64_t>(512, sh.block_size >> 4));
     const uint64_t pstride = (blk_room + 64 + 15) & ~15ull;
     CK(ctx->d_tmp.ensure(pstride * nblocks + 64));
     for (uint32_t b = 0; b < nblocks; b++) jobs[b].out_off = (uint64_t)b * pstride;
@@ -2440,7 +1936,7 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     for (uint32_t b = 0; b < nblocks; b++)
         if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid bitstream: block decoding failed");
     std::vector<uint32_t> olen;
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, (uint8_t*)d_dst, cap, olen, &out_off, sh.block_size, true);
+    rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, (uint8_t*)d_dst, cap, olen, &out_off, 0);
     if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     if (sh.checksum_bits) {  // decoded blocks lie back to back (every block but the last is block_size long)
@@ -2608,30 +2104,23 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
         if (worst) return ctx->fail(-worst, "block decoding failed");
         return 0;
     }
-    // inverse transforms into a packed scratch area, then out
+    // inverse transforms into a scratch area (block b at b * ostride), then out
     CK(ctx->d_tmp.ensure(ostride * nblocks + 64));
     std::vector<uint32_t> olen;
     uint64_t total = 0;
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride, ctx->d_tmp.as<uint8_t>(), ostride * nblocks, olen, &total, ostride, false);
+    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride, ctx->d_tmp.as<uint8_t>(), ostride * nblocks, olen, &total, ostride);
     if (rc) return rc;
     if (checksum_bits) {
         std::vector<uint64_t> hoff(nblocks);
-        uint64_t o = 0;
-        for (uint32_t b = 0; b < nblocks; b++) {
-            hoff[b] = (plan.lz() || plan.generic()) ? (uint64_t)b * ostride : o;
-            o += olen[b];
-        }
+        for (uint32_t b = 0; b < nblocks; b++) hoff[b] = (uint64_t)b * ostride;
         int vrc = verify_checksums(ctx, ctx->d_tmp.as<uint8_t>(), hoff, olen, checksum_bits, jobs);
         if (vrc) return vrc;
     }
-    uint64_t off = 0;
     for (uint32_t b = 0; b < nblocks; b++) {
         if (status) status[b] = 0;
         out_len[b] = olen[b];
         if (olen[b] > out_stride) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-        const uint64_t from = (plan.lz() || plan.generic()) ? (uint64_t)b * ostride : off;
-        CK(cudaMemcpyAsync(out + b * out_stride, ctx->d_tmp.as<uint8_t>() + from, olen[b], cudaMemcpyDeviceToHost, ctx->stream));
-        off += olen[b];
+        CK(cudaMemcpyAsync(out + b * out_stride, ctx->d_tmp.as<uint8_t>() + (uint64_t)b * ostride, olen[b], cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
@@ -2694,144 +2183,67 @@ int kz_entropy_decode(kz_ctx* ctx, uint32_t type, const uint8_t* src, size_t src
     return 0;
 }
 
+// One transform on one block: the argument checks of each reference codec, then the stage a sequence of that one transform runs
 int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     ctx->stream_bs = ctx->user_stream_bs;
     *out_n = 0;
-    if (type == KZ_T_LZ || type == KZ_T_LZX) {  // LZXCodec.Forward (reads ctx["dataType"], never writes it)
-        if (n == 0) return 0;
-        if (n > (1u << 30)) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
-        if (cap < kz_transform_max_encoded_len(type, n)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Output buffer is too small");
-        TransformPlan plan;
-        plan.nt = 1;
-        plan.ids[0] = type;
-        CK(ctx->d_in.ensure(n + 64));
-        CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-        const uint32_t len = (uint32_t)n;
-        const uint8_t* d_data = nullptr;
-        std::vector<EncJob> jobs;
-        const std::vector<int32_t> dt1(1, data_type ? *data_type : 0);
-        int rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), n, 0, 0, &len, 1, &d_data, jobs, &dt1, false);
-        if (rc) return rc;
-        if (jobs[0].skip_flags & 0x80) return 1;
-        CK(cudaMemcpyAsync(dst, d_data, jobs[0].post_len, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *out_n = jobs[0].post_len;
-        return 0;
-    }
-    if (type == KZ_T_RANK || type == KZ_T_MTFT || type == KZ_T_ZRLT || type == KZ_T_BWTS || type == KZ_T_ROLZ || type == KZ_T_PACK || type == KZ_T_DNA || type == KZ_T_MM || type == KZ_T_TEXT || type == KZ_T_UTF || type == KZ_T_EXE) {  // SBRT / ZRLT / BWTS / ROLZ / Alias / FSD / Text / UTF / EXE Forward
-        if (n == 0) return 0;
-        if (n > (1u << 30)) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
-        if (cap < kz_transform_max_encoded_len(type, n)) return 1;  // Forward returns an error: the sequence skips the transform
-        const uint64_t stride = ((uint64_t)n + n / 8 + 8192 + 1024 + 64 + 64 + 15) & ~15ull;
-        CK(ctx->d_in.ensure(stride));
-        CK(ctx->d_out.ensure(stride));
-        CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-        std::vector<uint32_t> len(1, (uint32_t)n);
-        std::vector<uint8_t> active(1, 1), applied;
-        std::vector<int32_t> dt1(1, data_type ? *data_type : 0);
-        int rc = apply_forward(ctx, type, ctx->d_in.as<uint8_t>(), stride, ctx->d_out.as<uint8_t>(), stride, len, active, applied, &dt1);
-        if (rc) return rc;
-        if (data_type) *data_type = dt1[0];
-        if (!applied[0]) return 1;
-        CK(cudaMemcpyAsync(dst, ctx->d_out.p, len[0], cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *out_n = len[0];
-        return 0;
-    }
-    if (type != KZ_T_BWT) return ctx->fail(KZ_ERR_CREATE_CODEC, "transform not available on the GPU path (BWT, LZ, LZX, RANK, MTFT, ZRLT are)");
+    if (!TransformPlan::seq_id(type)) return ctx->fail(KZ_ERR_CREATE_CODEC, NO_GPU_TRANSFORM);
     if (n == 0) return 0;
-    if (n > (1u << 30)) return ctx->fail(KZ_ERR_BLOCK_SIZE, "The max BWT block size is 1 GiB");
-    if (cap < n + 33) return ctx->fail(KZ_ERR_INVALID_PARAM, "Output buffer is too small");
-    if (n < 2) return 1;  // BWTBlockCodec.Forward: invalid index size -> the sequence skips the transform
-    CK(ctx->d_in.ensure(n + 64));
-    CK(ctx->d_out.ensure(n + 128));
-    CK(ctx->d_ws.ensure(bwt_forward_workspace((uint32_t)n)));
-    CK(ctx->d_lens.ensure(64));
-    CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-    cudaError_t e;
-    {
-        LaunchScope ls(ctx, "bwt_forward");
-        e = bwt_forward_device(ctx->d_in.as<uint8_t>(), (uint32_t)n, ctx->d_out.as<uint8_t>(), ctx->d_lens.as<uint32_t>(), ctx->d_ws.as<uint8_t>(),
-                               ctx->d_ws.cap, ctx->stream, &ctx->launches);
+    if (n > (1u << 30)) return ctx->fail(KZ_ERR_BLOCK_SIZE, type == KZ_T_BWT ? "The max BWT block size is 1 GiB" : "block too large");
+    if (cap < kz_transform_max_encoded_len(type, n)) {
+        // BWTBlockCodec and LZXCodec refuse the call; every other Forward returns an error, and the sequence skips the transform
+        if (type == KZ_T_BWT || type == KZ_T_LZ || type == KZ_T_LZX) return ctx->fail(KZ_ERR_INVALID_PARAM, "Output buffer is too small");
+        return 1;
     }
-    if (e == cudaErrorInvalidValue) return 1;
-    if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_forward");
-    uint32_t produced = 0;
-    CK(cudaMemcpyAsync(&produced, ctx->d_lens.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if (type == KZ_T_BWT && n < 2) return 1;  // BWTBlockCodec.Forward: invalid index size -> the sequence skips the transform
+    const uint64_t stride = ((uint64_t)n + n / 8 + 8192 + 1024 + 64 + 64 + 15) & ~15ull;
+    CK(ctx->d_in.ensure(stride));
+    CK(ctx->d_out.ensure(stride));
+    CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<uint32_t> len(1, (uint32_t)n);
+    std::vector<uint8_t> active(1, 1), applied;
+    std::vector<int32_t> dt1(1, data_type ? *data_type : 0);  // ctx["dataType"]; BWT / BWTS / LZ / LZX / RANK / MTFT / ZRLT leave it as it is
+    int rc = apply_forward(ctx, type, ctx->d_in.as<uint8_t>(), stride, ctx->d_out.as<uint8_t>(), stride, len, active, applied, &dt1);
+    if (rc) return rc;
+    if (data_type) *data_type = dt1[0];
+    if (!applied[0]) return 1;
+    CK(cudaMemcpyAsync(dst, ctx->d_out.p, len[0], cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaMemcpyAsync(dst, ctx->d_out.p, produced, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    *out_n = produced;
+    *out_n = len[0];
     return 0;
 }
 
+// cap = len(dst) of the reference call
 int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     ctx->stream_bs = ctx->user_stream_bs;
     *out_n = 0;
-    if (type == KZ_T_LZ || type == KZ_T_LZX) {  // LZXCodec.inverseV6; cap = len(dst) of the reference call
-        if (n == 0) return 0;
-        if (n > (1u << 30) || cap > (1u << 30) + 64) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
-        TransformPlan plan;
-        plan.nt = 1;
-        plan.ids[0] = type;
-        CK(ctx->d_in.ensure(n + 64));
-        CK(ctx->d_out.ensure(cap + 64));
-        CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-        std::vector<DecJob> jobs(1);
-        jobs[0] = DecJob();
-        jobs[0].pre_len = (uint32_t)n;
-        std::vector<uint32_t> olen;
-        uint64_t total = 0;
-        int rc = inverse_stage(ctx, plan, jobs, ctx->d_in.as<uint8_t>(), n, ctx->d_out.as<uint8_t>(), cap, olen, &total, cap, false);
-        if (rc) return rc;
-        if (olen[0]) CK(cudaMemcpyAsync(dst, ctx->d_out.p, olen[0], cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *out_n = olen[0];
-        return 0;
-    }
-    if (type == KZ_T_RANK || type == KZ_T_MTFT || type == KZ_T_ZRLT || type == KZ_T_BWTS || type == KZ_T_ROLZ || type == KZ_T_PACK || type == KZ_T_DNA || type == KZ_T_MM || type == KZ_T_TEXT || type == KZ_T_UTF || type == KZ_T_EXE) {  // SBRT / ZRLT / BWTS / ROLZ / Alias / FSD / Text / UTF / EXE Inverse; cap = len(dst)
-        if (n == 0 || cap == 0) return 0;
-        if (n > (1u << 30) || cap > (1u << 30) + 4096) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
-        const uint64_t stride = ((uint64_t)std::max(n, cap) + 64 + 15) & ~15ull;
-        CK(ctx->d_in.ensure(stride));
-        CK(ctx->d_out.ensure(stride));
-        CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-        std::vector<uint32_t> len(1, (uint32_t)n);
-        std::vector<uint8_t> active(1, 1);
-        int rc = apply_inverse(ctx, type, ctx->d_in.as<uint8_t>(), ctx->d_out.as<uint8_t>(), stride, (uint32_t)cap, len, active);
-        if (rc) return rc;
-        if (len[0]) CK(cudaMemcpyAsync(dst, ctx->d_out.p, len[0], cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *out_n = len[0];
-        return 0;
-    }
-    if (type != KZ_T_BWT) return ctx->fail(KZ_ERR_CREATE_CODEC, "transform not available on the GPU path (BWT, LZ, LZX, RANK, MTFT, ZRLT are)");
+    if (!TransformPlan::seq_id(type)) return ctx->fail(KZ_ERR_CREATE_CODEC, NO_GPU_TRANSFORM);
     if (n == 0) return 0;
-    if (n == 1) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid size");
-    if (n > (1u << 30) + 33) return ctx->fail(KZ_ERR_BLOCK_SIZE, "The max BWT block size is 1 GiB");
-    CK(ctx->d_in.ensure(n + 64));
-    CK(ctx->d_out.ensure(n + 64));
-    CK(ctx->d_ws.ensure(bwt_inverse_workspace((uint32_t)n)));
-    CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
-    uint8_t head[64];
-    memset(head, 0, sizeof(head));
-    memcpy(head, src, std::min<size_t>(n, 33));
-    uint32_t produced = 0;
-    cudaError_t e;
-    {
-        LaunchScope ls(ctx, "bwt_inverse");
-        e = bwt_inverse_device(ctx->d_in.as<uint8_t>(), head, (uint32_t)n, ctx->d_out.as<uint8_t>(), (uint32_t)std::min<size_t>(cap, 0xFFFFFFFFu), &produced,
-                               ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
+    if (type == KZ_T_BWT) {
+        if (n == 1) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid size");
+        if (n > (1u << 30) + 33) return ctx->fail(KZ_ERR_BLOCK_SIZE, "The max BWT block size is 1 GiB");
+        cap = std::min(cap, n);  // the block is shorter than its header + BWT bytes: more room changes nothing
+    } else if (type == KZ_T_LZ || type == KZ_T_LZX) {  // LZXCodec.inverseV6
+        if (n > (1u << 30) || cap > (1u << 30) + 64) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
+    } else {
+        if (cap == 0) return 0;
+        if (n > (1u << 30) || cap > (1u << 30) + 4096) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
     }
-    if (e == cudaErrorInvalidValue) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header");
-    if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
-    if (produced) CK(cudaMemcpyAsync(dst, ctx->d_out.p, produced, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint64_t stride = ((uint64_t)std::max(n, cap) + 64 + 15) & ~15ull;
+    CK(ctx->d_in.ensure(stride));
+    CK(ctx->d_out.ensure(stride));
+    CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<uint32_t> len(1, (uint32_t)n);
+    std::vector<uint8_t> active(1, 1);
+    int rc = apply_inverse(ctx, type, ctx->d_in.as<uint8_t>(), ctx->d_out.as<uint8_t>(), stride, (uint32_t)cap, len, active);
+    if (rc) return rc;
+    if (len[0]) CK(cudaMemcpyAsync(dst, ctx->d_out.p, len[0], cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    *out_n = produced;
+    *out_n = len[0];
     return 0;
 }
 

@@ -190,67 +190,7 @@ __global__ void bwt_header_kernel(const uint32_t* __restrict__ primary, uint32_t
 }
 
 // ---------------- inverse ----------------
-// key = BWT byte, value = index of the next suffix' rank for the suffix that starts with this byte (BWT.go:246-258):
-// position 0 -> END, positions 1..pidx-1 -> i-1, positions >= pidx -> i
-__global__ void ibwt_init_kernel(const uint8_t* __restrict__ src, uint32_t n, uint32_t pidx, uint8_t* __restrict__ keys, uint32_t* __restrict__ vals) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    keys[i] = src[i];
-    vals[i] = i == 0 ? 0xFFFFFFFFu : (i < pidx ? i - 1 : i);
-}
-
 static const uint32_t IBWT_STRIDE = 64;  // a sub-list starts at every rank that is a multiple of this (1024 left < 1 warp per SM for a 4 MiB block)
-
-KZ_D bool ibwt_is_head(uint32_t t, const uint32_t* prim, uint32_t nprim) {
-    if ((t & (IBWT_STRIDE - 1)) == 0) return true;
-    for (uint32_t k = 0; k < nprim; k++)
-        if (t == prim[k]) return true;
-    return false;
-}
-
-// head id of rank t: multiples of the stride first, then the primary ranks
-KZ_D uint32_t ibwt_head_id(uint32_t t, uint32_t nstride, const uint32_t* prim, uint32_t nprim) {
-    if ((t & (IBWT_STRIDE - 1)) == 0) return t / IBWT_STRIDE;
-    for (uint32_t k = 0; k < nprim; k++)
-        if (t == prim[k]) return nstride + k;
-    return 0xFFFFFFFFu;
-}
-
-// walk 1: one thread per sub-list head: length of the sub-list and id of the next head (END = 0xFFFFFFFF)
-__global__ void ibwt_measure_kernel(const uint32_t* __restrict__ next, uint32_t n, const uint32_t* __restrict__ prim_rank, uint32_t nprim,
-                                    uint32_t nstride, uint32_t* __restrict__ succ, uint32_t* __restrict__ len) {
-    // the primary ranks are staged by the first 8 threads of EVERY CTA before any thread leaves: the last CTA holds the primary heads and
-    // may have fewer than 8 live threads (a block whose head count is 1..7 modulo the CTA size used to read stale shared memory here)
-    __shared__ uint32_t s_prim[8];
-    if (threadIdx.x < 8) s_prim[threadIdx.x] = threadIdx.x < nprim ? prim_rank[threadIdx.x] : 0xFFFFFFFFu;
-    __syncthreads();
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nstride + nprim) return;
-    uint32_t t = j < nstride ? j * IBWT_STRIDE : s_prim[j - nstride];
-    if (t >= n || (j >= nstride && (t & (IBWT_STRIDE - 1)) == 0)) {  // duplicate head (primary rank on a stride multiple) or out of range
-        succ[j] = 0xFFFFFFFEu;                                        // marks "unused"
-        len[j] = 0;
-        return;
-    }
-    uint32_t l = 0;
-    for (;;) {
-        t = next[t];
-        l++;
-        if (t == 0xFFFFFFFFu) {
-            succ[j] = 0xFFFFFFFFu;
-            break;
-        }
-        if (t >= n || l > n) {  // corrupt permutation
-            succ[j] = 0xFFFFFFFDu;
-            break;
-        }
-        if (ibwt_is_head(t, s_prim, nprim)) {
-            succ[j] = ibwt_head_id(t, nstride, s_prim, nprim);
-            break;
-        }
-    }
-    len[j] = l;
-}
 
 // Wyllie pointer doubling over the heads: after the rounds dist[j] = number of bytes from head j to the end of the list
 __global__ void ibwt_jump_kernel(const uint32_t* __restrict__ succ_in, const uint64_t* __restrict__ dist_in, uint32_t nheads, uint32_t* __restrict__ succ_out,
@@ -266,33 +206,6 @@ __global__ void ibwt_jump_kernel(const uint32_t* __restrict__ succ_in, const uin
     }
     succ_out[j] = s2;
     dist_out[j] = d;
-}
-
-// walk 2: writes the first byte of every visited rank at its final position
-__global__ void ibwt_write_kernel(const uint32_t* __restrict__ next, const uint8_t* __restrict__ first, uint32_t n, const uint32_t* __restrict__ prim_rank,
-                                  uint32_t nprim, uint32_t nstride, const uint32_t* __restrict__ succ0, const uint32_t* __restrict__ len,
-                                  const uint64_t* __restrict__ dist, uint64_t total, uint8_t* __restrict__ dst, int32_t* __restrict__ status) {
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nstride + nprim) return;
-    if (succ0[j] == 0xFFFFFFFEu) return;
-    uint32_t t = j < nstride ? j * IBWT_STRIDE : prim_rank[j - nstride];
-    const uint64_t d = dist[j];
-    if (d > total) {  // head not on the main list (corrupt input)
-        return;
-    }
-    uint64_t off = total - d;
-    const uint32_t l = len[j];
-    for (uint32_t i = 0; i < l; i++) {
-        if (off + i < n) dst[off + i] = first[t];
-        t = next[t];
-        if (t >= n) break;
-    }
-    (void)status;
-}
-
-__global__ void ibwt_first_kernel(const uint8_t* __restrict__ sorted_keys, uint32_t n, uint8_t* __restrict__ first) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) first[i] = sorted_keys[i];
 }
 
 }  // namespace
@@ -680,100 +593,11 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
     return cudaGetLastError();
 }
 
-size_t bwt_inverse_workspace(uint32_t n) {
-    size_t temp = 0;
-    cub::DoubleBuffer<uint8_t> k(nullptr, nullptr);
-    cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
-    cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int)n, 0, 8);
-    const size_t nheads = (size_t)n / IBWT_STRIDE + 16;
-    return (size_t)n * (1 * 2 + 4 * 2 + 1) + nheads * (4 * 3 + 8 * 2) + 4096 + temp + 4096;
-}
-
-// d_src: header + BWT bytes (len bytes); d_dst: receives the original block. Returns cudaErrorInvalidValue for malformed headers.
-cudaError_t bwt_inverse_device(const uint8_t* d_src, const uint8_t* h_header /*first 33 bytes on the host*/, uint32_t len, uint8_t* d_dst, uint32_t cap,
-                               uint32_t* out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches) {
-    if (len < 2) return cudaErrorInvalidValue;
-    const uint8_t mode = h_header[0];
-    const uint32_t log_chunks = (mode >> 2) & 7;
-    const int pidx_size = (int)(mode & 3) + 1;
-    const uint32_t chunks = 1u << log_chunks;
-    const uint32_t header = chunks * pidx_size + 1;
-    if (len < header || chunks > 8) return cudaErrorInvalidValue;
-    const uint32_t n = len - header;
-    if (chunks != (n < 256 ? 1u : 8u)) return cudaErrorInvalidValue;
-    *out_len = n;
-    if (n == 0) return cudaSuccess;
-    if (n > cap) return cudaErrorInvalidValue;
-    uint32_t prim[8];
-    for (uint32_t i = 0, idx = 1; i < chunks; i++) {
-        uint32_t p = 0;
-        for (int k = 0; k < pidx_size; k++) p = (p << 8) | h_header[idx++];
-        prim[i] = p + 1;
-        if (prim[i] == 0 || prim[i] > n) return cudaErrorInvalidValue;
-    }
-    const uint8_t* bw = d_src + header;
-    if (n == 1) return cudaMemcpyAsync(d_dst, bw, 1, cudaMemcpyDeviceToDevice, stream);
-    auto align = [](size_t x) { return (x + 255) & ~size_t(255); };
-    size_t off = 0;
-    uint8_t* keys_a = ws + off; off = align(off + n);
-    uint8_t* keys_b = ws + off; off = align(off + n);
-    uint32_t* val_a = (uint32_t*)(ws + off); off = align(off + (size_t)n * 4);
-    uint32_t* val_b = (uint32_t*)(ws + off); off = align(off + (size_t)n * 4);
-    const uint32_t nstride = (n + IBWT_STRIDE - 1) / IBWT_STRIDE;
-    const uint32_t nprim = chunks;
-    const uint32_t nheads = nstride + nprim;
-    uint32_t* succ_a = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* succ_b = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* succ0 = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* lenv = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint64_t* dist_a = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
-    uint64_t* dist_b = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
-    uint32_t* d_prim = (uint32_t*)(ws + off); off = align(off + 64);
-    void* temp = ws + off;
-    size_t temp_bytes = ws_bytes > off ? ws_bytes - off : 0;
-    uint32_t prim_rank[8];
-    for (uint32_t i = 0; i < 8; i++) prim_rank[i] = i < chunks ? prim[i] - 1 : 0xFFFFFFFFu;
-    cudaError_t e = cudaMemcpyAsync(d_prim, prim_rank, sizeof(prim_rank), cudaMemcpyHostToDevice, stream);
-    if (e != cudaSuccess) return e;
-    const uint32_t T = 256, G = (n + T - 1) / T;
-    ibwt_init_kernel<<<G, T, 0, stream>>>(bw, n, prim[0], keys_a, val_a);
-    cub::DoubleBuffer<uint8_t> k(keys_a, keys_b);
-    cub::DoubleBuffer<uint32_t> v(val_a, val_b);
-    size_t tb = temp_bytes;
-    e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int)n, 0, 8, stream);  // stable: LF mapping
-    if (e != cudaSuccess) return e;
-    const uint8_t* first = k.Current();
-    const uint32_t* next = v.Current();
-    const uint32_t GH = (nheads + T - 1) / T;
-    ibwt_measure_kernel<<<GH, T, 0, stream>>>(next, n, d_prim, nprim, nstride, succ0, lenv);
-    // dist[j] = len[j] initially; doubling
-    // (len -> 64-bit) reuse jump kernel with succ pointing nowhere for the first copy
-    {
-        // initialise dist_a from len, succ_a from succ0
-        cudaMemcpyAsync(succ_a, succ0, (size_t)nheads * 4, cudaMemcpyDeviceToDevice, stream);
-        // widen len into dist_a with a tiny kernel-free trick: use cudaMemset + 2D copy of the low words
-        cudaMemsetAsync(dist_a, 0, (size_t)nheads * 8, stream);
-        cudaMemcpy2DAsync(dist_a, 8, lenv, 4, 4, nheads, cudaMemcpyDeviceToDevice, stream);
-    }
-    (*launches) += 4;
-    uint32_t rounds = 1;
-    while ((1u << rounds) < nheads) rounds++;
-    for (uint32_t r = 0; r < rounds + 1; r++) {
-        ibwt_jump_kernel<<<GH, T, 0, stream>>>(succ_a, dist_a, nheads, succ_b, dist_b);
-        std::swap(succ_a, succ_b);
-        std::swap(dist_a, dist_b);
-        (*launches)++;
-    }
-    ibwt_write_kernel<<<GH, T, 0, stream>>>(next, first, n, d_prim, nprim, nstride, succ0, lenv, dist_a, (uint64_t)n, d_dst, nullptr);
-    (*launches)++;
-    return cudaGetLastError();
-}
-
-
 // ---- inverse, all blocks of a batch together ---------------------------------------------------------------------------------------------------
-// Same algorithm as bwt_inverse_device; one position space for the batch (block b = [base, base + n)), the block index above the byte in the
-// key of the stable sort (so the LF mapping of block b lands in its own range), one head list for all blocks, one set of launches: a 4 MiB
-// block is 17 pointer-doubling launches of a few hundred threads each, 48 blocks one after another were mostly launch latency.
+// The inverse of the file header (LF mapping by a stable sort, sub-lists cut every IBWT_STRIDE ranks, heads ranked by pointer doubling) in
+// one position space for the batch (block b = [base, base + n)), the block index above the byte in the key of the stable sort (so the LF
+// mapping of block b lands in its own range), one head list for all blocks, one set of launches: a 4 MiB block is 17 pointer-doubling
+// launches of a few hundred threads each, so blocks inverted one after another would be mostly launch latency.
 namespace {
 struct IbwtBatchBlock {
     uint64_t src_off, dst_off;  // BWT bytes (behind the header) / output

@@ -4,7 +4,6 @@
 
 namespace kz {
 size_t bwt_forward_workspace(uint32_t n);
-size_t bwt_inverse_workspace(uint32_t n);
 // BWTBlockCodec.Forward of one block: d_dst receives header + BWT bytes (n + 1 + chunks * index size), *d_out_len its length
 cudaError_t bwt_forward_device(const uint8_t* d_src, uint32_t n, uint8_t* d_dst, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream,
                                uint64_t* launches);
@@ -14,9 +13,6 @@ uint64_t bwt_forward_batch_max_total();
 uint32_t bwt_forward_batch_max_blocks();
 cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_t* src_off, const uint64_t* dst_off, const uint32_t* n_of, const uint32_t* number,
                               uint32_t nb, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches);
-// BWTBlockCodec.Inverse of one block; h_header = the first min(len, 33) bytes of d_src copied to the host
-cudaError_t bwt_inverse_device(const uint8_t* d_src, const uint8_t* h_header, uint32_t len, uint8_t* d_dst, uint32_t cap, uint32_t* out_len, uint8_t* ws,
-                               size_t ws_bytes, cudaStream_t stream, uint64_t* launches);
 // BWTBlockCodec.Inverse of a batch (one sort, one head list, one set of launches for all blocks); h_headers + 64 k = first 33 bytes of block k's stream
 size_t bwt_inverse_batch_workspace(uint64_t total, uint32_t nblocks);
 uint64_t bwt_inverse_batch_max_total();

@@ -114,6 +114,25 @@ struct BitWriter {
     }
 };
 
+// ---- per-block descriptor and result of the transform stages TEXT, UTF, EXE, MM, PACK / DNA (ROLZ: result only) ---------
+struct StageBlock {
+    uint64_t src_off;   // byte offset of the block in the source buffer
+    uint64_t dst_off;   // byte offset of the block in the destination buffer
+    uint32_t len;       // input length (0 = inactive block)
+    uint32_t cap;       // destination capacity (forward: MaxEncodedLen; inverse: len(dst) of the reference call)
+    int32_t data_type;  // forward: ctx["dataType"] before the call
+    uint32_t flags;     // PACK / DNA forward: 1 for the DNA flavour (Factory.go:151-153 "packOnlyDNA"); TEXT inverse (set inside
+                        // text_inverse_batch): 1 = decoded by the data-parallel path
+};
+struct StageResult {
+    int32_t status;     // forward: 0 = transformed, 1 = skip, negative = -(error code) where the reference panics (EXE);
+                        // inverse: 0 = ok, negative = -(error code)
+    uint32_t out_len;
+    int32_t data_type;  // forward: ctx["dataType"] after the call
+    uint32_t mode;      // forward, stage specific: TEXT the mode byte (CRLF / XML flags); MM 0 delta / 1 xor coding, distance in bits
+                        // 8..15; PACK 0 skip, 1 one symbol, 2 four symbols, 3 sixteen symbols, 4 digram aliases
+};
+
 // ---- block framing shared by host and device (io/CompressedStream.go) --------------------------------------
 struct BlockHeader {
     uint8_t mode;

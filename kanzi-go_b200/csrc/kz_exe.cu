@@ -6,16 +6,16 @@
 
 namespace kz {
 
-__global__ void __launch_bounds__(32) exe_forward_kernel(const uint8_t* __restrict__ in, const ExeBlock* __restrict__ blocks, int nblocks, uint8_t* __restrict__ out,
-                                                          ExeResult* __restrict__ res) {
+__global__ void __launch_bounds__(32) exe_forward_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks, uint8_t* __restrict__ out,
+                                                          StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const ExeBlock blk = blocks[b];
-    ExeResult r;
+    const StageBlock blk = blocks[b];
+    StageResult r;
     r.status = 1;
     r.out_len = 0;
     r.data_type = blk.data_type;
-    r.pad = 0;
+    r.mode = 0;
     if (blk.len != 0) {
         int dt = blk.data_type;
         const int64_t n = exec::forward(in + blk.src_off, (int64_t)blk.len, out + blk.dst_off, (int64_t)blk.cap, &dt);
@@ -30,16 +30,16 @@ __global__ void __launch_bounds__(32) exe_forward_kernel(const uint8_t* __restri
     res[b] = r;
 }
 
-__global__ void __launch_bounds__(32) exe_inverse_kernel(const uint8_t* __restrict__ in, const ExeBlock* __restrict__ blocks, int nblocks, uint8_t* __restrict__ out,
-                                                          ExeResult* __restrict__ res) {
+__global__ void __launch_bounds__(32) exe_inverse_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks, uint8_t* __restrict__ out,
+                                                          StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const ExeBlock blk = blocks[b];
-    ExeResult r;
+    const StageBlock blk = blocks[b];
+    StageResult r;
     r.status = 0;
     r.out_len = 0;
     r.data_type = 0;
-    r.pad = 0;
+    r.mode = 0;
     if (blk.len != 0 && blk.cap != 0) {
         const int64_t n = exec::inverse(in + blk.src_off, (int64_t)blk.len, out + blk.dst_off, (int64_t)blk.cap);
         if (n < 0) r.status = -KZ_E_PROCESS_BLOCK;

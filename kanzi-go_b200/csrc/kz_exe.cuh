@@ -4,22 +4,7 @@
 
 namespace kz {
 
-struct ExeBlock {
-    uint64_t src_off;
-    uint64_t dst_off;
-    uint32_t len;       // input length (0 = inactive block)
-    uint32_t cap;       // destination capacity (len(dst) of the reference call)
-    int32_t data_type;  // forward: ctx["dataType"] before the call
-    uint32_t pad;
-};
-struct ExeResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip, negative = -(error code) where the reference panics; inverse: 0 / negative
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call
-    uint32_t pad;
-};
-
-__global__ void exe_forward_kernel(const uint8_t* in, const ExeBlock* blocks, int nblocks, uint8_t* out, ExeResult* res);
-__global__ void exe_inverse_kernel(const uint8_t* in, const ExeBlock* blocks, int nblocks, uint8_t* out, ExeResult* res);
+__global__ void exe_forward_kernel(const uint8_t* in, const StageBlock* blocks, int nblocks, uint8_t* out, StageResult* res);
+__global__ void exe_inverse_kernel(const uint8_t* in, const StageBlock* blocks, int nblocks, uint8_t* out, StageResult* res);
 
 }  // namespace kz

@@ -110,10 +110,10 @@ KZ_D bool magic_allows_fsd(const uint8_t* p, uint32_t n) {
 
 KZ_D uint32_t fsd_dist(uint32_t idx) { return idx < 5 ? idx : (idx == 5 ? 8u : 16u); }  // distances {0, 1, 2, 3, 4, 8, 16}
 
-__global__ void __launch_bounds__(256) fsd_sample_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, uint32_t* __restrict__ hist7) {
+__global__ void __launch_bounds__(256) fsd_sample_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, uint32_t* __restrict__ hist7) {
     __shared__ uint32_t h[7 * 256];
     const int b = blockIdx.y;
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if (blk.len < 1024) return;
     for (int i = threadIdx.x; i < 7 * 256; i += 256) h[i] = 0;
     __syncthreads();
@@ -140,13 +140,13 @@ __global__ void __launch_bounds__(256) fsd_sample_kernel(const uint8_t* __restri
         if (h[i]) atomicAdd(&g[i], h[i]);
 }
 
-__global__ void __launch_bounds__(32) fsd_plan_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) fsd_plan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                        const uint32_t* __restrict__ hist7, const uint32_t* __restrict__ T, FsdInfo* __restrict__ infos,
-                                                       uint8_t* __restrict__ out, FsdResult* __restrict__ res) {
+                                                       uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks) return;
     const int lane = threadIdx.x;
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     FsdInfo& I = infos[b];
     const uint32_t count = blk.len;
     const uint8_t* src = in + blk.src_off;
@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(32) fsd_plan_kernel(const uint8_t* __restrict_
             dst[1] = (uint8_t)dist;
             for (uint32_t i = 0; i < dist; i++) dst[2 + i] = src[i];
         }
-        FsdResult r;
+        StageResult r;
         r.status = 1;
         r.out_len = 0;
         r.data_type = dt_out;
@@ -216,12 +216,12 @@ KZ_D uint32_t fsd_token_len(const uint8_t* src, uint32_t i, uint32_t dist) {
 }
 
 // delta mode: bytes produced by every tile of 4096 positions (position p codes byte dist + p)
-__global__ void __launch_bounds__(256) fsd_tiles_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) fsd_tiles_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos,
                                                          uint32_t* __restrict__ tile_sum, uint32_t ntiles) {
     const int b = blockIdx.y;
     const FsdInfo& I = infos[b];
     if (!I.go || I.mode != 0) return;
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t npos = blk.len - I.dist;
     if ((uint64_t)blockIdx.x * FSD_TILE >= npos) return;
     __shared__ uint32_t s_sum[8];
@@ -241,13 +241,13 @@ __global__ void __launch_bounds__(256) fsd_tiles_kernel(const uint8_t* __restric
     }
 }
 
-__global__ void __launch_bounds__(32) fsd_scan_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, int nblocks, FsdInfo* __restrict__ infos,
+__global__ void __launch_bounds__(32) fsd_scan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks, FsdInfo* __restrict__ infos,
                                                        const uint32_t* __restrict__ tile_sum, uint32_t* __restrict__ tile_off, uint32_t ntiles) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     FsdInfo& I = infos[b];
     if (!I.go) return;
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t count = blk.len, dist = I.dist;
     if (I.mode == 1) {  // xor coding: one byte per byte, the loop has no bound test (:287-293)
         I.out_len = count + 2;
@@ -270,12 +270,12 @@ __global__ void __launch_bounds__(32) fsd_scan_kernel(const uint8_t* __restrict_
     I.out_len = (uint32_t)off;
 }
 
-__global__ void __launch_bounds__(256) fsd_emit_kernel(const uint8_t* __restrict__ in, const FsdBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos,
+__global__ void __launch_bounds__(256) fsd_emit_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos,
                                                         const uint32_t* __restrict__ tile_off, uint32_t ntiles, uint8_t* __restrict__ out) {
     const int b = blockIdx.y;
     const FsdInfo& I = infos[b];
     if (!I.go) return;
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t dist = I.dist, npos = blk.len - dist;
     if ((uint64_t)blockIdx.x * FSD_TILE >= npos) return;
     const uint8_t* src = in + blk.src_off;
@@ -324,7 +324,7 @@ __global__ void __launch_bounds__(256) fsd_emit_kernel(const uint8_t* __restrict
 }
 
 // :296-310 histogram of two sub-ranges of the output
-__global__ void __launch_bounds__(256) fsd_post_hist_kernel(const FsdBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos, const uint8_t* __restrict__ out,
+__global__ void __launch_bounds__(256) fsd_post_hist_kernel(const StageBlock* __restrict__ blocks, const FsdInfo* __restrict__ infos, const uint8_t* __restrict__ out,
                                                              uint32_t* __restrict__ hpost) {
     __shared__ uint32_t h[256];
     const int b = blockIdx.y;
@@ -332,7 +332,7 @@ __global__ void __launch_bounds__(256) fsd_post_hist_kernel(const FsdBlock* __re
     if (!I.go) return;
     h[threadIdx.x] = 0;
     __syncthreads();
-    const FsdBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const uint32_t count10 = blk.len / 10, count5 = 2 * count10;
     const uint8_t* dst = out + blk.dst_off;
     for (uint32_t k = blockIdx.x * 256 + threadIdx.x; k < count10; k += gridDim.x * 256) {
@@ -343,15 +343,15 @@ __global__ void __launch_bounds__(256) fsd_post_hist_kernel(const FsdBlock* __re
     if (h[threadIdx.x]) atomicAdd(&hpost[(size_t)b * 256 + threadIdx.x], h[threadIdx.x]);
 }
 
-__global__ void __launch_bounds__(32) fsd_final_kernel(const FsdBlock* __restrict__ blocks, int nblocks, const FsdInfo* __restrict__ infos,
-                                                        const uint32_t* __restrict__ hpost, const uint32_t* __restrict__ T, FsdResult* __restrict__ res) {
+__global__ void __launch_bounds__(32) fsd_final_kernel(const StageBlock* __restrict__ blocks, int nblocks, const FsdInfo* __restrict__ infos,
+                                                        const uint32_t* __restrict__ hpost, const uint32_t* __restrict__ T, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     const FsdInfo& I = infos[b];
     if (!I.go) return;
     const uint32_t count10 = blocks[b].len / 10, count5 = 2 * count10;
     if (entropy_1024(count5, hpost + (size_t)b * 256, T) >= I.ent0) return;  // "no improvement": skip
-    FsdResult r = res[b];
+    StageResult r = res[b];
     r.status = 0;
     r.out_len = I.out_len;
     res[b] = r;
@@ -365,8 +365,8 @@ size_t fsd_workspace(uint32_t nblocks, uint32_t max_len) {
            2 * align256((size_t)nblocks * ntiles * 4) + 256;
 }
 
-cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                              FsdResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                              StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
     if (ws_bytes < fsd_workspace(nblocks, max_len)) return cudaErrorInvalidValue;
     const Ws w = carve(ws, nblocks, max_len);
@@ -764,10 +764,10 @@ __global__ void __launch_bounds__(128) fsdi_k5_kernel(const uint8_t* __restrict_
     }
     if ((uint32_t)lane < m) out[B.dst_off + di0 + lane] = (uint8_t)v;
 }
-__global__ void fsdi_result_kernel(const FsdiBlock* __restrict__ blocks, int nblocks, const FsdiState* __restrict__ st, FsdResult* __restrict__ res) {
+__global__ void fsdi_result_kernel(const FsdiBlock* __restrict__ blocks, int nblocks, const FsdiState* __restrict__ st, StageResult* __restrict__ res) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nblocks) return;
-    FsdResult r;
+    StageResult r;
     r.status = 0, r.out_len = 0, r.data_type = 0, r.mode = 0;
     if (blocks[b].active) {
         r.out_len = st[b].total;
@@ -783,7 +783,7 @@ size_t fsd_inverse_workspace(uint32_t nblocks, uint64_t total_len) {
 }
 
 // FSDCodec.Inverse of a batch over tiles (kernels above); h_blocks: the descriptors on the host.
-cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, FsdResult* d_res,
+cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const StageBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
     std::vector<FsdiBlock> hb(nblocks);

@@ -5,31 +5,16 @@
 
 namespace kz {
 
-struct FsdBlock {
-    uint64_t src_off;
-    uint64_t dst_off;
-    uint32_t len;       // input length (0 = inactive block)
-    uint32_t cap;       // destination capacity (len(dst) of the reference call)
-    int32_t data_type;  // forward: ctx["dataType"] before the call
-    uint32_t pad;
-};
-struct FsdResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip; inverse: 0 = ok, negative = -(error code)
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call
-    uint32_t mode;      // forward: 0 delta coding, 1 xor coding (dst[0]); distance in bits 8..15
-};
-
 static const uint32_t FSD_TILE = 4096;
 
 static inline __host__ __device__ uint32_t fsd_max_encoded_len(uint32_t n) { return n + ((n >> 4) > 64 ? (n >> 4) : 64); }
 size_t fsd_workspace(uint32_t nblocks, uint32_t max_len);
 
-cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
-                              FsdResult* d_res, cudaStream_t stream, uint64_t* launches);
+cudaError_t fsd_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint32_t max_len, uint8_t* ws, size_t ws_bytes,
+                              StageResult* d_res, cudaStream_t stream, uint64_t* launches);
 // FSDCodec.Inverse over tiles of 32 source bytes, all blocks together (h_blocks: descriptors on the host; ws of fsd_inverse_workspace bytes)
 size_t fsd_inverse_workspace(uint32_t nblocks, uint64_t total_len);
-cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const FsdBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, FsdResult* d_res,
+cudaError_t fsd_inverse_tiles(const uint8_t* d_in, uint8_t* d_out, const StageBlock* h_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches);
 
 }  // namespace kz

@@ -626,11 +626,11 @@ size_t rolz_scratch_bytes(size_t n) {
 
 // ---- forward: ROLZCodec.Forward :150-168 + rolzCodec1.Forward :301-596. res[b]: status 0 = ok, 1 = skip
 __global__ void __launch_bounds__(32) rolz_forward_kernel(const uint8_t* __restrict__ in, const RolzBlock* __restrict__ blocks, int nblocks,
-                                                          uint8_t* __restrict__ scratch_all, uint8_t* __restrict__ out, RolzResult* __restrict__ res) {
+                                                          uint8_t* __restrict__ scratch_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x, lane = threadIdx.x;
     if (b >= nblocks) return;
     const RolzBlock blk = blocks[b];
-    RolzResult r;
+    StageResult r;
     r.status = 1;
     r.out_len = 0;
     r.data_type = blk.data_type;
@@ -802,11 +802,11 @@ __global__ void __launch_bounds__(32) rolz_forward_kernel(const uint8_t* __restr
 
 // ---- inverse: ROLZCodec.Inverse :173-191 + rolzCodec1.Inverse :601-913 (bitstream version 6). status: 0 ok, -13 error
 __global__ void __launch_bounds__(32) rolz_inverse_kernel(const uint8_t* __restrict__ in, const RolzBlock* __restrict__ blocks, int nblocks,
-                                                          uint8_t* __restrict__ scratch_all, uint8_t* __restrict__ out, RolzResult* __restrict__ res) {
+                                                          uint8_t* __restrict__ scratch_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x, lane = threadIdx.x;
     if (b >= nblocks) return;
     const RolzBlock blk = blocks[b];
-    RolzResult r;
+    StageResult r;
     r.status = -KZ_E_PROCESS_BLOCK;
     r.out_len = 0;
     r.data_type = 0;

@@ -13,12 +13,7 @@ struct RolzBlock {
     int32_t data_type;     // ctx["dataType"] (internal/Global.go DataType); forward only
     uint32_t pad;
 };
-struct RolzResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip; inverse: 0 = ok, negative = -(error code)
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call (DetectSimpleType may set it)
-    uint32_t pad;
-};
+// result: StageResult (kz_common.cuh); forward data_type = ctx["dataType"] after the call (DetectSimpleType may set it)
 
 // bytes of the nested rANS buffer for a ROLZ chunk of `chunk` bytes (>= the reference's max(min(2 len, 9/8 chunk), 64 KiB))
 static inline __host__ __device__ size_t rolz_ans_buffer(size_t chunk) {
@@ -28,7 +23,7 @@ static inline __host__ __device__ size_t rolz_ans_buffer(size_t chunk) {
 }
 size_t rolz_scratch_bytes(size_t n);  // n = block length (forward) or destination capacity (inverse)
 
-__global__ void rolz_forward_kernel(const uint8_t* in, const RolzBlock* blocks, int nblocks, uint8_t* scratch_all, uint8_t* out, RolzResult* res);
-__global__ void rolz_inverse_kernel(const uint8_t* in, const RolzBlock* blocks, int nblocks, uint8_t* scratch_all, uint8_t* out, RolzResult* res);
+__global__ void rolz_forward_kernel(const uint8_t* in, const RolzBlock* blocks, int nblocks, uint8_t* scratch_all, uint8_t* out, StageResult* res);
+__global__ void rolz_inverse_kernel(const uint8_t* in, const RolzBlock* blocks, int nblocks, uint8_t* scratch_all, uint8_t* out, StageResult* res);
 
 }  // namespace kz

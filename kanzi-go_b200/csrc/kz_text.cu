@@ -98,17 +98,17 @@ KZ_D bool has_magic(const uint8_t* p, uint32_t n) {
     return false;
 }
 
-KZ_D bool forward_candidate(const TextBlock& blk) {  // wrapper :549-560, Forward :1228-1241
+KZ_D bool forward_candidate(const StageBlock& blk) {  // wrapper :549-560, Forward :1228-1241
     if (blk.len < 1024 || blk.len > (1u << 30) || blk.cap < blk.len) return false;
     return blk.data_type == DT_UNDEFINED || blk.data_type == DT_TEXT || blk.data_type == DT_BIN;
 }
 
 // byte histogram (shared memory) and the read part of the (previous byte, byte) histogram (L2 atomics), previous = 0 for the first byte (:196-222)
-__global__ void __launch_bounds__(256) text_hist_kernel(const uint8_t* __restrict__ in, const TextBlock* __restrict__ blocks, uint32_t* __restrict__ hist0,
+__global__ void __launch_bounds__(256) text_hist_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, uint32_t* __restrict__ hist0,
                                                          uint32_t* __restrict__ hist1) {
     __shared__ uint32_t h[256];
     const int b = blockIdx.y;
-    const TextBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if (!forward_candidate(blk)) return;
     h[threadIdx.x] = 0;
     __syncthreads();
@@ -128,13 +128,13 @@ __global__ void __launch_bounds__(256) text_hist_kernel(const uint8_t* __restric
     if (h[threadIdx.x]) atomicAdd(&hist0[(size_t)b * 256 + threadIdx.x], h[threadIdx.x]);
 }
 
-__global__ void __launch_bounds__(32) text_plan_kernel(const uint8_t* __restrict__ in, const TextBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) text_plan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                         const uint32_t* __restrict__ hist0, const uint32_t* __restrict__ hist1, uint32_t* __restrict__ go,
-                                                        TextResult* __restrict__ res) {
+                                                        StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const TextBlock blk = blocks[b];
-    TextResult r;
+    const StageBlock blk = blocks[b];
+    StageResult r;
     r.status = 1;
     r.out_len = 0;
     r.data_type = blk.data_type;
@@ -187,32 +187,32 @@ KZ_D Dict make_dict(int32_t* map, uint32_t log, Entry* list, int static_n, const
     return D;
 }
 
-__global__ void __launch_bounds__(32) text_forward_walk_kernel(const uint8_t* __restrict__ in, const TextBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) text_forward_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                                 const uint32_t* __restrict__ go, int static_n, const uint8_t* __restrict__ swords,
                                                                 int32_t* __restrict__ map_all, uint32_t log, Entry* __restrict__ list_all,
-                                                                uint8_t* __restrict__ out, TextResult* __restrict__ res) {
+                                                                uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     if (!(go[b] & 0x100u)) return;
-    const TextBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     Dict D = make_dict(map_all + ((size_t)b << log), log, list_all + (size_t)b * MAX_DICT_SIZE, static_n, swords, (int)blk.len);
     const int n = forward_walk(in + blk.src_off, (int)blk.len, out + blk.dst_off, (uint8_t)(go[b] & 0xFF), D);
     if (n >= 0) {
-        TextResult r = res[b];
+        StageResult r = res[b];
         r.status = 0;
         r.out_len = (uint32_t)n;
         res[b] = r;
     }
 }
 
-__global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __restrict__ in, const TextBlock* __restrict__ blocks, int nblocks, int static_n,
+__global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks, int static_n,
                                                                 const uint8_t* __restrict__ swords, int32_t* __restrict__ map_all, uint32_t log,
-                                                                Entry* __restrict__ list_all, uint8_t* __restrict__ out, TextResult* __restrict__ res) {
+                                                                Entry* __restrict__ list_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const TextBlock blk = blocks[b];
-    if (blk.pad == 1) return;  // decoded by the data-parallel path
-    TextResult r;
+    const StageBlock blk = blocks[b];
+    if (blk.flags == 1) return;  // decoded by the data-parallel path
+    StageResult r;
     r.status = 0;
     r.out_len = 0;
     r.data_type = 0;
@@ -243,8 +243,8 @@ size_t text_workspace_inverse(uint32_t nblocks, uint64_t stream_block_size, uint
     return align256(text_workspace_serial(nblocks, stream_block_size)) + text_inverse_parallel_workspace(nblocks, max_len, stream_block_size) + 256;
 }
 
-cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
-                               uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
+                               uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
 #if !KZ_HAVE_TEXT_DICT
     (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)max_len; (void)stream_block_size; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
     return cudaErrorNotSupported;
@@ -263,7 +263,7 @@ cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
     // data-parallel path (kz_text_par.cu); blocks it does not cover come back in `fallback` and take the serial walk below
     uint8_t* pws = ws + align256(text_workspace_serial(nblocks, stream_block_size));
     const size_t pws_bytes = ws_bytes - align256(text_workspace_serial(nblocks, stream_block_size));
-    std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
+    std::vector<StageBlock> tb(h_blocks, h_blocks + nblocks);
     std::vector<uint32_t> fallback;
     if ((e = text_forward_parallel(d_in, d_out, tb, w.go, stream_block_size, w.sdict, w.swords, S.n, pws, pws_bytes, d_res, stream, fallback, launches)) != cudaSuccess)
         return e;
@@ -285,8 +285,8 @@ cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
 #endif
 }
 
-cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,
-                               uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,
+                               uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
 #if !KZ_HAVE_TEXT_DICT
     (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)stream_block_size; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
     return cudaErrorNotSupported;
@@ -300,7 +300,7 @@ cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
     if ((e = cudaMemcpyAsync(w.swords, S.words.data(), SWORDS_BYTES, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     // data-parallel path (kz_text_par.cu); trivial blocks and every anomaly come back in `fallback` and take the serial walk below
     const size_t used = align256(text_workspace_serial(nblocks, stream_block_size));
-    std::vector<TextBlock> tb(h_blocks, h_blocks + nblocks);
+    std::vector<StageBlock> tb(h_blocks, h_blocks + nblocks);
     std::vector<uint32_t> fallback;
     if ((e = text_inverse_parallel(d_in, d_out, tb, stream_block_size, w.sdict, w.swords, S.n, ws + used, ws_bytes - used, d_res, stream, fallback, launches)) != cudaSuccess)
         return e;
@@ -309,9 +309,9 @@ cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBl
     if (!any) return cudaGetLastError();
     // the serial kernel writes res[b] for every block: give it a descriptor list in which the finished blocks are marked
     for (uint32_t b = 0; b < nblocks; b++)
-        if (!fallback[b]) tb[b].pad = 1;
-    TextBlock* d_tmp = reinterpret_cast<TextBlock*>(w.hist1);  // the forward-only histogram area is free here
-    if ((e = cudaMemcpyAsync(d_tmp, tb.data(), nblocks * sizeof(TextBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+        if (!fallback[b]) tb[b].flags = 1;
+    StageBlock* d_tmp = reinterpret_cast<StageBlock*>(w.hist1);  // the forward-only histogram area is free here
+    if ((e = cudaMemcpyAsync(d_tmp, tb.data(), nblocks * sizeof(StageBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
     text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(nullptr, w.sdict, S.n, w.map, w.log, w.list);
     text_inverse_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_tmp, (int)nblocks, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);

@@ -5,21 +5,6 @@
 
 namespace kz {
 
-struct TextBlock {
-    uint64_t src_off;
-    uint64_t dst_off;
-    uint32_t len;       // input length (0 = inactive block)
-    uint32_t cap;       // destination capacity (inverse: len(dst) of the reference call)
-    int32_t data_type;  // forward: ctx["dataType"] before the call
-    uint32_t pad;
-};
-struct TextResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip; inverse: 0 = ok, negative = -(error code)
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call
-    uint32_t mode;      // forward: the mode byte (CRLF / XML flags)
-};
-
 bool text_available();  // false when the library was built without the static dictionary (kanzi-go_b200/gen_text_dict.py)
 // device workspace for a batch; stream_block_size = ctx["blockSize"] (sizes the hash map: 2^clamp(log2(bs / 32), 13, 24) slots)
 size_t text_workspace(uint32_t nblocks, uint64_t stream_block_size, uint32_t max_len);  // forward (serial + data-parallel scratch)
@@ -27,9 +12,9 @@ size_t text_workspace_serial(uint32_t nblocks, uint64_t stream_block_size);     
 size_t text_workspace_inverse(uint32_t nblocks, uint64_t stream_block_size, uint32_t max_len);  // inverse (serial + data-parallel scratch)
 
 // h_blocks: host copy of d_blocks (the data-parallel path builds its own descriptors from it)
-cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
-                               uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream, uint64_t* launches);
-cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const TextBlock* d_blocks, const TextBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,
-                               uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream, uint64_t* launches);
+cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
+                               uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches);
+cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,
+                               uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches);
 
 }  // namespace kz

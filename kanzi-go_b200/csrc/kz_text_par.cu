@@ -425,7 +425,7 @@ __global__ void __launch_bounds__(256) tp_found_cost_kernel(const uint8_t* __res
 }
 __global__ void __launch_bounds__(32) tp_finalize_kernel(const TpBlock* __restrict__ blocks, int nblocks, TpState* __restrict__ st, const FoundW* __restrict__ found_all,
                                                           const uint32_t* __restrict__ cp_all, const uint32_t* __restrict__ found_total, uint8_t* __restrict__ out,
-                                                          TextResult* __restrict__ res, const uint32_t* __restrict__ fallback) {
+                                                          StageResult* __restrict__ res, const uint32_t* __restrict__ fallback) {
     const int b = blockIdx.x, lane = threadIdx.x;
     if (b >= nblocks) return;
     const TpBlock B = blocks[b];
@@ -445,7 +445,7 @@ __global__ void __launch_bounds__(32) tp_finalize_kernel(const TpBlock* __restri
         S.total = ok ? (uint32_t)total : 0u;
         if (ok) {
             dst[0] = (uint8_t)(B.go & 0xFF);
-            TextResult r = res[b];
+            StageResult r = res[b];
             r.status = 0;
             r.out_len = (uint32_t)total;
             res[b] = r;
@@ -856,7 +856,7 @@ __global__ void __launch_bounds__(256) ti_output_kernel(const uint8_t* __restric
         pos += (uint32_t)lens[j];
     }
 }
-__global__ void ti_finalize_kernel(const TiBlock* __restrict__ blocks, int nblocks, TiState* __restrict__ st, const uint32_t* __restrict__ tot, TextResult* __restrict__ res) {
+__global__ void ti_finalize_kernel(const TiBlock* __restrict__ blocks, int nblocks, TiState* __restrict__ st, const uint32_t* __restrict__ tot, StageResult* __restrict__ res) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nblocks) return;
     const TiBlock B = blocks[b];
@@ -865,7 +865,7 @@ __global__ void ti_finalize_kernel(const TiBlock* __restrict__ blocks, int nbloc
     if ((uint64_t)total + 64 >= (uint64_t)B.cap) st[b].anomaly = 1;  // too close to the checks of :1601 / :1661: the serial walk decides
     st[b].total = total;
     if (!st[b].anomaly) {
-        TextResult r;
+        StageResult r;
         r.status = 0;
         r.out_len = total;
         r.data_type = 0;
@@ -936,8 +936,8 @@ size_t text_parallel_workspace(uint32_t nblocks, uint32_t max_len, uint64_t stre
 }
 
 // d_go: the plan kernel's verdict per block (mode | 0x100 for text blocks). On return h_fallback[b] != 0 marks the text blocks the serial walk must do.
-cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<TextBlock>& tb, const uint32_t* d_go, uint64_t stream_block_size,
-                                  const void* d_sdict, const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream,
+cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, const uint32_t* d_go, uint64_t stream_block_size,
+                                  const void* d_sdict, const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream,
                                   std::vector<uint32_t>& h_fallback, uint64_t* launches) {
     const uint32_t nblocks = (uint32_t)tb.size();
     h_fallback.assign(nblocks, 0);
@@ -1050,8 +1050,8 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     return cudaGetLastError();
 }
 
-cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<TextBlock>& tb, uint64_t stream_block_size, const void* d_sdict,
-                                  const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, TextResult* d_res, cudaStream_t stream,
+cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, uint64_t stream_block_size, const void* d_sdict,
+                                  const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream,
                                   std::vector<uint32_t>& h_fallback, uint64_t* launches) {
     const uint32_t nblocks = (uint32_t)tb.size();
     h_fallback.assign(nblocks, 1);

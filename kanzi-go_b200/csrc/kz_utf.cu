@@ -43,18 +43,18 @@ Ws carve(uint8_t* ws, uint32_t nblocks) {
     return w;
 }
 
-KZ_D bool forward_candidate(const UtfBlock& blk) {  // :92-114
+KZ_D bool forward_candidate(const StageBlock& blk) {  // :92-114
     if (blk.len < (uint32_t)MIN_BLOCKSIZE || (uint64_t)blk.cap < (uint64_t)blk.len + 8192) return false;
     return blk.data_type == DT_UNDEFINED || blk.data_type == DT_UTF8;
 }
 
 // histograms of block = src[start : count - 4] for validateUTF (only needed when the data type is not already UTF-8)
-__global__ void __launch_bounds__(256) utf_hist_kernel(const uint8_t* __restrict__ in, const UtfBlock* __restrict__ blocks, uint32_t* __restrict__ hist0,
+__global__ void __launch_bounds__(256) utf_hist_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, uint32_t* __restrict__ hist0,
                                                         uint32_t* __restrict__ hist1, uint32_t* __restrict__ forb) {
     __shared__ uint32_t h[256];
     __shared__ uint32_t s_forb;
     const int b = blockIdx.y;
-    const UtfBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     if (!forward_candidate(blk) || blk.data_type == DT_UTF8) return;
     h[threadIdx.x] = 0;
     if (threadIdx.x == 0) s_forb = 0;
@@ -81,17 +81,17 @@ __global__ void __launch_bounds__(256) utf_hist_kernel(const uint8_t* __restrict
     if (threadIdx.x == 0 && s_forb) atomicAdd(&forb[b], s_forb);
 }
 
-__global__ void __launch_bounds__(32) utf_plan_kernel(const uint8_t* __restrict__ in, const UtfBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) utf_plan_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                        const uint32_t* __restrict__ hist0, const uint32_t* __restrict__ hist1, const uint32_t* __restrict__ forb,
-                                                       uint32_t* __restrict__ go, UtfResult* __restrict__ res) {
+                                                       uint32_t* __restrict__ go, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const UtfBlock blk = blocks[b];
-    UtfResult r;
+    const StageBlock blk = blocks[b];
+    StageResult r;
     r.status = 1;
     r.out_len = 0;
     r.data_type = blk.data_type;
-    r.pad = 0;
+    r.mode = 0;
     go[b] = 0;
     if (forward_candidate(blk)) {
         const int start = utf_start(in + blk.src_off);
@@ -113,33 +113,33 @@ __global__ void __launch_bounds__(256) utf_zero_kernel(const uint32_t* __restric
     for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < ALIAS_MAP_SIZE / 4; i += gridDim.x * 256) m[i] = make_int4(0, 0, 0, 0);
 }
 
-__global__ void __launch_bounds__(32) utf_forward_walk_kernel(const uint8_t* __restrict__ in, const UtfBlock* __restrict__ blocks, int nblocks,
+__global__ void __launch_bounds__(32) utf_forward_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                                const uint32_t* __restrict__ go, int32_t* __restrict__ alias_all, uint64_t* __restrict__ keys_all,
-                                                               uint8_t* __restrict__ out, UtfResult* __restrict__ res) {
+                                                               uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     if (!(go[b] & 0x100u)) return;
-    const UtfBlock blk = blocks[b];
+    const StageBlock blk = blocks[b];
     const int64_t n = forward_walk(in + blk.src_off, (int)blk.len, (int)(go[b] & 0xFF), out + blk.dst_off, alias_all + (size_t)b * ALIAS_MAP_SIZE,
                                    keys_all + (size_t)b * MAX_SYMBOLS);
     if (n >= 0) {
-        UtfResult r = res[b];
+        StageResult r = res[b];
         r.status = 0;
         r.out_len = (uint32_t)n;
         res[b] = r;
     }
 }
 
-__global__ void __launch_bounds__(32) utf_inverse_walk_kernel(const uint8_t* __restrict__ in, const UtfBlock* __restrict__ blocks, int nblocks,
-                                                               uint64_t* __restrict__ scratch_all, uint8_t* __restrict__ out, UtfResult* __restrict__ res) {
+__global__ void __launch_bounds__(32) utf_inverse_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
+                                                               uint64_t* __restrict__ scratch_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
-    const UtfBlock blk = blocks[b];
-    UtfResult r;
+    const StageBlock blk = blocks[b];
+    StageResult r;
     r.status = 0;
     r.out_len = 0;
     r.data_type = 0;
-    r.pad = 0;
+    r.mode = 0;
     if (blk.len != 0 && blk.cap != 0) {
         Sym* m = reinterpret_cast<Sym*>(scratch_all + (size_t)b * MAX_SYMBOLS);  // 8 bytes per entry, like the keys
         const int64_t n = inverse_walk(in + blk.src_off, (int)blk.len, out + blk.dst_off, (int64_t)blk.cap, m);
@@ -156,7 +156,7 @@ size_t utf_workspace(uint32_t nblocks) {
            align256((size_t)nblocks * ALIAS_MAP_SIZE * 4) + align256((size_t)nblocks * MAX_SYMBOLS * 8) + 256;
 }
 
-cudaError_t utf_forward_batch(const uint8_t* d_in, uint8_t* d_out, const UtfBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, UtfResult* d_res,
+cudaError_t utf_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches) {
     static_assert(sizeof(Sym) == 8, "inverse scratch shares the key array");
     if (nblocks == 0) return cudaSuccess;
@@ -174,7 +174,7 @@ cudaError_t utf_forward_batch(const uint8_t* d_in, uint8_t* d_out, const UtfBloc
     return cudaGetLastError();
 }
 
-cudaError_t utf_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const UtfBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, UtfResult* d_res,
+cudaError_t utf_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches) {
     if (nblocks == 0) return cudaSuccess;
     if (ws_bytes < utf_workspace(nblocks)) return cudaErrorInvalidValue;

@@ -5,25 +5,10 @@
 
 namespace kz {
 
-struct UtfBlock {
-    uint64_t src_off;
-    uint64_t dst_off;
-    uint32_t len;       // input length (0 = inactive block)
-    uint32_t cap;       // destination capacity (len(dst) of the reference call)
-    int32_t data_type;  // forward: ctx["dataType"] before the call
-    uint32_t pad;
-};
-struct UtfResult {
-    int32_t status;     // forward: 0 = transformed, 1 = skip; inverse: 0 = ok, negative = -(error code)
-    uint32_t out_len;
-    int32_t data_type;  // forward: ctx["dataType"] after the call
-    uint32_t pad;
-};
-
 size_t utf_workspace(uint32_t nblocks);
-cudaError_t utf_forward_batch(const uint8_t* d_in, uint8_t* d_out, const UtfBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, UtfResult* d_res,
+cudaError_t utf_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches);
-cudaError_t utf_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const UtfBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, UtfResult* d_res,
+cudaError_t utf_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, uint32_t nblocks, uint8_t* ws, size_t ws_bytes, StageResult* d_res,
                               cudaStream_t stream, uint64_t* launches);
 
 }  // namespace kz
