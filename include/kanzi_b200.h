@@ -113,6 +113,43 @@ int kz_compress_stream_device(kz_ctx* ctx, uint64_t transform48, uint32_t entrop
 /* Decompresses the complete stream of n bytes at d_src (must be followed by >= 64 readable bytes) into d_dst. */
 int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n);
 
+/* ---- many independent streams in one call (BlockCompressor / BlockDecompressor over a directory: every file is a stream of its own,
+ *      app/BlockCompressor.go:543-613). The blocks of all streams run through the stages together, so a call pays the per-batch kernels
+ *      and host synchronisations once instead of once per stream. -------------------------------------------------------------------------
+ * Stream s is read from src + src_off[s] (src_len[s] bytes) and written to dst + dst_off[s] (at most dst_cap[s] bytes); out_len[s] = bytes
+ * written. Nothing is written outside [dst_off[s], dst_off[s] + dst_cap[s]).
+ * Compress: stream s is byte for byte what kz_compress_stream(ctx, transform48, entropy, block_size, checksum_bits, input_size[s],
+ *   src + src_off[s], src_len[s], ...) writes (input_size NULL = 0 for every stream). Empty streams are allowed (header and end marker), as
+ *   are streams shorter than 16 bytes (COPY blocks). One call uses one block size: with `-b auto` every file has its own block size, and the
+ *   caller groups files by block size. When stream s needs more than dst_cap[s] bytes, status[s] = -KZ_ERR_WRITE_FILE, nothing is written
+ *   for it and out_len[s] = the bytes it needs.
+ * Decompress: streams may have different headers (transform, entropy, block size, checksum); the library groups them. Stream s decodes to
+ *   dst + dst_off[s]; out_len[s] = its length.
+ * Status: status[s] = 0 or -(kanzi error code). A stream with status 0 is complete and correct whatever happened to the others. These errors
+ *   belong to one stream: a bad header or version, a bad block prefix or block header, an entropy-decode failure, a checksum mismatch, a
+ *   failing inverse transform, and dst_cap[s] too small (-KZ_ERR_WRITE_FILE); each gets the code kz_decompress_stream gives for the same
+ *   bytes. A call-level failure (a bad argument, an unsupported transform or entropy codec, a CUDA error) sets every status to its code.
+ *   On the compress side a transform or entropy failure on one stream's data (EXE on a malformed executable header, an entropy coder
+ *   that fails on a block: where the reference fails that stream with ERR_PROCESS_BLOCK) is also call-level; compress such a batch
+ *   stream by stream to find the stream. The return value is 0 when every stream succeeded, otherwise the code of the first failing
+ *   stream.
+ * Memory: device scratch for the stages follows the blocks of one pass (at most STREAM_PASS_BUDGET = 1 GiB of slots and entropy
+ *   tables, kanzi-go_b200/csrc/kz_stream_plan.h), but a call also holds all of its inputs and all of its outputs on the device at once:
+ *   compress every input, every encoded block and every assembled stream; decompress every input and, for the host variant,
+ *   sum(dst_cap) bytes of staging. Split a batch larger than the GPU's memory into several calls.
+ * Device variants: src / dst are device pointers, the offset and length arrays are host arrays, src, dst and every offset are multiples
+ *   of 16, and >= 64 readable bytes follow each input (the rule of kz_decompress_stream_device). */
+int kz_compress_streams(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams,
+                        const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst,
+                        const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+int kz_decompress_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, uint8_t* dst,
+                          const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+int kz_compress_streams_device(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams,
+                               const void* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst,
+                               const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+int kz_decompress_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, void* d_dst,
+                                 const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+
 /* ---- sharded streams (io.Writer / io.Reader with the blocks of ONE stream spread over several GPUs; the NCCL scatter / gather of the
  *      byte ranges is the host side's business, kanzi-go_b200/parallel.py; blocks are independent: io/CompressedStream.go:896-898) ---------- */
 /* Block records (5 b | lw b | payload each, :951-976) of the n bytes at d_src: no stream header, no end marker. *out_bits = exact length. */

@@ -8,6 +8,7 @@ package gpu
 import "C"
 
 import (
+	"fmt"
 	"time"
 	"unsafe"
 
@@ -110,6 +111,112 @@ func (c *Context) DecodeBlocks(transformType uint64, entropyType uint32, ckBits 
 		}
 	}
 	return outLen, nil
+}
+
+// StreamResult is what one file of a many-stream call produced: the stream (or decoded bytes), or the kanzi error of that file alone.
+type StreamResult struct {
+	Data []byte
+	Err  error
+}
+
+// CompressStreams compresses every input as a stream of its own in one call, as BlockCompressor's multi-file path
+// (app/BlockCompressor.go:543-613) would use it instead of one Writer per file. Stream i is byte for byte what a Writer with
+// the same parameters and fileSize = inputSizes[i] writes for inputs[i]. All inputs share one block size: with `-b auto` the
+// caller groups its files by block size and makes one call per group. A file whose output does not fit fails alone; a transform or
+// entropy failure on one file's data (the reference fails that file with ERR_PROCESS_BLOCK) fails the whole call, and the caller
+// then compresses the files one by one. The call holds all inputs, encoded blocks and streams in device memory at once: split a
+// large directory into calls of a size the GPU holds.
+func (c *Context) CompressStreams(transformType uint64, entropyType uint32, blockSize uint32, ckBits uint, inputs [][]byte,
+	inputSizes []int64) ([]StreamResult, error) {
+	n := len(inputs)
+	srcOff, srcLen := make([]uint64, n), make([]uint64, n)
+	dstOff, dstCap := make([]uint64, n), make([]uint64, n)
+	var srcTotal, dstTotal uint64
+	for i, in := range inputs {
+		srcOff[i], srcLen[i] = srcTotal, uint64(len(in))
+		srcTotal += uint64(len(in))
+		dstOff[i], dstCap[i] = dstTotal, uint64(C.kz_max_stream_output(C.size_t(len(in)), C.uint32_t(blockSize)))
+		dstTotal += dstCap[i]
+	}
+	src := make([]byte, srcTotal+1)
+	for i, in := range inputs {
+		copy(src[srcOff[i]:], in)
+	}
+	dst := make([]byte, dstTotal+1)
+	outLen, status := make([]uint64, n+1), make([]C.int32_t, n+1)
+	var isz *C.int64_t
+	if len(inputSizes) == n && n > 0 {
+		isz = (*C.int64_t)(unsafe.Pointer(&inputSizes[0]))
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_compress_streams(c.h, C.uint64_t(transformType), C.uint32_t(entropyType), C.uint32_t(blockSize), C.uint32_t(ckBits), C.uint32_t(n),
+		(*C.uint8_t)(unsafe.Pointer(&src[0])), u64p(srcOff), u64p(srcLen), isz, (*C.uint8_t)(unsafe.Pointer(&dst[0])), u64p(dstOff), u64p(dstCap),
+		u64p(outLen), &status[0])
+	return c.streamResults(rc, dst, dstOff, outLen, status, n)
+}
+
+// DecompressStreams decodes many streams in one call, as BlockDecompressor's multi-file path would: the streams may have different
+// headers (transform, entropy, block size, checksum). caps[i] bounds the decoded size of stream i (the file size its header records,
+// or the caller's limit). A corrupt stream gets the error code a Reader would report for it; every other stream decodes normally.
+// A stream whose transform or entropy codec the GPU path lacks fails the whole call with ERR_INVALID_CODEC: the caller then keeps
+// the reference's Reader for the files of that call. The device holds every input and sum(caps) bytes of output at once.
+func (c *Context) DecompressStreams(streams [][]byte, caps []uint64) ([]StreamResult, error) {
+	n := len(streams)
+	srcOff, srcLen, dstOff := make([]uint64, n), make([]uint64, n), make([]uint64, n)
+	var srcTotal, dstTotal uint64
+	for i, s := range streams {
+		srcOff[i], srcLen[i] = srcTotal, uint64(len(s))
+		srcTotal += uint64(len(s))
+		dstOff[i] = dstTotal
+		dstTotal += caps[i]
+	}
+	src := make([]byte, srcTotal+1)
+	for i, s := range streams {
+		copy(src[srcOff[i]:], s)
+	}
+	dst := make([]byte, dstTotal+1)
+	outLen, status := make([]uint64, n+1), make([]C.int32_t, n+1)
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_decompress_streams(c.h, C.uint32_t(n), (*C.uint8_t)(unsafe.Pointer(&src[0])), u64p(srcOff), u64p(srcLen),
+		(*C.uint8_t)(unsafe.Pointer(&dst[0])), u64p(dstOff), u64p(caps), u64p(outLen), &status[0])
+	return c.streamResults(rc, dst, dstOff, outLen, status, n)
+}
+
+// StreamError is the kanzi error code (Definitions.go:25-46) one file of a many-stream call failed with.
+type StreamError struct {
+	Code int
+}
+
+func (e *StreamError) Error() string {
+	return fmt.Sprintf("kanzi gpu: stream failed with error code %d", e.Code)
+}
+
+// streamResults splits a many-stream call's output (called with mu held). Every file carries its own result: its bytes, or a
+// StreamError with its own code. The returned error is nil when every file succeeded; otherwise it is the context's message for the
+// call (kz_last_error) with the code of the first failing file. A call-level failure (a bad argument, an unsupported codec, a CUDA
+// error) gives every file that same code.
+func (c *Context) streamResults(rc C.int, dst []byte, dstOff, outLen []uint64, status []C.int32_t, n int) ([]StreamResult, error) {
+	res := make([]StreamResult, n)
+	for i := 0; i < n; i++ {
+		if status[i] != 0 {
+			res[i].Err = &StreamError{Code: -int(status[i])}
+			continue
+		}
+		res[i].Data = dst[dstOff[i] : dstOff[i]+outLen[i]]
+	}
+	if rc != 0 {
+		return res, fmt.Errorf("%v (code %d)", c.err(rc), -int(rc))
+	}
+	return res, nil
+}
+
+func u64p(a []uint64) *C.uint64_t {
+	if len(a) == 0 {
+		return nil
+	}
+	return (*C.uint64_t)(unsafe.Pointer(&a[0]))
 }
 
 // parseBlockHead reads post-transform length and checksum back from a block-local bit string (:869-886).

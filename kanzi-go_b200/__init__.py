@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "kz_compress_stream_device", "kz_decompress_stream_device", "kz_profile", "kz_kernel_time", "kz_profile_reset", "kz_set_stream_block_size",
     "kz_stage_bytes", "kz_profile_names",
     "kz_compress_fragment_device", "kz_stream_header", "kz_concat_bits_device", "kz_stream_index_device", "kz_decompress_fragment_device",
+    "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
 ]
 
 
@@ -133,6 +134,10 @@ def load_library(build_if_missing=True):
     L.kz_profile_names.argtypes = [vp, C.c_char_p, sz]
     L.kz_profile_names.restype = sz
     L.kz_set_stream_block_size.restype = None
+    L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_decompress_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -145,6 +150,18 @@ def _u8(a):
 
 def _p(a):
     return a.ctypes.data if a.size else None
+
+
+def _offsets(lens):
+    """Exclusive prefix sums of lens (uint64)."""
+    off = np.zeros(len(lens), np.uint64)
+    if len(lens) > 1:
+        off[1:] = np.cumsum(lens[:-1], dtype=np.uint64)
+    return off
+
+
+def _dptr(t):
+    return t.data_ptr() if hasattr(t, "data_ptr") else t
 
 
 class Context:
@@ -268,6 +285,60 @@ class Context:
         n = C.c_size_t(0)
         self._check(self.lib.kz_decompress_stream(self.h, _p(s), s.size, out.ctypes.data, out_cap, C.byref(n)))
         return out[: n.value]
+
+    # ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams) -----------------------------------
+    # Per-stream failures do not raise: status[s] = 0 or -(kanzi error code), and outputs[s] is None for a failed stream.
+    def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None):
+        """One compressed stream per input, each equal to compress(inputs[s], ..., input_size=input_sizes[s]) -> (outputs, status)."""
+        arrs = [_u8(x) for x in inputs]
+        t48 = transform_type(transform) if isinstance(transform, str) else transform
+        et = entropy_type(entropy) if isinstance(entropy, str) else entropy
+        src_len = np.array([a.size for a in arrs], np.uint64)
+        src_off = _offsets(src_len)
+        src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
+        cap = np.array([self.lib.kz_max_stream_output(a.size, block_size) for a in arrs], np.uint64)
+        dst_off = _offsets(cap)
+        dst = np.empty(max(int(cap.sum()), 1), np.uint8)
+        isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
+        out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
+        self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len), None if isz is None else _p(isz),
+                                     dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
+        outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
+        return outs, status
+
+    def decompress_streams(self, streams, caps):
+        """Decodes every stream (headers may differ) into at most caps[s] bytes -> (outputs, status)."""
+        arrs = [_u8(x) for x in streams]
+        src_len = np.array([a.size for a in arrs], np.uint64)
+        src_off = _offsets(src_len)
+        src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
+        cap = np.ascontiguousarray(caps, np.uint64)
+        dst_off = _offsets(cap)
+        dst = np.empty(max(int(cap.sum()), 1), np.uint8)
+        out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
+        self.lib.kz_decompress_streams(self.h, len(arrs), _p(src), _p(src_off), _p(src_len), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len),
+                                       _p(status))
+        outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
+        return outs, status
+
+    def compress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, transform, entropy, block_size, checksum_bits=0,
+                                input_sizes=None):
+        """src / dst: CUDA uint8 tensors (or device addresses); offsets (multiples of 16) and lengths: host sequences -> (out_len, status)."""
+        t48 = transform_type(transform) if isinstance(transform, str) else transform
+        et = entropy_type(entropy) if isinstance(entropy, str) else entropy
+        so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
+        isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
+        out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
+        self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl), None if isz is None else _p(isz),
+                                            _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+        return out_len, status
+
+    def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap):
+        """Device-resident decompress_streams: inputs need >= 64 readable bytes behind each -> (out_len, status)."""
+        so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
+        out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
+        self.lib.kz_decompress_streams_device(self.h, len(sl), _dptr(src), _p(so), _p(sl), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+        return out_len, status
 
     # ---- device-resident entry points (pointers are CUDA device addresses, e.g. torch tensors' data_ptr()) -------
     def compress_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, input_size=0):

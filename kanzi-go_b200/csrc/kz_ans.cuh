@@ -82,4 +82,12 @@ struct ExtractJob {
 };
 __global__ void extract_copy_kernel(const uint32_t* words, const ExtractJob* jobs, int njobs, uint8_t* dst);
 
+// A list of byte copies between device addresses, one CTA per job. The host cuts longer copies into pieces of at most COPY_PIECE bytes.
+struct CopyJob {
+    uint64_t src, dst;  // device addresses
+    uint64_t len;
+};
+static const uint64_t COPY_PIECE = 64 * 1024;
+__global__ void batch_copy_kernel(const CopyJob* jobs, int njobs);
+
 }  // namespace kz

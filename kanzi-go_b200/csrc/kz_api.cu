@@ -24,8 +24,11 @@
 #include "kz_text.cuh"
 #include "kz_utf.cuh"
 #include "kz_exe.cuh"
+#include "kz_stream_plan.h"
 
+#include <map>
 #include <memory>
+#include <tuple>
 
 using namespace kz;
 
@@ -188,6 +191,28 @@ int upload(kz_ctx* ctx, Packer& pk) {
     return 0;
 }
 
+// Device-to-device copies collected on the host and run by one batch_copy_kernel launch.
+struct CopyList {
+    std::vector<CopyJob> jobs;
+    void add(const void* src, void* dst, uint64_t len) {
+        for (uint64_t o = 0; o < len; o += COPY_PIECE)
+            jobs.push_back({(uint64_t)(uintptr_t)src + o, (uint64_t)(uintptr_t)dst + o, std::min<uint64_t>(COPY_PIECE, len - o)});
+    }
+};
+int run_copies(kz_ctx* ctx, const CopyList& cl) {
+    if (cl.jobs.empty()) return 0;
+    const size_t bytes = cl.jobs.size() * sizeof(CopyJob);
+    CK(ctx->d_copy.ensure(bytes));
+    // from pageable memory: the runtime has taken the list when the call returns, and the copy is ordered behind earlier kernels
+    CK(cudaMemcpyAsync(ctx->d_copy.p, cl.jobs.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+    {
+        LaunchScope ls(ctx, "batch_copy");
+        batch_copy_kernel<<<(int)cl.jobs.size(), 256, 0, ctx->stream>>>(ctx->d_copy.as<CopyJob>(), (int)cl.jobs.size());
+    }
+    CK(cudaGetLastError());
+    return 0;
+}
+
 // XXHash32/64 of a set of blocks (hash/XXHash32.go, XXHash64.go; seed "KANZ", io/CompressedStream.go:354-356). Synchronous.
 int hash_blocks(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint32_t bits,
                 std::vector<uint64_t>& out) {
@@ -235,6 +260,32 @@ int verify_checksums(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint6
 }
 
 bool etype_supported(uint32_t e) { return e == KZ_E_NONE || e == KZ_E_ANS0 || e == KZ_E_HUFFMAN || e == KZ_E_ANS1 || e == KZ_E_RANGE; }
+
+// The gather of every bit-granular output (kz_concat.cu): segment i, seg_bits[i] bits at address seg_src[i], lands at bit seg_dst[i] of
+// d_out. The three tables are device arrays. encode_batch, the many-stream assembly and kz_concat_bits_device all write through it.
+int concat_segments(kz_ctx* ctx, const uint64_t* d_seg_src, const uint64_t* d_seg_bits, const uint64_t* d_seg_dst, int nsegs, uint8_t* d_out) {
+    if (nsegs <= 0) return 0;
+    {
+        LaunchScope ls(ctx, "concat_zero");
+        concat_zero_kernel<<<(nsegs + 255) / 256, 256, 0, ctx->stream>>>(d_seg_bits, d_seg_dst, nsegs, (uint32_t*)d_out);
+    }
+    {
+        LaunchScope ls(ctx, "concat");
+        concat_copy_kernel<<<nsegs, 128, 0, ctx->stream>>>(d_seg_src, d_seg_bits, d_seg_dst, nsegs, (uint32_t*)d_out);
+    }
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// The per-chunk scratch encode_batch allocates for codec e (d_enc_tab, d_hdr, d_pay, d_hist), for the pass planner (kz_stream_plan.h)
+EntropyScratch entropy_scratch(uint32_t e) {
+    EntropyScratch s;
+    if (e == KZ_E_ANS1) s = {ANS1_CHUNK, 65536 * 4 + 256 * ANS1_CTX_HDR_STRIDE + 32 + 112 + ANS1_HIST_WORDS * 4 + 256 * 4, 2};
+    else if (e == KZ_E_RANGE) s = {RANGE_CHUNK, RC_OUT_STRIDE, 0};
+    else if (e == KZ_E_HUFFMAN) s = {HUF_CHUNK, 256 * 2 + HUF_HDR_STRIDE + HUF_FRAG_STRIDE * 4, 0};
+    else if (e == KZ_E_ANS0) s = {ANS0_CHUNK, 256 * 4 + HDR_STRIDE + PAY_STRIDE, 0};
+    return s;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // entropy encode of a batch of blocks + bit-granular assembly
@@ -364,7 +415,7 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
                 }
             }
             if (layout == LAYOUT_STREAM) {
-                add_seg((uint64_t)(uintptr_t)(d_small + small_zero_off), ctx->fragment ? 0 : 8);  // end marker: 5+3 zero bits (Close :593-594); none behind a fragment
+                add_seg((uint64_t)(uintptr_t)(d_small + small_zero_off), ctx->fragment ? 0 : END_MARKER_BITS);  // end marker (Close :593-594); none behind a fragment
                 blk_first[nblocks] = (uint32_t)seg_src.size();
             } else {
                 blk_first[nblocks] = (uint32_t)seg_src.size();
@@ -532,14 +583,8 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
             if (blk_base_bits[b] + res.blk_bits[b] + 64 > lim) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
         }
     }
-    if (nsegs > 0) {
-        {
-            LaunchScope ls(ctx, "concat_zero");
-            concat_zero_kernel<<<(nsegs + 255) / 256, 256, 0, ctx->stream>>>(d_seg_bits, d_seg_dst, nsegs, (uint32_t*)d_dst);
-        }
-        LaunchScope ls(ctx, "concat");
-        concat_copy_kernel<<<nsegs, 128, 0, ctx->stream>>>(d_seg_src, d_seg_bits, d_seg_dst, nsegs, (uint32_t*)d_dst);
-    }
+    rc = concat_segments(ctx, d_seg_src, d_seg_bits, d_seg_dst, nsegs, d_dst);
+    if (rc) return rc;
     CK(cudaGetLastError());
     return 0;
 }
@@ -554,12 +599,24 @@ __global__ void block_header_kernel(const uint32_t* __restrict__ words, const ui
     out[b] = parse_block_header(words, bit_off[b], bits[b], checksum_bits, block_size);
 }
 
-// Serial walk over the block length prefixes of a complete stream (decodingTask.decode :1816-1852). One thread.
-// stop_after != 0: a fragment of that many block records (no end marker behind them)
-__global__ void stream_walk_kernel(const uint32_t* __restrict__ words, uint64_t start_bit, uint64_t end_bit, uint32_t max_blocks,
-                                   uint64_t* __restrict__ bit_off, uint64_t* __restrict__ bits, uint32_t* __restrict__ count_status, uint32_t stop_after = 0) {
-    if (blockIdx.x != 0 || threadIdx.x != 0) return;
-    BitReader br(words, start_bit, end_bit);
+// The block records of one stream for stream_walk_kernel: bits [start_bit, end_bit) of the word buffer, found records go to entries
+// out .. out + max_blocks - 1 of bit_off / bits. stop_after != 0: a fragment of that many block records (no end marker behind them).
+struct WalkJob {
+    uint64_t start_bit, end_bit, out;
+    uint32_t max_blocks, stop_after;
+};
+
+// Serial walk over the block length prefixes of complete streams (decodingTask.decode :1816-1852), one thread per stream: jobs[s], or
+// `one` when jobs is null. count_status[2s] = records found, count_status[2s + 1] = 0 or -(error code).
+__global__ void stream_walk_kernel(const uint32_t* __restrict__ words, const WalkJob* __restrict__ jobs, WalkJob one, int nstreams,
+                                   uint64_t* __restrict__ bit_off_all, uint64_t* __restrict__ bits_all, uint32_t* __restrict__ count_status) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nstreams) return;
+    const WalkJob job = jobs ? jobs[s] : one;
+    const uint32_t max_blocks = job.max_blocks, stop_after = job.stop_after;
+    uint64_t* bit_off = bit_off_all + job.out;
+    uint64_t* bits = bits_all + job.out;
+    BitReader br(words, job.start_bit, job.end_bit);
     uint32_t n = 0;
     int32_t st = 0;
     for (;;) {
@@ -594,8 +651,8 @@ __global__ void stream_walk_kernel(const uint32_t* __restrict__ words, uint64_t 
             break;
         }
     }
-    count_status[0] = n;
-    count_status[1] = (uint32_t)st;
+    count_status[2 * s] = n;
+    count_status[2 * s + 1] = (uint32_t)st;
 }
 
 // jobs[b].bit_off / bits / out_off must be set; fills pre_len, mode, ..., status. d_words = device stream buffer.
@@ -1448,10 +1505,13 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
         if (rc) return rc;
         for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
         note_stage_bytes(ctx, "fwd", plan.ids[i], bytes_in, bytes_out);
+        CopyList declined;
         for (uint32_t b = 0; b < nblocks; b++) {
             if (applied[b]) flags[b] &= (uint8_t)~(1u << (7 - i));
-            else if (len[b]) CK(cudaMemcpyAsync(outb + b * gstride, cur + b * cur_stride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
+            else declined.add(cur + b * cur_stride, outb + b * gstride, len[b]);
         }
+        rc = run_copies(ctx, declined);
+        if (rc) return rc;
         cur = outb;
         cur_stride = gstride;
     }
@@ -1467,13 +1527,14 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
 
 // Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186) of every block of a batch. The entropy
 // stage left block b's pre_len bytes at d_pre + b*pstride, a scratch buffer of this context with room for pstride - 64 bytes per
-// block; the stages alternate between it and ctx->d_tmp2. Decoded blocks go to d_dst back to back (slot = 0) or at b * slot.
-// *total = bytes produced.
-int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, uint8_t* d_dst, size_t cap,
-                  std::vector<uint32_t>& out_len, uint64_t* total, uint64_t slot) {
+// block; the stages alternate between it and ctx->d_tmp2. out_len[b] = decoded length of block b. Once the lengths are known,
+// place(b, len, &at) is called for every block in order and gives its destination: at = nullptr drops the block, a false return fails
+// the call with KZ_ERR_WRITE_FILE (no room). All blocks are then copied by one batch_copy_kernel launch.
+template <class Place>
+int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, Place&& place,
+                  std::vector<uint32_t>& out_len) {
     const uint32_t nblocks = (uint32_t)jobs.size();
     out_len.assign(nblocks, 0);
-    *total = 0;
     if (nblocks == 0) return 0;
     const uint32_t blk_cap = (uint32_t)std::min<uint64_t>(pstride - 64, 0xFFFFFFF0u);
     std::vector<uint32_t> len(nblocks);
@@ -1496,22 +1557,38 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
         if (rc) return rc;
         for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
         note_stage_bytes(ctx, "inv", plan.ids[i], bytes_in, bytes_out);
+        CopyList skipped;
         for (uint32_t b = 0; b < nblocks; b++)
-            if (!active[b] && len[b]) CK(cudaMemcpyAsync(other + b * pstride, cur + b * pstride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
+            if (!active[b]) skipped.add(cur + b * pstride, other + b * pstride, len[b]);
+        rc = run_copies(ctx, skipped);
+        if (rc) return rc;
         std::swap(cur, other);
     }
-    uint64_t off = 0;
+    CopyList out;
     for (uint32_t b = 0; b < nblocks; b++) {
-        const uint64_t at = slot ? (uint64_t)b * slot : off;
-        if (at + len[b] > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-        if (len[b]) CK(cudaMemcpyAsync(d_dst + at, cur + b * pstride, len[b], cudaMemcpyDeviceToDevice, ctx->stream));
+        uint8_t* at = nullptr;
+        if (!place(b, len[b], &at)) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
+        if (at) out.add(cur + b * pstride, at, len[b]);
         out_len[b] = len[b];
-        off += len[b];
     }
-    *total = off;
+    int rc = run_copies(ctx, out);
+    if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
+
+// Destinations of blocks decoded back to back into d_dst (cap bytes): what inverse_stage's place() does for one stream.
+struct BackToBack {
+    uint8_t* d_dst;
+    uint64_t cap, off = 0;
+    bool operator()(uint32_t, uint32_t len, uint8_t** at) {
+        if (off + len > cap) return false;
+        *at = d_dst + off;
+        off += len;
+        return true;
+    }
+};
+
 
 }  // namespace
 
@@ -1551,10 +1628,12 @@ void kz_destroy(kz_ctx* ctx) {
     cudaStreamSynchronize(ctx->stream);
     drain_profile(ctx);
     for (auto e : ctx->event_pool) cudaEventDestroy(e);
-    DevBuf* bufs[] = {&ctx->d_in, &ctx->d_out, &ctx->d_tmp, &ctx->d_tmp2, &ctx->d_seg, &ctx->d_chunks, &ctx->d_tables, &ctx->d_enc_tab, &ctx->d_hdr, &ctx->d_pay, &ctx->d_small, &ctx->d_dl, &ctx->d_rcp, &ctx->d_ws, &ctx->d_lens, &ctx->d_hist};
+    DevBuf* bufs[] = {&ctx->d_in, &ctx->d_out, &ctx->d_tmp, &ctx->d_tmp2, &ctx->d_seg, &ctx->d_chunks, &ctx->d_tables, &ctx->d_enc_tab, &ctx->d_hdr, &ctx->d_pay, &ctx->d_small, &ctx->d_dl, &ctx->d_rcp, &ctx->d_ws, &ctx->d_lens, &ctx->d_hist,
+                      &ctx->d_copy, &ctx->d_slots, &ctx->d_enc, &ctx->d_bits, &ctx->d_asm};
     for (auto b : bufs) b->release();
     ctx->h_stage.release();
     ctx->h_dl.release();
+    ctx->h_io.release();
     cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -1755,15 +1834,8 @@ int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, 
         LaunchScope ls(ctx, "scan");
         scan_bits_kernel<<<1, 1024, 0, ctx->stream>>>((const uint64_t*)(T + o_bits), (uint64_t*)(T + o_dst), nsegs + 1, 0, (uint64_t*)(T + o_total));
     }
-    {
-        LaunchScope ls(ctx, "concat_zero");
-        concat_zero_kernel<<<(nsegs + 255) / 256, 256, 0, ctx->stream>>>((const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), nsegs, (uint32_t*)d_dst);
-    }
-    {
-        LaunchScope ls(ctx, "concat");
-        concat_copy_kernel<<<nsegs, 128, 0, ctx->stream>>>((const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), nsegs, (uint32_t*)d_dst);
-    }
-    CK(cudaGetLastError());
+    rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), nsegs, (uint8_t*)d_dst);
+    if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
 }
@@ -1813,7 +1885,7 @@ int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t ma
     uint32_t* d_cnt = (uint32_t*)(d_bbits + max_blocks);
     {
         LaunchScope ls(ctx, "stream_walk");
-        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>((const uint32_t*)d_src, sh.bits, 8ull * n, max_blocks, d_boff, d_bbits, d_cnt);
+        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>((const uint32_t*)d_src, nullptr, WalkJob{sh.bits, 8ull * n, 0, max_blocks, 0}, 1, d_boff, d_bbits, d_cnt);
     }
     uint32_t cs[2] = {0, 0};
     CK(cudaMemcpyAsync(cs, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1862,7 +1934,7 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     uint32_t* d_cnt = (uint32_t*)(d_bbits + max_blocks);
     {
         LaunchScope ls(ctx, "stream_walk");
-        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>(d_words, sh.bits, 8ull * n, max_blocks, d_boff, d_bbits, d_cnt, stop_after);
+        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>(d_words, nullptr, WalkJob{sh.bits, 8ull * n, 0, max_blocks, stop_after}, 1, d_boff, d_bbits, d_cnt);
     }
     // count + the first SPEC block descriptors in one round trip (streams with more blocks pay a second copy)
     const uint32_t SPEC = std::min<uint32_t>(max_blocks, 1024);
@@ -1936,8 +2008,10 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     for (uint32_t b = 0; b < nblocks; b++)
         if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid bitstream: block decoding failed");
     std::vector<uint32_t> olen;
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, (uint8_t*)d_dst, cap, olen, &out_off, 0);
+    BackToBack place{(uint8_t*)d_dst, cap};
+    rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen);
     if (rc) return rc;
+    out_off = place.off;
     CK(cudaStreamSynchronize(ctx->stream));
     if (sh.checksum_bits) {  // decoded blocks lie back to back (every block but the last is block_size long)
         std::vector<uint64_t> hoff(nblocks);
@@ -1986,6 +2060,515 @@ int kz_decompress_stream(kz_ctx* ctx, const uint8_t* src, size_t n, uint8_t* dst
     CK(cudaStreamSynchronize(ctx->stream));
     *out_n = produced;
     return 0;
+}
+
+// ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams and their _device variants) ------------
+// Every input file of BlockCompressor is a stream of its own (app/BlockCompressor.go:543-613); blocks are independent
+// (io/CompressedStream.go:896-898), so the blocks of all streams run through the stages together, pass by pass (kz_stream_plan.h).
+
+// Grows b to n bytes and keeps its first `used` bytes (DevBuf::ensure does not keep them).
+static int ensure_keep(kz_ctx* ctx, DevBuf& b, size_t used, size_t n) {
+    if (n + 256 <= b.cap) return 0;
+    DevBuf nb;
+    CK(nb.ensure(std::max(n, 2 * b.cap)));
+    if (used) CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    b.release();
+    b = nb;
+    return 0;
+}
+
+static int check_stream_args(kz_ctx* ctx, uint32_t nstreams, const void* src, const uint64_t* src_off, const uint64_t* src_len, const void* dst,
+                             const uint64_t* dst_off, const uint64_t* dst_cap, const uint64_t* out_len, const int32_t* status, bool device) {
+    if (nstreams && (!src_off || !src_len || !dst_off || !dst_cap || !out_len || !status)) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
+    uint64_t src_end = 0, dst_end = 0;
+    for (uint32_t s = 0; s < nstreams; s++) {
+        if (src_off[s] + src_len[s] < src_off[s] || dst_off[s] + dst_cap[s] < dst_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+        src_end = std::max(src_end, src_off[s] + src_len[s]);
+        dst_end = std::max(dst_end, dst_off[s] + dst_cap[s]);
+        if (device && ((src_off[s] | dst_off[s]) & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
+    }
+    if ((src_end && !src) || (dst_end && !dst)) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    if (device && (((uintptr_t)src & 15) || ((uintptr_t)dst & 15))) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    return 0;
+}
+
+// The return value and statuses of a many-stream call: a call-level failure rc sets every status; otherwise the first failing stream's code.
+static int finish_streams(uint32_t nstreams, int32_t* status, uint64_t* out_len, int rc) {
+    if (rc) {
+        for (uint32_t s = 0; s < nstreams; s++) {
+            if (status) status[s] = rc;
+            if (out_len) out_len[s] = 0;
+        }
+        return rc;
+    }
+    for (uint32_t s = 0; s < nstreams; s++)
+        if (status[s]) return status[s];
+    return 0;
+}
+
+// Compresses stream s = d_src[src_off[s] : + src_len[s]]. Stream s is assembled in ctx->d_asm at 8 * stage_off[s] (16-byte aligned, behind
+// the header / prefix table of `small_bytes`); its length is out_len[s], status[s] = -KZ_ERR_WRITE_FILE when it exceeds dst_cap[s].
+static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams,
+                                 const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size,
+                                 const uint64_t* dst_cap, uint64_t* out_len, int32_t* status, std::vector<uint64_t>& stage_off, uint64_t* stage_base,
+                                 uint64_t* stage_total) {
+    ctx->stream_bs = block_size;
+    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
+    if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+    TransformPlan plan;
+    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    // the blocks of every stream, stream after stream (Writer.Write cuts the input into blockSize pieces)
+    std::vector<uint64_t> boff;
+    std::vector<uint32_t> blen, first(nstreams + 1);
+    for (uint32_t s = 0; s < nstreams; s++) {
+        first[s] = (uint32_t)blen.size();
+        for (uint64_t o = 0; o < src_len[s]; o += block_size) {
+            boff.push_back(src_off[s] + o);
+            blen.push_back((uint32_t)std::min<uint64_t>(block_size, src_len[s] - o));
+        }
+    }
+    const uint32_t nb = (uint32_t)blen.size();
+    first[nstreams] = nb;
+    // ctx["dataType"] of every block from its first four bytes (encodingTask.encode :806-816), gathered in one copy
+    std::vector<int32_t> dts(nb, 0);
+    if (plan.uses_magic() && nb) {
+        CK(ctx->d_asm.ensure((size_t)nb * 4));
+        CK(cudaMemsetAsync(ctx->d_asm.p, 0, (size_t)nb * 4, ctx->stream));
+        CopyList heads;
+        for (uint32_t b = 0; b < nb; b++) heads.add(d_src + boff[b], ctx->d_asm.as<uint8_t>() + 4 * (size_t)b, std::min<uint32_t>(4, blen[b]));
+        rc = run_copies(ctx, heads);
+        if (rc) return rc;
+        std::vector<uint8_t> h((size_t)nb * 4);
+        CK(cudaMemcpyAsync(h.data(), ctx->d_asm.p, h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t b = 0; b < nb; b++) dts[b] = magic_data_type(&h[(size_t)b * 4], blen[b]);
+    }
+    std::vector<uint64_t> hv;
+    if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
+        rc = hash_blocks(ctx, d_src, boff, blen, checksum_bits, hv);
+        if (rc) return rc;
+    }
+    // passes: transforms and entropy coding of the blocks of a pass, then their bit strings packed into ctx->d_bits
+    const EntropyScratch es = entropy_scratch(etype);
+    const PassPlan P = plan_compress_passes(blen, [&](uint64_t s) { return compress_block_cost(s, es); });
+    std::vector<uint64_t> bbits(nb), barena(nb);
+    uint64_t arena = 0;
+    for (uint32_t p = 0; p < P.npasses(); p++) {
+        const uint32_t i0 = P.first[p], k = P.first[p + 1] - i0;
+        const uint64_t s = P.stride[p];
+        CK(ctx->d_slots.ensure(s * k + 64));
+        uint8_t* slots = ctx->d_slots.as<uint8_t>();
+        std::vector<uint32_t> lens(k);
+        std::vector<int32_t> pdt(k);
+        CopyList place;
+        uint32_t max_len = 0;
+        for (uint32_t j = 0; j < k; j++) {
+            const uint32_t b = P.order[i0 + j];
+            lens[j] = blen[b];
+            pdt[j] = dts[b];
+            max_len = std::max(max_len, blen[b]);
+            place.add(d_src + boff[b], slots + j * s, blen[b]);
+        }
+        rc = run_copies(ctx, place);
+        if (rc) return rc;
+        const uint8_t* d_data = nullptr;
+        std::vector<EncJob> jobs;
+        rc = forward_stage(ctx, plan, slots, 0, block_size, s, lens.data(), k, &d_data, jobs, &pdt);
+        if (rc) return rc;
+        if (checksum_bits)
+            for (uint32_t j = 0; j < k; j++) jobs[j].checksum = hv[P.order[i0 + j]];
+        const uint64_t ostride = round16(kz_max_block_output(max_len));
+        CK(ctx->d_enc.ensure(ostride * k + 64));
+        std::vector<uint64_t> base(k);
+        for (uint32_t j = 0; j < k; j++) base[j] = 8 * (uint64_t)j * ostride;
+        EncResult res;
+        rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, ctx->d_enc.as<uint8_t>(), ostride * k, base, res);
+        if (rc) return rc;
+        uint64_t need = arena;
+        for (uint32_t j = 0; j < k; j++) need += round16((res.blk_bits[j] + 7) / 8);
+        rc = ensure_keep(ctx, ctx->d_bits, arena, need + 64);
+        if (rc) return rc;
+        CopyList pack;
+        for (uint32_t j = 0; j < k; j++) {
+            const uint32_t b = P.order[i0 + j];
+            const uint64_t nbytes = (res.blk_bits[j] + 7) / 8;
+            bbits[b] = res.blk_bits[j];
+            barena[b] = arena;
+            pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + arena, nbytes);
+            arena += round16(nbytes);
+        }
+        rc = run_copies(ctx, pack);
+        if (rc) return rc;
+    }
+    // assembly (Writer.processBlock :951-976, Close :593-594): stream header, then 5 b | lw b prefix and bit string of every block, then the
+    // end marker. Lengths are known here, so the host lays out every segment; one concat_zero / concat_copy pair writes all streams.
+    const size_t o_zero = 64 * (size_t)nstreams + 8 * (size_t)nb;
+    const uint64_t small_bytes = (o_zero + 16 + 255) & ~255ull;
+    std::vector<uint8_t> small(small_bytes, 0);
+    std::vector<uint32_t> hdr_bits(nstreams), pre_bits(nb);
+    stage_off.assign(nstreams, 0);
+    uint64_t stage = 0, nsegs = 0;
+    for (uint32_t s = 0; s < nstreams; s++) {
+        std::vector<uint8_t> hdr;
+        hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size ? input_size[s] : 0);
+        memcpy(&small[64 * (size_t)s], hdr.data(), 64);
+        uint64_t bits = hdr_bits[s] + END_MARKER_BITS;
+        for (uint32_t b = first[s]; b < first[s + 1]; b++) {
+            pre_bits[b] = write_block_prefix(&small[64 * (size_t)nstreams + 8 * (size_t)b], bbits[b]);
+            bits += pre_bits[b] + bbits[b];
+            nsegs += 1 + (bbits[b] + 8 * RAW_PIECE - 1) / (8 * RAW_PIECE);
+        }
+        out_len[s] = (bits + 7) / 8;
+        status[s] = out_len[s] > dst_cap[s] ? -KZ_ERR_WRITE_FILE : 0;
+        stage_off[s] = stage;
+        if (!status[s]) stage += round16(out_len[s]);
+        nsegs += 2;
+    }
+    *stage_base = small_bytes;
+    *stage_total = stage;
+    CK(ctx->d_asm.ensure(small_bytes + stage + 64));
+    uint8_t* A = ctx->d_asm.as<uint8_t>();
+    CK(cudaMemcpyAsync(A, small.data(), small_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<uint64_t> seg_src, seg_bits, seg_dst;
+    seg_src.reserve(nsegs), seg_bits.reserve(nsegs), seg_dst.reserve(nsegs);
+    for (uint32_t s = 0; s < nstreams; s++) {
+        if (status[s]) continue;
+        uint64_t d = 8 * (small_bytes + stage_off[s]);
+        auto add = [&](const uint8_t* src, uint64_t nbits) {
+            seg_src.push_back((uint64_t)(uintptr_t)src);
+            seg_bits.push_back(nbits);
+            seg_dst.push_back(d);
+            d += nbits;
+        };
+        add(A + 64 * (size_t)s, hdr_bits[s]);
+        for (uint32_t b = first[s]; b < first[s + 1]; b++) {
+            add(A + 64 * (size_t)nstreams + 8 * (size_t)b, pre_bits[b]);
+            for (uint64_t o = 0; o < bbits[b]; o += 8 * RAW_PIECE) add(ctx->d_bits.as<uint8_t>() + barena[b] + o / 8, std::min<uint64_t>(8 * RAW_PIECE, bbits[b] - o));
+        }
+        add(A + o_zero, END_MARKER_BITS);
+    }
+    const int ns = (int)seg_src.size();
+    if (ns) {
+        Packer pk;
+        const size_t o_src = pk.add(seg_src.data(), seg_src.size() * 8);
+        const size_t o_bits = pk.add(seg_bits.data(), seg_bits.size() * 8);
+        const size_t o_dst = pk.add(seg_dst.data(), seg_dst.size() * 8);
+        rc = upload(ctx, pk);
+        if (rc) return rc;
+        uint8_t* T = ctx->d_tables.as<uint8_t>();
+        rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), ns, A);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));  // the segment tables live in d_tables
+    }
+    return 0;
+}
+
+// One group of streams with the same header fields: walk, entropy decode and inverse transforms of all their blocks, pass by pass, each
+// block written behind the previous one of its stream at d_dst + dst_off[s]. A stream on which anything goes wrong (a bad record, block
+// header, entropy payload or checksum, too little room, a block longer than the decode slot) is put on `alone`; the caller decodes it
+// again on its own with the single-stream path, so that its status is the code kz_decompress_stream_device gives for the same bytes. A
+// failing inverse transform does not say which block failed: then every stream of the group goes on `alone`.
+static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan, const std::vector<uint32_t>& grp,
+                               const std::vector<uint64_t>& hdr_bits, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off,
+                               const uint64_t* src_len, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len,
+                               int32_t* status, std::vector<uint32_t>& alone) {
+    const uint32_t ng = (uint32_t)grp.size();
+    const uint32_t* d_words = (const uint32_t*)d_src;
+    const uint64_t words_len = (src_bytes + 3) / 4 + 16;
+    // walk: one thread per stream; as many records per stream as the single-stream path allows, and no more than its bytes can hold
+    std::vector<WalkJob> wj(ng);
+    uint64_t nrec = 0;
+    for (uint32_t g = 0; g < ng; g++) {
+        const uint32_t s = grp[g];
+        const uint64_t by_cap = std::min<uint64_t>(dst_cap[s] / 1024 + 16, 1u << 22);
+        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), nrec, (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1), 0};
+        nrec += wj[g].max_blocks;
+    }
+    CK(ctx->d_dl.ensure((size_t)nrec * 16 + (size_t)ng * 8 + 64));
+    uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
+    uint64_t* d_bbits = d_boff + nrec;
+    uint32_t* d_cnt = (uint32_t*)(d_bbits + nrec);
+    {
+        Packer pk;
+        const size_t o_wj = pk.add(wj.data(), wj.size() * sizeof(WalkJob));
+        int rc = upload(ctx, pk);
+        if (rc) return rc;
+        LaunchScope ls(ctx, "stream_walk");
+        stream_walk_kernel<<<(ng + 127) / 128, 128, 0, ctx->stream>>>(d_words, (const WalkJob*)(ctx->d_tables.as<uint8_t>() + o_wj), WalkJob{}, (int)ng, d_boff,
+                                                                       d_bbits, d_cnt);
+    }
+    CK(cudaGetLastError());
+    std::vector<uint32_t> cs((size_t)ng * 2);
+    std::vector<uint64_t> hoff(nrec), hbits(nrec);
+    CK(cudaMemcpyAsync(cs.data(), d_cnt, cs.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(hoff.data(), d_boff, nrec * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(hbits.data(), d_bbits, nrec * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::vector<uint8_t> bad(ng, 0);
+    std::vector<uint64_t> written(ng, 0);
+    std::vector<DecJob> all;
+    std::vector<uint32_t> bgrp;   // group index of every block
+    std::vector<uint8_t> blast;   // last block of its stream
+    for (uint32_t g = 0; g < ng; g++) {
+        if (cs[2 * g + 1]) {
+            bad[g] = 1;
+            continue;
+        }
+        for (uint32_t r = 0; r < cs[2 * g]; r++) {
+            DecJob j = DecJob();
+            j.bit_off = hoff[wj[g].out + r];
+            j.bits = hbits[wj[g].out + r];
+            all.push_back(j);
+            bgrp.push_back(g);
+            blast.push_back(r + 1 == cs[2 * g]);
+        }
+    }
+    const uint64_t pstride = decompress_slot(sh.block_size);
+    const PassPlan P = plan_decompress_passes((uint32_t)all.size(), pstride, decompress_block_cost(sh.block_size));
+    bool group_failed = false;
+    for (uint32_t p = 0; p < P.npasses() && !group_failed; p++) {
+        std::vector<DecJob> jobs;
+        std::vector<uint32_t> jg;
+        std::vector<uint8_t> jl;
+        auto keep_good = [&]() {  // drops the blocks of streams that went bad
+            size_t w = 0;
+            for (size_t i = 0; i < jobs.size(); i++)
+                if (!bad[jg[i]]) jobs[w] = jobs[i], jg[w] = jg[i], jl[w] = jl[i], w++;
+            jobs.resize(w), jg.resize(w), jl.resize(w);
+        };
+        for (uint32_t i = P.first[p]; i < P.first[p + 1]; i++)
+            if (!bad[bgrp[i]]) jobs.push_back(all[i]), jg.push_back(bgrp[i]), jl.push_back(blast[i]);
+        int rc = decode_parse_headers(ctx, d_words, jobs, sh.checksum_bits, sh.block_size);
+        if (rc) return rc;
+        for (size_t i = 0; i < jobs.size(); i++)
+            if (jobs[i].status || jobs[i].pre_len > pstride - 64 || (plan.none() && !jl[i] && (jobs[i].pre_len & 15))) bad[jg[i]] = 1;
+        keep_good();
+        const uint32_t k = (uint32_t)jobs.size();
+        if (k == 0) continue;
+        CK(ctx->d_tmp.ensure(pstride * k + 64));
+        for (uint32_t i = 0; i < k; i++) jobs[i].out_off = (uint64_t)i * pstride;
+        rc = decode_batch(ctx, sh.etype, d_words, words_len, jobs, ctx->d_tmp.as<uint8_t>());
+        if (rc) return rc;
+        for (uint32_t i = 0; i < k; i++)
+            if (jobs[i].status) bad[jg[i]] = 1;
+        keep_good();
+        // destinations: behind the stream's earlier blocks, within its dst_cap
+        std::vector<uint64_t> at(jobs.size(), 0);
+        auto place = [&](uint32_t i, uint32_t len, uint8_t** to) {
+            const uint32_t g = jg[i], s = grp[g];
+            if (bad[g] || written[g] + len > dst_cap[s]) {
+                bad[g] = 1;
+                *to = nullptr;
+                return true;
+            }
+            at[i] = dst_off[s] + written[g];
+            *to = d_dst + at[i];
+            written[g] += len;
+            return true;
+        };
+        std::vector<uint32_t> olen(jobs.size(), 0);
+        if (plan.none()) {
+            CopyList out;
+            for (uint32_t i = 0; i < jobs.size(); i++) {
+                uint8_t* to = nullptr;
+                place(i, jobs[i].pre_len, &to);
+                olen[i] = jobs[i].pre_len;
+                if (to) out.add(ctx->d_tmp.as<uint8_t>() + (uint64_t)i * pstride, to, olen[i]);
+            }
+            rc = run_copies(ctx, out);
+            if (rc) return rc;
+        } else if (inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen)) {
+            group_failed = true;
+            break;
+        }
+        if (sh.checksum_bits) {  // decodingTask.decode :1990-2006, on the bytes where they landed
+            std::vector<uint64_t> hoffs, hv;
+            std::vector<uint32_t> hlens;
+            std::vector<uint32_t> hidx;
+            for (uint32_t i = 0; i < jobs.size(); i++)
+                if (!bad[jg[i]]) hoffs.push_back(at[i]), hlens.push_back(olen[i]), hidx.push_back(i);
+            rc = hash_blocks(ctx, d_dst, hoffs, hlens, sh.checksum_bits, hv);
+            if (rc) return rc;
+            for (size_t q = 0; q < hidx.size(); q++) {
+                const uint64_t want = sh.checksum_bits == 32 ? (jobs[hidx[q]].checksum & 0xFFFFFFFFull) : jobs[hidx[q]].checksum;
+                if (hv[q] != want) bad[jg[hidx[q]]] = 1;
+            }
+        }
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (uint32_t g = 0; g < ng; g++) {
+        const uint32_t s = grp[g];
+        if (group_failed || bad[g]) {
+            alone.push_back(s);
+        } else {
+            status[s] = 0;
+            out_len[s] = written[g];
+        }
+    }
+    return 0;
+}
+
+static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, const void* d_src, size_t n, void* d_dst,
+                                  size_t cap, size_t* out_n);
+
+// Decodes stream s = d_src[src_off[s] : + src_len[s]] (>= 64 readable bytes behind it) to d_dst + dst_off[s]. src_bytes: readable bytes at d_src.
+static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off, const uint64_t* src_len,
+                                   uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    for (uint32_t s = 0; s < nstreams; s++) status[s] = 0, out_len[s] = 0;
+    if (nstreams == 0) return 0;
+    // headers: the first 64 bytes of every stream in one gather and one transfer, parsed by parse_stream_header
+    CK(ctx->d_asm.ensure(64 * (size_t)nstreams));
+    CK(cudaMemsetAsync(ctx->d_asm.p, 0, 64 * (size_t)nstreams, ctx->stream));
+    CopyList heads;
+    for (uint32_t s = 0; s < nstreams; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
+    int rc = run_copies(ctx, heads);
+    if (rc) return rc;
+    std::vector<uint8_t> head(64 * (size_t)nstreams);
+    CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::vector<StreamHeader> sh(nstreams);
+    std::vector<uint64_t> hdr_bits(nstreams, 0);
+    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
+    for (uint32_t s = 0; s < nstreams; s++) {
+        status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
+        if (status[s]) continue;
+        TransformPlan plan;
+        rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan, KZ_ERR_INVALID_CODEC);
+        if (rc) return rc;
+        if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
+        hdr_bits[s] = sh[s].bits;
+        groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
+    }
+    std::vector<uint32_t> alone;
+    for (auto& kv : groups) {
+        const StreamHeader& h = sh[kv.second[0]];
+        ctx->stream_bs = h.block_size;
+        TransformPlan plan;
+        rc = plan_transforms(ctx, h.t48, h.etype, plan, KZ_ERR_INVALID_CODEC);
+        if (rc) return rc;
+        rc = decode_stream_group(ctx, h, plan, kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
+        if (rc) return rc;
+    }
+    for (uint32_t s : alone) {  // only corrupt input (or too little room) gets here
+        size_t n = 0;
+        status[s] = decompress_device_impl(ctx, nullptr, 0, 0, d_src + src_off[s], src_len[s], d_dst + dst_off[s], dst_cap[s], &n);
+        out_len[s] = status[s] ? 0 : n;
+    }
+    return 0;
+}
+
+int kz_compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const void* d_src,
+                               const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst, const uint64_t* dst_off,
+                               const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_stream_args(ctx, nstreams, d_src, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, true);
+    if (rc) return finish_streams(nstreams, status, out_len, rc);
+    if (cudaSetDevice(ctx->device) != cudaSuccess) return finish_streams(nstreams, status, out_len, -KZ_ERR_PROCESS_BLOCK);
+    std::vector<uint64_t> stage_off;
+    uint64_t stage_base = 0, stage_total = 0;
+    rc = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, (const uint8_t*)d_src, src_off, src_len, input_size, dst_cap, out_len,
+                               status, stage_off, &stage_base, &stage_total);
+    if (!rc) {
+        CopyList out;
+        for (uint32_t s = 0; s < nstreams; s++)
+            if (!status[s]) out.add(ctx->d_asm.as<uint8_t>() + stage_base + stage_off[s], (uint8_t*)d_dst + dst_off[s], out_len[s]);
+        rc = run_copies(ctx, out);
+        if (!rc && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = ctx->cuda_fail(cudaGetLastError(), "compress_streams");
+    }
+    return finish_streams(nstreams, status, out_len, rc);
+}
+
+int kz_compress_streams(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const uint8_t* src,
+                        const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                        uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_stream_args(ctx, nstreams, src, src_off, src_len, dst, dst_off, dst_cap, out_len, status, false);
+    if (rc) return finish_streams(nstreams, status, out_len, rc);
+    rc = [&]() -> int {
+        CK(cudaSetDevice(ctx->device));
+        // the inputs packed at 16-byte aligned offsets and moved in one transfer
+        std::vector<uint64_t> in_off(nstreams);
+        uint64_t total = 0;
+        for (uint32_t s = 0; s < nstreams; s++) in_off[s] = total, total += round16(src_len[s]);
+        CK(ctx->h_io.ensure(total + 64));
+        CK(ctx->d_in.ensure(total + 64));
+        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
+        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+        std::vector<uint64_t> stage_off;
+        uint64_t stage_base = 0, stage_total = 0;
+        int r = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, ctx->d_in.as<uint8_t>(), in_off.data(), src_len, input_size, dst_cap,
+                                      out_len, status, stage_off, &stage_base, &stage_total);
+        if (r) return r;
+        CK(ctx->h_io.ensure(stage_total + 64));
+        if (stage_total) CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.as<uint8_t>() + stage_base, stage_total, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t s = 0; s < nstreams; s++)
+            if (!status[s]) memcpy(dst + dst_off[s], (uint8_t*)ctx->h_io.p + stage_off[s], out_len[s]);
+        return 0;
+    }();
+    return finish_streams(nstreams, status, out_len, rc);
+}
+
+int kz_decompress_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, void* d_dst,
+                                 const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_stream_args(ctx, nstreams, d_src, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, true);
+    if (rc) return finish_streams(nstreams, status, out_len, rc);
+    uint64_t src_bytes = 0;
+    for (uint32_t s = 0; s < nstreams; s++) src_bytes = std::max(src_bytes, src_off[s] + src_len[s]);
+    rc = [&]() -> int {
+        CK(cudaSetDevice(ctx->device));
+        return decompress_streams_impl(ctx, nstreams, (const uint8_t*)d_src, src_bytes, src_off, src_len, (uint8_t*)d_dst, dst_off, dst_cap, out_len, status);
+    }();
+    return finish_streams(nstreams, status, out_len, rc);
+}
+
+int kz_decompress_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, uint8_t* dst,
+                          const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_stream_args(ctx, nstreams, src, src_off, src_len, dst, dst_off, dst_cap, out_len, status, false);
+    if (rc) return finish_streams(nstreams, status, out_len, rc);
+    rc = [&]() -> int {
+        CK(cudaSetDevice(ctx->device));
+        // inputs packed at 16-byte aligned offsets with 64 zero bytes behind each (what kz_decompress_stream gives a single stream);
+        // outputs staged at 16-byte aligned offsets of dst_cap[s] bytes each, packed by length and moved back in one transfer
+        std::vector<uint64_t> in_off(nstreams), st_off(nstreams), pk_off(nstreams);
+        uint64_t total = 0, st_total = 0;
+        for (uint32_t s = 0; s < nstreams; s++) {
+            in_off[s] = total, total += round16(src_len[s]) + 64;
+            st_off[s] = st_total, st_total += round16(dst_cap[s]);
+        }
+        CK(ctx->h_io.ensure(total + 64));
+        CK(ctx->d_in.ensure(total + 64));
+        CK(ctx->d_out.ensure(st_total + 64));
+        memset(ctx->h_io.p, 0, total);
+        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
+        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+        int r = decompress_streams_impl(ctx, nstreams, ctx->d_in.as<uint8_t>(), total, in_off.data(), src_len, ctx->d_out.as<uint8_t>(), st_off.data(), dst_cap,
+                                        out_len, status);
+        if (r) return r;
+        uint64_t pk_total = 0;
+        for (uint32_t s = 0; s < nstreams; s++) {
+            pk_off[s] = pk_total;
+            if (!status[s]) pk_total += round16(out_len[s]);
+        }
+        CK(ctx->d_asm.ensure(pk_total + 64));
+        CopyList pack;
+        for (uint32_t s = 0; s < nstreams; s++)
+            if (!status[s]) pack.add(ctx->d_out.as<uint8_t>() + st_off[s], ctx->d_asm.as<uint8_t>() + pk_off[s], out_len[s]);
+        r = run_copies(ctx, pack);
+        if (r) return r;
+        CK(ctx->h_io.ensure(pk_total + 64));
+        if (pk_total) CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.p, pk_total, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t s = 0; s < nstreams; s++)
+            if (!status[s]) memcpy(dst + dst_off[s], (uint8_t*)ctx->h_io.p + pk_off[s], out_len[s]);
+        return 0;
+    }();
+    return finish_streams(nstreams, status, out_len, rc);
 }
 
 // ---- block batch, host buffers (Writer.processBlock / Reader.processBlock replacement) -----------------------
@@ -2107,8 +2690,14 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     // inverse transforms into a scratch area (block b at b * ostride), then out
     CK(ctx->d_tmp.ensure(ostride * nblocks + 64));
     std::vector<uint32_t> olen;
-    uint64_t total = 0;
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride, ctx->d_tmp.as<uint8_t>(), ostride * nblocks, olen, &total, ostride);
+    uint8_t* d_res = ctx->d_tmp.as<uint8_t>();
+    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride,
+                       [&](uint32_t b, uint32_t len, uint8_t** at) {
+                           if ((uint64_t)b * ostride + len > ostride * nblocks) return false;
+                           *at = d_res + (uint64_t)b * ostride;
+                           return true;
+                       },
+                       olen);
     if (rc) return rc;
     if (checksum_bits) {
         std::vector<uint64_t> hoff(nblocks);

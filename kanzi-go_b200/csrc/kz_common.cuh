@@ -114,6 +114,25 @@ struct BitWriter {
     }
 };
 
+// ---- stream records (Writer.processBlock io/CompressedStream.go:951-976, Close :593-594) ----------------------------------
+// Every block of a stream is preceded by 5 bits (lw - 3) and lw bits holding its bit length `written`; the stream ends with
+// END_MARKER_BITS zero bits (a record of length 0). Writes the prefix into p (8 zeroed bytes) and returns its bit count. The one
+// statement of the rule: block_prefix_kernel (single-stream assembly) and the many-stream assembly of kz_api.cu both call it.
+static const uint32_t END_MARKER_BITS = 8;
+KZ_HD uint32_t write_block_prefix(uint8_t* p, uint64_t written) {
+    uint32_t lw = 3;
+    if (written >= 8) lw = log2_floor((uint32_t)(written >> 3)) + 4;
+    BitWriter bw(p);
+    bw.write(lw - 3, 5);
+    if (lw > 32) {
+        bw.write((uint32_t)(written >> 32), lw - 32);
+        bw.write((uint32_t)written, 32);
+    } else {
+        bw.write((uint32_t)written, lw);
+    }
+    return bw.pos;
+}
+
 // ---- per-block descriptor and result of the transform stages TEXT, UTF, EXE, MM, PACK / DNA (ROLZ: result only) ---------
 struct StageBlock {
     uint64_t src_off;   // byte offset of the block in the source buffer

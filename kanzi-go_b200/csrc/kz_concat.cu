@@ -75,19 +75,10 @@ __global__ void block_prefix_kernel(const uint64_t* __restrict__ seg_off, const 
     const uint32_t next_prefix = blk_first[b + 1] - 1;
     const uint64_t written = seg_off[next_prefix] - seg_off[first];
     blk_bits[b] = written;
-    uint32_t lw = 3;
-    if (written >= 8) lw = log2_floor((uint32_t)(written >> 3)) + 4;
     uint8_t* p = prefix_bytes + 8 * (size_t)b;
-    BitWriter bw(p);
-    bw.write(lw - 3, 5);
-    if (lw > 32) {
-        bw.write((uint32_t)(written >> 32), lw - 32);
-        bw.write((uint32_t)written, 32);
-    } else {
-        bw.write((uint32_t)written, lw);
-    }
+    const uint32_t nbits = write_block_prefix(p, written);
     seg_src[first - 1] = (uint64_t)(uintptr_t)p;
-    seg_bits[first - 1] = bw.pos;
+    seg_bits[first - 1] = nbits;
 }
 
 __global__ void concat_zero_kernel(const uint64_t* __restrict__ seg_bits, const uint64_t* __restrict__ seg_dst, int nsegs, uint32_t* __restrict__ dst_words) {
@@ -154,5 +145,29 @@ __global__ void __launch_bounds__(256) extract_copy_kernel(const uint32_t* __res
     for (uint32_t i = threadIdx.x; i < nw; i += blockDim.x) dw[i] = bswap32(bits_at(words, sb + 32ull * i, 32));
     const uint32_t done = head + (nw << 2);
     if (threadIdx.x < n - done) d[done + threadIdx.x] = (uint8_t)bits_at(words, job.src_bit + 8ull * (done + threadIdx.x), 8);
+}
+
+// Device-to-device byte copies (blocks a transform stage declined, decoded blocks to their destination, streams to the caller's buffer).
+// When source and destination share their alignment modulo 16, the body moves in 16-byte words; otherwise byte by byte.
+__global__ void __launch_bounds__(256) batch_copy_kernel(const CopyJob* __restrict__ jobs, int njobs) {
+    const int j = blockIdx.x;
+    if (j >= njobs) return;
+    const CopyJob job = jobs[j];
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(job.src);
+    uint8_t* d = reinterpret_cast<uint8_t*>(job.dst);
+    const uint64_t n = job.len;
+    if (((job.src ^ job.dst) & 15) != 0) {
+        for (uint64_t i = threadIdx.x; i < n; i += blockDim.x) d[i] = s[i];
+        return;
+    }
+    uint64_t head = (16 - (job.dst & 15)) & 15;
+    if (head > n) head = n;
+    if (threadIdx.x < head) d[threadIdx.x] = s[threadIdx.x];
+    const uint64_t nv = (n - head) >> 4;
+    const uint4* sv = reinterpret_cast<const uint4*>(s + head);
+    uint4* dv = reinterpret_cast<uint4*>(d + head);
+    for (uint64_t i = threadIdx.x; i < nv; i += blockDim.x) dv[i] = sv[i];
+    const uint64_t done = head + (nv << 4);
+    if (threadIdx.x < n - done) d[done + threadIdx.x] = s[done + threadIdx.x];
 }
 }  // namespace kz

@@ -141,7 +141,9 @@ struct kz_ctx {
 
     // scratch
     kz::DevBuf d_in, d_out, d_tmp, d_tmp2, d_seg, d_chunks, d_tables, d_enc_tab, d_hdr, d_pay, d_small, d_dl, d_rcp, d_ws, d_lens, d_hist;
-    kz::PinnedBuf h_stage, h_dl;
+    // many-stream entry points: copy lists, pass slots, pass entropy output, compact block bit strings, stream assembly / staging
+    kz::DevBuf d_copy, d_slots, d_enc, d_bits, d_asm;
+    kz::PinnedBuf h_stage, h_dl, h_io;  // h_io: packed inputs / outputs of the host-buffer many-stream entry points
 
     int fail(int code, const std::string& msg) {
         err = msg;
