@@ -185,6 +185,62 @@ size_t kz_profile_names(kz_ctx* ctx, char* buf, size_t cap);
  * 0 (default) = the longest block of the call. kz_decode_blocks and the stream entry points know the value themselves. */
 void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size);
 
+/* ---- streaming sessions: CompressedOutputStream / CompressedInputStream (io/CompressedStream.go:524-710, :1556-1744) for a stream of any
+ *      length, or one that arrives in pieces (a pipe, a socket), in memory that does not grow with the stream ------------------------------
+ * A zlib-style pump. The session takes ctx over until kz_*_free: the caller makes no other call on ctx in between except kz_device_bytes and
+ * kz_last_error (the one-thread-at-a-time rule; one session per context). batch_blocks = blocks per GPU batch (the role of kanzi's `jobs`),
+ * 1 .. 1024; kz_reader_open also takes 0: about 256 MiB of blocks per batch, resolved from the block size in the stream's header.
+ * Bytes: the writer's output, concatenated, is byte for byte what kz_compress_stream writes for the concatenated input with the same
+ *   parameters and input_size_hint, whatever the piece sizes, batch_blocks and output caps. The reader's output is what kz_decompress_stream
+ *   gives for the same stream. Bytes after the end marker are ignored, as kz_decompress_stream ignores them.
+ * Progress: every call consumes or produces at least one byte, or returns an error, except: n == 0 and cap == 0; n == 0 and nothing is in
+ *   flight (all input so far waits in a partly filled slot for more input or for finish); cap == 0 while finished bytes wait to be handed
+ *   out (give the call room). A call may block until the batch in flight ends; it never spins.
+ * Pipeline: each session owns one worker thread (created at open, joined at finish or free), one copy stream and two pinned slots each for
+ *   input and output. The caller's thread fills an input slot, copies it to the device on the copy stream and hands it to the worker, which
+ *   computes on ctx's stream, copies the finished bytes into an output slot and publishes them. So the caller's I/O and the copies of batch
+ *   k + 1 overlap the kernels of batch k.
+ * Memory: device and pinned memory depend only on (block_size, batch_blocks, chain, entropy), never on the stream's length. With
+ *   B = batch_blocks * block_size:
+ *   writer: pinned 2 x B input + 2 x O output, device 2 x B input + O output, O = kz_max_stream_output(B, block_size) + 64; plus the
+ *     context's scratch for one batch of batch_blocks blocks (transform ping-pong buffers, entropy tables), as kz_compress_stream of B bytes.
+ *   reader: pinned 2 x B input + 2 x D output, device 2 x B input, 2 x (kz_max_block_output(block_size) + 64 + B) window (at least one
+ *     maximal record plus one input slot) and D decoded bytes, D = batch_blocks x (max(block_size + max(512, block_size / 16),
+ *     min(max(2048, 1.5 x block_size), 2^30)) + 64), rounded up to 16 per block; plus the context's scratch for one batch. The reader sizes
+ *     its buffers from the stream header.
+ *   kz_device_bytes: the device bytes held by ctx's scratch and an open session's buffers (the sum of their capacities); while a session is
+ *   open, the scratch as it was after the worker's last batch.
+ * Errors: the first failure is sticky: every later call returns the same code, and kz_last_error(ctx) gives its message. The reader gives a
+ *   stream with a single defect (bad header or version, bad block prefix, bad block header, entropy failure, checksum mismatch, failing
+ *   inverse transform, truncation) the code kz_decompress_stream gives for those bytes (given a cap large enough that its record count limit,
+ *   cap / 1024 + 16 records, does not apply). It reports in kz_decompress_stream's order: a block-level failure (block header, entropy
+ *   decode, inverse transform, checksum) is held until the walk over the record prefixes reaches the end marker, since a walk error found
+ *   later (a length past the end of the stream, truncation) takes precedence; among block-level failures the earliest stage wins, then the
+ *   earliest block. Truncation is reported by kz_reader_finish, because until then more input may come. Nothing is handed out after the
+ *   first block-level failure; the blocks decoded before it may have been, and without checksums a corrupt record length is only found
+ *   when the walk fails, so blocks decoded from the records the defect made up may have been handed out too. With checksums on, no block
+ *   whose checksum fails is handed out (nor any block of its batch). A record longer than kz_max_block_output(block_size) bytes fails with
+ *   -KZ_ERR_PROCESS_BLOCK when the reader meets it (the code kz_decompress_stream gives when such a length runs past the end of the stream;
+ *   the reader cannot hold a longer record to find out whether it does). Writing or reading after finish fails with -KZ_ERR_INVALID_PARAM.
+ *   kz_*_free is legal at any point, also with a batch in flight: it joins the worker and leaves ctx usable. kz_destroy with a session open
+ *   closes the session first; its handle then answers -KZ_ERR_INVALID_PARAM and must still be given to kz_*_free. */
+typedef struct kz_writer kz_writer;
+typedef struct kz_reader kz_reader;
+/* Checks the parameters as kz_compress_stream does (unsupported chain or codec: -KZ_ERR_CREATE_CODEC) and allocates every buffer. */
+int kz_writer_open(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t block_size, uint32_t checksum_bits, uint32_t batch_blocks,
+                   int64_t input_size_hint, kz_writer** out);
+/* Consumes up to n bytes of src, writes up to cap finished stream bytes to dst. */
+int kz_writer_write(kz_writer* w, const uint8_t* src, size_t n, size_t* consumed, uint8_t* dst, size_t cap, size_t* produced);
+/* End of input: last (partial) block, end marker. 0 = every byte handed out, 1 = call again with room, < 0 = error. */
+int kz_writer_finish(kz_writer* w, uint8_t* dst, size_t cap, size_t* produced);
+void kz_writer_free(kz_writer* w);
+int kz_reader_open(kz_ctx* ctx, uint32_t batch_blocks, kz_reader** out);
+int kz_reader_read(kz_reader* r, const uint8_t* src, size_t n, size_t* consumed, uint8_t* dst, size_t cap, size_t* produced);
+/* End of input. 0 = end marker seen and all output handed out, 1 = call again with room, < 0 = error (e.g. truncated stream). */
+int kz_reader_finish(kz_reader* r, uint8_t* dst, size_t cap, size_t* produced);
+void kz_reader_free(kz_reader* r);
+size_t kz_device_bytes(kz_ctx* ctx);
+
 #ifdef __cplusplus
 }
 #endif

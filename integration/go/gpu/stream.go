@@ -1,0 +1,177 @@
+// Streaming sessions: an io.WriteCloser / io.Reader over kz_writer_* / kz_reader_*, for a stream of any length or one that arrives from a
+// pipe, in device and pinned memory that follows batchBlocks x blockSize, not the stream's length (the shape of CompressedOutputStream /
+// CompressedInputStream, io/CompressedStream.go:524-710, :1556-1744). Lives at v2/gpu/stream.go. Not compiled (no Go toolchain here).
+package gpu
+
+/*
+#include "kanzi_b200.h"
+*/
+import "C"
+
+import (
+	"io"
+	"unsafe"
+)
+
+const streamBufSize = 4 << 20 // bytes handed to / taken from the pump per call
+
+// StreamWriter compresses everything written to it into w. The session holds c until Close: make no other call on c meanwhile.
+type StreamWriter struct {
+	c      *Context
+	w      io.Writer
+	h      *C.kz_writer
+	out    []byte
+	closed bool
+}
+
+// NewStreamWriter opens a writer session: the bytes written to w are what CompressStream writes for the whole input with the same
+// parameters. batchBlocks in [1..1024] is the role of kanzi's jobs; 0 takes about 256 MiB per batch.
+func NewStreamWriter(c *Context, w io.Writer, transformType uint64, entropyType uint32, blockSize uint32, ckBits uint, batchBlocks uint32,
+	inputSizeHint int64) (*StreamWriter, error) {
+	if batchBlocks == 0 {
+		batchBlocks = uint32(max(1, min(1024, (256<<20)/int(blockSize))))
+	}
+	c.mu.Lock() // held until Close: the session owns the context
+	var h *C.kz_writer
+	rc := C.kz_writer_open(c.h, C.uint64_t(transformType), C.uint32_t(entropyType), C.uint32_t(blockSize), C.uint32_t(ckBits),
+		C.uint32_t(batchBlocks), C.int64_t(inputSizeHint), &h)
+	if rc != 0 {
+		err := c.err(rc)
+		c.mu.Unlock()
+		return nil, err
+	}
+	return &StreamWriter{c: c, w: w, h: h, out: make([]byte, streamBufSize)}, nil
+}
+
+func (s *StreamWriter) Write(p []byte) (int, error) {
+	n := 0
+	for n < len(p) {
+		var used, made C.size_t
+		rc := C.kz_writer_write(s.h, (*C.uint8_t)(unsafe.Pointer(&p[n])), C.size_t(len(p)-n), &used, (*C.uint8_t)(unsafe.Pointer(&s.out[0])),
+			C.size_t(len(s.out)), &made)
+		if rc != 0 {
+			return n, s.c.err(rc)
+		}
+		n += int(used)
+		if made > 0 {
+			if _, err := s.w.Write(s.out[:made]); err != nil {
+				return n, err
+			}
+		}
+	}
+	return n, nil
+}
+
+// Close writes the last block and the end marker, then frees the session and gives c back.
+func (s *StreamWriter) Close() error {
+	if s.closed {
+		return nil
+	}
+	s.closed = true
+	defer s.c.mu.Unlock()
+	defer C.kz_writer_free(s.h)
+	for {
+		var made C.size_t
+		rc := C.kz_writer_finish(s.h, (*C.uint8_t)(unsafe.Pointer(&s.out[0])), C.size_t(len(s.out)), &made)
+		if rc < 0 {
+			return s.c.err(rc)
+		}
+		if made > 0 {
+			if _, err := s.w.Write(s.out[:made]); err != nil {
+				return err
+			}
+		}
+		if rc == 0 {
+			return nil
+		}
+	}
+}
+
+// StreamReader decompresses the stream read from r. The session holds c until the end of the stream or Close. It feeds input only while
+// no decoded bytes are pending, so its own memory stays at two 4 MiB buffers whatever the compression ratio.
+type StreamReader struct {
+	c          *Context
+	r          io.Reader
+	h          *C.kz_reader
+	in, out    []byte
+	inOff, inN int    // s.in[inOff:inN] is read from r and not yet consumed by the session
+	pending    []byte // decoded bytes not yet returned (a slice of s.out)
+	inEOF      bool
+	finished   bool
+	err        error
+}
+
+// NewStreamReader opens a reader session. batchBlocks in [1..1024]; 0 takes about 256 MiB per batch once the stream's block size is known.
+func NewStreamReader(c *Context, r io.Reader, batchBlocks uint32) (*StreamReader, error) {
+	c.mu.Lock()
+	var h *C.kz_reader
+	rc := C.kz_reader_open(c.h, C.uint32_t(batchBlocks), &h)
+	if rc != 0 {
+		err := c.err(rc)
+		c.mu.Unlock()
+		return nil, err
+	}
+	return &StreamReader{c: c, r: r, h: h, in: make([]byte, streamBufSize), out: make([]byte, streamBufSize)}, nil
+}
+
+func (s *StreamReader) Read(p []byte) (int, error) {
+	for len(s.pending) == 0 {
+		if s.err != nil {
+			return 0, s.err
+		}
+		if s.finished {
+			return 0, io.EOF
+		}
+		var made C.size_t
+		if s.inOff < s.inN {
+			var used C.size_t
+			rc := C.kz_reader_read(s.h, (*C.uint8_t)(unsafe.Pointer(&s.in[s.inOff])), C.size_t(s.inN-s.inOff), &used,
+				(*C.uint8_t)(unsafe.Pointer(&s.out[0])), C.size_t(len(s.out)), &made)
+			if rc != 0 {
+				s.fail(rc)
+				return 0, s.err
+			}
+			s.inOff += int(used)
+			s.pending = s.out[:made]
+			continue
+		}
+		if !s.inEOF {
+			k, err := s.r.Read(s.in)
+			if err == io.EOF {
+				s.inEOF = true
+			} else if err != nil {
+				return 0, err
+			}
+			s.inOff, s.inN = 0, k
+			continue
+		}
+		rc := C.kz_reader_finish(s.h, (*C.uint8_t)(unsafe.Pointer(&s.out[0])), C.size_t(len(s.out)), &made)
+		if rc < 0 {
+			s.fail(rc)
+			return 0, s.err
+		}
+		s.pending = s.out[:made]
+		if rc == 0 {
+			s.finished = true
+			s.Close()
+		}
+	}
+	n := copy(p, s.pending)
+	s.pending = s.pending[n:]
+	return n, nil
+}
+
+func (s *StreamReader) fail(rc C.int) {
+	s.err = s.c.err(rc)
+	s.Close()
+}
+
+// Close frees the session (also in the middle of the stream) and gives c back.
+func (s *StreamReader) Close() error {
+	if s.h != nil {
+		C.kz_reader_free(s.h)
+		s.h = nil
+		s.c.mu.Unlock()
+	}
+	return nil
+}

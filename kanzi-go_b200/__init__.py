@@ -37,6 +37,8 @@ ABI_SYMBOLS = [
     "kz_stage_bytes", "kz_profile_names",
     "kz_compress_fragment_device", "kz_stream_header", "kz_concat_bits_device", "kz_stream_index_device", "kz_decompress_fragment_device",
     "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
+    "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
+    "kz_reader_free", "kz_device_bytes",
 ]
 
 
@@ -138,6 +140,18 @@ def load_library(build_if_missing=True):
     L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_writer_open.argtypes = [vp, u64, u32, u32, u32, u32, C.c_int64, C.POINTER(vp)]
+    L.kz_writer_write.argtypes = [vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
+    L.kz_writer_finish.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.kz_writer_free.argtypes = [vp]
+    L.kz_writer_free.restype = None
+    L.kz_reader_open.argtypes = [vp, u32, C.POINTER(vp)]
+    L.kz_reader_read.argtypes = [vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
+    L.kz_reader_finish.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.kz_reader_free.argtypes = [vp]
+    L.kz_reader_free.restype = None
+    L.kz_device_bytes.argtypes = [vp]
+    L.kz_device_bytes.restype = sz
     _lib = L
     return L
 
@@ -400,6 +414,31 @@ class Context:
     def cuda_stream(self):
         return self.lib.kz_cuda_stream(self.h)
 
+    # ---- streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded memory -------------------------------
+    def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0):
+        """A StreamSession: write(data) -> bytes and finish() -> bytes give the stream compress() writes for the concatenated input.
+        batch_blocks=None: about 256 MiB of input per batch."""
+        t48 = transform_type(transform) if isinstance(transform, str) else transform
+        et = entropy_type(entropy) if isinstance(entropy, str) else entropy
+        if batch_blocks is None:
+            batch_blocks = default_batch_blocks(block_size)
+        h = C.c_void_p()
+        self._check(self.lib.kz_writer_open(self.h, t48, et, block_size, checksum_bits, batch_blocks, input_size, C.byref(h)))
+        return StreamSession(self, h, self.lib.kz_writer_write, self.lib.kz_writer_finish, self.lib.kz_writer_free)
+
+    def stream_reader(self, batch_blocks=None):
+        """A StreamSession: write(data) -> decoded bytes and finish() -> the rest. batch_blocks=None: about 256 MiB per batch, resolved
+        from the block size in the stream's header."""
+        if batch_blocks is None:
+            batch_blocks = 0
+        h = C.c_void_p()
+        self._check(self.lib.kz_reader_open(self.h, batch_blocks, C.byref(h)))
+        return StreamSession(self, h, self.lib.kz_reader_read, self.lib.kz_reader_finish, self.lib.kz_reader_free)
+
+    def device_bytes(self):
+        """Device bytes held by this context's scratch and an open session's buffers (kz_device_bytes)."""
+        return int(self.lib.kz_device_bytes(self.h))
+
     # ---- instrumentation ---------------------------------------------------------------------------------------
     def profile(self, on=True):
         self.lib.kz_profile(self.h, 1 if on else 0)
@@ -426,6 +465,68 @@ class Context:
 
     def launch_count(self, reset=False):
         return self.lib.kz_launch_count(self.h, 1 if reset else 0)
+
+
+def default_batch_blocks(block_size):
+    """Blocks per session batch that make about 256 MiB of input, in [1..1024]."""
+    return max(1, min(1024, (256 << 20) // block_size))
+
+
+class StreamSession:
+    """One writer or reader session (Context.stream_writer / stream_reader) driven through its pump. A context manager: leaving the
+    block frees the session, also mid-stream. out_cap: the output buffer each pump call fills."""
+
+    def __init__(self, ctx, h, step, fin, free, out_cap=64 << 20):
+        self.ctx, self.h, self._step, self._fin, self._free = ctx, h, step, fin, free
+        self._out = np.empty(out_cap, np.uint8)
+
+    def _live(self):
+        if self.h is None or self.ctx.h is None:
+            raise KanziError(18, "the session or its context is closed")
+
+    def write(self, data):
+        """Hands data to the session -> the finished bytes it gave back meanwhile."""
+        self._live()
+        a = _u8(data)
+        parts, pos = [], 0
+        used, made = C.c_size_t(0), C.c_size_t(0)
+        while pos < a.size:  # bytes still in flight at the end come out of a later write() or finish()
+            self.ctx._check(self._step(self.h, a.ctypes.data + pos, a.size - pos, C.byref(used), self._out.ctypes.data, self._out.size, C.byref(made)))
+            pos += used.value
+            if made.value:
+                parts.append(self._out[: made.value].copy())
+        return np.concatenate(parts) if parts else np.zeros(0, np.uint8)
+
+    def finish(self):
+        """End of input -> every remaining byte."""
+        self._live()
+        parts = []
+        made = C.c_size_t(0)
+        while True:
+            rc = self.ctx._check(self._fin(self.h, self._out.ctypes.data, self._out.size, C.byref(made)))
+            if made.value:
+                parts.append(self._out[: made.value].copy())
+            if rc == 0:
+                break
+        return np.concatenate(parts) if parts else np.zeros(0, np.uint8)
+
+    def close(self):
+        """Frees the session; legal after the context was closed too (kz_destroy closed the session then)."""
+        if self.h:
+            self._free(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 _default_ctx = None

@@ -26,8 +26,11 @@
 #include "kz_exe.cuh"
 #include "kz_stream_plan.h"
 
+#include <condition_variable>
 #include <map>
 #include <memory>
+#include <mutex>
+#include <thread>
 #include <tuple>
 
 using namespace kz;
@@ -316,16 +319,19 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
     CK(ctx->d_small.ensure(small_size));
     uint8_t* d_small = ctx->d_small.as<uint8_t>();
     std::vector<uint8_t> key;
+    // a streaming writer's leading segment (header, then the carry) changes from batch to batch: it stays out of the key and is
+    // written into the kept tables below
+    const bool lead = ctx->volatile_lead && layout == LAYOUT_STREAM;
     {
         auto put = [&](const void* p, size_t n) {
             const uint8_t* q = (const uint8_t*)p;
             key.insert(key.end(), q, q + n);
         };
-        const uint64_t scal[8] = {(uint64_t)layout | (ctx->fragment ? 0x100u : 0u), etype, checksum_bits, (uint64_t)(uintptr_t)d_data, (uint64_t)(uintptr_t)d_small, (uint64_t)nblocks,
-                                  stream_hdr_bits, (uint64_t)stream_hdr.size()};
+        const uint64_t scal[8] = {(uint64_t)layout | (ctx->fragment ? 0x100u : 0u) | (lead ? 0x200u : 0u), etype, checksum_bits, (uint64_t)(uintptr_t)d_data,
+                                  (uint64_t)(uintptr_t)d_small, (uint64_t)nblocks, lead ? 0 : stream_hdr_bits, (uint64_t)stream_hdr.size()};
         key.reserve(sizeof(scal) + stream_hdr.size() + jobs.size() * 40 + blk_base_bits.size() * 8);
         put(scal, sizeof(scal));
-        put(stream_hdr.data(), stream_hdr.size());
+        if (!lead) put(stream_hdr.data(), stream_hdr.size());
         for (const EncJob& j : jobs) {
             const uint64_t f[4] = {j.data_off, ((uint64_t)j.post_len << 32) | j.ntransforms, ((uint64_t)j.skip_flags << 8) | (j.copy ? 1u : 0u), j.checksum};
             put(f, sizeof(f));
@@ -445,6 +451,10 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
         });
     }
     Packer& pk = plan.pk;
+    if (lead) {  // segment 0 is the leading segment; its bytes sit at the start of the small strings
+        memcpy(pk.bytes.data() + plan.o_small + small_hdr_off, stream_hdr.data(), std::min<size_t>(stream_hdr.size(), small_blk_off));
+        memcpy(pk.bytes.data() + plan.o_bits, &stream_hdr_bits, 8);
+    }
     const int nsegs = plan.nsegs, nchunks = plan.nchunks;
     const size_t o_small = plan.o_small, o_src = plan.o_src, o_bits = plan.o_bits, o_first = plan.o_first, o_chunks = plan.o_chunks, o_cseg = plan.o_cseg,
                  o_base = plan.o_base, o_off = plan.o_off, o_dst = plan.o_dst, o_blkbits = plan.o_blkbits, o_total = plan.o_total, o_hbits = plan.o_hbits,
@@ -621,14 +631,7 @@ __global__ void stream_walk_kernel(const uint32_t* __restrict__ words, const Wal
     int32_t st = 0;
     for (;;) {
         if (stop_after && n == stop_after) break;
-        const uint32_t lr = br.read(5) + 3;
-        uint64_t len;
-        if (lr > 32) {
-            uint64_t hi = br.read(lr - 32);
-            len = (hi << 32) | br.read(32);
-        } else {
-            len = br.read(lr);
-        }
+        const uint64_t len = read_block_prefix(br);
         if (br.overrun) {
             st = -KZ_E_PROCESS_BLOCK;
             break;
@@ -653,6 +656,12 @@ __global__ void stream_walk_kernel(const uint32_t* __restrict__ words, const Wal
     }
     count_status[2 * s] = n;
     count_status[2 * s + 1] = (uint32_t)st;
+}
+
+// The streaming reader's walk over its window (walk_records), one thread.
+__global__ void record_walk_kernel(const uint32_t* __restrict__ words, uint64_t start, uint64_t end, uint32_t max_records, uint64_t max_bits,
+                                   uint64_t* __restrict__ bit_off, uint64_t* __restrict__ bits, WalkResult* __restrict__ out) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) *out = walk_records(words, start, end, max_records, max_bits, bit_off, bits);
 }
 
 // jobs[b].bit_off / bits / out_off must be set; fills pre_len, mode, ..., status. d_words = device stream buffer.
@@ -1625,12 +1634,11 @@ int kz_init(int device, kz_ctx** out) {
 void kz_destroy(kz_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
+    if (ctx->session) close_session(ctx->session);
     cudaStreamSynchronize(ctx->stream);
     drain_profile(ctx);
     for (auto e : ctx->event_pool) cudaEventDestroy(e);
-    DevBuf* bufs[] = {&ctx->d_in, &ctx->d_out, &ctx->d_tmp, &ctx->d_tmp2, &ctx->d_seg, &ctx->d_chunks, &ctx->d_tables, &ctx->d_enc_tab, &ctx->d_hdr, &ctx->d_pay, &ctx->d_small, &ctx->d_dl, &ctx->d_rcp, &ctx->d_ws, &ctx->d_lens, &ctx->d_hist,
-                      &ctx->d_copy, &ctx->d_slots, &ctx->d_enc, &ctx->d_bits, &ctx->d_asm};
-    for (auto b : bufs) b->release();
+    ctx->each_dev_buf([](DevBuf& b) { b.release(); });
     ctx->h_stage.release();
     ctx->h_dl.release();
     ctx->h_io.release();
@@ -1727,6 +1735,8 @@ size_t kz_transform_max_encoded_len(uint64_t type, size_t n) {
 // ---- whole stream, device resident ---------------------------------------------------------------------------
 static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size, const void* d_src,
                                 size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits);
+static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src,
+                                size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res);
 int kz_compress_stream_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size,
                               const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, out_n, false, nullptr);
@@ -1747,11 +1757,31 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
     if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
     if (((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    const uint32_t nblocks = (uint32_t)((n + block_size - 1) / block_size);
-    std::vector<EncJob> jobs;
     TransformPlan plan;
     int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
     if (rc) return rc;
+    std::vector<uint8_t> hdr;
+    uint32_t hdr_bits = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size);
+    if (fragment) hdr_bits = 0;
+    EncResult res;
+    ctx->fragment = fragment;
+    rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, d_src, n, hdr, hdr_bits, d_dst, cap, res);
+    ctx->fragment = false;
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    *out_n = (size_t)((res.total_bits + 7) / 8);
+    if (out_bits) *out_bits = res.total_bits;
+    return 0;
+}
+
+// What compress_device_impl runs on the n bytes at d_src, cut into blocks of block_size: the initial dataType of every block from its magic
+// number, the forward transforms, the block checksums and the LAYOUT_STREAM encode behind the leading segment `lead` (lead_bits bits: the
+// stream header, or a writer session's carry). A writer session runs every batch of its stream through it.
+static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src,
+                                size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res) {
+    const uint32_t nblocks = (uint32_t)((n + block_size - 1) / block_size);
+    std::vector<EncJob> jobs;
+    int rc = 0;
     const uint8_t* d_data = nullptr;
     std::vector<int32_t> init_dt;
     if (plan.uses_magic() && nblocks) {  // the first four bytes of every block decide its initial data type
@@ -1778,18 +1808,7 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
         if (rc) return rc;
         for (uint32_t b = 0; b < nblocks; b++) jobs[b].checksum = hv[b];
     }
-    std::vector<uint8_t> hdr;
-    uint32_t hdr_bits = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size);
-    if (fragment) hdr_bits = 0;
-    EncResult res;
-    ctx->fragment = fragment;
-    rc = encode_batch(ctx, LAYOUT_STREAM, etype, checksum_bits, d_data, jobs, hdr, hdr_bits, (uint8_t*)d_dst, cap, {}, res);
-    ctx->fragment = false;
-    if (rc) return rc;
-    CK(cudaStreamSynchronize(ctx->stream));
-    *out_n = (size_t)((res.total_bits + 7) / 8);
-    if (out_bits) *out_bits = res.total_bits;
-    return 0;
+    return encode_batch(ctx, LAYOUT_STREAM, etype, checksum_bits, d_data, jobs, lead, lead_bits, (uint8_t*)d_dst, cap, {}, res);
 }
 
 // Stream header bytes (Writer.writeHeader, io/CompressedStream.go:429-519) for the rank that commits a sharded stream. out: >= 32 bytes.
@@ -2834,6 +2853,677 @@ int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t 
     CK(cudaStreamSynchronize(ctx->stream));
     *out_n = len[0];
     return 0;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------
+// Streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded device and pinned memory, the role of
+// CompressedOutputStream / CompressedInputStream (io/CompressedStream.go:524-710, :1556-1744), which cut `jobs` blocks per batch.
+// ------------------------------------------------------------------------------------------------------------
+namespace kz {
+
+const int SESSION_STOPPED = 1;                 // a worker step that saw the session being freed
+const uint64_t READER_BATCH_BYTES = 256ull << 20;  // kz_reader_open with batch_blocks 0: about this many decoded bytes per batch
+
+// The pump both sessions share. The caller's thread fills pinned input slot (given % 2), issues its host-to-device copy on `copy` and
+// hands it to the worker; the worker is the only thread that drives ctx while the session is open: it waits on the slot's event on
+// ctx->stream, computes, copies the finished bytes into pinned output slot (made % 2) and publishes them; the caller's thread hands them
+// out. So the caller's I/O and the copies of batch k + 1 overlap the kernels of batch k. All counters are guarded by m.
+struct Session {
+    kz_ctx* ctx;
+    uint32_t batch_blocks;
+    std::thread worker;
+    std::mutex m;
+    std::condition_variable cv;
+    cudaStream_t copy = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    PinnedBuf h_in[2], h_out[2];
+    DevBuf d_in[2];
+    size_t in_cap = 0;                        // bytes per input slot
+    size_t in_len[2] = {0, 0};                // filled bytes of each input slot
+    bool in_last[2] = {false, false};
+    size_t out_len[2] = {0, 0}, out_pos = 0;  // published bytes of each output slot, bytes of slot (taken % 2) handed out
+    uint64_t given = 0, done = 0;             // input slots handed to the worker / finished by it
+    uint64_t made = 0, taken = 0;             // output slots published / handed out completely
+    bool last_given = false, finished = false, stop = false;
+    int err = 0;                              // sticky: 0 or -(error code)
+    size_t scratch = 0;                       // ctx->scratch_bytes() after the worker's last step
+
+    explicit Session(kz_ctx* c, uint32_t bb) : ctx(c), batch_blocks(bb) {}
+    virtual ~Session() {}
+    virtual int run(int k, bool last) = 0;  // worker: input slot k
+    virtual size_t own_device_bytes() = 0;
+    virtual void release_own() = 0;
+
+    int open_common() {
+        if (cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking) != cudaSuccess) return ctx->fail(KZ_ERR_CREATE_COMPRESSOR, "cannot create the copy stream");
+        for (auto& e : ev)
+            if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return ctx->fail(KZ_ERR_CREATE_COMPRESSOR, "cannot create events");
+        scratch = ctx->scratch_bytes();
+        ctx->session = this;
+        worker = std::thread([this] { main(); });
+        return 0;
+    }
+    int alloc_inputs(size_t cap) {
+        in_cap = cap;
+        for (int k = 0; k < 2; k++) {
+            CK(h_in[k].ensure(cap));
+            CK(d_in[k].ensure(cap));
+        }
+        return 0;
+    }
+
+    void main() {
+        cudaSetDevice(ctx->device);
+        for (;;) {
+            int k;
+            bool last;
+            {
+                std::unique_lock<std::mutex> l(m);
+                cv.wait(l, [&] { return stop || done < given; });
+                if (stop) return;
+                k = (int)(done % 2);
+                last = in_last[k];
+            }
+            int rc = run(k, last);
+            std::lock_guard<std::mutex> l(m);
+            scratch = ctx->scratch_bytes();
+            in_len[k] = 0;
+            done++;
+            if (rc < 0 && !err) err = rc;
+            if (rc == 0 && last) finished = true;
+            cv.notify_all();
+            if (rc || last) return;
+        }
+    }
+
+    // worker: copies copy_n finished bytes at d_src into the next free output slot and publishes the first give_n of them; *tail = the
+    // byte behind them (the writer's carry)
+    int publish(const void* d_src, size_t copy_n, size_t give_n, uint8_t* tail = nullptr) {
+        if (copy_n == 0) return 0;
+        int j;
+        {
+            std::unique_lock<std::mutex> l(m);
+            cv.wait(l, [&] { return stop || made - taken < 2; });
+            if (stop) return SESSION_STOPPED;
+            j = (int)(made % 2);
+        }
+        CK(cudaMemcpyAsync(h_out[j].p, d_src, copy_n, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (tail) *tail = give_n < copy_n ? ((const uint8_t*)h_out[j].p)[give_n] : 0;
+        std::lock_guard<std::mutex> l(m);
+        out_len[j] = give_n;
+        made++;
+        cv.notify_all();
+        return 0;
+    }
+
+    // caller: a failure found on the caller's side; the worker is joined before ctx is touched
+    int fail(int code, const std::string& msg) {
+        bool mine = false;
+        {
+            std::lock_guard<std::mutex> l(m);
+            if (!err) {
+                err = -code;
+                mine = true;
+            }
+            stop = true;
+            cv.notify_all();
+        }
+        if (worker.joinable()) worker.join();
+        if (mine) ctx->err = msg;
+        return err;
+    }
+    int cuda_fail(cudaError_t e, const char* what) { return fail(KZ_ERR_PROCESS_BLOCK, std::string(what) + ": " + cudaGetErrorString(e)); }
+
+    // caller: hands out published bytes; returns the count
+    size_t take(uint8_t* dst, size_t cap) {
+        size_t got = 0;
+        for (;;) {
+            int j;
+            size_t avail;
+            {
+                std::lock_guard<std::mutex> l(m);
+                if (taken == made) return got;
+                j = (int)(taken % 2);
+                avail = out_len[j] - out_pos;
+                if (avail == 0 || got == cap) {
+                    if (avail == 0) {
+                        out_pos = 0;
+                        taken++;
+                        cv.notify_all();
+                        continue;
+                    }
+                    return got;
+                }
+            }
+            const size_t c = std::min(avail, cap - got);
+            memcpy(dst + got, (const uint8_t*)h_out[j].p + out_pos, c);
+            got += c;
+            out_pos += c;
+        }
+    }
+    bool slot_free() {
+        std::lock_guard<std::mutex> l(m);
+        return given - done < 2;
+    }
+    // caller: hands input slot k (filled) to the worker
+    int give(int k, bool last) {
+        if (in_len[k]) {
+            cudaError_t e = cudaMemcpyAsync(d_in[k].p, h_in[k].p, in_len[k], cudaMemcpyHostToDevice, copy);
+            if (e != cudaSuccess) return cuda_fail(e, "session input copy");
+        }
+        cudaError_t e = cudaEventRecord(ev[k], copy);
+        if (e != cudaSuccess) return cuda_fail(e, "session input event");
+        std::lock_guard<std::mutex> l(m);
+        in_last[k] = last;
+        given++;
+        if (last) last_given = true;
+        cv.notify_all();
+        return 0;
+    }
+    // caller: copies up to n bytes into the input slots, handing over every full one; returns the count or a negative error
+    int64_t feed(const uint8_t* src, size_t n) {
+        size_t c = 0;
+        while (c < n && slot_free()) {
+            const int k = (int)(given % 2);
+            const size_t t = std::min(n - c, in_cap - in_len[k]);
+            memcpy((uint8_t*)h_in[k].p + in_len[k], src + c, t);
+            in_len[k] += t;
+            c += t;
+            if (in_len[k] == in_cap) {
+                int rc = give(k, false);
+                if (rc) return rc;
+            }
+        }
+        return (int64_t)c;
+    }
+    // caller: nothing could be done without waiting. 1 = return to the caller empty-handed (nothing in flight that could change it)
+    int wait_for_worker(bool have_input, bool have_room) {
+        std::unique_lock<std::mutex> l(m);
+        if (err) return err;
+        if (!have_room && taken < made) return 1;  // finished bytes wait for room
+        if (!have_input && done == given) return 1;
+        const uint64_t d0 = done, m0 = made;
+        cv.wait(l, [&] { return err || done != d0 || made != m0; });
+        return err;
+    }
+
+    // the zlib-style pump of write / read: consume or produce at least one byte unless nothing can happen
+    int pump(const uint8_t* src, size_t n, size_t* consumed, uint8_t* dst, size_t cap, size_t* produced) {
+        for (;;) {
+            bool lg;
+            {
+                std::lock_guard<std::mutex> l(m);
+                if (err) return err;
+                lg = last_given;
+            }
+            if (lg) return fail(KZ_ERR_INVALID_PARAM, "session: write or read after finish");
+            *produced += take(dst + *produced, cap - *produced);
+            int64_t c = accept(src + *consumed, n - *consumed);
+            if (c < 0) return (int)c;
+            *consumed += (size_t)c;
+            if (*consumed || *produced || (n == 0 && cap == 0)) return 0;
+            int rc = wait_for_worker(n > 0, cap > 0);
+            if (rc < 0) return rc;
+            if (rc == 1) return 0;
+        }
+    }
+    // end of input: 0 = every byte handed out, 1 = call again with room
+    int finish(uint8_t* dst, size_t cap, size_t* produced) {
+        for (;;) {
+            {
+                std::lock_guard<std::mutex> l(m);
+                if (err) return err;
+            }
+            *produced += take(dst + *produced, cap - *produced);
+            bool lg;
+            {
+                std::lock_guard<std::mutex> l(m);
+                lg = last_given;
+            }
+            if (!lg && slot_free()) {
+                int rc = hand_last();
+                if (rc) return rc;
+            }
+            std::unique_lock<std::mutex> l(m);
+            if (err) return err;
+            if (finished && taken == made) return 0;
+            if (*produced == cap) return 1;
+            if (taken < made) continue;
+            const uint64_t d0 = done, m0 = made;
+            cv.wait(l, [&] { return err || done != d0 || made != m0; });
+        }
+    }
+    virtual int64_t accept(const uint8_t* src, size_t n) { return feed(src, n); }
+    virtual int hand_last() { return give((int)(given % 2), true); }
+
+    // kz_*_free: joins the worker (after the step in flight), waits for the copies in flight and leaves ctx usable
+    void close() {
+        {
+            std::lock_guard<std::mutex> l(m);
+            stop = true;
+            cv.notify_all();
+        }
+        if (worker.joinable()) worker.join();
+        cudaSetDevice(ctx->device);
+        if (copy) cudaStreamSynchronize(copy);
+        cudaStreamSynchronize(ctx->stream);
+        ctx->fragment = false;
+        ctx->volatile_lead = false;
+        for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        if (copy) cudaStreamDestroy(copy);
+        for (int k = 0; k < 2; k++) {
+            h_in[k].release();
+            h_out[k].release();
+            d_in[k].release();
+        }
+        release_own();
+        if (ctx->session == this) ctx->session = nullptr;
+        ctx = nullptr;  // closed: only kz_*_free may follow
+    }
+    size_t device_bytes() {
+        std::lock_guard<std::mutex> l(m);
+        return scratch + d_in[0].cap + d_in[1].cap + own_device_bytes();
+    }
+};
+
+// kz_destroy with a session open: the session is closed first; its handle is then only good for kz_*_free
+void close_session(Session* s) { s->close(); }
+
+}  // namespace kz
+
+struct kz_writer : kz::Session {
+    TransformPlan plan;
+    uint64_t t48 = 0;
+    uint32_t etype = 0, block_size = 0, checksum_bits = 0;
+    int64_t input_size = 0;
+    DevBuf d_out;            // the finished bytes of one batch
+    size_t out_cap = 0;
+    uint64_t batches = 0;    // batches encoded (worker)
+    uint8_t carry = 0;       // the last total_bits mod 8 bits of the previous batch, MSB first (worker)
+    uint32_t carry_bits = 0;
+
+    using Session::Session;
+    size_t own_device_bytes() override { return d_out.cap; }
+    void release_own() override { d_out.release(); }
+
+    // worker: one batch = the blocks of input slot k behind the stream header (first batch) or the carry; the end marker only in the last
+    int run(int k, bool last) override {
+        CK(cudaStreamWaitEvent(ctx->stream, ev[k], 0));
+        std::vector<uint8_t> lead(64, 0);
+        uint32_t lead_bits = carry_bits;
+        if (batches == 0) lead_bits = build_stream_header(lead, t48, etype, block_size, checksum_bits, input_size);
+        else lead[0] = carry;
+        EncResult res;
+        ctx->stream_bs = block_size;
+        ctx->fragment = !last;
+        ctx->volatile_lead = true;
+        int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, d_in[k].p, in_len[k], lead, lead_bits, d_out.p, out_cap, res);
+        ctx->fragment = false;
+        ctx->volatile_lead = false;
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));
+        batches++;
+        const uint64_t give_n = batch_bytes_out(res.total_bits, last, &carry_bits);
+        return publish(d_out.p, (size_t)((res.total_bits + 7) / 8), (size_t)give_n, &carry);
+    }
+};
+
+struct kz_reader : kz::Session {
+    StreamHeader sh;
+    TransformPlan plan;
+    uint8_t head[64];
+    size_t head_len = 0;
+    bool have_header = false;
+    DevBuf win[2], d_dec, d_walk;  // window buffers (the unconsumed bits move between them), decoded bytes of one batch, walk results
+    size_t win_cap = 0, dec_cap = 0;
+    uint64_t pstride_max = 0, max_rec_bits = 0;
+    // worker state
+    int cur = 0;
+    uint64_t fill = 0, start_bit = 0;  // valid bytes of win[cur], first bit not yet walked
+    bool ended = false;                // the end marker was read (guarded by m: the caller drops input after it)
+    bool odd_tail = false;             // NONE: the last block handed out has a length that is not a multiple of 16
+
+    using Session::Session;
+    size_t own_device_bytes() override { return win[0].cap + win[1].cap + d_dec.cap + d_walk.cap; }
+    void release_own() override {
+        win[0].release();
+        win[1].release();
+        d_dec.release();
+        d_walk.release();
+    }
+
+    // caller: the stream header is parsed from the first 64 bytes (or fewer at finish, as kz_decompress_stream does); the buffers are
+    // sized from it
+    int start() {
+        int rc = parse_stream_header(ctx, head, head_len, sh);
+        if (rc == 0) rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_INVALID_CODEC);
+        if (rc) return fail(-rc, ctx->err);
+        const uint64_t bs = sh.block_size;
+        if (batch_blocks == 0) batch_blocks = (uint32_t)std::min<uint64_t>(1024, std::max<uint64_t>(1, READER_BATCH_BYTES / bs));
+        // Reader.processBlock :1649-1653 and parse_block_header's bound on a block's pre-transform length
+        const uint64_t max_len = std::min<uint64_t>(std::max<uint64_t>(2048, bs + bs / 2), 1ull << 30);
+        pstride_max = (std::max<uint64_t>(max_len, bs + std::max<uint64_t>(512, bs >> 4)) + 64 + 15) & ~15ull;
+        max_rec_bits = 8ull * kz_max_block_output(bs);
+        dec_cap = (size_t)(batch_blocks * pstride_max);
+        const size_t in_bytes = (size_t)batch_blocks * bs;
+        win_cap = (size_t)(max_rec_bits / 8 + 64 + in_bytes);
+        cudaError_t e = cudaSuccess;
+        for (int k = 0; k < 2 && e == cudaSuccess; k++) {
+            e = h_in[k].ensure(in_bytes);
+            if (e == cudaSuccess) e = d_in[k].ensure(in_bytes);
+            if (e == cudaSuccess) e = h_out[k].ensure(dec_cap);
+            if (e == cudaSuccess) e = win[k].ensure(win_cap);
+        }
+        if (e == cudaSuccess) e = d_dec.ensure(dec_cap);
+        if (e == cudaSuccess) e = d_walk.ensure((size_t)batch_blocks * 16 + sizeof(WalkResult) + 64);
+        if (e != cudaSuccess) return cuda_fail(e, "session buffers");
+        in_cap = in_bytes;
+        start_bit = sh.bits;
+        have_header = true;
+        memcpy(h_in[0].p, head, head_len);  // slot 0 is the first one filled (in_cap >= 1024 > head_len)
+        in_len[0] = head_len;
+        return 0;
+    }
+    int64_t accept(const uint8_t* src, size_t n) override {
+        size_t c = 0;
+        if (!have_header) {
+            c = std::min(n, sizeof(head) - head_len);
+            memcpy(head + head_len, src, c);
+            head_len += c;
+            if (head_len < sizeof(head)) return (int64_t)c;
+            int rc = start();
+            if (rc) return rc;
+        }
+        {
+            std::lock_guard<std::mutex> l(m);
+            if (ended) return (int64_t)n;  // bytes behind the end marker are ignored
+        }
+        int64_t f = feed(src + c, n - c);
+        return f < 0 ? f : (int64_t)c + f;
+    }
+    int hand_last() override {
+        if (!have_header) {
+            int rc = start();
+            if (rc) return rc;
+        }
+        return give((int)(given % 2), true);
+    }
+
+    // worker: appends input slot k to the window, then walks and decodes every complete record, batch_blocks at a time
+    int run(int k, bool last) override {
+        bool end_seen;
+        {
+            std::lock_guard<std::mutex> l(m);
+            end_seen = ended;
+        }
+        if (!end_seen) {
+            CK(cudaStreamWaitEvent(ctx->stream, ev[k], 0));
+            if (fill + in_len[k] + 64 > win[cur].cap) return ctx->fail(KZ_ERR_UNKNOWN, "internal: reader window overflow");
+            CopyList cl;
+            cl.add(d_in[k].p, win[cur].as<uint8_t>() + fill, in_len[k]);
+            int rc = run_copies(ctx, cl);
+            if (rc) return rc;
+            fill += in_len[k];
+            rc = walk_and_decode();
+            if (rc) return rc;
+            {
+                std::lock_guard<std::mutex> l(m);
+                end_seen = ended;
+            }
+            if (!end_seen) {  // the unconsumed bits move to the start of the other window buffer (from a 16-byte boundary)
+                const uint64_t from = (start_bit / 8) & ~15ull;
+                CopyList tail;
+                tail.add(win[cur].as<uint8_t>() + from, win[cur ^ 1].as<uint8_t>(), fill - from);
+                rc = run_copies(ctx, tail);
+                if (rc) return rc;
+                CK(cudaStreamSynchronize(ctx->stream));
+                cur ^= 1;
+                fill -= from;
+                start_bit -= 8 * from;
+            }
+        }
+        CK(cudaStreamSynchronize(ctx->stream));  // input slot k is free again
+        if (last && !end_seen) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "Invalid bitstream: truncated stream");
+        return 0;
+    }
+
+    int walk_and_decode() {
+        const uint32_t* W = win[cur].as<uint32_t>();
+        uint64_t* d_boff = d_walk.as<uint64_t>();
+        uint64_t* d_bbits = d_boff + batch_blocks;
+        WalkResult* d_res = (WalkResult*)(d_bbits + batch_blocks);
+        std::vector<uint64_t> boff(batch_blocks), bbits(batch_blocks);
+        for (;;) {
+            {
+                LaunchScope ls(ctx, "record_walk");
+                record_walk_kernel<<<1, 1, 0, ctx->stream>>>(W, start_bit, 8 * fill, batch_blocks, max_rec_bits, d_boff, d_bbits, d_res);
+            }
+            CK(cudaGetLastError());
+            WalkResult r;
+            CK(cudaMemcpyAsync(&r, d_res, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(boff.data(), d_boff, (size_t)batch_blocks * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(bbits.data(), d_bbits, (size_t)batch_blocks * 8, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            if (r.status) return ctx->fail(-r.status, "Invalid bitstream: corrupted block length");
+            if (r.count) {
+                int rc = decode(r.count, boff, bbits);
+                if (rc) return rc;
+            }
+            start_bit = r.next_bit;
+            if (r.ended) {
+                {
+                    std::lock_guard<std::mutex> l(m);
+                    ended = true;
+                }
+                return pend_stage == STAGE_NONE ? 0 : ctx->fail(-pend_code, pend_msg);
+            }
+            if (r.count < batch_blocks) return 0;
+        }
+    }
+
+    // A block-level failure (block header, entropy decode, inverse transform, checksum) is not reported when it is found:
+    // decompress_device_impl walks every record of the stream before it decodes any, so a walk error (a length over the limits, a
+    // truncated stream) found later takes precedence, and after the walk the failure of the earliest stage wins (headers of every block,
+    // then entropy decode, inverse transforms, checksums), the earliest block within a stage. The reader keeps the failure that wins so
+    // far, hands out nothing more, runs each later batch only through the stages whose failures could still win, and reports at the end
+    // marker or at the walk error.
+    enum { STAGE_NONE = 0, STAGE_HEADER = 1, STAGE_DECODE = 2, STAGE_INVERSE = 3, STAGE_CHECKSUM = 4 };
+    int pend_stage = STAGE_NONE, pend_code = 0;
+    std::string pend_msg;
+    void note(int stage, int rc) {  // rc = -(error code); ctx->err holds its message
+        if (pend_stage != STAGE_NONE && stage >= pend_stage) return;
+        pend_stage = stage;
+        pend_code = rc;
+        pend_msg = ctx->err;
+    }
+    int note_fail(int stage, int code, const char* msg) {
+        note(stage, ctx->fail(code, msg));
+        return 0;
+    }
+
+    // the records of one batch, as decompress_device_impl decodes a whole stream; the decoded bytes are published back to back
+    int decode(uint32_t nb, const std::vector<uint64_t>& boff, const std::vector<uint64_t>& bbits) {
+        if (pend_stage == STAGE_HEADER) return 0;  // only a walk error could still win
+        const uint32_t* W = win[cur].as<uint32_t>();
+        const uint64_t words_len = (fill + 3) / 4 + 16;
+        std::vector<DecJob> jobs(nb);
+        for (uint32_t b = 0; b < nb; b++) {
+            jobs[b] = DecJob();
+            jobs[b].bit_off = boff[b];
+            jobs[b].bits = bbits[b];
+        }
+        ctx->stream_bs = sh.block_size;
+        int rc = decode_parse_headers(ctx, W, jobs, sh.checksum_bits, sh.block_size);
+        if (rc) return rc;
+        uint64_t total = 0;
+        std::vector<uint32_t> olen(nb);
+        uint64_t pstride = 0;
+        // headers (and, for NONE, the rule that every block but the stream's last is a multiple of 16 long: the last block of the
+        // previous batch was not the last one), in block order as decompress_device_impl checks them
+        if (plan.none() && odd_tail) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+        uint32_t max_pre = 0;
+        for (uint32_t b = 0; b < nb; b++) {
+            if (jobs[b].status) return note_fail(STAGE_HEADER, -jobs[b].status, "Invalid compressed block header");
+            if (plan.none()) {
+                jobs[b].out_off = total;
+                total += jobs[b].pre_len;
+                olen[b] = jobs[b].pre_len;
+                if (b + 1 < nb && (jobs[b].pre_len & 15)) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+            }
+            max_pre = std::max(max_pre, jobs[b].pre_len);
+        }
+        if (plan.none()) odd_tail = (jobs[nb - 1].pre_len & 15) != 0;
+        if (pend_stage == STAGE_DECODE) return 0;
+        uint8_t* d_ent = d_dec.as<uint8_t>();
+        if (!plan.none()) {
+            const uint64_t blk_room = std::max<uint64_t>(max_pre, (uint64_t)sh.block_size + std::max<uint64_t>(512, sh.block_size >> 4));
+            pstride = (blk_room + 64 + 15) & ~15ull;
+            CK(ctx->d_tmp.ensure(pstride * nb + 64));
+            for (uint32_t b = 0; b < nb; b++) jobs[b].out_off = (uint64_t)b * pstride;
+            d_ent = ctx->d_tmp.as<uint8_t>();
+        }
+        rc = decode_batch(ctx, sh.etype, W, words_len, jobs, d_ent);
+        if (rc) {
+            note(STAGE_DECODE, rc);
+            return 0;
+        }
+        for (uint32_t b = 0; b < nb; b++)
+            if (jobs[b].status) return note_fail(STAGE_DECODE, -jobs[b].status, "Invalid bitstream: block decoding failed");
+        if (pend_stage == STAGE_INVERSE) return 0;
+        if (!plan.none()) {
+            BackToBack place{d_dec.as<uint8_t>(), dec_cap};
+            rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen);
+            if (rc) {
+                note(STAGE_INVERSE, rc);
+                return 0;
+            }
+            total = place.off;
+        }
+        if (pend_stage == STAGE_CHECKSUM) return 0;
+        if (sh.checksum_bits) {  // before anything of the batch is handed out
+            std::vector<uint64_t> hoff(nb);
+            uint64_t o = 0;
+            for (uint32_t b = 0; b < nb; b++) {
+                hoff[b] = o;
+                o += olen[b];
+            }
+            rc = verify_checksums(ctx, d_dec.as<uint8_t>(), hoff, olen, sh.checksum_bits, jobs);
+            if (rc == -KZ_ERR_CRC_CHECK) {
+                note(STAGE_CHECKSUM, rc);
+                return 0;
+            }
+            if (rc) return rc;
+        }
+        return publish(d_dec.p, (size_t)total, (size_t)total);
+    }
+};
+
+extern "C" {
+
+int kz_writer_open(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t batch_blocks, int64_t input_size_hint,
+                   kz_writer** out) {
+    if (!ctx || !out) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is already open on this context");
+    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
+    if (batch_blocks < 1 || batch_blocks > 1024) return ctx->fail(KZ_ERR_INVALID_PARAM, "batch_blocks must be in [1..1024]");
+    if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+    TransformPlan plan;
+    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    kz_writer* w = new kz_writer(ctx, batch_blocks);
+    w->plan = plan;
+    w->t48 = t48;
+    w->etype = etype;
+    w->block_size = block_size;
+    w->checksum_bits = checksum_bits;
+    w->input_size = input_size_hint;
+    const size_t in_bytes = (size_t)batch_blocks * block_size;
+    w->out_cap = kz_max_stream_output(in_bytes, block_size) + 64;
+    rc = w->alloc_inputs(in_bytes);
+    for (int k = 0; k < 2 && rc == 0; k++)
+        if (w->h_out[k].ensure(w->out_cap) != cudaSuccess) rc = ctx->fail(KZ_ERR_CREATE_COMPRESSOR, "cannot allocate pinned output slots");
+    if (rc == 0 && w->d_out.ensure(w->out_cap) != cudaSuccess) rc = ctx->fail(KZ_ERR_CREATE_COMPRESSOR, "cannot allocate the device output buffer");
+    if (rc == 0) rc = w->open_common();
+    if (rc) {
+        w->close();
+        delete w;
+        return rc;
+    }
+    *out = w;
+    return 0;
+}
+
+int kz_writer_write(kz_writer* w, const uint8_t* src, size_t n, size_t* consumed, uint8_t* dst, size_t cap, size_t* produced) {
+    if (!w || !consumed || !produced || (!src && n) || (!dst && cap)) return -KZ_ERR_INVALID_PARAM;
+    *consumed = *produced = 0;
+    if (!w->ctx) return -KZ_ERR_INVALID_PARAM;  // its context was destroyed
+    if (cudaSetDevice(w->ctx->device) != cudaSuccess) return w->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    return w->pump(src, n, consumed, dst, cap, produced);
+}
+
+int kz_writer_finish(kz_writer* w, uint8_t* dst, size_t cap, size_t* produced) {
+    if (!w || !produced || (!dst && cap)) return -KZ_ERR_INVALID_PARAM;
+    *produced = 0;
+    if (!w->ctx) return -KZ_ERR_INVALID_PARAM;  // its context was destroyed
+    if (cudaSetDevice(w->ctx->device) != cudaSuccess) return w->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    return w->finish(dst, cap, produced);
+}
+
+void kz_writer_free(kz_writer* w) {
+    if (!w) return;
+    if (w->ctx) w->close();
+    delete w;
+}
+
+int kz_reader_open(kz_ctx* ctx, uint32_t batch_blocks, kz_reader** out) {
+    if (!ctx || !out) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is already open on this context");
+    if (batch_blocks > 1024) return ctx->fail(KZ_ERR_INVALID_PARAM, "batch_blocks must be in [0..1024]");
+    kz_reader* r = new kz_reader(ctx, batch_blocks);
+    int rc = r->open_common();
+    if (rc) {
+        r->close();
+        delete r;
+        return rc;
+    }
+    *out = r;
+    return 0;
+}
+
+int kz_reader_read(kz_reader* r, const uint8_t* src, size_t n, size_t* consumed, uint8_t* dst, size_t cap, size_t* produced) {
+    if (!r || !consumed || !produced || (!src && n) || (!dst && cap)) return -KZ_ERR_INVALID_PARAM;
+    *consumed = *produced = 0;
+    if (!r->ctx) return -KZ_ERR_INVALID_PARAM;  // its context was destroyed
+    if (cudaSetDevice(r->ctx->device) != cudaSuccess) return r->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    return r->pump(src, n, consumed, dst, cap, produced);
+}
+
+int kz_reader_finish(kz_reader* r, uint8_t* dst, size_t cap, size_t* produced) {
+    if (!r || !produced || (!dst && cap)) return -KZ_ERR_INVALID_PARAM;
+    *produced = 0;
+    if (!r->ctx) return -KZ_ERR_INVALID_PARAM;  // its context was destroyed
+    if (cudaSetDevice(r->ctx->device) != cudaSuccess) return r->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    return r->finish(dst, cap, produced);
+}
+
+void kz_reader_free(kz_reader* r) {
+    if (!r) return;
+    if (r->ctx) r->close();
+    delete r;
+}
+
+size_t kz_device_bytes(kz_ctx* ctx) {
+    if (!ctx) return 0;
+    return ctx->session ? ctx->session->device_bytes() : ctx->scratch_bytes();
 }
 
 }  // extern "C"

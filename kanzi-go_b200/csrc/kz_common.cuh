@@ -133,6 +133,66 @@ KZ_HD uint32_t write_block_prefix(uint8_t* p, uint64_t written) {
     return bw.pos;
 }
 
+// The reader's side of write_block_prefix (Reader.processBlock :1816-1852): 5 bits lw - 3, then the record's bit length on lw bits
+// (0 = the end marker). A prefix that runs past br.end leaves br.overrun set. stream_walk_kernel and walk_records both read through it.
+KZ_HD uint64_t read_block_prefix(BitReader& br) {
+    const uint32_t lr = br.read(5) + 3;
+    if (lr > 32) {
+        uint64_t hi = br.read(lr - 32);
+        return (hi << 32) | br.read(32);
+    }
+    return br.read(lr);
+}
+
+// Resumable walk over the block records of a window [start, end) of a stream that may still be incomplete (the streaming reader):
+// at most max_records records that lie completely inside the window, their payload bit offsets and lengths in bit_off / bits. It stops
+// cleanly before the first record whose prefix or payload is not completely inside, and at the end marker. status is an error only for
+// real corruption: a length over 2^34 bits (-KZ_E_BLOCK_SIZE, as stream_walk_kernel) or over max_bits, more than any block of the
+// stream can take (-KZ_E_PROCESS_BLOCK: the code a whole-stream walk gives when such a length runs past the end of the stream).
+struct WalkResult {
+    uint64_t next_bit;  // first bit behind the last record found (behind the end marker when ended)
+    uint32_t count;     // records found
+    int32_t status;     // 0 or -(error code)
+    uint32_t ended;     // 1: the end marker was read
+    uint32_t pad;
+};
+KZ_HD WalkResult walk_records(const uint32_t* words, uint64_t start, uint64_t end, uint32_t max_records, uint64_t max_bits, uint64_t* bit_off,
+                              uint64_t* bits) {
+    WalkResult r = {start, 0, 0, 0, 0};
+    BitReader br(words, start, end);
+    while (r.count < max_records) {
+        const uint64_t len = read_block_prefix(br);
+        if (br.overrun) break;
+        if (len == 0) {
+            r.ended = 1;
+            r.next_bit = br.pos;
+            break;
+        }
+        if (len > (1ull << 34)) {
+            r.status = -KZ_E_BLOCK_SIZE;
+            break;
+        }
+        if (len > max_bits) {
+            r.status = -KZ_E_PROCESS_BLOCK;
+            break;
+        }
+        if (br.pos + len > end) break;
+        bit_off[r.count] = br.pos;
+        bits[r.count] = len;
+        r.count++;
+        br.skip(len);
+        r.next_bit = br.pos;
+    }
+    return r;
+}
+
+// A writer session's batch of total_bits bits (its leading carry included) hands out the whole bytes and carries the last total_bits mod 8
+// bits into the next batch; the last batch hands out every byte, zero padded. Returns the bytes handed out.
+KZ_HD uint64_t batch_bytes_out(uint64_t total_bits, bool last, uint32_t* carry_bits) {
+    *carry_bits = last ? 0 : (uint32_t)(total_bits % 8);
+    return last ? (total_bits + 7) / 8 : total_bits / 8;
+}
+
 // ---- per-block descriptor and result of the transform stages TEXT, UTF, EXE, MM, PACK / DNA (ROLZ: result only) ---------
 struct StageBlock {
     uint64_t src_off;   // byte offset of the block in the source buffer

@@ -11,6 +11,9 @@
 
 namespace kz {
 
+struct Session;
+void close_session(Session* s);
+
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
@@ -128,7 +131,8 @@ struct kz_ctx {
     uint64_t launches = 0;
     bool profile = false;
     kz::EncPlan enc_plan;
-    bool fragment = false;        // encode_batch: LAYOUT_STREAM without the end marker (kz_compress_fragment_device)
+    bool fragment = false;        // encode_batch: LAYOUT_STREAM without the end marker (kz_compress_fragment_device, a writer session)
+    bool volatile_lead = false;   // encode_batch: the leading segment is a writer session's header or carry, kept out of the plan key
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
     uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
     std::map<std::string, kz::ProfEntry> prof;
@@ -144,6 +148,21 @@ struct kz_ctx {
     // many-stream entry points: copy lists, pass slots, pass entropy output, compact block bit strings, stream assembly / staging
     kz::DevBuf d_copy, d_slots, d_enc, d_bits, d_asm;
     kz::PinnedBuf h_stage, h_dl, h_io;  // h_io: packed inputs / outputs of the host-buffer many-stream entry points
+    // the open writer / reader session (the end of kz_api.cu), if any; kz_destroy closes it. kz_device_bytes asks it, because its
+    // worker thread grows the scratch
+    kz::Session* session = nullptr;
+
+    template <class F>
+    void each_dev_buf(F&& f) {
+        kz::DevBuf* bufs[] = {&d_in, &d_out, &d_tmp, &d_tmp2, &d_seg, &d_chunks, &d_tables, &d_enc_tab, &d_hdr, &d_pay, &d_small, &d_dl, &d_rcp, &d_ws, &d_lens,
+                              &d_hist, &d_copy, &d_slots, &d_enc, &d_bits, &d_asm};
+        for (auto b : bufs) f(*b);
+    }
+    size_t scratch_bytes() {
+        size_t s = 0;
+        each_dev_buf([&](kz::DevBuf& b) { s += b.cap; });
+        return s;
+    }
 
     int fail(int code, const std::string& msg) {
         err = msg;
