@@ -18,6 +18,8 @@
 //                          broadcasts key(c), every lane counts its larger keys, one REDUX gives r.
 // Inverse: the list itself is the decoder state (r -> c needs the list, which needs all earlier symbols), so a block is
 // one serial chain: one CTA per block walks it with the list in registers (blocks run concurrently).
+#include <algorithm>
+
 #include "kz_sbrt.cuh"
 
 namespace kz {
@@ -409,14 +411,26 @@ __global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_
 // A chain is serial and latency-bound: a CTA that shares its SM with another chain's CTA runs at a fraction of its speed for the whole launch, and
 // the block scheduler does pack CTAs (six per SM were seen: 1.6 s instead of 0.26 s) when kernels of other streams occupy the GPU at launch time.
 // Dynamic shared memory that nobody touches caps the chains per SM at ceil(nblocks / SMs): the chains spread over the GPU whatever runs beside them.
+// The chains of an SM take all of its shared memory, so that no CTA of another kernel shares their schedulers either: with room left for one
+// (half an SM per chain), a chain beside the -l 3 round trip of another context took 256 ms instead of the 224 ms it takes alone.
 template <typename K>
 static size_t spread_chains(K kernel, int nblocks) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return 0;
+    int dev = 0, sms = 0, sm_bytes = 0, block_max = 0, reserved = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0 ||
+        cudaDeviceGetAttribute(&sm_bytes, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&block_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess)
+        return 0;
     const int per = (nblocks + sms - 1) / sms;
     if (per > 5) return 0;  // small blocks in large numbers: several chains per SM overlap their latencies, no cap
-    const size_t sm_bytes = 228 * 1024;
-    const size_t dyn = sm_bytes / (size_t)(per + 1);
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    const size_t room = (size_t)sm_bytes / (size_t)per, fixed = (size_t)reserved + fa.sharedSizeBytes;
+    if (room <= fixed) return 0;
+    const size_t dyn = std::min(room - fixed, (size_t)block_max - fa.sharedSizeBytes);
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess) {
         cudaGetLastError();
         return 0;
