@@ -185,10 +185,25 @@ size_t kz_profile_names(kz_ctx* ctx, char* buf, size_t cap);
  * 0 (default) = the longest block of the call. kz_decode_blocks and the stream entry points know the value themselves. */
 void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size);
 
+/* ctx["from"] / ctx["to"] (kanzi d --from / --to): decode only a range of blocks. Block ids start at 1 with the stream's first record
+ * (io/CompressedStream.go:1684); block id is skipped iff id < from_block (when from_block >= 0) or id >= to_block (when to_block >= 0)
+ * (:1858-1871). So to_block is exclusive, from 0 acts as from 1, and to_block <= from_block or to_block == 1 decodes nothing. A negative value
+ * means "not given"; the default (-1, -1) decodes every block. Returns 0, or -KZ_ERR_INVALID_PARAM without a context.
+ * Read by kz_decompress_stream, kz_decompress_stream_device, kz_decompress_streams and kz_decompress_streams_device (the same range for every
+ * stream, as BlockDecompressor applies one from / to to every file) and kz_reader_open, which captures the range when the session opens
+ * (later calls do not change an open session, and the call is allowed while one is open). kz_decode_blocks, kz_decompress_fragment_device, kz_entropy_* and kz_transform_* ignore it:
+ * their block numbers are not stream ids.
+ * Semantics: every record of the stream is still walked to the end marker, so a bad record length, a record past the end or a truncated
+ * stream is reported wherever it lies. A skipped block is never parsed, entropy decoded, inverse transformed or checksummed: a defect inside
+ * it is not an error. The output is the decoded blocks of the range back to back (out_n / out_len = their length, 0 for an empty range). The
+ * error order of the sessions (below) applies to the decoded blocks. The record count limit of the whole-stream entry points (cap / 1024 + 16
+ * records) applies to the decoded blocks only; with a range set, the stream's length bounds the walk. */
+int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block);
+
 /* ---- streaming sessions: CompressedOutputStream / CompressedInputStream (io/CompressedStream.go:524-710, :1556-1744) for a stream of any
  *      length, or one that arrives in pieces (a pipe, a socket), in memory that does not grow with the stream ------------------------------
- * A zlib-style pump. The session takes ctx over until kz_*_free: the caller makes no other call on ctx in between except kz_device_bytes and
- * kz_last_error (the one-thread-at-a-time rule; one session per context). batch_blocks = blocks per GPU batch (the role of kanzi's `jobs`),
+ * A zlib-style pump. The session takes ctx over until kz_*_free: the caller makes no other call on ctx in between except kz_device_bytes,
+ * kz_last_error and kz_set_block_range (the one-thread-at-a-time rule; one session per context). batch_blocks = blocks per GPU batch (the role of kanzi's `jobs`),
  * 1 .. 1024; kz_reader_open also takes 0: about 256 MiB of blocks per batch, resolved from the block size in the stream's header.
  * Bytes: the writer's output, concatenated, is byte for byte what kz_compress_stream writes for the concatenated input with the same
  *   parameters and input_size_hint, whatever the piece sizes, batch_blocks and output caps. The reader's output is what kz_decompress_stream

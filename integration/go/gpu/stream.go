@@ -102,6 +102,7 @@ type StreamReader struct {
 }
 
 // NewStreamReader opens a reader session. batchBlocks in [1..1024]; 0 takes about 256 MiB per batch once the stream's block size is known.
+// The session decodes the block range last set with SetBlockRange (all blocks by default).
 func NewStreamReader(c *Context, r io.Reader, batchBlocks uint32) (*StreamReader, error) {
 	c.mu.Lock()
 	var h *C.kz_reader
@@ -174,4 +175,43 @@ func (s *StreamReader) Close() error {
 		s.c.mu.Unlock()
 	}
 	return nil
+}
+
+// BlockRange reads kanzi's ctx["from"] / ctx["to"], which NewReaderWithCtx checks to be ints (io/CompressedStream.go:1149-1159) and
+// BlockDecompressor sets only when they are >= 0 (app/BlockDecompressor.go:411-417). A missing key gives -1, "not given".
+func BlockRange(ctx map[string]any) (from, to int64) {
+	from, to = -1, -1
+	if v, ok := ctx["from"].(int); ok {
+		from = int64(v)
+	}
+	if v, ok := ctx["to"].(int); ok {
+		to = int64(v)
+	}
+	return from, to
+}
+
+// SetBlockRange is kz_set_block_range: the stream-level decodes that follow on c (DecompressStreams, and NewStreamReader, which keeps
+// the range for its session) decode only the blocks with from <= id < to, ids counted from 1; a negative bound is not given.
+func (c *Context) SetBlockRange(from, to int64) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	if rc := C.kz_set_block_range(c.h, C.int64_t(from), C.int64_t(to)); rc != 0 {
+		return c.err(rc)
+	}
+	return nil
+}
+
+// NewStreamReaderWithCtx is NewStreamReader for the reader paths that carry a kanzi ctx (NewReaderWithCtx): the session decodes the
+// block range of ctx["from"] / ctx["to"]. c's range is set for the open and restored to "not given" afterwards.
+func NewStreamReaderWithCtx(c *Context, r io.Reader, batchBlocks uint32, ctx map[string]any) (*StreamReader, error) {
+	from, to := BlockRange(ctx)
+	if from < 0 && to < 0 {
+		return NewStreamReader(c, r, batchBlocks)
+	}
+	if err := c.SetBlockRange(from, to); err != nil {
+		return nil, err
+	}
+	s, err := NewStreamReader(c, r, batchBlocks)
+	C.kz_set_block_range(c.h, -1, -1) // without c.mu, which the open session holds: the call is allowed while a session is open
+	return s, err
 }

@@ -11,6 +11,7 @@ shows the cgo binding a kanzi-go maintainer would add). Names follow the referen
 There is no CPU fallback: importing works without a GPU (so that the library's symbols can be checked), but creating a
 Context without a CUDA device raises.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -38,7 +39,7 @@ ABI_SYMBOLS = [
     "kz_compress_fragment_device", "kz_stream_header", "kz_concat_bits_device", "kz_stream_index_device", "kz_decompress_fragment_device",
     "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
     "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
-    "kz_reader_free", "kz_device_bytes",
+    "kz_reader_free", "kz_device_bytes", "kz_set_block_range",
 ]
 
 
@@ -136,6 +137,7 @@ def load_library(build_if_missing=True):
     L.kz_profile_names.argtypes = [vp, C.c_char_p, sz]
     L.kz_profile_names.restype = sz
     L.kz_set_stream_block_size.restype = None
+    L.kz_set_block_range.argtypes = [vp, C.c_int64, C.c_int64]
     L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -189,6 +191,7 @@ class Context:
             raise KanziError(-rc, "cannot create the engine on CUDA device %d (no GPU / no driver?) - there is no CPU fallback" % device)
         self.h = h
         self.device = device
+        self._range = (-1, -1)  # kz_set_block_range's (from, to) on this context
 
     def close(self):
         if getattr(self, "h", None):
@@ -293,12 +296,34 @@ class Context:
         self._check(self.lib.kz_compress_stream(self.h, t48, et, block_size, checksum_bits, input_size, _p(a), a.size, out.ctypes.data, cap, C.byref(n)))
         return out[: n.value].copy()
 
-    def decompress(self, stream, out_cap):
+    def decompress(self, stream, out_cap, from_block=None, to_block=None):
+        """from_block / to_block: decode only that range of blocks (see set_block_range) for this call."""
         s = _u8(stream)
         out = np.empty(max(out_cap, 1), np.uint8)
         n = C.c_size_t(0)
-        self._check(self.lib.kz_decompress_stream(self.h, _p(s), s.size, out.ctypes.data, out_cap, C.byref(n)))
+        with self._block_range(from_block, to_block):
+            self._check(self.lib.kz_decompress_stream(self.h, _p(s), s.size, out.ctypes.data, out_cap, C.byref(n)))
         return out[: n.value]
+
+    # ---- block range (kz_set_block_range): kanzi's ctx["from"] / ctx["to"] ---------------------------------------------------------
+    def set_block_range(self, from_block=-1, to_block=-1):
+        """Decode only blocks from_block <= id < to_block (ids start at 1; a negative value = not given) in the stream-level decodes that
+        follow: decompress*, decompress_streams* and stream_reader (captured when the session opens)."""
+        self._check(self.lib.kz_set_block_range(self.h, from_block, to_block))
+        self._range = (from_block if from_block >= 0 else -1, to_block if to_block >= 0 else -1)
+
+    @contextlib.contextmanager
+    def _block_range(self, from_block, to_block):
+        """Sets the range for one call when either bound is given, and restores the previous range afterwards."""
+        if from_block is None and to_block is None:
+            yield
+            return
+        prev = self._range
+        self.set_block_range(-1 if from_block is None else from_block, -1 if to_block is None else to_block)
+        try:
+            yield
+        finally:
+            self.set_block_range(*prev)
 
     # ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams) -----------------------------------
     # Per-stream failures do not raise: status[s] = 0 or -(kanzi error code), and outputs[s] is None for a failed stream.
@@ -320,8 +345,9 @@ class Context:
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
         return outs, status
 
-    def decompress_streams(self, streams, caps):
-        """Decodes every stream (headers may differ) into at most caps[s] bytes -> (outputs, status)."""
+    def decompress_streams(self, streams, caps, from_block=None, to_block=None):
+        """Decodes every stream (headers may differ) into at most caps[s] bytes -> (outputs, status). from_block / to_block: the same block
+        range for every stream."""
         arrs = [_u8(x) for x in streams]
         src_len = np.array([a.size for a in arrs], np.uint64)
         src_off = _offsets(src_len)
@@ -330,8 +356,9 @@ class Context:
         dst_off = _offsets(cap)
         dst = np.empty(max(int(cap.sum()), 1), np.uint8)
         out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
-        self.lib.kz_decompress_streams(self.h, len(arrs), _p(src), _p(src_off), _p(src_len), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len),
-                                       _p(status))
+        with self._block_range(from_block, to_block):
+            self.lib.kz_decompress_streams(self.h, len(arrs), _p(src), _p(src_off), _p(src_len), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len),
+                                           _p(status))
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
         return outs, status
 
@@ -347,11 +374,12 @@ class Context:
                                             _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
 
-    def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap):
+    def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, from_block=None, to_block=None):
         """Device-resident decompress_streams: inputs need >= 64 readable bytes behind each -> (out_len, status)."""
         so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
         out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
-        self.lib.kz_decompress_streams_device(self.h, len(sl), _dptr(src), _p(so), _p(sl), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+        with self._block_range(from_block, to_block):
+            self.lib.kz_decompress_streams_device(self.h, len(sl), _dptr(src), _p(so), _p(sl), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
 
     # ---- device-resident entry points (pointers are CUDA device addresses, e.g. torch tensors' data_ptr()) -------
@@ -360,9 +388,10 @@ class Context:
         self._check(self.lib.kz_compress_stream_device(self.h, transform48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, C.byref(out_n)))
         return out_n.value
 
-    def decompress_device(self, d_src, n, d_dst, cap):
+    def decompress_device(self, d_src, n, d_dst, cap, from_block=None, to_block=None):
         out_n = C.c_size_t(0)
-        self._check(self.lib.kz_decompress_stream_device(self.h, d_src, n, d_dst, cap, C.byref(out_n)))
+        with self._block_range(from_block, to_block):
+            self._check(self.lib.kz_decompress_stream_device(self.h, d_src, n, d_dst, cap, C.byref(out_n)))
         return out_n.value
 
     def compress_host(self, src_ptr, n, dst_ptr, cap, transform48, etype, block_size, checksum_bits=0, input_size=0):
@@ -426,13 +455,14 @@ class Context:
         self._check(self.lib.kz_writer_open(self.h, t48, et, block_size, checksum_bits, batch_blocks, input_size, C.byref(h)))
         return StreamSession(self, h, self.lib.kz_writer_write, self.lib.kz_writer_finish, self.lib.kz_writer_free)
 
-    def stream_reader(self, batch_blocks=None):
+    def stream_reader(self, batch_blocks=None, from_block=None, to_block=None):
         """A StreamSession: write(data) -> decoded bytes and finish() -> the rest. batch_blocks=None: about 256 MiB per batch, resolved
-        from the block size in the stream's header."""
+        from the block size in the stream's header. from_block / to_block: the session decodes only that range of blocks."""
         if batch_blocks is None:
             batch_blocks = 0
         h = C.c_void_p()
-        self._check(self.lib.kz_reader_open(self.h, batch_blocks, C.byref(h)))
+        with self._block_range(from_block, to_block):
+            self._check(self.lib.kz_reader_open(self.h, batch_blocks, C.byref(h)))
         return StreamSession(self, h, self.lib.kz_reader_read, self.lib.kz_reader_finish, self.lib.kz_reader_free)
 
     def device_bytes(self):
@@ -673,11 +703,13 @@ class Writer:
 
 
 class Reader:
-    """io.Reader (CompressedInputStream): NewReader(is, jobs) (io/CompressedStream.go:1047)."""
+    """io.Reader (CompressedInputStream): NewReader(is, jobs) (io/CompressedStream.go:1047); from_block / to_block are ctx["from"] /
+    ctx["to"] of NewReaderWithCtx (negative = not given): only blocks from_block <= id < to_block are decoded."""
 
-    def __init__(self, stream, jobs=1, ctx=None):
+    def __init__(self, stream, jobs=1, ctx=None, from_block=-1, to_block=-1):
         self.stream = _u8(stream)
         self.ctx = ctx or default_context()
+        self.from_block, self.to_block = from_block, to_block
 
     def read_all(self, max_size):
-        return self.ctx.decompress(self.stream, max_size)
+        return self.ctx.decompress(self.stream, max_size, self.from_block, self.to_block)

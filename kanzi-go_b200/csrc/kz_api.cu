@@ -611,9 +611,12 @@ __global__ void block_header_kernel(const uint32_t* __restrict__ words, const ui
 
 // The block records of one stream for stream_walk_kernel: bits [start_bit, end_bit) of the word buffer, found records go to entries
 // out .. out + max_blocks - 1 of bit_off / bits. stop_after != 0: a fragment of that many block records (no end marker behind them).
+// Only records keep_lo .. keep_hi - 1 (0-based) are stored, record r at entry out + r - keep_lo (a block range, kz_set_block_range); the
+// others are walked all the same.
 struct WalkJob {
     uint64_t start_bit, end_bit, out;
     uint32_t max_blocks, stop_after;
+    uint64_t keep_lo = 0, keep_hi = ~0ull;
 };
 
 // Serial walk over the block length prefixes of complete streams (decodingTask.decode :1816-1852), one thread per stream: jobs[s], or
@@ -645,8 +648,10 @@ __global__ void stream_walk_kernel(const uint32_t* __restrict__ words, const Wal
             st = -KZ_E_BLOCK_SIZE;
             break;
         }
-        bit_off[n] = br.pos;
-        bits[n] = len;
+        if (n >= job.keep_lo && n < job.keep_hi) {
+            bit_off[n - job.keep_lo] = br.pos;
+            bits[n - job.keep_lo] = len;
+        }
         n++;
         br.skip(len);
         if (br.overrun) {
@@ -1708,6 +1713,13 @@ size_t kz_max_stream_output(size_t n, uint32_t block_size) {
     return n + (n >> 3) + 64 * (n / 16384 + 1) + 32 * nblocks + 1024 + 106496 * (n / (4u << 20) + nblocks + 1);
 }
 
+int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    ctx->range_from = from_block < 0 ? -1 : from_block;
+    ctx->range_to = to_block < 0 ? -1 : to_block;
+    return 0;
+}
+
 void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size) {
     if (ctx) ctx->user_stream_bs = block_size;
 }
@@ -1859,10 +1871,10 @@ int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, 
     return 0;
 }
 
-static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, const void* d_src, size_t n, void* d_dst,
-                                  size_t cap, size_t* out_n);
+static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
+                                  size_t n, void* d_dst, size_t cap, size_t* out_n);
 int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
-    return decompress_device_impl(ctx, nullptr, 0, 0, d_src, n, d_dst, cap, out_n);
+    return decompress_device_impl(ctx, nullptr, 0, 0, ctx ? ctx->range_from : -1, ctx ? ctx->range_to : -1, d_src, n, d_dst, cap, out_n);
 }
 // Decodes `nblocks` block records that start at bit `start_bit` of the fragment at d_src (frag_bytes bytes, >= 64 readable bytes behind them):
 // what one rank of a sharded decompression does with its part of the stream. The stream parameters come from the header rank 0 parsed.
@@ -1878,7 +1890,7 @@ int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uin
     sh.checksum_bits = checksum_bits;
     sh.input_size = 0;
     sh.bits = 0;
-    return decompress_device_impl(ctx, &sh, start_bit, nblocks, d_src, frag_bytes, d_dst, cap, out_n);
+    return decompress_device_impl(ctx, &sh, start_bit, nblocks, -1, -1, d_src, frag_bytes, d_dst, cap, out_n);
 }
 // Parses the header of the stream at d_src and walks its block records: rec_bit[b] = first bit of record b (its 5-bit prefix), rec_bit[nblocks] =
 // first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries.
@@ -1922,8 +1934,8 @@ int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t ma
     *nblocks = nb;
     return 0;
 }
-static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, const void* d_src, size_t n, void* d_dst,
-                                  size_t cap, size_t* out_n) {
+static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
+                                  size_t n, void* d_dst, size_t cap, size_t* out_n) {
     if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     if (((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
@@ -1945,18 +1957,25 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     if (rc) return rc;
     const uint32_t* d_words = (const uint32_t*)d_src;
     const uint64_t words_len = (n + 3) / 4 + 16;  // callers guarantee >= 64 readable bytes past n
-    // block prefixes
-    uint32_t max_blocks = (uint32_t)std::min<uint64_t>((uint64_t)cap / 1024 + 16, 1u << 22);
-    CK(ctx->d_dl.ensure((size_t)max_blocks * 16 + 64));
+    // block prefixes: at most cap / 1024 + 16 decoded blocks are stored (blocks are at least 1 KiB). Without a block range that also
+    // bounds the walk. With one, the walk goes over every record to the end marker, so that a walk error behind the range is still found,
+    // and only the stream's bytes bound it (a record takes at least 9 bits); the records outside the range are not stored.
+    const bool ranged = from >= 0 || to >= 0;
+    uint64_t keep_lo = 0, keep_hi = ~0ull;
+    if (ranged) block_range_records(from, to, &keep_lo, &keep_hi);
+    const uint32_t max_blocks = (uint32_t)std::min<uint64_t>((uint64_t)cap / 1024 + 16, 1u << 22);
+    const uint32_t slots = (uint32_t)std::min<uint64_t>(max_blocks, keep_hi - keep_lo);
+    CK(ctx->d_dl.ensure((size_t)slots * 16 + 64));
     uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
-    uint64_t* d_bbits = d_boff + max_blocks;
-    uint32_t* d_cnt = (uint32_t*)(d_bbits + max_blocks);
+    uint64_t* d_bbits = d_boff + slots;
+    uint32_t* d_cnt = (uint32_t*)(d_bbits + slots);
     {
         LaunchScope ls(ctx, "stream_walk");
-        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>(d_words, nullptr, WalkJob{sh.bits, 8ull * n, 0, max_blocks, stop_after}, 1, d_boff, d_bbits, d_cnt);
+        const WalkJob wj{sh.bits, 8ull * n, 0, ranged ? 0xFFFFFFFFu : max_blocks, stop_after, keep_lo, keep_lo + slots};
+        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>(d_words, nullptr, wj, 1, d_boff, d_bbits, d_cnt);
     }
     // count + the first SPEC block descriptors in one round trip (streams with more blocks pay a second copy)
-    const uint32_t SPEC = std::min<uint32_t>(max_blocks, 1024);
+    const uint32_t SPEC = std::min<uint32_t>(slots, 1024);
     CK(ctx->h_dl.ensure((size_t)SPEC * 16 + 64));
     uint32_t* cs = (uint32_t*)ctx->h_dl.p;
     uint64_t* h_boff = (uint64_t*)((uint8_t*)ctx->h_dl.p + 64);
@@ -1966,7 +1985,10 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     CK(cudaMemcpyAsync(h_bbits, d_bbits, (size_t)SPEC * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if ((int32_t)cs[1] != 0) return ctx->fail(-(int32_t)cs[1], "Invalid bitstream: corrupted block length");
-    const uint32_t nblocks = cs[0];
+    const uint64_t nrec = cs[0];  // records of the stream; the decoded ones are records keep_lo .. keep_lo + nblocks - 1
+    const uint64_t in_range = std::min(nrec, keep_hi) - std::min(nrec, keep_lo);
+    if (in_range > slots) return ctx->fail(KZ_ERR_BLOCK_SIZE, "Invalid bitstream: more blocks than the output buffer can hold");
+    const uint32_t nblocks = (uint32_t)in_range;
     std::vector<uint64_t> boff(nblocks), bbits(nblocks);
     if (nblocks && nblocks <= SPEC) {
         memcpy(boff.data(), h_boff, (size_t)nblocks * 8);
@@ -1992,7 +2014,7 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
             jobs[b].out_off = out_off;  // NONE transform: decoded length == pre_len; every block but the last is block_size (multiple of 16)
             out_off += jobs[b].pre_len;
             if (out_off > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-            if (b + 1 < nblocks && (jobs[b].pre_len & 15)) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+            if (keep_lo + b + 1 < nrec && (jobs[b].pre_len & 15)) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "unexpected block length");
         }
         rc = decode_batch(ctx, sh.etype, d_words, words_len, jobs, (uint8_t*)d_dst);
         if (rc) return rc;
@@ -2297,14 +2319,21 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     const uint32_t ng = (uint32_t)grp.size();
     const uint32_t* d_words = (const uint32_t*)d_src;
     const uint64_t words_len = (src_bytes + 3) / 4 + 16;
-    // walk: one thread per stream; as many records per stream as the single-stream path allows, and no more than its bytes can hold
+    // walk: one thread per stream; as many records per stream as the single-stream path allows, and no more than its bytes can hold. With
+    // a block range (the same for every stream) the walk goes to the end marker and stores as many records of the range as the
+    // single-stream path would.
+    const bool ranged = ctx->range_from >= 0 || ctx->range_to >= 0;
+    uint64_t keep_lo = 0, keep_hi = ~0ull;
+    if (ranged) block_range_records(ctx->range_from, ctx->range_to, &keep_lo, &keep_hi);
     std::vector<WalkJob> wj(ng);
     uint64_t nrec = 0;
     for (uint32_t g = 0; g < ng; g++) {
         const uint32_t s = grp[g];
         const uint64_t by_cap = std::min<uint64_t>(dst_cap[s] / 1024 + 16, 1u << 22);
-        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), nrec, (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1), 0};
-        nrec += wj[g].max_blocks;
+        const uint32_t max_blocks = (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1);
+        const uint32_t slots = (uint32_t)std::min<uint64_t>(max_blocks, keep_hi - keep_lo);
+        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), nrec, ranged ? 0xFFFFFFFFu : max_blocks, 0, keep_lo, keep_lo + slots};
+        nrec += slots;
     }
     CK(ctx->d_dl.ensure((size_t)nrec * 16 + (size_t)ng * 8 + 64));
     uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
@@ -2332,17 +2361,18 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     std::vector<uint32_t> bgrp;   // group index of every block
     std::vector<uint8_t> blast;   // last block of its stream
     for (uint32_t g = 0; g < ng; g++) {
-        if (cs[2 * g + 1]) {
+        const uint64_t n = cs[2 * g], kept = std::min(n, keep_hi) - std::min(n, keep_lo);
+        if (cs[2 * g + 1] || kept > wj[g].keep_hi - keep_lo) {
             bad[g] = 1;
             continue;
         }
-        for (uint32_t r = 0; r < cs[2 * g]; r++) {
+        for (uint32_t r = 0; r < kept; r++) {
             DecJob j = DecJob();
             j.bit_off = hoff[wj[g].out + r];
             j.bits = hbits[wj[g].out + r];
             all.push_back(j);
             bgrp.push_back(g);
-            blast.push_back(r + 1 == cs[2 * g]);
+            blast.push_back(keep_lo + r + 1 == n);
         }
     }
     const uint64_t pstride = decompress_slot(sh.block_size);
@@ -2430,8 +2460,8 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     return 0;
 }
 
-static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, const void* d_src, size_t n, void* d_dst,
-                                  size_t cap, size_t* out_n);
+static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
+                                  size_t n, void* d_dst, size_t cap, size_t* out_n);
 
 // Decodes stream s = d_src[src_off[s] : + src_len[s]] (>= 64 readable bytes behind it) to d_dst + dst_off[s]. src_bytes: readable bytes at d_src.
 static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off, const uint64_t* src_len,
@@ -2473,7 +2503,8 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     }
     for (uint32_t s : alone) {  // only corrupt input (or too little room) gets here
         size_t n = 0;
-        status[s] = decompress_device_impl(ctx, nullptr, 0, 0, d_src + src_off[s], src_len[s], d_dst + dst_off[s], dst_cap[s], &n);
+        status[s] = decompress_device_impl(ctx, nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s], d_dst + dst_off[s],
+                                           dst_cap[s], &n);
         out_len[s] = status[s] ? 0 : n;
     }
     return 0;
@@ -3186,6 +3217,8 @@ struct kz_reader : kz::Session {
     uint64_t fill = 0, start_bit = 0;  // valid bytes of win[cur], first bit not yet walked
     bool ended = false;                // the end marker was read (guarded by m: the caller drops input after it)
     bool odd_tail = false;             // NONE: the last block handed out has a length that is not a multiple of 16
+    int64_t range_from = -1, range_to = -1;  // the context's block range when the session opened (kz_set_block_range)
+    uint64_t walked = 0;                     // records walked so far
 
     using Session::Session;
     size_t own_device_bytes() override { return win[0].cap + win[1].cap + d_dec.cap + d_walk.cap; }
@@ -3310,8 +3343,17 @@ struct kz_reader : kz::Session {
             CK(cudaStreamSynchronize(ctx->stream));
             if (r.status) return ctx->fail(-r.status, "Invalid bitstream: corrupted block length");
             if (r.count) {
-                int rc = decode(r.count, boff, bbits);
-                if (rc) return rc;
+                // only the records in the block range are decoded; the others were walked and their bits are dropped with the window
+                uint32_t lo, hi;
+                block_range_slice(range_from, range_to, walked, r.count, &lo, &hi);
+                walked += r.count;
+                // NONE: a decoded block that was not the stream's last record must be a multiple of 16 long
+                if (plan.none() && odd_tail && pend_stage != STAGE_HEADER) note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+                odd_tail = false;
+                if (hi > lo) {
+                    int rc = decode(hi - lo, &boff[lo], &bbits[lo], hi == r.count);
+                    if (rc) return rc;
+                }
             }
             start_bit = r.next_bit;
             if (r.ended) {
@@ -3345,8 +3387,9 @@ struct kz_reader : kz::Session {
         return 0;
     }
 
-    // the records of one batch, as decompress_device_impl decodes a whole stream; the decoded bytes are published back to back
-    int decode(uint32_t nb, const std::vector<uint64_t>& boff, const std::vector<uint64_t>& bbits) {
+    // nb records of one batch, as decompress_device_impl decodes a whole stream; the decoded bytes are published back to back.
+    // ends_batch: the last of them is the last record walked so far.
+    int decode(uint32_t nb, const uint64_t* boff, const uint64_t* bbits, bool ends_batch) {
         if (pend_stage == STAGE_HEADER) return 0;  // only a walk error could still win
         const uint32_t* W = win[cur].as<uint32_t>();
         const uint64_t words_len = (fill + 3) / 4 + 16;
@@ -3362,9 +3405,8 @@ struct kz_reader : kz::Session {
         uint64_t total = 0;
         std::vector<uint32_t> olen(nb);
         uint64_t pstride = 0;
-        // headers (and, for NONE, the rule that every block but the stream's last is a multiple of 16 long: the last block of the
-        // previous batch was not the last one), in block order as decompress_device_impl checks them
-        if (plan.none() && odd_tail) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+        // headers (and, for NONE, the rule that every block but the stream's last is a multiple of 16 long), in block order as
+        // decompress_device_impl checks them
         uint32_t max_pre = 0;
         for (uint32_t b = 0; b < nb; b++) {
             if (jobs[b].status) return note_fail(STAGE_HEADER, -jobs[b].status, "Invalid compressed block header");
@@ -3372,7 +3414,7 @@ struct kz_reader : kz::Session {
                 jobs[b].out_off = total;
                 total += jobs[b].pre_len;
                 olen[b] = jobs[b].pre_len;
-                if (b + 1 < nb && (jobs[b].pre_len & 15)) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+                if ((b + 1 < nb || !ends_batch) && (jobs[b].pre_len & 15)) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
             }
             max_pre = std::max(max_pre, jobs[b].pre_len);
         }
@@ -3489,6 +3531,8 @@ int kz_reader_open(kz_ctx* ctx, uint32_t batch_blocks, kz_reader** out) {
     if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is already open on this context");
     if (batch_blocks > 1024) return ctx->fail(KZ_ERR_INVALID_PARAM, "batch_blocks must be in [0..1024]");
     kz_reader* r = new kz_reader(ctx, batch_blocks);
+    r->range_from = ctx->range_from;
+    r->range_to = ctx->range_to;
     int rc = r->open_common();
     if (rc) {
         r->close();

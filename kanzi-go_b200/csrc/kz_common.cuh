@@ -193,6 +193,27 @@ KZ_HD uint64_t batch_bytes_out(uint64_t total_bits, bool last, uint32_t* carry_b
     return last ? (total_bits + 7) / 8 : total_bits / 8;
 }
 
+// kanzi's ctx["from"] / ctx["to"] (kz_set_block_range): block ids start at 1 with the stream's first record
+// (io/CompressedStream.go:1684), and a block is skipped iff id < from (from given) or id >= to (to given) (:1858-1871); a negative value is
+// "not given". As 0-based record indices: the records [*lo, *hi) are decoded (*hi >= *lo; ~0 = no end).
+KZ_HD void block_range_records(int64_t from, int64_t to, uint64_t* lo, uint64_t* hi) {
+    *lo = from > 1 ? (uint64_t)(from - 1) : 0;
+    *hi = to < 0 ? ~0ull : to > 1 ? (uint64_t)(to - 1) : 0;
+    if (*hi < *lo) *hi = *lo;
+}
+
+// The records of one walk batch that are decoded: records first .. first + count - 1 of the stream (0-based) were walked; the slice
+// [*lo, *hi) of the batch lies in the range (*lo == *hi: none).
+KZ_HD void block_range_slice(int64_t from, int64_t to, uint64_t first, uint32_t count, uint32_t* lo, uint32_t* hi) {
+    uint64_t rlo, rhi;
+    block_range_records(from, to, &rlo, &rhi);
+    const uint64_t end = first + count;
+    const uint64_t a = rlo < first ? first : rlo > end ? end : rlo;
+    const uint64_t b = rhi < a ? a : rhi > end ? end : rhi;
+    *lo = (uint32_t)(a - first);
+    *hi = (uint32_t)(b - first);
+}
+
 // ---- per-block descriptor and result of the transform stages TEXT, UTF, EXE, MM, PACK / DNA (ROLZ: result only) ---------
 struct StageBlock {
     uint64_t src_off;   // byte offset of the block in the source buffer

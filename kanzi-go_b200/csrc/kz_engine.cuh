@@ -135,6 +135,7 @@ struct kz_ctx {
     bool volatile_lead = false;   // encode_batch: the leading segment is a writer session's header or carry, kept out of the plan key
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
     uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
+    int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)
     std::map<std::string, kz::ProfEntry> prof;
     struct Pending {
         std::string name;
