@@ -179,6 +179,10 @@ void kz_profile_reset(kz_ctx* ctx);
  * Also "kernel names" (enumeration): kz_profile_names writes up to cap bytes of newline separated names, returns the full size. */
 uint32_t kz_stage_bytes(kz_ctx* ctx, const char* name, uint64_t* bytes_in, uint64_t* bytes_out);
 size_t kz_profile_names(kz_ctx* ctx, char* buf, size_t cap);
+/* BWT forward doubling rounds of this context (a profiling aid; the default is 0 and the output bytes never depend on it):
+ * bit 0: with kz_profile(ctx,1), time every round's parts under "bwt_round:<r>:<part>" (parts: small, sort, large, select, gap);
+ * bit 1: run the 56-bit global sort in every round, also where the blocks would take the small-group / narrow-key rounds. */
+void kz_bwt_profile(kz_ctx* ctx, int flags);
 
 /* ctx["blockSize"] of the stream the following kz_encode_blocks / kz_transform_forward / kz_transform_inverse calls belong to
  * (io/CompressedStream.go:220,1406). Only TEXT reads it (it sizes its hash map from it, transform/TextCodec.go:1143-1156);

@@ -39,7 +39,7 @@ ABI_SYMBOLS = [
     "kz_compress_fragment_device", "kz_stream_header", "kz_concat_bits_device", "kz_stream_index_device", "kz_decompress_fragment_device",
     "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
     "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
-    "kz_reader_free", "kz_device_bytes", "kz_set_block_range",
+    "kz_reader_free", "kz_device_bytes", "kz_set_block_range", "kz_bwt_profile",
 ]
 
 
@@ -136,6 +136,8 @@ def load_library(build_if_missing=True):
     L.kz_stage_bytes.restype = u32
     L.kz_profile_names.argtypes = [vp, C.c_char_p, sz]
     L.kz_profile_names.restype = sz
+    L.kz_bwt_profile.argtypes = [vp, i32]
+    L.kz_bwt_profile.restype = None
     L.kz_set_stream_block_size.restype = None
     L.kz_set_block_range.argtypes = [vp, C.c_int64, C.c_int64]
     L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -492,6 +494,10 @@ class Context:
         buf = C.create_string_buffer(n + 16)
         self.lib.kz_profile_names(self.h, buf, n + 16)
         return [x for x in buf.value.decode().split("\n") if x]
+
+    def bwt_profile(self, time_rounds=False, wide_rounds=False):
+        """BWT forward rounds (kz_bwt_profile): time every round under "bwt_round:<r>:<part>" / run the 56-bit global sort in every round"""
+        self.lib.kz_bwt_profile(self.h, (1 if time_rounds else 0) | (2 if wide_rounds else 0))
 
     def launch_count(self, reset=False):
         return self.lib.kz_launch_count(self.h, 1 if reset else 0)

@@ -1093,8 +1093,10 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             if (nn.empty()) continue;
             CK(ctx->d_ws.ensure(bwt_forward_batch_workspace(total, (uint32_t)nn.size())));
             LaunchScope ls(ctx, "bwt_forward");
+            CtxLzHook round_hook(ctx);  // kz_bwt_profile bit 0: every round timed under its own name
             cudaError_t e = bwt_forward_batch(d_in, d_out, so.data(), dof.data(), nn.data(), num.data(), (uint32_t)nn.size(), d_post, ctx->d_ws.as<uint8_t>(),
-                                              ctx->d_ws.cap, ctx->stream, &ctx->launches);
+                                              ctx->d_ws.cap, ctx->stream, &ctx->launches, (ctx->profile && (ctx->bwt_profile & 1)) ? &round_hook : nullptr,
+                                              (ctx->bwt_profile & 2) != 0);
             if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_forward");
             for (uint32_t k : num) applied[k] = 1;
         }
@@ -1683,6 +1685,9 @@ uint32_t kz_kernel_time(kz_ctx* ctx, const char* name, double* total_ms) {
     }
     if (total_ms) *total_ms = it->second.ms;
     return it->second.launches;
+}
+void kz_bwt_profile(kz_ctx* ctx, int flags) {
+    if (ctx) ctx->bwt_profile = flags;
 }
 void kz_profile_reset(kz_ctx* ctx) {
     drain_profile(ctx);

@@ -20,12 +20,17 @@
 #include <cub/device/dispatch/dispatch_segmented_sort.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include <cub/device/device_select.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 
 #include <algorithm>
+#include <string>
 #include <vector>
 
 #include "kz_bwt.cuh"
+#include "kz_bwt_core.cuh"
+#include "kz_lz.cuh"
 
 namespace kz {
 
@@ -435,6 +440,141 @@ __global__ void __launch_bounds__(256) bwtu_apply_kernel(uint32_t* __restrict__ 
     sa[cpos[u]] = v;
     rank[v] = g;
 }
+
+// ---- narrow rounds (every block of the batch at most BWT_NARROW_MAX_N bytes) --------------------------------------------------------------
+// The same rounds without a 56-bit global sort. Members u < m (cpos[u]: sorted position, ascending; groups are contiguous runs of u) get
+// their suffix v = sa[cpos[u]] and a 32-bit second key (rank of v + h relative to the block's base, + 1; 0 past the end of the block: at
+// most n <= 2^22, 23 bits) in one pass, before any rank changes. Then:
+//  - groups of at most BWT_SMALL_GROUP members are sorted by that key inside the CTA that owns their first member (kz_bwt_core.cuh), which
+//    writes sa, the new ranks and the "still unresolved" flag of every member directly;
+//  - the members of the larger groups are selected and radix sorted on (ordinal of the large group << 23 | second key): the ordinal has at
+//    most log2(m_large / (G + 1)) bits, so the key is 32 bits or a few passes above instead of 2 x 28 bits;
+//  - one select of the sorted positions that are still unresolved gives the next round's members (their suffixes are read from sa).
+const uint32_t BWT_NARROW_MAX_N = 1u << 22;
+const uint32_t BWTN_G = bwtc::BWT_SMALL_GROUP;
+const uint32_t BWTN_TILE = 2048;                          // members per CTA of the small-group pass
+const uint32_t BWTN_ITEMS = (BWTN_TILE + 2 * BWTN_G + 2 + 255) / 256;
+const uint32_t BWTN_WIN = BWTN_ITEMS * 256;               // window of a CTA: G members before its tile, G + 1 after (+ the end of the list)
+const uint32_t BWTN_START = 1u << 31;                     // bit of a second key: the member heads its group
+const uint16_t BWTN_NONE = 0xFFFF;
+
+__global__ void __launch_bounds__(256) bwtn_keys_kernel(const uint32_t* __restrict__ sa, const uint32_t* __restrict__ rank, const uint32_t* __restrict__ cpos, uint32_t m,
+                                                         const BwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t h, uint32_t* __restrict__ key2,
+                                                         uint32_t* __restrict__ val) {
+    __shared__ uint32_t s_base[BWT_BATCH_MAX];
+    __shared__ uint32_t s_n[BWT_BATCH_MAX];
+    for (uint32_t k = threadIdx.x; k < nb; k += 256) s_base[k] = blocks[k].base, s_n[k] = blocks[k].n;
+    __syncthreads();
+    const uint32_t u = blockIdx.x * 256 + threadIdx.x;
+    if (u >= m) return;
+    const uint32_t p = cpos[u];
+    const uint32_t v = sa[p];
+    const uint32_t b = bwtb_find(s_base, nb, v);
+    const uint32_t base = s_base[b];
+    const uint32_t k = (uint64_t)v + h < (uint64_t)base + s_n[b] ? rank[v + h] - base + 1 : 0u;
+    key2[u] = k | (rank[v] == p ? BWTN_START : 0u);
+    val[u] = v;
+}
+
+// CTA t owns the groups whose first member lies in [t * TILE, (t + 1) * TILE). A member's group runs from the last start at or before it to the
+// first start after it; the window (G before the tile, G + 1 after) holds both ends of every group of at most G members the CTA owns or
+// touches, so big[u] (member of a group of more than G) is exact for the CTA's own members.
+__global__ void __launch_bounds__(256) bwtn_small_kernel(const uint32_t* __restrict__ cpos, const uint32_t* __restrict__ key2, const uint32_t* __restrict__ val, uint32_t m,
+                                                          uint32_t* __restrict__ sa, uint32_t* __restrict__ rank, uint8_t* __restrict__ keep, uint8_t* __restrict__ big) {
+    using Scan = cub::BlockScan<uint32_t, 256>;
+    __shared__ typename Scan::TempStorage s_scan;
+    __shared__ uint32_t s_key[BWTN_WIN];
+    __shared__ uint16_t s_prev[BWTN_WIN];  // window index of the last group start at or before w
+    __shared__ uint16_t s_next[BWTN_WIN];  // window index of the first group start at or after w (W: the end of the list)
+    const uint32_t t0 = blockIdx.x * BWTN_TILE;
+    const uint32_t t1 = min(m, t0 + BWTN_TILE);
+    const uint32_t lo = t0 > BWTN_G ? t0 - BWTN_G : 0u;
+    const uint32_t hi = (uint32_t)min((uint64_t)m, (uint64_t)t0 + BWTN_TILE + BWTN_G + 1);
+    const uint32_t W = hi - lo;
+    for (uint32_t w = threadIdx.x; w < W; w += 256) s_key[w] = key2[lo + w];
+    __syncthreads();
+    uint32_t x[BWTN_ITEMS];
+#pragma unroll
+    for (uint32_t q = 0; q < BWTN_ITEMS; q++) {
+        const uint32_t w = threadIdx.x * BWTN_ITEMS + q;
+        x[q] = w < W && (s_key[w] & BWTN_START) ? w + 1 : 0u;
+    }
+    Scan(s_scan).InclusiveScan(x, x, cub::Max());
+#pragma unroll
+    for (uint32_t q = 0; q < BWTN_ITEMS; q++) {
+        const uint32_t w = threadIdx.x * BWTN_ITEMS + q;
+        if (w < W) s_prev[w] = x[q] ? (uint16_t)(x[q] - 1) : BWTN_NONE;
+    }
+    __syncthreads();
+#pragma unroll
+    for (uint32_t q = 0; q < BWTN_ITEMS; q++) {  // right to left: thread 0 takes the end of the window
+        const uint32_t w = BWTN_WIN - 1 - (threadIdx.x * BWTN_ITEMS + q);
+        x[q] = w < W ? ((s_key[w] & BWTN_START) ? w : BWTN_NONE) : (w == W && hi == m ? W : BWTN_NONE);
+    }
+    Scan(s_scan).InclusiveScan(x, x, cub::Min());
+#pragma unroll
+    for (uint32_t q = 0; q < BWTN_ITEMS; q++) {
+        const uint32_t w = BWTN_WIN - 1 - (threadIdx.x * BWTN_ITEMS + q);
+        if (w <= W) s_next[w] = (uint16_t)x[q];
+    }
+    __syncthreads();
+    for (uint32_t w = threadIdx.x; w < W; w += 256) s_key[w] &= ~BWTN_START;
+    __syncthreads();
+    for (uint32_t w = threadIdx.x; w < W; w += 256) {
+        const uint32_t u = lo + w;
+        const uint32_t s = s_prev[w], e = s_next[w + 1];
+        const bool small = s != BWTN_NONE && e != BWTN_NONE && e - s <= BWTN_G;
+        if (u >= t0 && u < t1) big[u] = small ? 0 : 1;
+        if (!small || lo + s < t0 || lo + s >= t1) continue;
+        const bwtc::GroupRank g = bwtc::bwt_group_rank(s_key + s, e - s, w - s);
+        const uint32_t gs = lo + s, head = cpos[gs], v = val[u];
+        sa[head + g.r] = v;
+        rank[v] = head + g.lt;
+        keep[gs + g.r] = g.eq > 1 ? 1 : 0;
+    }
+}
+
+// members l < mL of the large groups (lidx: their member indices, ascending): group starts, counted by a scan into ordinals
+__global__ void __launch_bounds__(256) bwtn_lstart_kernel(const uint32_t* __restrict__ lidx, const uint32_t* __restrict__ key2, uint32_t mL, uint32_t* __restrict__ ord) {
+    const uint32_t l = blockIdx.x * 256 + threadIdx.x;
+    if (l < mL) ord[l] = key2[lidx[l]] >> 31;
+}
+template <typename K>
+__global__ void __launch_bounds__(256) bwtn_lkeys_kernel(const uint32_t* __restrict__ lidx, const uint32_t* __restrict__ key2, const uint32_t* __restrict__ val,
+                                                          const uint32_t* __restrict__ ord, uint32_t mL, uint32_t kb, K* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint32_t l = blockIdx.x * 256 + threadIdx.x;
+    if (l >= mL) return;
+    const uint32_t u = lidx[l];
+    keys[l] = ((K)(ord[l] - 1) << kb) | (K)(key2[u] & ~BWTN_START);
+    vals[l] = val[u];
+}
+template <typename K>
+__global__ void __launch_bounds__(256) bwtn_lheads_kernel(const K* __restrict__ keys, const uint32_t* __restrict__ lidx, const uint32_t* __restrict__ cpos, uint32_t mL,
+                                                           uint32_t* __restrict__ f) {
+    const uint32_t l = blockIdx.x * 256 + threadIdx.x;
+    if (l >= mL) return;
+    f[l] = (l == 0 || keys[l] != keys[l - 1]) ? cpos[lidx[l]] : 0u;
+}
+__global__ void __launch_bounds__(256) bwtn_lapply_kernel(uint32_t* __restrict__ f, const uint32_t* __restrict__ block_max, const uint32_t* __restrict__ lidx,
+                                                           const uint32_t* __restrict__ cpos, const uint32_t* __restrict__ vals, uint32_t mL, uint32_t* __restrict__ sa,
+                                                           uint32_t* __restrict__ rank) {
+    const uint32_t l = blockIdx.x * 256 + threadIdx.x;
+    if (l >= mL) return;
+    const uint32_t blk = l / (256 * 8);
+    uint32_t g = f[l];
+    if (blk > 0) g = max(g, block_max[blk - 1]);
+    f[l] = g;
+    const uint32_t v = vals[l];
+    sa[cpos[lidx[l]]] = v;
+    rank[v] = g;
+}
+__global__ void __launch_bounds__(256) bwtn_lflags_kernel(const uint32_t* __restrict__ f, const uint32_t* __restrict__ lidx, const uint32_t* __restrict__ cpos, uint32_t mL,
+                                                           uint8_t* __restrict__ keep) {
+    const uint32_t l = blockIdx.x * 256 + threadIdx.x;
+    if (l >= mL) return;
+    const uint32_t g = f[l], u = lidx[l];
+    keep[u] = (g != cpos[u] || (l + 1 < mL && f[l + 1] == g)) ? 1 : 0;
+}
 }  // namespace
 
 size_t bwt_forward_batch_workspace(uint64_t total, uint32_t nblocks) {
@@ -447,16 +587,135 @@ size_t bwt_forward_batch_workspace(uint64_t total, uint32_t nblocks) {
     size_t temp3 = 0;  // no round runs a segmented sort, but its scratch size is still part of the workspace bound
     cub::DeviceSegmentedSort::SortPairs(nullptr, temp3, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)total,
                                         (int64_t)total, (const uint32_t*)nullptr, (const uint32_t*)nullptr);
-    return (size_t)total * (8 * 2 + 4 * 2 + 4 + 4 + 4 * 4 + 1) + 4 * ((size_t)total / 2048 + 16) + (size_t)nblocks * sizeof(BwtBatchBlock) + 16 * 256 +
-           std::max(std::max(temp, temp2), temp3) + 4096;
+    size_t temp4 = 0;  // ordinals of the large groups of a narrow round
+    cub::DeviceScan::InclusiveSum(nullptr, temp4, (uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)total);
+    // + the narrow rounds' large-group flags and member list (1 + 4 bytes per position)
+    return (size_t)total * (8 * 2 + 4 * 2 + 4 + 4 + 4 * 4 + 1 + 1 + 4) + 4 * ((size_t)total / 2048 + 16) + (size_t)nblocks * sizeof(BwtBatchBlock) + 18 * 256 +
+           std::max(std::max(temp, temp2), std::max(temp3, temp4)) + 4096;
 }
+
+namespace {
+// the rounds after the first one of bwt_forward_batch when every block has at most BWT_NARROW_MAX_N bytes; the workspace buffers of the
+// 56-bit rounds are reused (kv: 2 x 8 bytes per position for the large groups' keys, vv: 2 x 4 bytes for their suffixes)
+struct NarrowBufs {
+    uint32_t *sa, *rank, *cpos_a, *cpos_b, *key2, *val, *lidx, *count;
+    uint8_t *keep, *big;
+    uint64_t *kv_a, *kv_b;
+    uint32_t *vv_a, *vv_b, *block_max;
+    void* temp;
+    size_t temp_bytes;
+};
+struct RoundScope {  // a part of round r timed through the hook, if any
+    LzHook* hook;
+    std::string name;  // the hook keeps the pointer until end()
+    RoundScope(LzHook* h, int r, const char* part) : hook(h) {
+        if (!hook) return;
+        name = "bwt_round:" + std::to_string(r) + ":" + part;
+        hook->begin(name.c_str());
+    }
+    ~RoundScope() {
+        if (hook) hook->end();
+    }
+};
+
+template <typename K>
+cudaError_t bwtn_large(const NarrowBufs& B, uint32_t mL, uint32_t ob, uint32_t kb, cudaStream_t stream, uint64_t* launches, LzHook* hook, int round) {
+    const uint32_t T = 256, GL = (mL + T - 1) / T, nscan = (mL + 2047) / 2048;
+    K* keys_a = (K*)B.kv_a;
+    K* keys_b = (K*)B.kv_b;
+    {
+        RoundScope rs(hook, round, "large");
+        uint32_t* ord = (uint32_t*)B.kv_b;  // consumed before the sort writes there
+        bwtn_lstart_kernel<<<GL, T, 0, stream>>>(B.lidx, B.key2, mL, ord);
+        size_t tb = B.temp_bytes;
+        cudaError_t e = cub::DeviceScan::InclusiveSum(B.temp, tb, ord, ord, (int64_t)mL, stream);
+        if (e != cudaSuccess) return e;
+        bwtn_lkeys_kernel<K><<<GL, T, 0, stream>>>(B.lidx, B.key2, B.val, ord, mL, kb, keys_a, B.vv_a);
+        (*launches) += 4;
+    }
+    cub::DoubleBuffer<K> k(keys_a, keys_b);
+    cub::DoubleBuffer<uint32_t> v(B.vv_a, B.vv_b);
+    {
+        RoundScope rs(hook, round, "sort");
+        size_t tb = B.temp_bytes;
+        const int end_bit = (int)(ob + kb);
+        cudaError_t e = cub::DeviceRadixSort::SortPairs(B.temp, tb, k, v, (int64_t)mL, 0, end_bit, stream);
+        if (e != cudaSuccess) return e;
+        (*launches) += (end_bit + 7) / 8 + 1;
+    }
+    RoundScope rs(hook, round, "large");
+    uint32_t* f = (uint32_t*)(k.Current() == keys_a ? keys_b : keys_a);  // the key buffer the sort left free
+    bwtn_lheads_kernel<K><<<GL, T, 0, stream>>>(k.Current(), B.lidx, B.cpos_a, mL, f);
+    scan_max_local_kernel<<<nscan, 256, 0, stream>>>(f, mL, B.block_max);
+    scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(B.block_max, nscan);
+    bwtn_lapply_kernel<<<GL, T, 0, stream>>>(f, B.block_max, B.lidx, B.cpos_a, v.Current(), mL, B.sa, B.rank);
+    bwtn_lflags_kernel<<<GL, T, 0, stream>>>(f, B.lidx, B.cpos_a, mL, B.keep);
+    (*launches) += 5;
+    return cudaSuccess;
+}
+
+// rounds h = 6, 12, 24, ... over the m members in B.cpos_a (sorted positions of the unresolved groups after round 0)
+cudaError_t bwtn_rounds(NarrowBufs B, uint32_t m, const BwtBatchBlock* d_blocks, uint32_t nb, uint32_t max_n, cudaStream_t stream, uint64_t* launches,
+                        LzHook* hook) {
+    const uint32_t T = 256;
+    const uint32_t kb = bwtc::bwt_bits_for(max_n);  // second key: 0 .. n
+    uint32_t h = 6;
+    for (int round = 1; round < 48 && m > 0; round++) {
+        const uint32_t GM = (m + T - 1) / T, tiles = (m + BWTN_TILE - 1) / BWTN_TILE;
+        {
+            RoundScope rs(hook, round, "small");
+            bwtn_keys_kernel<<<GM, T, 0, stream>>>(B.sa, B.rank, B.cpos_a, m, d_blocks, nb, h, B.key2, B.val);
+            bwtn_small_kernel<<<tiles, T, 0, stream>>>(B.cpos_a, B.key2, B.val, m, B.sa, B.rank, B.keep, B.big);
+            (*launches) += 2;
+        }
+        uint32_t mL = 0;
+        {
+            RoundScope rs(hook, round, "select");
+            size_t tb = B.temp_bytes;
+            cudaError_t e = cub::DeviceSelect::Flagged(B.temp, tb, cub::CountingInputIterator<uint32_t>(0), B.big, B.lidx, B.count, (int64_t)m, stream);
+            if (e != cudaSuccess) return e;
+            (*launches) += 2;
+            if ((e = cudaMemcpyAsync(&mL, B.count, 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+        }
+        {
+            RoundScope rs(hook, round, "gap");
+            cudaError_t e = cudaStreamSynchronize(stream);
+            if (e != cudaSuccess) return e;
+        }
+        if (mL > 0) {
+            const uint32_t ob = bwtc::bwt_bits_for(mL / (BWTN_G + 1) - 1);  // ordinals 0 .. (large groups - 1), every large group has > G members
+            const cudaError_t e = ob + kb <= 32 ? bwtn_large<uint32_t>(B, mL, ob, kb, stream, launches, hook, round)
+                                                : bwtn_large<uint64_t>(B, mL, ob, kb, stream, launches, hook, round);
+            if (e != cudaSuccess) return e;
+        }
+        h *= 2;
+        if (h >= 2 * (uint64_t)max_n) break;  // every suffix pair has been compared past the end of its block
+        {
+            RoundScope rs(hook, round, "select");
+            size_t tb = B.temp_bytes;
+            cudaError_t e = cub::DeviceSelect::Flagged(B.temp, tb, (const uint32_t*)B.cpos_a, B.keep, B.cpos_b, B.count, (int64_t)m, stream);
+            if (e != cudaSuccess) return e;
+            (*launches) += 2;
+            if ((e = cudaMemcpyAsync(&m, B.count, 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+        }
+        {
+            RoundScope rs(hook, round, "gap");
+            cudaError_t e = cudaStreamSynchronize(stream);
+            if (e != cudaSuccess) return e;
+        }
+        std::swap(B.cpos_a, B.cpos_b);
+    }
+    return cudaSuccess;
+}
+}  // namespace
 // at most this many positions / blocks in one call (keys: 2 * lg bits with total < 2^lg; 10 bits of block index in the first key)
 uint64_t bwt_forward_batch_max_total() { return (1ull << 30) - 1; }
 uint32_t bwt_forward_batch_max_blocks() { return BWT_BATCH_MAX; }
 
 // BWTBlockCodec.Forward of blocks[k] = (src offset, dst offset, n >= 2, caller's block number): d_out_len[number] = n + header
 cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_t* src_off, const uint64_t* dst_off, const uint32_t* n_of, const uint32_t* number,
-                              uint32_t nb, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches) {
+                              uint32_t nb, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches, LzHook* hook,
+                              bool wide_rounds) {
     if (nb == 0) return cudaSuccess;
     if (nb > (uint32_t)BWT_BATCH_MAX) return cudaErrorInvalidValue;
     std::vector<BwtBatchBlock> hb(nb);
@@ -492,6 +751,8 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
     uint32_t* cpos_a = (uint32_t*)(ws + off); off = align(off + (size_t)total * 4);
     uint32_t* cpos_b = (uint32_t*)(ws + off); off = align(off + (size_t)total * 4);
     uint8_t* uflags = ws + off; off = align(off + (size_t)total);
+    uint8_t* big = ws + off; off = align(off + (size_t)total);
+    uint32_t* lidx = (uint32_t*)(ws + off); off = align(off + (size_t)total * 4);
     uint32_t* d_count = flags + 8;
     void* temp = ws + off;
     if (ws_bytes < off) return cudaErrorInvalidValue;
@@ -512,23 +773,32 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
     {
         cub::DoubleBuffer<uint64_t> k(keys_a, keys_b);
         cub::DoubleBuffer<uint32_t> v(idx_a, idx_b);
-        size_t tb = temp_bytes;
-        e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)total, 0, end_bit, stream);
-        if (e != cudaSuccess) return e;
-        (*launches) += 8;
+        {
+            RoundScope rs(hook, 0, "sort");
+            size_t tb = temp_bytes;
+            e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)total, 0, end_bit, stream);
+            if (e != cudaSuccess) return e;
+            (*launches) += 8;
+        }
         const uint64_t* sk = k.Current();
         sa = v.Current();
-        cudaMemsetAsync(flags, 0, 4, stream);
-        bwt_flag_kernel<<<G, T, 0, stream>>>(sk, total, head);
-        scan_max_local_kernel<<<nscan, 256, 0, stream>>>(head, total, block_max);
-        scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(block_max, nscan);
-        bwt_apply_rank_kernel<<<G, T, 0, stream>>>(head, block_max, sa, total, rank, flags);
-        (*launches) += 4;
+        {
+            RoundScope rs(hook, 0, "large");
+            cudaMemsetAsync(flags, 0, 4, stream);
+            bwt_flag_kernel<<<G, T, 0, stream>>>(sk, total, head);
+            scan_max_local_kernel<<<nscan, 256, 0, stream>>>(head, total, block_max);
+            scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(block_max, nscan);
+            bwt_apply_rank_kernel<<<G, T, 0, stream>>>(head, block_max, sa, total, rank, flags);
+            (*launches) += 4;
+        }
         uint32_t unsorted = 0;
         e = cudaMemcpyAsync(&unsorted, flags, 4, cudaMemcpyDeviceToHost, stream);
         if (e != cudaSuccess) return e;
-        e = cudaStreamSynchronize(stream);
-        if (e != cudaSuccess) return e;
+        {
+            RoundScope rs(hook, 0, "gap");
+            e = cudaStreamSynchronize(stream);
+            if (e != cudaSuccess) return e;
+        }
         if (!unsorted || h >= max_n) {
             bwtb_emit_kernel<<<G, T, 0, stream>>>(d_in, d_blocks, nb, total, sa, rank, d_out);
             bwtb_header_kernel<<<(nb + 63) / 64, 64, 0, stream>>>(d_blocks, nb, rank, d_out, d_out_len);
@@ -537,53 +807,86 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
         }
     }
     // later rounds: the members of groups with more than one suffix only
+    const bool narrow = !wide_rounds && max_n <= BWT_NARROW_MAX_N;
     uint32_t m = 0;
     {
+        RoundScope rs(hook, 0, "select");
         bwtu_flags_full_kernel<<<G, T, 0, stream>>>(head, total, uflags);
         size_t tb = temp_bytes;
         e = cub::DeviceSelect::Flagged(temp, tb, cub::CountingInputIterator<uint32_t>(0), uflags, cpos_a, d_count, (int64_t)total, stream);
         if (e != cudaSuccess) return e;
-        tb = temp_bytes;
-        e = cub::DeviceSelect::Flagged(temp, tb, (const uint32_t*)sa, uflags, cval_a, d_count, (int64_t)total, stream);
-        if (e != cudaSuccess) return e;
-        (*launches) += 5;
+        (*launches) += 3;
+        if (!narrow) {  // the narrow rounds read the suffixes from sa
+            tb = temp_bytes;
+            e = cub::DeviceSelect::Flagged(temp, tb, (const uint32_t*)sa, uflags, cval_a, d_count, (int64_t)total, stream);
+            if (e != cudaSuccess) return e;
+            (*launches) += 2;
+        }
         e = cudaMemcpyAsync(&m, d_count, 4, cudaMemcpyDeviceToHost, stream);
         if (e != cudaSuccess) return e;
+    }
+    {
+        RoundScope rs(hook, 0, "gap");
         e = cudaStreamSynchronize(stream);
         if (e != cudaSuccess) return e;
+    }
+    if (narrow) {
+        NarrowBufs B;
+        B.sa = sa, B.rank = rank, B.cpos_a = cpos_a, B.cpos_b = cpos_b;
+        B.key2 = sa == idx_a ? idx_b : idx_a, B.val = head, B.lidx = lidx, B.count = d_count;
+        B.keep = uflags, B.big = big, B.kv_a = keys_a, B.kv_b = keys_b, B.vv_a = cval_a, B.vv_b = cval_b, B.block_max = block_max;
+        B.temp = temp, B.temp_bytes = temp_bytes;
+        e = bwtn_rounds(B, m, d_blocks, nb, max_n, stream, launches, hook);
+        if (e != cudaSuccess) return e;
+        m = 0;
     }
     end_bit = 2 * (int)lg;
     uint32_t* nhead = head;  // reused: new group heads of the compacted members
     // later rounds: 64-bit radix sorts of (group head, second key) over the compacted members
     for (int round = 1; round < 48 && m > 0; round++) {
         const uint32_t GM = (m + T - 1) / T, nscan_m = (m + 2047) / 2048;
-        bwtu_keys_kernel<<<GM, T, 0, stream>>>(rank, cval_a, m, d_blocks, nb, h, lg, keys_a);
         cub::DoubleBuffer<uint64_t> k(keys_a, keys_b);
         cub::DoubleBuffer<uint32_t> v(cval_a, cval_b);
-        size_t tb = temp_bytes;
-        e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)m, 0, end_bit, stream);
-        if (e != cudaSuccess) return e;
-        bwtu_heads_kernel<<<GM, T, 0, stream>>>(k.Current(), cpos_a, m, nhead);
+        {
+            RoundScope rs(hook, round, "large");
+            bwtu_keys_kernel<<<GM, T, 0, stream>>>(rank, cval_a, m, d_blocks, nb, h, lg, keys_a);
+        }
+        {
+            RoundScope rs(hook, round, "sort");
+            size_t tb = temp_bytes;
+            e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)m, 0, end_bit, stream);
+            if (e != cudaSuccess) return e;
+        }
         const uint32_t* sorted_val = v.Current();
         uint32_t* other = v.Current() == cval_a ? cval_b : cval_a;
-        scan_max_local_kernel<<<nscan_m, 256, 0, stream>>>(nhead, m, block_max);
-        scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(block_max, nscan_m);
-        bwtu_apply_kernel<<<GM, T, 0, stream>>>(nhead, block_max, cpos_a, sorted_val, m, sa, rank);
+        {
+            RoundScope rs(hook, round, "large");
+            bwtu_heads_kernel<<<GM, T, 0, stream>>>(k.Current(), cpos_a, m, nhead);
+            scan_max_local_kernel<<<nscan_m, 256, 0, stream>>>(nhead, m, block_max);
+            scan_max_blocks_kernel<<<1, 1024, 0, stream>>>(block_max, nscan_m);
+            bwtu_apply_kernel<<<GM, T, 0, stream>>>(nhead, block_max, cpos_a, sorted_val, m, sa, rank);
+        }
         (*launches) += 13;
         h *= 2;
         if (h >= 2 * (uint64_t)max_n) break;  // every suffix pair has been compared past the end of its block
-        bwtu_flags_kernel<<<GM, T, 0, stream>>>(nhead, cpos_a, m, uflags);
-        tb = temp_bytes;
-        e = cub::DeviceSelect::Flagged(temp, tb, (const uint32_t*)cpos_a, uflags, cpos_b, d_count, (int64_t)m, stream);
-        if (e != cudaSuccess) return e;
-        tb = temp_bytes;
-        e = cub::DeviceSelect::Flagged(temp, tb, sorted_val, uflags, other, d_count, (int64_t)m, stream);
-        if (e != cudaSuccess) return e;
-        (*launches) += 5;
-        e = cudaMemcpyAsync(&m, d_count, 4, cudaMemcpyDeviceToHost, stream);
-        if (e != cudaSuccess) return e;
-        e = cudaStreamSynchronize(stream);
-        if (e != cudaSuccess) return e;
+        {
+            RoundScope rs(hook, round, "select");
+            bwtu_flags_kernel<<<GM, T, 0, stream>>>(nhead, cpos_a, m, uflags);
+            size_t tb = temp_bytes;
+            e = cub::DeviceSelect::Flagged(temp, tb, (const uint32_t*)cpos_a, uflags, cpos_b, d_count, (int64_t)m, stream);
+            if (e != cudaSuccess) return e;
+            tb = temp_bytes;
+            e = cub::DeviceSelect::Flagged(temp, tb, sorted_val, uflags, other, d_count, (int64_t)m, stream);
+            if (e != cudaSuccess) return e;
+            (*launches) += 5;
+            e = cudaMemcpyAsync(&m, d_count, 4, cudaMemcpyDeviceToHost, stream);
+            if (e != cudaSuccess) return e;
+        }
+        {
+            RoundScope rs(hook, round, "gap");
+            e = cudaStreamSynchronize(stream);
+            if (e != cudaSuccess) return e;
+        }
         std::swap(cpos_a, cpos_b);
         if (other != cval_a) std::swap(cval_a, cval_b);  // the compacted suffixes are the next round's input
     }

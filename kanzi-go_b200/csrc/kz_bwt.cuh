@@ -8,11 +8,15 @@ size_t bwt_forward_workspace(uint32_t n);
 cudaError_t bwt_forward_device(const uint8_t* d_src, uint32_t n, uint8_t* d_dst, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream,
                                uint64_t* launches);
 // BWTBlockCodec.Forward of a batch of blocks sorted together (block k: n_of[k] >= 2 bytes at d_in + src_off[k] -> d_out + dst_off[k]; d_out_len[number[k]] = length)
+// hook (optional): every part of every doubling round timed under "bwt_round:<r>:<part>"; wide_rounds: the 56-bit global sort in every round
+// (the rounds the batches with a block above 4 MiB take), same output
 size_t bwt_forward_batch_workspace(uint64_t total, uint32_t nblocks);
 uint64_t bwt_forward_batch_max_total();
 uint32_t bwt_forward_batch_max_blocks();
+struct LzHook;
 cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_t* src_off, const uint64_t* dst_off, const uint32_t* n_of, const uint32_t* number,
-                              uint32_t nb, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches);
+                              uint32_t nb, uint32_t* d_out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches, LzHook* hook = nullptr,
+                              bool wide_rounds = false);
 // BWTBlockCodec.Inverse of a batch (one sort, one head list, one set of launches for all blocks); h_headers + 64 k = first 33 bytes of block k's stream
 size_t bwt_inverse_batch_workspace(uint64_t total, uint32_t nblocks);
 uint64_t bwt_inverse_batch_max_total();

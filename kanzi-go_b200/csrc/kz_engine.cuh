@@ -130,6 +130,7 @@ struct kz_ctx {
     std::string err;
     uint64_t launches = 0;
     bool profile = false;
+    int bwt_profile = 0;  // kz_bwt_profile: bit 0 times the BWT forward rounds (with profile), bit 1 forces the 56-bit rounds
     kz::EncPlan enc_plan;
     bool fragment = false;        // encode_batch: LAYOUT_STREAM without the end marker (kz_compress_fragment_device, a writer session)
     bool volatile_lead = false;   // encode_batch: the leading segment is a writer session's header or carry, kept out of the plan key
