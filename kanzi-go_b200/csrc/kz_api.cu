@@ -1212,7 +1212,7 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
     } else if (t == KZ_T_RANK || t == KZ_T_MTFT) {  // SBRT.Forward never declines (buffers are sized for MaxEncodedLen)
         std::vector<SbrtBlock> sb(nblocks);
         std::vector<uint32_t> seg_block;
-        uint32_t max_segs = 0;
+        uint32_t max_segs = 0, max_len = 0;
         for (uint32_t b = 0; b < nblocks; b++) {
             sb[b].src_off = b * istride;
             sb[b].dst_off = b * ostride;
@@ -1222,6 +1222,7 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             sb[b].pad = 0;
             const uint32_t nseg = sb[b].active ? (len[b] + SBRT_SEG_BYTES - 1) / SBRT_SEG_BYTES : 0;
             max_segs = std::max(max_segs, nseg);
+            if (sb[b].active) max_len = std::max(max_len, len[b]);
             for (uint32_t s = 0; s < nseg; s++) seg_block.push_back(b);
             applied[b] = sb[b].active ? 1 : 0;
         }
@@ -1246,8 +1247,7 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             }
             {
                 LaunchScope ls(ctx, "sbrt_rank");
-                sbrt_rank_kernel<<<(nsegs + 3) / 4, 128, 0, ctx->stream>>>(d_in, d_sb, (int)nblocks, mode, (const uint32_t*)(T + o_map), nsegs,
-                                                                          ctx->d_seg.as<int32_t>(), d_out);
+                sbrt_rank_launch(d_in, d_sb, mode, (const uint32_t*)(T + o_map), nsegs, ctx->d_seg.as<int32_t>(), d_out, max_len, ctx->stream);
             }
             CK(cudaGetLastError());
             CK(cudaStreamSynchronize(ctx->stream));  // the tables live in d_tables, which the next stage reuses

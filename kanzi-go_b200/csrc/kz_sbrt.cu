@@ -14,13 +14,15 @@
 // segments are processed concurrently, each starting from the per-symbol (last, second last) positions before it:
 //   1. sbrt_last2_kernel   per segment: last two positions of every symbol inside the segment (shared-memory atomics);
 //   2. sbrt_carry_kernel   per block: running (last, second last) over the segments, one thread per symbol;
-//   3. sbrt_rank_kernel    per segment, one warp: lane l owns the keys of symbols l, l+32, ...; per byte the owner of c
-//                          broadcasts key(c), every lane counts its larger keys, one REDUX gives r.
+//   3. sbrt_rank_kernel    per segment, one warp: the keys of the 256 symbols in a shared-memory table (32-bit keys,
+//                          kz_sbrt_core.cuh); per byte every lane counts the keys larger than key(c) among 8 of them, one REDUX
+//                          gives r. Blocks above 16 MiB take sbrt_rank_wide_kernel (64-bit keys in registers).
 // Inverse: the list itself is the decoder state (r -> c needs the list, which needs all earlier symbols), so a block is
 // one serial chain: one CTA per block walks it with the list in registers (blocks run concurrently).
 #include <algorithm>
 
 #include "kz_sbrt.cuh"
+#include "kz_sbrt_core.cuh"
 
 namespace kz {
 
@@ -63,20 +65,116 @@ __global__ void __launch_bounds__(256) sbrt_carry_kernel(const SbrtBlock* __rest
         const int32_t a = t[0], b = t[1];
         t[0] = l1;
         t[1] = l2;
-        if (a >= 0) {
-            l2 = b >= 0 ? b : l1;
-            l1 = a;
+        sbrtc::sbrt_carry(l1, l2, a, b);
+    }
+}
+
+// acc + inc for every key of k above kc. Stated in PTX so that each key costs one compare and one predicated add (the C++ sum compiles to a
+// compare, an add and a predicated move per key).
+KZ_D uint32_t add_if_above(uint32_t acc, uint32_t kd, uint32_t kc, uint32_t inc) {
+    asm("{\n\t.reg .pred p;\n\tsetp.gt.u32 p, %1, %2;\n\t@p add.u32 %0, %0, %3;\n\t}" : "+r"(acc) : "r"(kd), "r"(kc), "r"(inc));
+    return acc;
+}
+KZ_D uint32_t count_above(uint32_t acc, uint4 k, uint32_t kc, uint32_t inc) {
+    return add_if_above(add_if_above(add_if_above(add_if_above(acc, k.x, kc, inc), k.y, kc, inc), k.z, kc, inc), k.w, kc, inc);
+}
+// the tie terms of the 4 symbols d0 .. d0 + 3 held in k / t
+KZ_D uint32_t count_ties(uint4 k, uint4 t, uint32_t d0, uint32_t kc, uint32_t tc, uint32_t c) {
+    using namespace sbrtc;
+    return sbrt_tie(k.x, t.x, d0, kc, tc, c) + sbrt_tie(k.y, t.y, d0 + 1, kc, tc, c) + sbrt_tie(k.z, t.z, d0 + 2, kc, tc, c) +
+           sbrt_tie(k.w, t.w, d0 + 3, kc, tc, c);
+}
+
+// ---- 3. ranks of one segment by one warp, blocks of at most SBRT_KEY_MAX_LEN bytes. MODE: 1 = MTFT, 2 = RANK
+// The 32-bit keys and last positions of the 256 symbols (kz_sbrt_core.cuh) sit in a per-warp table in shared memory. Per byte every lane
+// reads key(c) and t(c) with one broadcast load each, and counts the larger keys among its 8 with two 16-byte loads. The tie terms are added
+// only for a key that can tie (clipped, or a symbol never seen). The counts of the 4 bytes of a word share one register, one byte each, so one
+// REDUX per word gives 4 ranks. Every lane then writes the same new entry: the same value to the same word, so each lane reads it back in
+// program order and no warp barrier is needed between bytes.
+template <int MODE>
+__global__ void __launch_bounds__(128) sbrt_rank_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks,
+                                                        const uint32_t* __restrict__ seg_block, uint32_t nsegs_total,
+                                                        const int32_t* __restrict__ table, uint8_t* __restrict__ out) {
+    using namespace sbrtc;
+    struct Table {
+        uint32_t key[256];
+        uint32_t t[256];
+    };
+    __shared__ __align__(16) uint8_t s_in[4][SBRT_SEG];
+    __shared__ __align__(16) Table s_tab[4];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t g = blockIdx.x * 4 + warp;  // global segment id
+    if (g >= nsegs_total) return;
+    const SbrtBlock blk = blocks[seg_block[g]];
+    if (!blk.active) return;
+    const uint32_t s0 = (g - blk.seg_base) * SBRT_SEG;
+    const uint32_t cnt = min((uint32_t)SBRT_SEG, blk.len - s0);
+    const uint8_t* src = data + blk.src_off + s0;
+    uint8_t* dst = out + blk.dst_off + s0;
+    // stage the segment (block offsets are 16-byte aligned, segments are multiples of 16); zeros up to the next multiple of 128, whose ranks
+    // are computed and never stored
+    {
+        const uint32_t n16 = cnt >> 4, end = (cnt + 127) & ~127u;
+        const uint4* s4 = reinterpret_cast<const uint4*>(src);
+        uint4* d4 = reinterpret_cast<uint4*>(s_in[warp]);
+        for (uint32_t i = lane; i < n16; i += 32) d4[i] = __ldg(&s4[i]);
+        for (uint32_t i = (n16 << 4) + lane; i < end; i += 32) s_in[warp][i] = i < cnt ? src[i] : 0;
+    }
+    uint32_t* keys = s_tab[warp].key;
+    uint32_t* ts = s_tab[warp].t;
+    const int32_t* t0 = table + (size_t)g * 512;
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const int sym = lane + 32 * k;
+        const SbrtEntry e = sbrt_start(MODE, t0[2 * sym], t0[2 * sym + 1]);
+        keys[sym] = e.key;
+        ts[sym] = e.t;
+    }
+    __syncwarp();
+    // lane l counts symbols 4 l .. 4 l + 3 and 128 + 4 l .. 128 + 4 l + 3 (conflict-free 16-byte loads)
+    const uint4* kv = reinterpret_cast<const uint4*>(keys);
+    const uint4* tv = reinterpret_cast<const uint4*>(ts);
+    const uint32_t* in4 = reinterpret_cast<const uint32_t*>(s_in[warp]);
+    uint32_t pos = s0;
+    for (uint32_t i0 = 0; i0 < cnt; i0 += 128) {  // 128 positions per round: lane l keeps the ranks of positions i0 + 4 l .. + 3
+        uint32_t pack = 0;
+#pragma unroll 2
+        for (uint32_t w = 0; w < 32; w++) {
+            const uint32_t word = in4[(i0 >> 2) + w];
+            uint32_t larger = 0;  // this lane's count for byte m of the word in byte m
+#pragma unroll
+            for (int m = 0; m < 4; m++, pos++) {
+                const uint32_t c = __byte_perm(word, 0u, 0x4440u + m), inc = 1u << (8 * m);
+                const uint32_t kc = keys[c], tc = ts[c];
+                const uint4 a = kv[lane], b = kv[32 + lane];
+                larger = count_above(count_above(larger, a, kc, inc), b, kc, inc);
+                if (sbrt_ties_possible(kc)) {  // the same in every lane
+                    const uint4 ta = tv[lane], tb = tv[32 + lane];
+                    larger += (count_ties(a, ta, 4 * lane, kc, tc, c) + count_ties(b, tb, 128 + 4 * lane, kc, tc, c)) << (8 * m);
+                }
+                const SbrtEntry e = sbrt_coded<MODE>(pos, tc);
+                keys[c] = e.key;
+                ts[c] = e.t;
+            }
+            const uint32_t ranks = __reduce_add_sync(0xFFFFFFFFu, larger);  // a rank is at most 255: no carry between the bytes
+            pack = w == (uint32_t)lane ? ranks : pack;
+        }
+        const uint32_t base = i0 + 4 * lane;
+        if (base + 4 <= cnt) {
+            *reinterpret_cast<uint32_t*>(dst + base) = pack;
+        } else {
+            for (uint32_t q = 0; q < 4 && base + q < cnt; q++) dst[base + q] = (uint8_t)(pack >> (8 * q));
         }
     }
 }
 
-// ---- 3. ranks of one segment by one warp. mode: 1 = MTFT, 2 = RANK
+// ---- 3'. the same for blocks longer than SBRT_KEY_MAX_LEN (kanzi allows up to 1 GiB): 64-bit keys in registers. mode: 1 = MTFT, 2 = RANK
 // key = q << 32 | (t + 2^31): unsigned 64-bit order = (q, t) order; t = -1-d for a symbol never seen
-KZ_D uint64_t sbrt_key(int32_t q, int32_t t) { return ((uint64_t)(uint32_t)q << 32) | (uint32_t)(t ^ 0x80000000); }
+KZ_D uint64_t sbrt_key_wide(int32_t q, int32_t t) { return ((uint64_t)(uint32_t)q << 32) | (uint32_t)(t ^ 0x80000000); }
 
-__global__ void __launch_bounds__(128) sbrt_rank_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks, int mode,
-                                                        const uint32_t* __restrict__ seg_block, uint32_t nsegs_total,
-                                                        const int32_t* __restrict__ table, uint8_t* __restrict__ out) {
+__global__ void __launch_bounds__(128) sbrt_rank_wide_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int mode,
+                                                             const uint32_t* __restrict__ seg_block, uint32_t nsegs_total,
+                                                             const int32_t* __restrict__ table, uint8_t* __restrict__ out) {
     __shared__ uint8_t s_in[4][SBRT_SEG];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t g = blockIdx.x * 4 + warp;  // global segment id
@@ -110,7 +208,7 @@ __global__ void __launch_bounds__(128) sbrt_rank_kernel(const uint8_t* __restric
             t = l1;
             q = mode == 1 ? l1 : (l1 + (l2 >= 0 ? l2 : 0)) >> 1;
         }
-        key[k] = sbrt_key(q, t);
+        key[k] = sbrt_key_wide(q, t);
         last[k] = l1 >= 0 ? l1 : 0;  // p[c] (0 before the first occurrence)
     }
     __syncwarp();
@@ -143,7 +241,7 @@ __global__ void __launch_bounds__(128) sbrt_rank_kernel(const uint8_t* __restric
             const int32_t pos = (int32_t)(s0 + i);
             const int32_t qc = mode == 1 ? pos : (pos + pc) >> 1;
             if (lane == owner) {
-                const uint64_t nk = sbrt_key(qc, pos);
+                const uint64_t nk = sbrt_key_wide(qc, pos);
 #pragma unroll
                 for (int k = 0; k < 8; k++) {
                     if (slot == k) {
@@ -436,6 +534,14 @@ static size_t spread_chains(K kernel, int nblocks) {
         return 0;
     }
     return dyn;
+}
+
+void sbrt_rank_launch(const uint8_t* data, const SbrtBlock* d_blocks, int mode, const uint32_t* seg_block, uint32_t nsegs, const int32_t* table,
+                      uint8_t* out, uint32_t max_len, cudaStream_t stream) {
+    const unsigned grid = (nsegs + 3) / 4;
+    if (max_len > sbrtc::SBRT_KEY_MAX_LEN) sbrt_rank_wide_kernel<<<grid, 128, 0, stream>>>(data, d_blocks, mode, seg_block, nsegs, table, out);
+    else if (mode == 2) sbrt_rank_kernel<2><<<grid, 128, 0, stream>>>(data, d_blocks, seg_block, nsegs, table, out);
+    else sbrt_rank_kernel<1><<<grid, 128, 0, stream>>>(data, d_blocks, seg_block, nsegs, table, out);
 }
 
 void sbrt_inverse_launch_len(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, uint32_t max_len, cudaStream_t stream) {
