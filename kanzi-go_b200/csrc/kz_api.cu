@@ -247,6 +247,7 @@ int hash_blocks(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>&
 }
 
 // decodingTask.decode :1990-2006: hash of the decoded block against the transmitted checksum
+const char* const CHECKSUM_MISMATCH = "Corrupted bitstream: block checksum mismatch";
 int verify_checksums(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint32_t bits,
                      std::vector<DecJob>& jobs) {
     std::vector<uint64_t> hv;
@@ -256,7 +257,7 @@ int verify_checksums(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint6
         const uint64_t want = bits == 32 ? (jobs[b].checksum & 0xFFFFFFFFull) : jobs[b].checksum;
         if (hv[b] != want) {
             jobs[b].status = -KZ_ERR_CRC_CHECK;
-            return ctx->fail(KZ_ERR_CRC_CHECK, "Corrupted bitstream: block checksum mismatch");
+            return ctx->fail(KZ_ERR_CRC_CHECK, CHECKSUM_MISMATCH);
         }
     }
     return 0;
@@ -667,6 +668,101 @@ __global__ void stream_walk_kernel(const uint32_t* __restrict__ words, const Wal
 __global__ void record_walk_kernel(const uint32_t* __restrict__ words, uint64_t start, uint64_t end, uint32_t max_records, uint64_t max_bits,
                                    uint64_t* __restrict__ bit_off, uint64_t* __restrict__ bits, WalkResult* __restrict__ out) {
     if (blockIdx.x == 0 && threadIdx.x == 0) *out = walk_records(words, start, end, max_records, max_bits, bit_off, bits);
+}
+
+// What walk_streams found in one stream: n records walked, status 0 or -(error code), overflow = the block range holds more records
+// than could be stored; bit_off / bits = the stored records, records first .. first + size - 1 of the stream.
+struct Walked {
+    uint64_t n = 0, first = 0;
+    int32_t status = 0;
+    bool overflow = false;
+    std::vector<uint64_t> bit_off, bits;
+    // appends the stored records as DecJobs of `own`; last[b]: the record is the stream's last
+    void append(uint32_t own, std::vector<DecJob>& jobs, std::vector<uint32_t>& owner, std::vector<uint8_t>& last) const {
+        for (size_t r = 0; r < bit_off.size(); r++) {
+            DecJob j = DecJob();
+            j.bit_off = bit_off[r];
+            j.bits = bits[r];
+            jobs.push_back(j);
+            owner.push_back(own);
+            last.push_back(first + r + 1 == n);
+        }
+    }
+};
+
+// Walks the complete streams of jobs (start_bit, end_bit, stop_after and max_blocks set: at most max_blocks records are stored) with
+// stream_walk_kernel, one thread per stream. Only the records of the block range from / to (kz_set_block_range, -1 = not given) are
+// stored. Without a range max_blocks also bounds the walk; with one the walk goes over every record to the end marker, so that a walk
+// error behind the range is still found, and only the stream's bytes bound it (a record takes at least 9 bits). The counts and the first
+// min(slots, 1024) records come back in one round trip; the rest only when more were stored.
+int walk_streams(kz_ctx* ctx, const uint32_t* d_words, std::vector<WalkJob>& jobs, int64_t from, int64_t to, std::vector<Walked>& out) {
+    const uint32_t ns = (uint32_t)jobs.size();
+    const bool ranged = from >= 0 || to >= 0;
+    uint64_t keep_lo = 0, keep_hi = ~0ull, slots = 0;
+    if (ranged) block_range_records(from, to, &keep_lo, &keep_hi);
+    for (WalkJob& j : jobs) {
+        const uint64_t k = std::min<uint64_t>(j.max_blocks, keep_hi - keep_lo);
+        if (ranged) j.max_blocks = 0xFFFFFFFFu;
+        j.out = slots;
+        j.keep_lo = keep_lo;
+        j.keep_hi = keep_lo + k;
+        slots += k;
+    }
+    CK(ctx->d_dl.ensure((size_t)slots * 16 + (size_t)ns * 8 + 64));
+    uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
+    uint64_t* d_bbits = d_boff + slots;
+    uint32_t* d_cnt = (uint32_t*)(d_bbits + slots);
+    const WalkJob* d_jobs = nullptr;  // one stream: its job goes as a kernel parameter
+    if (ns > 1) {
+        Packer pk;
+        const size_t o_wj = pk.add(jobs.data(), jobs.size() * sizeof(WalkJob));
+        int rc = upload(ctx, pk);
+        if (rc) return rc;
+        d_jobs = (const WalkJob*)(ctx->d_tables.as<uint8_t>() + o_wj);
+    }
+    {
+        LaunchScope ls(ctx, "stream_walk");
+        stream_walk_kernel<<<(ns + 127) / 128, 128, 0, ctx->stream>>>(d_words, d_jobs, jobs[0], (int)ns, d_boff, d_bbits, d_cnt);
+    }
+    CK(cudaGetLastError());
+    const uint64_t spec = std::min<uint64_t>(slots, 1024);
+    const size_t cs_bytes = round16((uint64_t)ns * 8);
+    CK(ctx->h_dl.ensure(cs_bytes + (size_t)spec * 16 + 64));
+    const uint32_t* cs = (uint32_t*)ctx->h_dl.p;
+    uint64_t* h_boff = (uint64_t*)((uint8_t*)ctx->h_dl.p + cs_bytes);
+    uint64_t* h_bbits = h_boff + spec;
+    CK(cudaMemcpyAsync(ctx->h_dl.p, d_cnt, (size_t)ns * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h_boff, d_boff, (size_t)spec * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h_bbits, d_bbits, (size_t)spec * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    out.assign(ns, Walked());
+    uint64_t used = 0;  // entries up to the last stored record
+    for (uint32_t s = 0; s < ns; s++) {
+        Walked& w = out[s];
+        w.n = cs[2 * s];
+        w.first = keep_lo;
+        w.status = (int32_t)cs[2 * s + 1];
+        const uint64_t in_range = std::min(w.n, keep_hi) - std::min(w.n, keep_lo), k = jobs[s].keep_hi - keep_lo;
+        w.overflow = in_range > k;
+        if (w.status || w.overflow) continue;
+        w.bit_off.resize(in_range);
+        w.bits.resize(in_range);
+        used = std::max(used, jobs[s].out + in_range);
+    }
+    if (used > spec) {  // the counts are read: h_dl now takes all stored records
+        CK(ctx->h_dl.ensure((size_t)used * 16 + 64));
+        h_boff = (uint64_t*)ctx->h_dl.p;
+        h_bbits = h_boff + used;
+        CK(cudaMemcpyAsync(h_boff, d_boff, (size_t)used * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(h_bbits, d_bbits, (size_t)used * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    for (uint32_t s = 0; s < ns; s++) {
+        Walked& w = out[s];
+        std::copy(h_boff + jobs[s].out, h_boff + jobs[s].out + w.bit_off.size(), w.bit_off.begin());
+        std::copy(h_bbits + jobs[s].out, h_bbits + jobs[s].out + w.bits.size(), w.bits.begin());
+    }
+    return 0;
 }
 
 // jobs[b].bit_off / bits / out_off must be set; fills pre_len, mode, ..., status. d_words = device stream buffer.
@@ -1544,10 +1640,11 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
 // Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186) of every block of a batch. The entropy
 // stage left block b's pre_len bytes at d_pre + b*pstride, a scratch buffer of this context with room for pstride - 64 bytes per
 // block; the stages alternate between it and ctx->d_tmp2. out_len[b] = decoded length of block b. Once the lengths are known,
-// place(b, len, &at) is called for every block in order and gives its destination: at = nullptr drops the block, a false return fails
-// the call with KZ_ERR_WRITE_FILE (no room). All blocks are then copied by one batch_copy_kernel launch.
+// place(b, len) is called for every block in order and gives its offset in d_dst, or NO_ROOM: the block is not copied. The placed
+// blocks are then copied by one batch_copy_kernel launch.
+const uint64_t NO_ROOM = ~0ull;
 template <class Place>
-int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, Place&& place,
+int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& jobs, uint8_t* d_pre, uint64_t pstride, uint8_t* d_dst, Place&& place,
                   std::vector<uint32_t>& out_len) {
     const uint32_t nblocks = (uint32_t)jobs.size();
     out_len.assign(nblocks, 0);
@@ -1582,9 +1679,8 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
     }
     CopyList out;
     for (uint32_t b = 0; b < nblocks; b++) {
-        uint8_t* at = nullptr;
-        if (!place(b, len[b], &at)) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-        if (at) out.add(cur + b * pstride, at, len[b]);
+        const uint64_t at = place(b, len[b]);
+        if (at != NO_ROOM) out.add(cur + b * pstride, d_dst + at, len[b]);
         out_len[b] = len[b];
     }
     int rc = run_copies(ctx, out);
@@ -1593,17 +1689,108 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
     return 0;
 }
 
-// Destinations of blocks decoded back to back into d_dst (cap bytes): what inverse_stage's place() does for one stream.
+// Destinations of blocks decoded back to back into an output buffer of cap bytes: decode_walked's place() for one stream.
 struct BackToBack {
-    uint8_t* d_dst;
     uint64_t cap, off = 0;
-    bool operator()(uint32_t, uint32_t len, uint8_t** at) {
-        if (off + len > cap) return false;
-        *at = d_dst + off;
+    uint64_t operator()(uint32_t, uint32_t len) {
+        if (off + len > cap) return NO_ROOM;
         off += len;
-        return true;
+        return off - len;
     }
 };
+
+// The block stages of walked records of one stream header: jobs (bit_off / bits set) are the blocks, in order; block b belongs to stream
+// owner[b], and last[b] says it is (or may be) its stream's last record, which exempts it from NONE's rule that a block is a multiple of
+// 16 long. place(b, len) gives block b's offset in d_dst, or NO_ROOM. fail[o] is the failure held for stream o: a block failure is noted
+// there (DecodeFailure: earliest stage, then earliest block), and the blocks of o skip every stage whose failure could not beat it. In
+// this order, as decompress_device_impl always checked them:
+//   1. headers: per block, its header status, then for NONE its place and the multiple-of-16 rule;
+//   2. entropy decode: NONE straight to the placed destination, other plans into ctx->d_tmp slots of decode_stride;
+//   3. inverse transforms into their place (KZ_ERR_WRITE_FILE when there is no room);
+//   4. checksums of the bytes where they landed.
+// A failing decode_batch or inverse_stage cannot name the block: its failure goes to every stream of the batch at that stage. The return
+// value is kept for call-level errors (CUDA, allocation, a bad hash launch).
+template <class Place>
+int decode_walked(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan, const uint32_t* d_words, uint64_t words_len, std::vector<DecJob>& jobs,
+                  const std::vector<uint32_t>& owner, const std::vector<uint8_t>& last, Place&& place, uint8_t* d_dst, DecodeFailure* fail) {
+    const uint32_t nb = (uint32_t)jobs.size();
+    std::vector<uint32_t> idx;  // the blocks of the stage in progress
+    std::vector<DecJob> run;
+    auto stage = [&](int s) {   // the blocks whose stream can still fail at stage s
+        idx.clear();
+        run.clear();
+        for (uint32_t b = 0; b < nb; b++)
+            if (fail[owner[b]].runs(s)) idx.push_back(b), run.push_back(jobs[b]);
+        return !run.empty();
+    };
+    auto done = [&]() {
+        for (size_t i = 0; i < idx.size(); i++) jobs[idx[i]] = run[i];
+    };
+    auto note_all = [&](int s, int rc) {
+        for (uint32_t b : idx) fail[owner[b]].note(s, rc, ctx->err);
+    };
+    ctx->stream_bs = sh.block_size;
+    if (!stage(STAGE_HEADER)) return 0;
+    int rc = decode_parse_headers(ctx, d_words, run, sh.checksum_bits, sh.block_size);
+    if (rc) return rc;
+    done();
+    for (uint32_t b = 0; b < nb; b++) {
+        DecodeFailure& f = fail[owner[b]];
+        DecJob& j = jobs[b];
+        if (!f.runs(STAGE_HEADER)) continue;
+        if (j.status) {
+            f.note(STAGE_HEADER, j.status, "Invalid compressed block header");
+        } else if (plan.none()) {  // NONE: the decoded length is pre_len
+            j.out_off = place(b, j.pre_len);
+            if (j.out_off == NO_ROOM) f.note(STAGE_HEADER, -KZ_ERR_WRITE_FILE, "output buffer too small");
+            else if (!last[b] && (j.pre_len & 15)) f.note(STAGE_HEADER, -KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+        }
+    }
+    if (!stage(STAGE_DECODE)) return 0;
+    uint64_t stride = 0;
+    if (!plan.none()) {
+        uint32_t max_pre = 0;
+        for (const DecJob& j : run) max_pre = std::max(max_pre, j.pre_len);
+        stride = decode_stride(sh.block_size, max_pre);
+        CK(ctx->d_tmp.ensure(stride * run.size() + 64));
+        for (size_t i = 0; i < run.size(); i++) run[i].out_off = i * stride;
+    }
+    rc = decode_batch(ctx, sh.etype, d_words, words_len, run, plan.none() ? d_dst : ctx->d_tmp.as<uint8_t>());
+    if (rc) note_all(STAGE_DECODE, rc);
+    done();
+    for (uint32_t b : idx)
+        if (jobs[b].status) fail[owner[b]].note(STAGE_DECODE, jobs[b].status, "Invalid bitstream: block decoding failed");
+    if (!stage(STAGE_INVERSE)) return 0;
+    std::vector<uint64_t> at(nb, NO_ROOM);
+    std::vector<uint32_t> len(nb, 0);
+    if (plan.none()) {
+        for (uint32_t b : idx) at[b] = jobs[b].out_off, len[b] = jobs[b].pre_len;
+    } else {
+        std::vector<uint32_t> olen;
+        auto put = [&](uint32_t i, uint32_t n) {
+            const uint32_t b = idx[i];
+            DecodeFailure& f = fail[owner[b]];
+            if (!f.runs(STAGE_INVERSE)) return NO_ROOM;  // an earlier block of the stream had no room
+            at[b] = place(b, n);
+            if (at[b] == NO_ROOM) f.note(STAGE_INVERSE, -KZ_ERR_WRITE_FILE, "output buffer too small");
+            return at[b];
+        };
+        rc = inverse_stage(ctx, plan, run, ctx->d_tmp.as<uint8_t>(), stride, d_dst, put, olen);
+        if (rc) note_all(STAGE_INVERSE, rc);
+        for (size_t i = 0; i < olen.size(); i++) len[idx[i]] = olen[i];
+    }
+    if (!sh.checksum_bits || !stage(STAGE_CHECKSUM)) return 0;
+    std::vector<uint64_t> hoff, hv;
+    std::vector<uint32_t> hlen;
+    for (uint32_t b : idx) hoff.push_back(at[b]), hlen.push_back(len[b]);
+    rc = hash_blocks(ctx, d_dst, hoff, hlen, sh.checksum_bits, hv);
+    if (rc) return rc;
+    for (size_t i = 0; i < idx.size(); i++) {
+        const uint64_t want = sh.checksum_bits == 32 ? (run[i].checksum & 0xFFFFFFFFull) : run[i].checksum;
+        if (hv[i] != want) fail[owner[idx[i]]].note(STAGE_CHECKSUM, -KZ_ERR_CRC_CHECK, CHECKSUM_MISMATCH);
+    }
+    return 0;
+}
 
 
 }  // namespace
@@ -1915,28 +2102,14 @@ int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t ma
     if (block_size) *block_size = sh.block_size;
     if (checksum_bits) *checksum_bits = sh.checksum_bits;
     if (input_size) *input_size = sh.input_size;
-    CK(ctx->d_dl.ensure((size_t)max_blocks * 16 + 64));
-    uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
-    uint64_t* d_bbits = d_boff + max_blocks;
-    uint32_t* d_cnt = (uint32_t*)(d_bbits + max_blocks);
-    {
-        LaunchScope ls(ctx, "stream_walk");
-        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>((const uint32_t*)d_src, nullptr, WalkJob{sh.bits, 8ull * n, 0, max_blocks, 0}, 1, d_boff, d_bbits, d_cnt);
-    }
-    uint32_t cs[2] = {0, 0};
-    CK(cudaMemcpyAsync(cs, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if ((int32_t)cs[1] != 0) return ctx->fail(-(int32_t)cs[1], "Invalid bitstream: corrupted block length");
-    const uint32_t nb = cs[0];
-    std::vector<uint64_t> boff(nb), bbits(nb);
-    if (nb) {
-        CK(cudaMemcpyAsync(boff.data(), d_boff, (size_t)nb * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(bbits.data(), d_bbits, (size_t)nb * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
+    std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, max_blocks, 0}};
+    std::vector<Walked> w;
+    rc = walk_streams(ctx, (const uint32_t*)d_src, wj, -1, -1, w);
+    if (rc) return rc;
+    if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
     rec_bit[0] = sh.bits;
-    for (uint32_t b = 0; b < nb; b++) rec_bit[b + 1] = boff[b] + bbits[b];
-    *nblocks = nb;
+    for (size_t b = 0; b < w[0].bit_off.size(); b++) rec_bit[b + 1] = w[0].bit_off[b] + w[0].bits[b];
+    *nblocks = (uint32_t)w[0].n;
     return 0;
 }
 static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
@@ -1961,115 +2134,23 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_INVALID_CODEC);
     if (rc) return rc;
     const uint32_t* d_words = (const uint32_t*)d_src;
-    const uint64_t words_len = (n + 3) / 4 + 16;  // callers guarantee >= 64 readable bytes past n
-    // block prefixes: at most cap / 1024 + 16 decoded blocks are stored (blocks are at least 1 KiB). Without a block range that also
-    // bounds the walk. With one, the walk goes over every record to the end marker, so that a walk error behind the range is still found,
-    // and only the stream's bytes bound it (a record takes at least 9 bits); the records outside the range are not stored.
-    const bool ranged = from >= 0 || to >= 0;
-    uint64_t keep_lo = 0, keep_hi = ~0ull;
-    if (ranged) block_range_records(from, to, &keep_lo, &keep_hi);
-    const uint32_t max_blocks = (uint32_t)std::min<uint64_t>((uint64_t)cap / 1024 + 16, 1u << 22);
-    const uint32_t slots = (uint32_t)std::min<uint64_t>(max_blocks, keep_hi - keep_lo);
-    CK(ctx->d_dl.ensure((size_t)slots * 16 + 64));
-    uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
-    uint64_t* d_bbits = d_boff + slots;
-    uint32_t* d_cnt = (uint32_t*)(d_bbits + slots);
-    {
-        LaunchScope ls(ctx, "stream_walk");
-        const WalkJob wj{sh.bits, 8ull * n, 0, ranged ? 0xFFFFFFFFu : max_blocks, stop_after, keep_lo, keep_lo + slots};
-        stream_walk_kernel<<<1, 32, 0, ctx->stream>>>(d_words, nullptr, wj, 1, d_boff, d_bbits, d_cnt);
-    }
-    // count + the first SPEC block descriptors in one round trip (streams with more blocks pay a second copy)
-    const uint32_t SPEC = std::min<uint32_t>(slots, 1024);
-    CK(ctx->h_dl.ensure((size_t)SPEC * 16 + 64));
-    uint32_t* cs = (uint32_t*)ctx->h_dl.p;
-    uint64_t* h_boff = (uint64_t*)((uint8_t*)ctx->h_dl.p + 64);
-    uint64_t* h_bbits = h_boff + SPEC;
-    CK(cudaMemcpyAsync(cs, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(h_boff, d_boff, (size_t)SPEC * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(h_bbits, d_bbits, (size_t)SPEC * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if ((int32_t)cs[1] != 0) return ctx->fail(-(int32_t)cs[1], "Invalid bitstream: corrupted block length");
-    const uint64_t nrec = cs[0];  // records of the stream; the decoded ones are records keep_lo .. keep_lo + nblocks - 1
-    const uint64_t in_range = std::min(nrec, keep_hi) - std::min(nrec, keep_lo);
-    if (in_range > slots) return ctx->fail(KZ_ERR_BLOCK_SIZE, "Invalid bitstream: more blocks than the output buffer can hold");
-    const uint32_t nblocks = (uint32_t)in_range;
-    std::vector<uint64_t> boff(nblocks), bbits(nblocks);
-    if (nblocks && nblocks <= SPEC) {
-        memcpy(boff.data(), h_boff, (size_t)nblocks * 8);
-        memcpy(bbits.data(), h_bbits, (size_t)nblocks * 8);
-    } else if (nblocks) {
-        CK(cudaMemcpyAsync(boff.data(), d_boff, (size_t)nblocks * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(bbits.data(), d_bbits, (size_t)nblocks * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    std::vector<DecJob> jobs(nblocks);
-    for (uint32_t b = 0; b < nblocks; b++) {
-        jobs[b] = DecJob();
-        jobs[b].bit_off = boff[b];
-        jobs[b].bits = bbits[b];
-    }
-    ctx->stream_bs = sh.block_size;
-    rc = decode_parse_headers(ctx, d_words, jobs, sh.checksum_bits, sh.block_size);
+    // at most cap / 1024 + 16 decoded blocks are stored (blocks are at least 1 KiB)
+    std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, (uint32_t)std::min<uint64_t>((uint64_t)cap / 1024 + 16, 1u << 22), stop_after}};
+    std::vector<Walked> w;
+    rc = walk_streams(ctx, d_words, wj, from, to, w);
     if (rc) return rc;
-    uint64_t out_off = 0;
-    if (plan.none()) {
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid compressed block header");
-            jobs[b].out_off = out_off;  // NONE transform: decoded length == pre_len; every block but the last is block_size (multiple of 16)
-            out_off += jobs[b].pre_len;
-            if (out_off > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-            if (keep_lo + b + 1 < nrec && (jobs[b].pre_len & 15)) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "unexpected block length");
-        }
-        rc = decode_batch(ctx, sh.etype, d_words, words_len, jobs, (uint8_t*)d_dst);
-        if (rc) return rc;
-        for (uint32_t b = 0; b < nblocks; b++)
-            if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid bitstream: block decoding failed");
-        if (sh.checksum_bits) {
-            std::vector<uint64_t> hoff(nblocks);
-            std::vector<uint32_t> hlen(nblocks);
-            for (uint32_t b = 0; b < nblocks; b++) {
-                hoff[b] = jobs[b].out_off;
-                hlen[b] = jobs[b].pre_len;
-            }
-            rc = verify_checksums(ctx, (const uint8_t*)d_dst, hoff, hlen, sh.checksum_bits, jobs);
-            if (rc) return rc;
-        }
-        *out_n = (size_t)out_off;
-        return 0;
-    }
-    // transforms: entropy-decode every block into scratch, then invert the transforms into d_dst
-    uint32_t max_pre = 0;
-    for (uint32_t b = 0; b < nblocks; b++) {
-        if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid compressed block header");
-        max_pre = std::max(max_pre, jobs[b].pre_len);
-    }
-    // Reader.processBlock :1649-1653: the task buffers hold blockSize + max(512, blockSize >> 4) bytes
-    const uint64_t blk_room = std::max<uint64_t>(max_pre, (uint64_t)sh.block_size + std::max<uint64_t>(512, sh.block_size >> 4));
-    const uint64_t pstride = (blk_room + 64 + 15) & ~15ull;
-    CK(ctx->d_tmp.ensure(pstride * nblocks + 64));
-    for (uint32_t b = 0; b < nblocks; b++) jobs[b].out_off = (uint64_t)b * pstride;
-    rc = decode_batch(ctx, sh.etype, d_words, words_len, jobs, ctx->d_tmp.as<uint8_t>());
+    if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
+    if (w[0].overflow) return ctx->fail(KZ_ERR_BLOCK_SIZE, "Invalid bitstream: more blocks than the output buffer can hold");
+    std::vector<DecJob> jobs;
+    std::vector<uint32_t> owner;
+    std::vector<uint8_t> last;
+    w[0].append(0, jobs, owner, last);
+    BackToBack place{cap};
+    DecodeFailure f;
+    rc = decode_walked(ctx, sh, plan, d_words, (n + 3) / 4 + 16, jobs, owner, last, place, (uint8_t*)d_dst, &f);  // >= 64 readable bytes past n
     if (rc) return rc;
-    for (uint32_t b = 0; b < nblocks; b++)
-        if (jobs[b].status) return ctx->fail(-jobs[b].status, "Invalid bitstream: block decoding failed");
-    std::vector<uint32_t> olen;
-    BackToBack place{(uint8_t*)d_dst, cap};
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen);
-    if (rc) return rc;
-    out_off = place.off;
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (sh.checksum_bits) {  // decoded blocks lie back to back (every block but the last is block_size long)
-        std::vector<uint64_t> hoff(nblocks);
-        uint64_t o = 0;
-        for (uint32_t b = 0; b < nblocks; b++) {
-            hoff[b] = o;
-            o += olen[b];
-        }
-        rc = verify_checksums(ctx, (const uint8_t*)d_dst, hoff, olen, sh.checksum_bits, jobs);
-        if (rc) return rc;
-    }
-    *out_n = (size_t)out_off;
+    if (f.failed()) return ctx->fail(-f.code, f.msg);
+    *out_n = (size_t)place.off;
     return 0;
 }
 
@@ -2312,150 +2393,53 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
     return 0;
 }
 
-// One group of streams with the same header fields: walk, entropy decode and inverse transforms of all their blocks, pass by pass, each
-// block written behind the previous one of its stream at d_dst + dst_off[s]. A stream on which anything goes wrong (a bad record, block
-// header, entropy payload or checksum, too little room, a block longer than the decode slot) is put on `alone`; the caller decodes it
-// again on its own with the single-stream path, so that its status is the code kz_decompress_stream_device gives for the same bytes. A
-// failing inverse transform does not say which block failed: then every stream of the group goes on `alone`.
+// One group of streams with the same header fields: walk, then decode_walked pass by pass, each block written behind the previous one of
+// its stream at d_dst + dst_off[s]. A stream on which anything goes wrong (a bad record, block header, entropy payload or checksum, too
+// little room, or a failing stage call of a pass it has blocks in) is put on `alone`; the caller decodes it again on its own with the
+// single-stream path, so that its status is the code kz_decompress_stream_device gives for the same bytes.
 static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan, const std::vector<uint32_t>& grp,
                                const std::vector<uint64_t>& hdr_bits, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off,
                                const uint64_t* src_len, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len,
                                int32_t* status, std::vector<uint32_t>& alone) {
     const uint32_t ng = (uint32_t)grp.size();
     const uint32_t* d_words = (const uint32_t*)d_src;
-    const uint64_t words_len = (src_bytes + 3) / 4 + 16;
-    // walk: one thread per stream; as many records per stream as the single-stream path allows, and no more than its bytes can hold. With
-    // a block range (the same for every stream) the walk goes to the end marker and stores as many records of the range as the
-    // single-stream path would.
-    const bool ranged = ctx->range_from >= 0 || ctx->range_to >= 0;
-    uint64_t keep_lo = 0, keep_hi = ~0ull;
-    if (ranged) block_range_records(ctx->range_from, ctx->range_to, &keep_lo, &keep_hi);
+    // as many records per stream as the single-stream path allows, and no more than its bytes can hold
     std::vector<WalkJob> wj(ng);
-    uint64_t nrec = 0;
     for (uint32_t g = 0; g < ng; g++) {
         const uint32_t s = grp[g];
         const uint64_t by_cap = std::min<uint64_t>(dst_cap[s] / 1024 + 16, 1u << 22);
-        const uint32_t max_blocks = (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1);
-        const uint32_t slots = (uint32_t)std::min<uint64_t>(max_blocks, keep_hi - keep_lo);
-        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), nrec, ranged ? 0xFFFFFFFFu : max_blocks, 0, keep_lo, keep_lo + slots};
-        nrec += slots;
+        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), 0, (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1), 0};
     }
-    CK(ctx->d_dl.ensure((size_t)nrec * 16 + (size_t)ng * 8 + 64));
-    uint64_t* d_boff = ctx->d_dl.as<uint64_t>();
-    uint64_t* d_bbits = d_boff + nrec;
-    uint32_t* d_cnt = (uint32_t*)(d_bbits + nrec);
-    {
-        Packer pk;
-        const size_t o_wj = pk.add(wj.data(), wj.size() * sizeof(WalkJob));
-        int rc = upload(ctx, pk);
-        if (rc) return rc;
-        LaunchScope ls(ctx, "stream_walk");
-        stream_walk_kernel<<<(ng + 127) / 128, 128, 0, ctx->stream>>>(d_words, (const WalkJob*)(ctx->d_tables.as<uint8_t>() + o_wj), WalkJob{}, (int)ng, d_boff,
-                                                                       d_bbits, d_cnt);
-    }
-    CK(cudaGetLastError());
-    std::vector<uint32_t> cs((size_t)ng * 2);
-    std::vector<uint64_t> hoff(nrec), hbits(nrec);
-    CK(cudaMemcpyAsync(cs.data(), d_cnt, cs.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(hoff.data(), d_boff, nrec * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(hbits.data(), d_bbits, nrec * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    std::vector<uint8_t> bad(ng, 0);
-    std::vector<uint64_t> written(ng, 0);
+    std::vector<Walked> w;
+    int rc = walk_streams(ctx, d_words, wj, ctx->range_from, ctx->range_to, w);
+    if (rc) return rc;
+    std::vector<DecodeFailure> fail(ng);
     std::vector<DecJob> all;
-    std::vector<uint32_t> bgrp;   // group index of every block
-    std::vector<uint8_t> blast;   // last block of its stream
+    std::vector<uint32_t> own;
+    std::vector<uint8_t> last;
     for (uint32_t g = 0; g < ng; g++) {
-        const uint64_t n = cs[2 * g], kept = std::min(n, keep_hi) - std::min(n, keep_lo);
-        if (cs[2 * g + 1] || kept > wj[g].keep_hi - keep_lo) {
-            bad[g] = 1;
-            continue;
-        }
-        for (uint32_t r = 0; r < kept; r++) {
-            DecJob j = DecJob();
-            j.bit_off = hoff[wj[g].out + r];
-            j.bits = hbits[wj[g].out + r];
-            all.push_back(j);
-            bgrp.push_back(g);
-            blast.push_back(keep_lo + r + 1 == n);
-        }
+        if (w[g].status || w[g].overflow) fail[g].note(STAGE_WALK, w[g].status ? w[g].status : -KZ_ERR_BLOCK_SIZE, "");
+        else w[g].append(g, all, own, last);
     }
-    const uint64_t pstride = decompress_slot(sh.block_size);
-    const PassPlan P = plan_decompress_passes((uint32_t)all.size(), pstride, decompress_block_cost(sh.block_size));
-    bool group_failed = false;
-    for (uint32_t p = 0; p < P.npasses() && !group_failed; p++) {
-        std::vector<DecJob> jobs;
-        std::vector<uint32_t> jg;
-        std::vector<uint8_t> jl;
-        auto keep_good = [&]() {  // drops the blocks of streams that went bad
-            size_t w = 0;
-            for (size_t i = 0; i < jobs.size(); i++)
-                if (!bad[jg[i]]) jobs[w] = jobs[i], jg[w] = jg[i], jl[w] = jl[i], w++;
-            jobs.resize(w), jg.resize(w), jl.resize(w);
-        };
-        for (uint32_t i = P.first[p]; i < P.first[p + 1]; i++)
-            if (!bad[bgrp[i]]) jobs.push_back(all[i]), jg.push_back(bgrp[i]), jl.push_back(blast[i]);
-        int rc = decode_parse_headers(ctx, d_words, jobs, sh.checksum_bits, sh.block_size);
+    std::vector<uint64_t> written(ng, 0);
+    auto place = [&](uint32_t g, uint32_t len) {  // behind the stream's earlier blocks, within its dst_cap
+        const uint32_t s = grp[g];
+        if (written[g] + len > dst_cap[s]) return NO_ROOM;
+        written[g] += len;
+        return dst_off[s] + written[g] - len;
+    };
+    const PassPlan P = plan_decompress_passes((uint32_t)all.size(), decompress_slot(sh.block_size), decompress_block_cost(sh.block_size));
+    for (uint32_t p = 0; p < P.npasses(); p++) {
+        const uint32_t a = P.first[p], e = P.first[p + 1];
+        std::vector<DecJob> jobs(all.begin() + a, all.begin() + e);
+        const std::vector<uint32_t> owner(own.begin() + a, own.begin() + e);
+        rc = decode_walked(ctx, sh, plan, d_words, (src_bytes + 3) / 4 + 16, jobs, owner, std::vector<uint8_t>(last.begin() + a, last.begin() + e),
+                           [&](uint32_t b, uint32_t len) { return place(owner[b], len); }, d_dst, fail.data());
         if (rc) return rc;
-        for (size_t i = 0; i < jobs.size(); i++)
-            if (jobs[i].status || jobs[i].pre_len > pstride - 64 || (plan.none() && !jl[i] && (jobs[i].pre_len & 15))) bad[jg[i]] = 1;
-        keep_good();
-        const uint32_t k = (uint32_t)jobs.size();
-        if (k == 0) continue;
-        CK(ctx->d_tmp.ensure(pstride * k + 64));
-        for (uint32_t i = 0; i < k; i++) jobs[i].out_off = (uint64_t)i * pstride;
-        rc = decode_batch(ctx, sh.etype, d_words, words_len, jobs, ctx->d_tmp.as<uint8_t>());
-        if (rc) return rc;
-        for (uint32_t i = 0; i < k; i++)
-            if (jobs[i].status) bad[jg[i]] = 1;
-        keep_good();
-        // destinations: behind the stream's earlier blocks, within its dst_cap
-        std::vector<uint64_t> at(jobs.size(), 0);
-        auto place = [&](uint32_t i, uint32_t len, uint8_t** to) {
-            const uint32_t g = jg[i], s = grp[g];
-            if (bad[g] || written[g] + len > dst_cap[s]) {
-                bad[g] = 1;
-                *to = nullptr;
-                return true;
-            }
-            at[i] = dst_off[s] + written[g];
-            *to = d_dst + at[i];
-            written[g] += len;
-            return true;
-        };
-        std::vector<uint32_t> olen(jobs.size(), 0);
-        if (plan.none()) {
-            CopyList out;
-            for (uint32_t i = 0; i < jobs.size(); i++) {
-                uint8_t* to = nullptr;
-                place(i, jobs[i].pre_len, &to);
-                olen[i] = jobs[i].pre_len;
-                if (to) out.add(ctx->d_tmp.as<uint8_t>() + (uint64_t)i * pstride, to, olen[i]);
-            }
-            rc = run_copies(ctx, out);
-            if (rc) return rc;
-        } else if (inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen)) {
-            group_failed = true;
-            break;
-        }
-        if (sh.checksum_bits) {  // decodingTask.decode :1990-2006, on the bytes where they landed
-            std::vector<uint64_t> hoffs, hv;
-            std::vector<uint32_t> hlens;
-            std::vector<uint32_t> hidx;
-            for (uint32_t i = 0; i < jobs.size(); i++)
-                if (!bad[jg[i]]) hoffs.push_back(at[i]), hlens.push_back(olen[i]), hidx.push_back(i);
-            rc = hash_blocks(ctx, d_dst, hoffs, hlens, sh.checksum_bits, hv);
-            if (rc) return rc;
-            for (size_t q = 0; q < hidx.size(); q++) {
-                const uint64_t want = sh.checksum_bits == 32 ? (jobs[hidx[q]].checksum & 0xFFFFFFFFull) : jobs[hidx[q]].checksum;
-                if (hv[q] != want) bad[jg[hidx[q]]] = 1;
-            }
-        }
     }
-    CK(cudaStreamSynchronize(ctx->stream));
     for (uint32_t g = 0; g < ng; g++) {
         const uint32_t s = grp[g];
-        if (group_failed || bad[g]) {
+        if (fail[g].failed()) {
             alone.push_back(s);
         } else {
             status[s] = 0;
@@ -2484,13 +2468,13 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     std::vector<StreamHeader> sh(nstreams);
+    std::vector<TransformPlan> plan(nstreams);
     std::vector<uint64_t> hdr_bits(nstreams, 0);
     std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
     for (uint32_t s = 0; s < nstreams; s++) {
         status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
         if (status[s]) continue;
-        TransformPlan plan;
-        rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan, KZ_ERR_INVALID_CODEC);
+        rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
         if (rc) return rc;
         if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
         hdr_bits[s] = sh[s].bits;
@@ -2498,15 +2482,11 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     }
     std::vector<uint32_t> alone;
     for (auto& kv : groups) {
-        const StreamHeader& h = sh[kv.second[0]];
-        ctx->stream_bs = h.block_size;
-        TransformPlan plan;
-        rc = plan_transforms(ctx, h.t48, h.etype, plan, KZ_ERR_INVALID_CODEC);
-        if (rc) return rc;
-        rc = decode_stream_group(ctx, h, plan, kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
+        const uint32_t s0 = kv.second[0];
+        rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
         if (rc) return rc;
     }
-    for (uint32_t s : alone) {  // only corrupt input (or too little room) gets here
+    for (uint32_t s : alone) {  // only corrupt input, too little room or a failing stage call gets here
         size_t n = 0;
         status[s] = decompress_device_impl(ctx, nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s], d_dst + dst_off[s],
                                            dst_cap[s], &n);
@@ -2745,13 +2725,8 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     // inverse transforms into a scratch area (block b at b * ostride), then out
     CK(ctx->d_tmp.ensure(ostride * nblocks + 64));
     std::vector<uint32_t> olen;
-    uint8_t* d_res = ctx->d_tmp.as<uint8_t>();
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride,
-                       [&](uint32_t b, uint32_t len, uint8_t** at) {
-                           if ((uint64_t)b * ostride + len > ostride * nblocks) return false;
-                           *at = d_res + (uint64_t)b * ostride;
-                           return true;
-                       },
+    // block b fits its slot at b * ostride: the block header bounds pre_len below ostride, and the stages cap their output at ostride - 64
+    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride, ctx->d_tmp.as<uint8_t>(), [&](uint32_t b, uint32_t) { return (uint64_t)b * ostride; },
                        olen);
     if (rc) return rc;
     if (checksum_bits) {
@@ -3216,7 +3191,7 @@ struct kz_reader : kz::Session {
     bool have_header = false;
     DevBuf win[2], d_dec, d_walk;  // window buffers (the unconsumed bits move between them), decoded bytes of one batch, walk results
     size_t win_cap = 0, dec_cap = 0;
-    uint64_t pstride_max = 0, max_rec_bits = 0;
+    uint64_t max_rec_bits = 0;
     // worker state
     int cur = 0;
     uint64_t fill = 0, start_bit = 0;  // valid bytes of win[cur], first bit not yet walked
@@ -3242,11 +3217,10 @@ struct kz_reader : kz::Session {
         if (rc) return fail(-rc, ctx->err);
         const uint64_t bs = sh.block_size;
         if (batch_blocks == 0) batch_blocks = (uint32_t)std::min<uint64_t>(1024, std::max<uint64_t>(1, READER_BATCH_BYTES / bs));
-        // Reader.processBlock :1649-1653 and parse_block_header's bound on a block's pre-transform length
+        // one decode slot per block, at the longest a block header can claim (parse_block_header's bound on the pre-transform length)
         const uint64_t max_len = std::min<uint64_t>(std::max<uint64_t>(2048, bs + bs / 2), 1ull << 30);
-        pstride_max = (std::max<uint64_t>(max_len, bs + std::max<uint64_t>(512, bs >> 4)) + 64 + 15) & ~15ull;
         max_rec_bits = 8ull * kz_max_block_output(bs);
-        dec_cap = (size_t)(batch_blocks * pstride_max);
+        dec_cap = (size_t)(batch_blocks * decode_stride(sh.block_size, (uint32_t)max_len));
         const size_t in_bytes = (size_t)batch_blocks * bs;
         win_cap = (size_t)(max_rec_bits / 8 + 64 + in_bytes);
         cudaError_t e = cudaSuccess;
@@ -3353,7 +3327,7 @@ struct kz_reader : kz::Session {
                 block_range_slice(range_from, range_to, walked, r.count, &lo, &hi);
                 walked += r.count;
                 // NONE: a decoded block that was not the stream's last record must be a multiple of 16 long
-                if (plan.none() && odd_tail && pend_stage != STAGE_HEADER) note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
+                if (plan.none() && odd_tail) pend.note(STAGE_HEADER, -KZ_ERR_PROCESS_BLOCK, "unexpected block length");
                 odd_tail = false;
                 if (hi > lo) {
                     int rc = decode(hi - lo, &boff[lo], &bbits[lo], hi == r.count);
@@ -3366,7 +3340,7 @@ struct kz_reader : kz::Session {
                     std::lock_guard<std::mutex> l(m);
                     ended = true;
                 }
-                return pend_stage == STAGE_NONE ? 0 : ctx->fail(-pend_code, pend_msg);
+                return pend.failed() ? ctx->fail(-pend.code, pend.msg) : 0;
             }
             if (r.count < batch_blocks) return 0;
         }
@@ -3374,98 +3348,28 @@ struct kz_reader : kz::Session {
 
     // A block-level failure (block header, entropy decode, inverse transform, checksum) is not reported when it is found:
     // decompress_device_impl walks every record of the stream before it decodes any, so a walk error (a length over the limits, a
-    // truncated stream) found later takes precedence, and after the walk the failure of the earliest stage wins (headers of every block,
-    // then entropy decode, inverse transforms, checksums), the earliest block within a stage. The reader keeps the failure that wins so
-    // far, hands out nothing more, runs each later batch only through the stages whose failures could still win, and reports at the end
-    // marker or at the walk error.
-    enum { STAGE_NONE = 0, STAGE_HEADER = 1, STAGE_DECODE = 2, STAGE_INVERSE = 3, STAGE_CHECKSUM = 4 };
-    int pend_stage = STAGE_NONE, pend_code = 0;
-    std::string pend_msg;
-    void note(int stage, int rc) {  // rc = -(error code); ctx->err holds its message
-        if (pend_stage != STAGE_NONE && stage >= pend_stage) return;
-        pend_stage = stage;
-        pend_code = rc;
-        pend_msg = ctx->err;
-    }
-    int note_fail(int stage, int code, const char* msg) {
-        note(stage, ctx->fail(code, msg));
-        return 0;
-    }
+    // truncated stream) found later takes precedence, and after the walk the failure of the earliest stage wins, the earliest block
+    // within a stage. The reader keeps the failure that wins so far, hands out nothing more, runs each later batch only through the
+    // stages whose failures could still win (decode_walked skips the others), and reports at the end marker or at the walk error.
+    DecodeFailure pend;
 
     // nb records of one batch, as decompress_device_impl decodes a whole stream; the decoded bytes are published back to back.
     // ends_batch: the last of them is the last record walked so far.
     int decode(uint32_t nb, const uint64_t* boff, const uint64_t* bbits, bool ends_batch) {
-        if (pend_stage == STAGE_HEADER) return 0;  // only a walk error could still win
-        const uint32_t* W = win[cur].as<uint32_t>();
-        const uint64_t words_len = (fill + 3) / 4 + 16;
         std::vector<DecJob> jobs(nb);
         for (uint32_t b = 0; b < nb; b++) {
             jobs[b] = DecJob();
             jobs[b].bit_off = boff[b];
             jobs[b].bits = bbits[b];
         }
-        ctx->stream_bs = sh.block_size;
-        int rc = decode_parse_headers(ctx, W, jobs, sh.checksum_bits, sh.block_size);
+        std::vector<uint8_t> last(nb, 0);
+        last[nb - 1] = ends_batch;
+        BackToBack place{dec_cap};
+        int rc = decode_walked(ctx, sh, plan, win[cur].as<uint32_t>(), (fill + 3) / 4 + 16, jobs, std::vector<uint32_t>(nb, 0), last, place,
+                               d_dec.as<uint8_t>(), &pend);
         if (rc) return rc;
-        uint64_t total = 0;
-        std::vector<uint32_t> olen(nb);
-        uint64_t pstride = 0;
-        // headers (and, for NONE, the rule that every block but the stream's last is a multiple of 16 long), in block order as
-        // decompress_device_impl checks them
-        uint32_t max_pre = 0;
-        for (uint32_t b = 0; b < nb; b++) {
-            if (jobs[b].status) return note_fail(STAGE_HEADER, -jobs[b].status, "Invalid compressed block header");
-            if (plan.none()) {
-                jobs[b].out_off = total;
-                total += jobs[b].pre_len;
-                olen[b] = jobs[b].pre_len;
-                if ((b + 1 < nb || !ends_batch) && (jobs[b].pre_len & 15)) return note_fail(STAGE_HEADER, KZ_ERR_PROCESS_BLOCK, "unexpected block length");
-            }
-            max_pre = std::max(max_pre, jobs[b].pre_len);
-        }
         if (plan.none()) odd_tail = (jobs[nb - 1].pre_len & 15) != 0;
-        if (pend_stage == STAGE_DECODE) return 0;
-        uint8_t* d_ent = d_dec.as<uint8_t>();
-        if (!plan.none()) {
-            const uint64_t blk_room = std::max<uint64_t>(max_pre, (uint64_t)sh.block_size + std::max<uint64_t>(512, sh.block_size >> 4));
-            pstride = (blk_room + 64 + 15) & ~15ull;
-            CK(ctx->d_tmp.ensure(pstride * nb + 64));
-            for (uint32_t b = 0; b < nb; b++) jobs[b].out_off = (uint64_t)b * pstride;
-            d_ent = ctx->d_tmp.as<uint8_t>();
-        }
-        rc = decode_batch(ctx, sh.etype, W, words_len, jobs, d_ent);
-        if (rc) {
-            note(STAGE_DECODE, rc);
-            return 0;
-        }
-        for (uint32_t b = 0; b < nb; b++)
-            if (jobs[b].status) return note_fail(STAGE_DECODE, -jobs[b].status, "Invalid bitstream: block decoding failed");
-        if (pend_stage == STAGE_INVERSE) return 0;
-        if (!plan.none()) {
-            BackToBack place{d_dec.as<uint8_t>(), dec_cap};
-            rc = inverse_stage(ctx, plan, jobs, ctx->d_tmp.as<uint8_t>(), pstride, place, olen);
-            if (rc) {
-                note(STAGE_INVERSE, rc);
-                return 0;
-            }
-            total = place.off;
-        }
-        if (pend_stage == STAGE_CHECKSUM) return 0;
-        if (sh.checksum_bits) {  // before anything of the batch is handed out
-            std::vector<uint64_t> hoff(nb);
-            uint64_t o = 0;
-            for (uint32_t b = 0; b < nb; b++) {
-                hoff[b] = o;
-                o += olen[b];
-            }
-            rc = verify_checksums(ctx, d_dec.as<uint8_t>(), hoff, olen, sh.checksum_bits, jobs);
-            if (rc == -KZ_ERR_CRC_CHECK) {
-                note(STAGE_CHECKSUM, rc);
-                return 0;
-            }
-            if (rc) return rc;
-        }
-        return publish(d_dec.p, (size_t)total, (size_t)total);
+        return pend.failed() ? 0 : publish(d_dec.p, (size_t)place.off, (size_t)place.off);
     }
 };
 

@@ -1,5 +1,6 @@
-// Pass planner of the many-stream entry points (kz_compress_streams / kz_decompress_streams, kz_api.cu). Pure host code: no CUDA
-// types, so that tests/host/stream_plan_host.cpp compiles it with g++ and checks its bounds on the CPU.
+// Pass planner of the many-stream entry points (kz_compress_streams / kz_decompress_streams, kz_api.cu), and the slot and error-order
+// rules of every stream-level decode. Pure host code: no CUDA types, so that tests/host/stream_plan_host.cpp compiles it with g++ and
+// checks it on the CPU.
 //
 // A pass is a set of blocks that run through the transform and entropy stages together. Every block of a pass gets a slot of the
 // pass's stride in the device scratch buffers, so the scratch of a pass is (number of blocks) x cost(stride). The planner keeps that
@@ -9,6 +10,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <numeric>
+#include <string>
 #include <vector>
 
 namespace kz {
@@ -48,6 +50,30 @@ inline uint64_t compress_block_cost(uint64_t s, const EntropyScratch& e) {
 // holds that plus 64 bytes of slack, and a block takes one slot in each of the two buffers the inverse stages alternate between.
 inline uint64_t decompress_slot(uint32_t block_size) { return round16((uint64_t)block_size + std::max<uint64_t>(512, block_size >> 4) + 64); }
 inline uint64_t decompress_block_cost(uint32_t block_size) { return 2 * decompress_slot(block_size); }
+// The slot stride of a batch of blocks whose longest entropy output is max_pre bytes: decompress_slot, or longer when a block header
+// claims more (parse_block_header bounds the claim by max(2048, 1.5 x block_size)).
+inline uint64_t decode_stride(uint32_t block_size, uint32_t max_pre) { return std::max(decompress_slot(block_size), round16((uint64_t)max_pre + 64)); }
+
+// The stages of a stream-level block decode (decode_walked in kz_api.cu), in the order they run. STAGE_WALK is the record walk before
+// them; STAGE_DONE is past the last stage.
+enum DecodeStage { STAGE_WALK = 0, STAGE_HEADER, STAGE_DECODE, STAGE_INVERSE, STAGE_CHECKSUM, STAGE_DONE };
+
+// The failure that decides one stream's status (DESIGN §5.2, "Error order"): the earliest stage wins, and within a stage the earliest
+// block. Blocks are noted in block order, so within a stage the failure noted first stays.
+struct DecodeFailure {
+    int stage = STAGE_DONE;
+    int code = 0;     // -(error code)
+    std::string msg;  // the message of ctx->err that goes with it
+    bool failed() const { return stage != STAGE_DONE; }
+    // whether a failure at stage s could still win: the stream's blocks skip every stage that could not
+    bool runs(int s) const { return s < stage; }
+    void note(int s, int c, const std::string& m) {
+        if (!runs(s)) return;
+        stage = s;
+        code = c;
+        msg = m;
+    }
+};
 
 // Compression: blocks of lengths len[], longest first. A pass opens with the longest block left, whose rounded length is the pass's
 // stride s; it admits shorter blocks while s <= 2 x len + 16 and while (blocks + 1) x cost(s) <= budget.

@@ -1,5 +1,7 @@
-// CPU harness of the pass planner of the many-stream entry points (kanzi-go_b200/csrc/kz_stream_plan.h), for tests/test_stream_plan_host.py.
+// CPU harness of the pass planner of the many-stream entry points and of the decode slot and error-order rules
+// (kanzi-go_b200/csrc/kz_stream_plan.h), for tests/test_stream_plan_host.py.
 #include <cstdint>
+#include <string>
 #include <vector>
 
 #include "../../kanzi-go_b200/csrc/kz_stream_plan.h"
@@ -34,4 +36,17 @@ uint32_t plan_decompress(uint32_t n, uint32_t block_size, uint64_t budget, uint3
     return P.npasses();
 }
 uint64_t decompress_cost(uint32_t block_size) { return kz::decompress_block_cost(block_size); }
+uint64_t decode_stride(uint32_t block_size, uint32_t max_pre) { return kz::decode_stride(block_size, max_pre); }
+
+// Notes n block failures (stage[i], code[i]) in the given order on one stream's DecodeFailure. runs_out[i] = whether stage[i] could
+// still win before note i. Returns the code that decides the stream (0: none); *out_stage = its stage (STAGE_DONE: none).
+int32_t note_failures(const int32_t* stage, const int32_t* code, uint32_t n, uint8_t* runs_out, int32_t* out_stage) {
+    kz::DecodeFailure f;
+    for (uint32_t i = 0; i < n; i++) {
+        runs_out[i] = f.runs(stage[i]);
+        f.note(stage[i], code[i], "failure " + std::to_string(i));
+    }
+    *out_stage = f.stage;
+    return f.failed() ? f.code : 0;
+}
 }

@@ -1,6 +1,7 @@
 """CPU check of the pass planner of kz_compress_streams / kz_decompress_streams (kanzi-go_b200/csrc/kz_stream_plan.h): every block lands in
 exactly one pass and one slot, each pass's stride holds its blocks and is at most twice each member's length plus 16, and the scratch
-bound and the pass budget hold, also for adversarial length mixes such as one 1 GiB block among 10^5 one-byte blocks."""
+bound and the pass budget hold, also for adversarial length mixes such as one 1 GiB block among 10^5 one-byte blocks. Also the decode
+slot stride and the error order of every stream-level decode (DecodeFailure): the earliest stage wins, then the earliest block."""
 import ctypes as C
 import os
 import subprocess
@@ -29,6 +30,10 @@ def plan():
     lib.plan_decompress.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.decompress_cost.restype = C.c_uint64
     lib.decompress_cost.argtypes = [C.c_uint32]
+    lib.decode_stride.restype = C.c_uint64
+    lib.decode_stride.argtypes = [C.c_uint32, C.c_uint32]
+    lib.note_failures.restype = C.c_int32
+    lib.note_failures.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_int32)]
     return lib
 
 
@@ -113,3 +118,51 @@ def test_decompress_passes(plan, n, bs):
             assert sl[ps == p].tolist() == list(range(int(counts[p])))
         assert scratch.value == int(counts.max()) * cost
         assert scratch.value <= max(BUDGET, cost)
+
+
+@pytest.mark.parametrize("bs", [1024, 65536, 4 << 20, 1 << 30])
+def test_decode_stride(plan, bs):
+    """Reader.processBlock's buffer plus 64 bytes, rounded to 16, or longer when a block header claims a longer entropy output"""
+    for max_pre in (0, 1, bs, bs + max(512, bs >> 4), bs + max(512, bs >> 4) + 1, max(2048, bs + bs // 2)):
+        want = (max(max_pre, bs + max(512, bs >> 4)) + 64 + 15) & ~15
+        assert plan.decode_stride(bs, max_pre) == want
+    assert plan.decode_stride(bs, 0) == plan.decompress_cost(bs) // 2
+
+
+WALK, HEADER, DECODE, INVERSE, CHECKSUM, DONE = range(6)
+
+
+def note_failures(lib, notes):
+    stage = np.array([s for s, _ in notes] or [0], np.int32)
+    code = np.array([c for _, c in notes] or [0], np.int32)
+    runs = np.zeros(max(len(notes), 1), np.uint8)
+    out_stage = C.c_int32(-1)
+    rc = lib.note_failures(stage.ctypes.data, code.ctypes.data, len(notes), runs.ctypes.data, C.byref(out_stage))
+    return rc, out_stage.value, runs[: len(notes)].astype(bool).tolist()
+
+
+def test_failure_none(plan):
+    assert note_failures(plan, []) == (0, DONE, [])
+
+
+def test_failure_earliest_stage_wins(plan):
+    """a later block's failure at an earlier stage beats an earlier block's at a later stage"""
+    rc, st, runs = note_failures(plan, [(CHECKSUM, -10), (INVERSE, -9), (DECODE, -7), (HEADER, -13)])
+    assert (rc, st) == (-13, HEADER)
+    assert runs == [True, True, True, True]
+
+
+def test_failure_earliest_block_within_a_stage(plan):
+    rc, st, runs = note_failures(plan, [(DECODE, -7), (DECODE, -13), (DECODE, -10)])
+    assert (rc, st) == (-7, DECODE)
+    assert runs == [True, False, False]
+
+
+def test_failure_skips_later_stages(plan):
+    """once a stream has failed, its blocks run no stage whose failure could not beat the one it holds"""
+    rc, st, runs = note_failures(plan, [(INVERSE, -13), (CHECKSUM, -10), (INVERSE, -9), (DECODE, -7), (INVERSE, -13), (CHECKSUM, -10)])
+    assert (rc, st) == (-7, DECODE)
+    assert runs == [True, False, False, True, False, False]
+    rc, st, runs = note_failures(plan, [(HEADER, -13), (DECODE, -7), (HEADER, -10), (WALK, -9)])
+    assert (rc, st) == (-9, WALK)
+    assert runs == [True, False, False, True]
