@@ -18,7 +18,7 @@
  *   - subsets of the v6 format the decoders accept (anything else answers an error, never wrong bytes; the Go caller keeps its own path then):
  *     ANS0 / ANS1 log range <= 12 (what every kanzi encoder writes; the format allows 8..15, entropy/ANSRangeCodec.go:606-609), ROLZ
  *     logPosChecks = 4 (what `-t ROLZ` writes), TEXT encoding 2 only (entropy NONE / ANS0 / HUFFMAN / RANGE, transform/Factory.go:99-119),
- *     bitstream version 6;
+ *     bitstream version 6 (in a header, and as the bsVersion of a headerless reader, kz_set_headerless_reader);
  *   - transform ids (transform/Factory.go:31-50): NONE 0, BWT 1, BWTS 2, LZ 3, ZRLT 6, MTFT 7, RANK 8, ROLZ 11, LZX 16; a "transform48"
  *     word packs up to 8 six-bit ids, first transform in the top 6 bits (Factory.go:26-54).
  */
@@ -204,11 +204,38 @@ void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size);
  * records) applies to the decoded blocks only; with a range set, the stream's length bounds the walk. */
 int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block);
 
+/* Headerless streams: kanzi's NewWriter(..., headerless = true) and NewHeaderlessReader (io/CompressedStream.go:216, :1060). Both are off by
+ * default. Callers that store the stream parameters once (object stores, record-level compression) use them to drop the 20 to 26 header
+ * bytes each stream carries.
+ * kz_set_headerless_writer(ctx, 1): kz_compress_stream[_device], kz_compress_streams[_device] and kz_writer_open write no stream header
+ *   (Writer.writeHeader returns at once, :430): a stream is its block records and the end marker, byte for byte the headered stream with its
+ *   first header-length bits removed. An empty input gives the 8-bit end marker alone. on = 0 brings back the headered bytes. Returns 0, or
+ *   -KZ_ERR_INVALID_PARAM without a context.
+ * kz_set_headerless_reader: kz_decompress_stream[_device], kz_decompress_streams[_device], kz_reader_open and kz_stream_index_device read
+ *   no header: they take the transform, entropy, block size and checksum of the setting and walk the records from bit 0. Every stream of
+ *   a many-stream call has these parameters. kz_stream_index_device returns the setting's fields (input_size = output_size) and
+ *   rec_bit[0] = 0. The block range (kz_set_block_range) applies as it does to a headered stream, and so do the error codes and their
+ *   order. The setting is checked when it is made, as Reader.validateHeaderless does (:1178-1280):
+ *   bs_version > 6 -KZ_ERR_INVALID_PARAM, bs_version < 6 -KZ_ERR_STREAM_VERSION (the decoders read version 6 only); an entropy id that is
+ *   no kanzi id (not 0..9, or PAQ = 3), a transform word with bits above 48 or a six-bit id that is no kanzi id (not 0..19, or SNAPPY = 4)
+ *   -KZ_ERR_INVALID_PARAM; block_size outside [1024, 1 GiB] -KZ_ERR_INVALID_PARAM (the reference takes any size in that range; a bad
+ *   block size in a header is -KZ_ERR_BLOCK_SIZE instead); checksum_bits not 0 / 32 / 64 -KZ_ERR_INVALID_PARAM; a kanzi chain or codec
+ *   the GPU path lacks -KZ_ERR_CREATE_CODEC. A failed call leaves the previous setting in place. output_size < 0 or >= 2^48 means "not
+ *   given" (0); it never changes the decoded bytes. kz_clear_headerless_reader turns the setting off.
+ * Both settings are read when a call starts; kz_writer_open and kz_reader_open capture them, so later changes do not reach an open session
+ * (and the calls are allowed while one is open). kz_compress_fragment_device, kz_decompress_fragment_device and the block entry points
+ * ignore them: they never read or write a header. */
+int kz_set_headerless_writer(kz_ctx* ctx, int on);
+int kz_set_headerless_reader(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t block_size, uint32_t checksum_bits, int64_t output_size,
+                             uint32_t bs_version);
+int kz_clear_headerless_reader(kz_ctx* ctx);
+
 /* ---- streaming sessions: CompressedOutputStream / CompressedInputStream (io/CompressedStream.go:524-710, :1556-1744) for a stream of any
  *      length, or one that arrives in pieces (a pipe, a socket), in memory that does not grow with the stream ------------------------------
  * A zlib-style pump. The session takes ctx over until kz_*_free: the caller makes no other call on ctx in between except kz_device_bytes,
- * kz_last_error and kz_set_block_range (the one-thread-at-a-time rule; one session per context). batch_blocks = blocks per GPU batch (the role of kanzi's `jobs`),
- * 1 .. 1024; kz_reader_open also takes 0: about 256 MiB of blocks per batch, resolved from the block size in the stream's header.
+ * kz_last_error, kz_set_block_range and the headerless settings (the one-thread-at-a-time rule; one session per context). batch_blocks =
+ * blocks per GPU batch (the role of kanzi's `jobs`), 1 .. 1024; kz_reader_open also takes 0: about 256 MiB of blocks per batch, resolved
+ * from the block size in the stream's header (or the headerless setting).
  * Bytes: the writer's output, concatenated, is byte for byte what kz_compress_stream writes for the concatenated input with the same
  *   parameters and input_size_hint, whatever the piece sizes, batch_blocks and output caps. The reader's output is what kz_decompress_stream
  *   gives for the same stream. Bytes after the end marker are ignored, as kz_decompress_stream ignores them.
@@ -226,7 +253,7 @@ int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block);
  *   reader: pinned 2 x B input + 2 x D output, device 2 x B input, 2 x (kz_max_block_output(block_size) + 64 + B) window (at least one
  *     maximal record plus one input slot) and D decoded bytes, D = batch_blocks x (max(block_size + max(512, block_size / 16),
  *     min(max(2048, 1.5 x block_size), 2^30)) + 64), rounded up to 16 per block; plus the context's scratch for one batch. The reader sizes
- *     its buffers from the stream header.
+ *     its buffers from the stream header, a headerless reader from its setting when it opens.
  *   kz_device_bytes: the device bytes held by ctx's scratch and an open session's buffers (the sum of their capacities); while a session is
  *   open, the scratch as it was after the worker's last batch.
  * Errors: the first failure is sticky: every later call returns the same code, and kz_last_error(ctx) gives its message. The reader gives a

@@ -125,7 +125,8 @@ type StreamResult struct {
 // caller groups its files by block size and makes one call per group. A file whose output does not fit fails alone; a transform or
 // entropy failure on one file's data (the reference fails that file with ERR_PROCESS_BLOCK) fails the whole call, and the caller
 // then compresses the files one by one. The call holds all inputs, encoded blocks and streams in device memory at once: split a
-// large directory into calls of a size the GPU holds.
+// large directory into calls of a size the GPU holds. After c.SetHeaderlessWriter(true) no stream carries a header (the Writer's
+// headerless = true): that saves 20 to 26 bytes per file for callers that store the parameters once.
 func (c *Context) CompressStreams(transformType uint64, entropyType uint32, blockSize uint32, ckBits uint, inputs [][]byte,
 	inputSizes []int64) ([]StreamResult, error) {
 	n := len(inputs)
@@ -161,6 +162,7 @@ func (c *Context) CompressStreams(transformType uint64, entropyType uint32, bloc
 // or the caller's limit). A corrupt stream gets the error code a Reader would report for it; every other stream decodes normally.
 // A stream whose transform or entropy codec the GPU path lacks fails the whole call with ERR_INVALID_CODEC: the caller then keeps
 // the reference's Reader for the files of that call. The device holds every input and sum(caps) bytes of output at once.
+// After c.SetHeaderlessReader(...) the streams have no header and all share its parameters (NewHeaderlessReader for every file).
 func (c *Context) DecompressStreams(streams [][]byte, caps []uint64) ([]StreamResult, error) {
 	n := len(streams)
 	srcOff, srcLen, dstOff := make([]uint64, n), make([]uint64, n), make([]uint64, n)

@@ -215,3 +215,61 @@ func NewStreamReaderWithCtx(c *Context, r io.Reader, batchBlocks uint32, ctx map
 	C.kz_set_block_range(c.h, -1, -1) // without c.mu, which the open session holds: the call is allowed while a session is open
 	return s, err
 }
+
+// Headerless reads kanzi's ctx["headerless"], which NewWriterWithCtx checks to be a bool (io/CompressedStream.go:366) and
+// NewHeaderlessReader sets to true (:1060). A missing key gives false.
+func Headerless(ctx map[string]any) bool {
+	v, ok := ctx["headerless"].(bool)
+	return ok && v
+}
+
+// SetHeaderlessWriter is kz_set_headerless_writer: the stream-level encodes that follow on c (CompressStreams, and NewStreamWriter, which
+// keeps the setting for its session) write no stream header, as Writer.writeHeader does for NewWriter(..., headerless = true) (:430).
+func (c *Context) SetHeaderlessWriter(on bool) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	v := C.int(0)
+	if on {
+		v = 1
+	}
+	if rc := C.kz_set_headerless_writer(c.h, v); rc != 0 {
+		return c.err(rc)
+	}
+	return nil
+}
+
+// SetHeaderlessReader is kz_set_headerless_reader: the stream-level decodes that follow on c (DecompressStreams, and NewStreamReader,
+// which keeps the setting for its session) read no header and take these parameters. They are checked as Reader.validateHeaderless
+// checks them (:1178-1280); a kanzi chain or codec the GPU lacks fails with ERR_CREATE_CODEC, and the caller keeps its CPU reader.
+func (c *Context) SetHeaderlessReader(transformType uint64, entropyType uint32, blockSize uint32, ckBits uint, outputSize int64, bsVersion uint) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	if rc := C.kz_set_headerless_reader(c.h, C.uint64_t(transformType), C.uint32_t(entropyType), C.uint32_t(blockSize), C.uint32_t(ckBits),
+		C.int64_t(outputSize), C.uint32_t(bsVersion)); rc != 0 {
+		return c.err(rc)
+	}
+	return nil
+}
+
+// ClearHeaderlessReader turns the headerless reader setting off: the stream-level decodes read a header again.
+func (c *Context) ClearHeaderlessReader() error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	if rc := C.kz_clear_headerless_reader(c.h); rc != 0 {
+		return c.err(rc)
+	}
+	return nil
+}
+
+// NewHeaderlessStreamReader is NewStreamReader for NewHeaderlessReader(is, jobs, transform, entropy, blockSize, checksum, originalSize,
+// bsVersion) (:1060): the session reads a stream without header, with these parameters. c's setting is made for the open and cleared
+// afterwards.
+func NewHeaderlessStreamReader(c *Context, r io.Reader, batchBlocks uint32, transformType uint64, entropyType uint32, blockSize uint32,
+	ckBits uint, originalSize int64, bsVersion uint) (*StreamReader, error) {
+	if err := c.SetHeaderlessReader(transformType, entropyType, blockSize, ckBits, originalSize, bsVersion); err != nil {
+		return nil, err
+	}
+	s, err := NewStreamReader(c, r, batchBlocks)
+	C.kz_clear_headerless_reader(c.h) // without c.mu, which the open session holds: the call is allowed while a session is open
+	return s, err
+}

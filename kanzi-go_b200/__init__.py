@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
     "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
     "kz_reader_free", "kz_device_bytes", "kz_set_block_range", "kz_bwt_profile",
+    "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader",
 ]
 
 
@@ -140,6 +141,9 @@ def load_library(build_if_missing=True):
     L.kz_bwt_profile.restype = None
     L.kz_set_stream_block_size.restype = None
     L.kz_set_block_range.argtypes = [vp, C.c_int64, C.c_int64]
+    L.kz_set_headerless_writer.argtypes = [vp, i32]
+    L.kz_set_headerless_reader.argtypes = [vp, u64, u32, u32, u32, C.c_int64, u32]
+    L.kz_clear_headerless_reader.argtypes = [vp]
     L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -194,6 +198,8 @@ class Context:
         self.h = h
         self.device = device
         self._range = (-1, -1)  # kz_set_block_range's (from, to) on this context
+        self._hl_writer = False  # kz_set_headerless_writer's setting
+        self._hl_reader = None   # kz_set_headerless_reader's arguments, None when it is off
 
     def close(self):
         if getattr(self, "h", None):
@@ -288,22 +294,25 @@ class Context:
                                               out.ctypes.data, ostride, lens.ctypes.data, status.ctypes.data))
         return [out[i * ostride: i * ostride + int(lens[i])].copy() for i in range(nb)]
 
-    def compress(self, data, transform="NONE", entropy="NONE", block_size=4 << 20, checksum_bits=0, input_size=0):
+    def compress(self, data, transform="NONE", entropy="NONE", block_size=4 << 20, checksum_bits=0, input_size=0, headerless=None):
+        """headerless: True / False sets the headerless writer setting for this call (None: the context's setting)."""
         a = _u8(data)
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         cap = self.lib.kz_max_stream_output(a.size, block_size)
         out = np.empty(cap, np.uint8)
         n = C.c_size_t(0)
-        self._check(self.lib.kz_compress_stream(self.h, t48, et, block_size, checksum_bits, input_size, _p(a), a.size, out.ctypes.data, cap, C.byref(n)))
+        with self._headerless(writer=headerless):
+            self._check(self.lib.kz_compress_stream(self.h, t48, et, block_size, checksum_bits, input_size, _p(a), a.size, out.ctypes.data, cap, C.byref(n)))
         return out[: n.value].copy()
 
-    def decompress(self, stream, out_cap, from_block=None, to_block=None):
-        """from_block / to_block: decode only that range of blocks (see set_block_range) for this call."""
+    def decompress(self, stream, out_cap, from_block=None, to_block=None, headerless=None):
+        """from_block / to_block: decode only that range of blocks (see set_block_range) for this call. headerless: a dict of
+        set_headerless_reader's arguments, the headerless reader setting for this call (None: the context's setting)."""
         s = _u8(stream)
         out = np.empty(max(out_cap, 1), np.uint8)
         n = C.c_size_t(0)
-        with self._block_range(from_block, to_block):
+        with self._block_range(from_block, to_block), self._headerless(reader=headerless):
             self._check(self.lib.kz_decompress_stream(self.h, _p(s), s.size, out.ctypes.data, out_cap, C.byref(n)))
         return out[: n.value]
 
@@ -327,9 +336,49 @@ class Context:
         finally:
             self.set_block_range(*prev)
 
+    # ---- headerless streams (kz_set_headerless_writer / kz_set_headerless_reader): NewWriter(..., headerless) and NewHeaderlessReader -----
+    def set_headerless_writer(self, on=True):
+        """The stream-level encodes that follow (compress*, compress_streams*, stream_writer when it opens) write no stream header."""
+        self._check(self.lib.kz_set_headerless_writer(self.h, 1 if on else 0))
+        self._hl_writer = bool(on)
+
+    def set_headerless_reader(self, transform, entropy, block_size, checksum_bits=0, output_size=-1, bs_version=6):
+        """The stream-level decodes that follow (decompress*, decompress_streams*, stream_reader when it opens, stream_index_device) read
+        no header and take these parameters (NewHeaderlessReader's). Checked now, as Reader.validateHeaderless does: a bad value raises and
+        leaves the previous setting."""
+        t48 = transform_type(transform) if isinstance(transform, str) else transform
+        et = entropy_type(entropy) if isinstance(entropy, str) else entropy
+        args = (t48, et, block_size, checksum_bits, output_size, bs_version)
+        self._check(self.lib.kz_set_headerless_reader(self.h, *args))
+        self._hl_reader = args
+
+    def clear_headerless_reader(self):
+        self._check(self.lib.kz_clear_headerless_reader(self.h))
+        self._hl_reader = None
+
+    @contextlib.contextmanager
+    def _headerless(self, writer=None, reader=None):
+        """Sets the headerless writer flag (writer: a bool) and / or the headerless reader parameters (reader: a dict of
+        set_headerless_reader's arguments) for one call, and restores the previous settings afterwards. None leaves a setting as it is."""
+        prev_w, prev_r = self._hl_writer, self._hl_reader
+        try:
+            if writer is not None:
+                self.set_headerless_writer(writer)
+            if reader is not None:
+                self.set_headerless_reader(**reader)
+            yield
+        finally:
+            if writer is not None:
+                self.set_headerless_writer(prev_w)
+            if reader is not None:
+                if prev_r is None:
+                    self.clear_headerless_reader()
+                else:
+                    self.set_headerless_reader(*prev_r)
+
     # ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams) -----------------------------------
     # Per-stream failures do not raise: status[s] = 0 or -(kanzi error code), and outputs[s] is None for a failed stream.
-    def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None):
+    def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None, headerless=None):
         """One compressed stream per input, each equal to compress(inputs[s], ..., input_size=input_sizes[s]) -> (outputs, status)."""
         arrs = [_u8(x) for x in inputs]
         t48 = transform_type(transform) if isinstance(transform, str) else transform
@@ -342,14 +391,15 @@ class Context:
         dst = np.empty(max(int(cap.sum()), 1), np.uint8)
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
-        self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len), None if isz is None else _p(isz),
-                                     dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
+        with self._headerless(writer=headerless):
+            self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len),
+                                         None if isz is None else _p(isz), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
         return outs, status
 
-    def decompress_streams(self, streams, caps, from_block=None, to_block=None):
+    def decompress_streams(self, streams, caps, from_block=None, to_block=None, headerless=None):
         """Decodes every stream (headers may differ) into at most caps[s] bytes -> (outputs, status). from_block / to_block: the same block
-        range for every stream."""
+        range for every stream. headerless: the same parameters for every stream (see decompress)."""
         arrs = [_u8(x) for x in streams]
         src_len = np.array([a.size for a in arrs], np.uint64)
         src_off = _offsets(src_len)
@@ -358,41 +408,44 @@ class Context:
         dst_off = _offsets(cap)
         dst = np.empty(max(int(cap.sum()), 1), np.uint8)
         out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
-        with self._block_range(from_block, to_block):
+        with self._block_range(from_block, to_block), self._headerless(reader=headerless):
             self.lib.kz_decompress_streams(self.h, len(arrs), _p(src), _p(src_off), _p(src_len), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len),
                                            _p(status))
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
         return outs, status
 
     def compress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, transform, entropy, block_size, checksum_bits=0,
-                                input_sizes=None):
+                                input_sizes=None, headerless=None):
         """src / dst: CUDA uint8 tensors (or device addresses); offsets (multiples of 16) and lengths: host sequences -> (out_len, status)."""
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
-        self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl), None if isz is None else _p(isz),
-                                            _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+        with self._headerless(writer=headerless):
+            self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl),
+                                                None if isz is None else _p(isz), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
 
-    def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, from_block=None, to_block=None):
+    def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, from_block=None, to_block=None, headerless=None):
         """Device-resident decompress_streams: inputs need >= 64 readable bytes behind each -> (out_len, status)."""
         so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
         out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
-        with self._block_range(from_block, to_block):
+        with self._block_range(from_block, to_block), self._headerless(reader=headerless):
             self.lib.kz_decompress_streams_device(self.h, len(sl), _dptr(src), _p(so), _p(sl), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
 
     # ---- device-resident entry points (pointers are CUDA device addresses, e.g. torch tensors' data_ptr()) -------
-    def compress_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, input_size=0):
+    def compress_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, input_size=0, headerless=None):
         out_n = C.c_size_t(0)
-        self._check(self.lib.kz_compress_stream_device(self.h, transform48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, C.byref(out_n)))
+        with self._headerless(writer=headerless):
+            self._check(self.lib.kz_compress_stream_device(self.h, transform48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap,
+                                                           C.byref(out_n)))
         return out_n.value
 
-    def decompress_device(self, d_src, n, d_dst, cap, from_block=None, to_block=None):
+    def decompress_device(self, d_src, n, d_dst, cap, from_block=None, to_block=None, headerless=None):
         out_n = C.c_size_t(0)
-        with self._block_range(from_block, to_block):
+        with self._block_range(from_block, to_block), self._headerless(reader=headerless):
             self._check(self.lib.kz_decompress_stream_device(self.h, d_src, n, d_dst, cap, C.byref(out_n)))
         return out_n.value
 
@@ -428,11 +481,12 @@ class Context:
         self._check(self.lib.kz_concat_bits_device(self.h, n, ptrs, bits, d_dst, cap, C.byref(total)))
         return total.value
 
-    def stream_index_device(self, d_src, n, max_blocks):
+    def stream_index_device(self, d_src, n, max_blocks, headerless=None):
         t48, et, bs, ck, isz, nb = C.c_uint64(0), C.c_uint32(0), C.c_uint32(0), C.c_uint32(0), C.c_int64(0), C.c_uint32(0)
         rec = (C.c_uint64 * (max_blocks + 1))()
-        self._check(self.lib.kz_stream_index_device(self.h, d_src, n, max_blocks, C.byref(t48), C.byref(et), C.byref(bs), C.byref(ck), C.byref(isz), rec,
-                                                    C.byref(nb)))
+        with self._headerless(reader=headerless):
+            self._check(self.lib.kz_stream_index_device(self.h, d_src, n, max_blocks, C.byref(t48), C.byref(et), C.byref(bs), C.byref(ck), C.byref(isz),
+                                                        rec, C.byref(nb)))
         return {"transform48": t48.value, "entropy": et.value, "block_size": bs.value, "checksum_bits": ck.value, "input_size": isz.value,
                 "rec_bit": [int(rec[i]) for i in range(nb.value + 1)], "nblocks": nb.value}
 
@@ -446,24 +500,26 @@ class Context:
         return self.lib.kz_cuda_stream(self.h)
 
     # ---- streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded memory -------------------------------
-    def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0):
+    def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0, headerless=None):
         """A StreamSession: write(data) -> bytes and finish() -> bytes give the stream compress() writes for the concatenated input.
-        batch_blocks=None: about 256 MiB of input per batch."""
+        batch_blocks=None: about 256 MiB of input per batch. headerless: as in compress (the session keeps the setting it opened with)."""
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         if batch_blocks is None:
             batch_blocks = default_batch_blocks(block_size)
         h = C.c_void_p()
-        self._check(self.lib.kz_writer_open(self.h, t48, et, block_size, checksum_bits, batch_blocks, input_size, C.byref(h)))
+        with self._headerless(writer=headerless):
+            self._check(self.lib.kz_writer_open(self.h, t48, et, block_size, checksum_bits, batch_blocks, input_size, C.byref(h)))
         return StreamSession(self, h, self.lib.kz_writer_write, self.lib.kz_writer_finish, self.lib.kz_writer_free)
 
-    def stream_reader(self, batch_blocks=None, from_block=None, to_block=None):
+    def stream_reader(self, batch_blocks=None, from_block=None, to_block=None, headerless=None):
         """A StreamSession: write(data) -> decoded bytes and finish() -> the rest. batch_blocks=None: about 256 MiB per batch, resolved
-        from the block size in the stream's header. from_block / to_block: the session decodes only that range of blocks."""
+        from the block size in the stream's header. from_block / to_block: the session decodes only that range of blocks. headerless: as
+        in decompress (the session keeps the setting it opened with)."""
         if batch_blocks is None:
             batch_blocks = 0
         h = C.c_void_p()
-        with self._block_range(from_block, to_block):
+        with self._block_range(from_block, to_block), self._headerless(reader=headerless):
             self._check(self.lib.kz_reader_open(self.h, batch_blocks, C.byref(h)))
         return StreamSession(self, h, self.lib.kz_reader_read, self.lib.kz_reader_finish, self.lib.kz_reader_free)
 
@@ -672,9 +728,9 @@ class Writer:
     """io.Writer (CompressedOutputStream): NewWriter(os, transform, entropy, blockSize, jobs, checksum, fileSize, headerless)
     (io/CompressedStream.go:216). write() buffers, close() compresses everything that was written in one GPU batch
     (the reference cuts batches of `jobs` blocks; batches do not change the bytes) and returns nothing; the stream
-    bytes are in .getvalue()."""
+    bytes are in .getvalue(). headerless=True writes no stream header: a HeaderlessReader with the same parameters reads it."""
 
-    def __init__(self, transform="NONE", entropy="NONE", block_size=4 << 20, jobs=1, checksum=0, file_size=0, ctx=None):
+    def __init__(self, transform="NONE", entropy="NONE", block_size=4 << 20, jobs=1, checksum=0, file_size=0, ctx=None, headerless=False):
         if not (1 <= jobs <= 64):
             raise KanziError(18, "The number of jobs must be in [1..64], got %d" % jobs)
         if block_size > (1 << 30):
@@ -688,6 +744,7 @@ class Writer:
         self.block_size = block_size
         self.checksum = checksum
         self.file_size = file_size
+        self.headerless = bool(headerless)
         self.ctx = ctx or default_context()
         self._chunks = []
         self._out = None
@@ -701,7 +758,7 @@ class Writer:
     def close(self):
         if self._out is None:
             data = np.concatenate(self._chunks) if self._chunks else np.zeros(0, np.uint8)
-            self._out = self.ctx.compress(data, self.t48, self.etype, self.block_size, self.checksum, self.file_size)
+            self._out = self.ctx.compress(data, self.t48, self.etype, self.block_size, self.checksum, self.file_size, headerless=self.headerless)
 
     def getvalue(self):
         self.close()
@@ -719,3 +776,20 @@ class Reader:
 
     def read_all(self, max_size):
         return self.ctx.decompress(self.stream, max_size, self.from_block, self.to_block)
+
+
+class HeaderlessReader(Reader):
+    """io.Reader over a stream without header: NewHeaderlessReader(is, jobs, transform, entropy, blockSize, checksum, originalSize,
+    bsVersion) (io/CompressedStream.go:1060). The parameters are checked here, as Reader.validateHeaderless does (:1178-1280); a bad
+    one raises KanziError with the code of kz_set_headerless_reader. original_size < 0 or >= 2^48 means "not given"."""
+
+    def __init__(self, stream, jobs=1, transform="NONE", entropy="NONE", block_size=4 << 20, checksum=0, original_size=0, bs_version=6, ctx=None,
+                 from_block=-1, to_block=-1):
+        super().__init__(stream, jobs, ctx, from_block, to_block)
+        self.params = dict(transform=transform, entropy=entropy, block_size=block_size, checksum_bits=checksum, output_size=original_size,
+                           bs_version=bs_version)
+        with self.ctx._headerless(reader=self.params):
+            pass
+
+    def read_all(self, max_size):
+        return self.ctx.decompress(self.stream, max_size, self.from_block, self.to_block, headerless=self.params)

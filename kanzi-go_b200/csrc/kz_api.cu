@@ -1003,6 +1003,20 @@ int parse_stream_header(kz_ctx* ctx, const uint8_t* bytes, size_t n, StreamHeade
     return 0;
 }
 
+// A headerless stream (kz_set_headerless_reader, NewHeaderlessReader io/CompressedStream.go:1060) has no header to parse (readHeader is
+// skipped, :1317): its fields are the setting's, and its first record starts at bit 0.
+StreamHeader headerless_header(const kz_ctx* ctx) {
+    const kz_ctx::Headerless& s = ctx->headerless_reader;
+    StreamHeader h;
+    h.t48 = s.t48;
+    h.etype = s.etype;
+    h.block_size = s.block_size;
+    h.checksum_bits = s.checksum_bits;
+    h.input_size = s.output_size;
+    h.bits = 0;
+    return h;
+}
+
 int count_transforms(uint64_t t48, uint64_t* ids) {
     int n = 0;
     for (int i = 0; i < 8; i++) {
@@ -1912,6 +1926,48 @@ int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block) {
     return 0;
 }
 
+int kz_set_headerless_writer(kz_ctx* ctx, int on) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    ctx->headerless_writer = on != 0;
+    return 0;
+}
+
+// Reader.validateHeaderless (io/CompressedStream.go:1178-1280) over ids instead of names: entropy.GetType and transform.GetType accept the
+// names of entropy ids 0..9 but PAQ (3) and of transform ids 0..19 but SNAPPY (4) (EntropyCodecFactory.go:170-206, Factory.go:330-395).
+int kz_set_headerless_reader(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t output_size,
+                             uint32_t bs_version) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    if (bs_version > BS_VERSION) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid bitstream version, cannot read this version of the stream");
+    if (bs_version < BS_VERSION) return ctx->fail(KZ_ERR_STREAM_VERSION, "Only bitstream version 6 is supported");
+    if (etype > 9 || etype == 3) return ctx->fail(KZ_ERR_INVALID_PARAM, "Unsupported entropy codec type");
+    if (t48 >> 48) return ctx->fail(KZ_ERR_INVALID_PARAM, "Unknown transform type");
+    for (int i = 0; i < 8; i++) {
+        const uint64_t t = (t48 >> (42 - 6 * i)) & 63;
+        if (t > 19 || t == 4) return ctx->fail(KZ_ERR_INVALID_PARAM, "Unknown transform type");
+    }
+    if (block_size < 1024 || block_size > (1u << 30)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64)
+        return ctx->fail(KZ_ERR_INVALID_PARAM, "The block checksum size must be 32 or 64 bits");
+    if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+    TransformPlan plan;
+    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    kz_ctx::Headerless& h = ctx->headerless_reader;
+    h.on = true;
+    h.t48 = t48;
+    h.etype = etype;
+    h.block_size = block_size;
+    h.checksum_bits = checksum_bits;
+    h.output_size = output_size < 0 || output_size >= ((int64_t)1 << 48) ? 0 : output_size;  // :1264-1268
+    return 0;
+}
+
+int kz_clear_headerless_reader(kz_ctx* ctx) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    ctx->headerless_reader = kz_ctx::Headerless();
+    return 0;
+}
+
 void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size) {
     if (ctx) ctx->user_stream_bs = block_size;
 }
@@ -1966,7 +2022,7 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     if (rc) return rc;
     std::vector<uint8_t> hdr;
     uint32_t hdr_bits = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size);
-    if (fragment) hdr_bits = 0;
+    if (fragment || ctx->headerless_writer) hdr_bits = 0;  // an empty leading segment (Writer.writeHeader :430)
     EncResult res;
     ctx->fragment = fragment;
     rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, d_src, n, hdr, hdr_bits, d_dst, cap, res);
@@ -2066,6 +2122,10 @@ int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, 
 static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
                                   size_t n, void* d_dst, size_t cap, size_t* out_n);
 int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
+    if (ctx && ctx->headerless_reader.on) {
+        const StreamHeader sh = headerless_header(ctx);
+        return decompress_device_impl(ctx, &sh, 0, 0, ctx->range_from, ctx->range_to, d_src, n, d_dst, cap, out_n);
+    }
     return decompress_device_impl(ctx, nullptr, 0, 0, ctx ? ctx->range_from : -1, ctx ? ctx->range_to : -1, d_src, n, d_dst, cap, out_n);
 }
 // Decodes `nblocks` block records that start at bit `start_bit` of the fragment at d_src (frag_bytes bytes, >= 64 readable bytes behind them):
@@ -2085,18 +2145,24 @@ int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uin
     return decompress_device_impl(ctx, &sh, start_bit, nblocks, -1, -1, d_src, frag_bytes, d_dst, cap, out_n);
 }
 // Parses the header of the stream at d_src and walks its block records: rec_bit[b] = first bit of record b (its 5-bit prefix), rec_bit[nblocks] =
-// first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries.
+// first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries. With a headerless reader setting the fields are
+// the setting's and rec_bit[0] = 0.
 int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t max_blocks, uint64_t* t48, uint32_t* etype, uint32_t* block_size,
                            uint32_t* checksum_bits, int64_t* input_size, uint64_t* rec_bit, uint32_t* nblocks) {
     if (!ctx || !d_src || !rec_bit || !nblocks) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    uint8_t head[64];
-    memset(head, 0, sizeof(head));
-    CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
     StreamHeader sh;
-    int rc = parse_stream_header(ctx, head, n, sh);
-    if (rc) return rc;
+    int rc = 0;
+    if (ctx->headerless_reader.on) {
+        sh = headerless_header(ctx);
+    } else {
+        uint8_t head[64];
+        memset(head, 0, sizeof(head));
+        CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        rc = parse_stream_header(ctx, head, n, sh);
+        if (rc) return rc;
+    }
     if (t48) *t48 = sh.t48;
     if (etype) *etype = sh.etype;
     if (block_size) *block_size = sh.block_size;
@@ -2339,9 +2405,12 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
     stage_off.assign(nstreams, 0);
     uint64_t stage = 0, nsegs = 0;
     for (uint32_t s = 0; s < nstreams; s++) {
-        std::vector<uint8_t> hdr;
-        hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size ? input_size[s] : 0);
-        memcpy(&small[64 * (size_t)s], hdr.data(), 64);
+        hdr_bits[s] = 0;
+        if (!ctx->headerless_writer) {  // Writer.writeHeader :430
+            std::vector<uint8_t> hdr;
+            hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size ? input_size[s] : 0);
+            memcpy(&small[64 * (size_t)s], hdr.data(), 64);
+        }
         uint64_t bits = hdr_bits[s] + END_MARKER_BITS;
         for (uint32_t b = first[s]; b < first[s + 1]; b++) {
             pre_bits[b] = write_block_prefix(&small[64 * (size_t)nstreams + 8 * (size_t)b], bbits[b]);
@@ -2370,7 +2439,7 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
             seg_dst.push_back(d);
             d += nbits;
         };
-        add(A + 64 * (size_t)s, hdr_bits[s]);
+        if (hdr_bits[s]) add(A + 64 * (size_t)s, hdr_bits[s]);
         for (uint32_t b = first[s]; b < first[s + 1]; b++) {
             add(A + 64 * (size_t)nstreams + 8 * (size_t)b, pre_bits[b]);
             for (uint64_t o = 0; o < bbits[b]; o += 8 * RAW_PIECE) add(ctx->d_bits.as<uint8_t>() + barena[b] + o / 8, std::min<uint64_t>(8 * RAW_PIECE, bbits[b] - o));
@@ -2457,39 +2526,54 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
                                    uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
     for (uint32_t s = 0; s < nstreams; s++) status[s] = 0, out_len[s] = 0;
     if (nstreams == 0) return 0;
-    // headers: the first 64 bytes of every stream in one gather and one transfer, parsed by parse_stream_header
-    CK(ctx->d_asm.ensure(64 * (size_t)nstreams));
-    CK(cudaMemsetAsync(ctx->d_asm.p, 0, 64 * (size_t)nstreams, ctx->stream));
-    CopyList heads;
-    for (uint32_t s = 0; s < nstreams; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
-    int rc = run_copies(ctx, heads);
-    if (rc) return rc;
-    std::vector<uint8_t> head(64 * (size_t)nstreams);
-    CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    std::vector<StreamHeader> sh(nstreams);
-    std::vector<TransformPlan> plan(nstreams);
-    std::vector<uint64_t> hdr_bits(nstreams, 0);
-    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
-    for (uint32_t s = 0; s < nstreams; s++) {
-        status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
-        if (status[s]) continue;
-        rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
-        if (rc) return rc;
-        if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
-        hdr_bits[s] = sh[s].bits;
-        groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
-    }
+    int rc = 0;
     std::vector<uint32_t> alone;
-    for (auto& kv : groups) {
-        const uint32_t s0 = kv.second[0];
-        rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
+    const bool headerless = ctx->headerless_reader.on;
+    const StreamHeader hl = headerless ? headerless_header(ctx) : StreamHeader();
+    if (headerless) {  // no headers to gather: every stream has the setting's fields, so all of them form one group
+        TransformPlan plan;
+        rc = plan_transforms(ctx, hl.t48, hl.etype, plan, KZ_ERR_INVALID_CODEC);
         if (rc) return rc;
+        std::vector<uint32_t> all(nstreams);
+        for (uint32_t s = 0; s < nstreams; s++) all[s] = s;
+        rc = decode_stream_group(ctx, hl, plan, all, std::vector<uint64_t>(nstreams, 0), d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len,
+                                 status, alone);
+        if (rc) return rc;
+    } else {
+        // headers: the first 64 bytes of every stream in one gather and one transfer, parsed by parse_stream_header
+        CK(ctx->d_asm.ensure(64 * (size_t)nstreams));
+        CK(cudaMemsetAsync(ctx->d_asm.p, 0, 64 * (size_t)nstreams, ctx->stream));
+        CopyList heads;
+        for (uint32_t s = 0; s < nstreams; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
+        rc = run_copies(ctx, heads);
+        if (rc) return rc;
+        std::vector<uint8_t> head(64 * (size_t)nstreams);
+        CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        std::vector<StreamHeader> sh(nstreams);
+        std::vector<TransformPlan> plan(nstreams);
+        std::vector<uint64_t> hdr_bits(nstreams, 0);
+        std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
+        for (uint32_t s = 0; s < nstreams; s++) {
+            status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
+            if (status[s]) continue;
+            rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
+            if (rc) return rc;
+            if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
+            hdr_bits[s] = sh[s].bits;
+            groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
+        }
+        for (auto& kv : groups) {
+            const uint32_t s0 = kv.second[0];
+            rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status,
+                                     alone);
+            if (rc) return rc;
+        }
     }
     for (uint32_t s : alone) {  // only corrupt input, too little room or a failing stage call gets here
         size_t n = 0;
-        status[s] = decompress_device_impl(ctx, nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s], d_dst + dst_off[s],
-                                           dst_cap[s], &n);
+        status[s] = decompress_device_impl(ctx, headerless ? &hl : nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s],
+                                           d_dst + dst_off[s], dst_cap[s], &n);
         out_len[s] = status[s] ? 0 : n;
     }
     return 0;
@@ -3151,6 +3235,7 @@ struct kz_writer : kz::Session {
     uint64_t t48 = 0;
     uint32_t etype = 0, block_size = 0, checksum_bits = 0;
     int64_t input_size = 0;
+    bool headerless = false;  // the context's headerless writer setting when the session opened (kz_set_headerless_writer)
     DevBuf d_out;            // the finished bytes of one batch
     size_t out_cap = 0;
     uint64_t batches = 0;    // batches encoded (worker)
@@ -3161,12 +3246,13 @@ struct kz_writer : kz::Session {
     size_t own_device_bytes() override { return d_out.cap; }
     void release_own() override { d_out.release(); }
 
-    // worker: one batch = the blocks of input slot k behind the stream header (first batch) or the carry; the end marker only in the last
+    // worker: one batch = the blocks of input slot k behind the stream header (first batch; nothing when headerless) or the carry; the end
+    // marker only in the last
     int run(int k, bool last) override {
         CK(cudaStreamWaitEvent(ctx->stream, ev[k], 0));
         std::vector<uint8_t> lead(64, 0);
         uint32_t lead_bits = carry_bits;
-        if (batches == 0) lead_bits = build_stream_header(lead, t48, etype, block_size, checksum_bits, input_size);
+        if (batches == 0) lead_bits = headerless ? 0 : build_stream_header(lead, t48, etype, block_size, checksum_bits, input_size);
         else lead[0] = carry;
         EncResult res;
         ctx->stream_bs = block_size;
@@ -3210,9 +3296,9 @@ struct kz_reader : kz::Session {
     }
 
     // caller: the stream header is parsed from the first 64 bytes (or fewer at finish, as kz_decompress_stream does); the buffers are
-    // sized from it
-    int start() {
-        int rc = parse_stream_header(ctx, head, head_len, sh);
+    // sized from it. A headerless session has sh from the setting and starts at open.
+    int start(bool headerless) {
+        int rc = headerless ? 0 : parse_stream_header(ctx, head, head_len, sh);
         if (rc == 0) rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_INVALID_CODEC);
         if (rc) return fail(-rc, ctx->err);
         const uint64_t bs = sh.block_size;
@@ -3247,7 +3333,7 @@ struct kz_reader : kz::Session {
             memcpy(head + head_len, src, c);
             head_len += c;
             if (head_len < sizeof(head)) return (int64_t)c;
-            int rc = start();
+            int rc = start(false);
             if (rc) return rc;
         }
         {
@@ -3259,7 +3345,7 @@ struct kz_reader : kz::Session {
     }
     int hand_last() override {
         if (!have_header) {
-            int rc = start();
+            int rc = start(false);
             if (rc) return rc;
         }
         return give((int)(given % 2), true);
@@ -3395,6 +3481,7 @@ int kz_writer_open(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_siz
     w->block_size = block_size;
     w->checksum_bits = checksum_bits;
     w->input_size = input_size_hint;
+    w->headerless = ctx->headerless_writer;
     const size_t in_bytes = (size_t)batch_blocks * block_size;
     w->out_cap = kz_max_stream_output(in_bytes, block_size) + 64;
     rc = w->alloc_inputs(in_bytes);
@@ -3443,6 +3530,10 @@ int kz_reader_open(kz_ctx* ctx, uint32_t batch_blocks, kz_reader** out) {
     r->range_from = ctx->range_from;
     r->range_to = ctx->range_to;
     int rc = r->open_common();
+    if (rc == 0 && ctx->headerless_reader.on) {
+        r->sh = headerless_header(ctx);
+        rc = r->start(true);
+    }
     if (rc) {
         r->close();
         delete r;

@@ -137,6 +137,13 @@ struct kz_ctx {
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
     uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
     int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)
+    bool headerless_writer = false;          // kz_set_headerless_writer: the stream-level encodes write no stream header
+    struct Headerless {                      // kz_set_headerless_reader: the stream-level decodes take these instead of a header
+        bool on = false;
+        uint64_t t48 = 0;
+        uint32_t etype = 0, block_size = 0, checksum_bits = 0;
+        int64_t output_size = 0;             // 0 = not given
+    } headerless_reader;
     std::map<std::string, kz::ProfEntry> prof;
     struct Pending {
         std::string name;
