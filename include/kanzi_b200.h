@@ -230,6 +230,20 @@ int kz_set_headerless_reader(kz_ctx* ctx, uint64_t transform48, uint32_t entropy
                              uint32_t bs_version);
 int kz_clear_headerless_reader(kz_ctx* ctx);
 
+/* kanzi's skipBlocks option (kanzi c --skip, ctx["skipBlocks"]): store incompressible blocks raw. Off by default. With on != 0, the encodes
+ * that follow (kz_encode_blocks, kz_compress_stream[_device], kz_compress_streams[_device], kz_compress_fragment_device and kz_writer_open,
+ * which captures the setting when the session opens, as it does the headerless writer setting) decide for every block of more than 15
+ * bytes what encodingTask.encode decides (io/CompressedStream.go:778-800): the block is stored when its first four bytes are the magic
+ * number of a compressed format (IsDataCompressed(GetMagicType), internal/Magic.go:73-149: only FFD8FFE0 among the JPEG keys) or when
+ * ComputeFirstOrderEntropy1024 of its order-0 histogram reaches INCOMPRESSIBLE_THRESHOLD (973 of 1024, entropy/EntropyUtils.go:26). A
+ * stored block is written like a block of at most 15 bytes: COPY_BLOCK_MASK set, no transform and no entropy codec, its bytes raw and the
+ * checksum of the block. No transform stage runs on it, in either direction. Blocks that are not stored, and every byte with the setting
+ * off, are unchanged; a stored block differs from a plain NONE & NONE block in its mode byte. The decoders need no setting.
+ * Cost: one order-0 histogram pass over the input and one device-to-host copy per batch (the block heads and entropy flags together).
+ * With kz_profile(ctx,1), kz_stage_bytes("skip:magic" / "skip:entropy") gives the blocks (*bytes_in) and bytes (*bytes_out) stored for
+ * each reason, and kz_kernel_time("skip_hist" / "skip_decide") the test's kernels. Returns 0, or -KZ_ERR_INVALID_PARAM without a context. */
+int kz_set_skip_blocks(kz_ctx* ctx, int on);
+
 /* ---- streaming sessions: CompressedOutputStream / CompressedInputStream (io/CompressedStream.go:524-710, :1556-1744) for a stream of any
  *      length, or one that arrives in pieces (a pipe, a socket), in memory that does not grow with the stream ------------------------------
  * A zlib-style pump. The session takes ctx over until kz_*_free: the caller makes no other call on ctx in between except kz_device_bytes,

@@ -273,3 +273,26 @@ func NewHeaderlessStreamReader(c *Context, r io.Reader, batchBlocks uint32, tran
 	C.kz_clear_headerless_reader(c.h) // without c.mu, which the open session holds: the call is allowed while a session is open
 	return s, err
 }
+
+// SkipBlocks reads kanzi's ctx["skipBlocks"], which NewWriterWithCtx checks to be a bool (io/CompressedStream.go:370-374) and
+// `kanzi c -s/--skip` sets (app/BlockCompressor.go:504). A missing key gives false.
+func SkipBlocks(ctx map[string]any) bool {
+	v, ok := ctx["skipBlocks"].(bool)
+	return ok && v
+}
+
+// SetSkipBlocks is kz_set_skip_blocks: the encodes that follow on c (EncodeBlocks, CompressStreams, and NewStreamWriter, which keeps the
+// setting for its session) store every block of more than 15 bytes that starts with a compressed format's magic number or whose order-0
+// entropy reaches INCOMPRESSIBLE_THRESHOLD raw, as encodingTask.encode does with ctx["skipBlocks"] (:778-800).
+func (c *Context) SetSkipBlocks(on bool) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	v := C.int(0)
+	if on {
+		v = 1
+	}
+	if rc := C.kz_set_skip_blocks(c.h, v); rc != 0 {
+		return c.err(rc)
+	}
+	return nil
+}

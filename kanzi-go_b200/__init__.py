@@ -40,7 +40,7 @@ ABI_SYMBOLS = [
     "kz_compress_streams", "kz_decompress_streams", "kz_compress_streams_device", "kz_decompress_streams_device",
     "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
     "kz_reader_free", "kz_device_bytes", "kz_set_block_range", "kz_bwt_profile",
-    "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader",
+    "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader", "kz_set_skip_blocks",
 ]
 
 
@@ -144,6 +144,7 @@ def load_library(build_if_missing=True):
     L.kz_set_headerless_writer.argtypes = [vp, i32]
     L.kz_set_headerless_reader.argtypes = [vp, u64, u32, u32, u32, C.c_int64, u32]
     L.kz_clear_headerless_reader.argtypes = [vp]
+    L.kz_set_skip_blocks.argtypes = [vp, i32]
     L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -200,6 +201,7 @@ class Context:
         self._range = (-1, -1)  # kz_set_block_range's (from, to) on this context
         self._hl_writer = False  # kz_set_headerless_writer's setting
         self._hl_reader = None   # kz_set_headerless_reader's arguments, None when it is off
+        self._skip = False       # kz_set_skip_blocks's setting
 
     def close(self):
         if getattr(self, "h", None):
@@ -256,8 +258,9 @@ class Context:
         self._check(self.lib.kz_transform_inverse(self.h, ttype, _p(a), a.size, out.ctypes.data, cap, C.byref(n)))
         return out[: n.value].copy()
 
-    def encode_blocks(self, transform48, etype, blocks, checksum_bits=0):
-        """blocks: list of byte arrays -> list of (bytes, nbits). One kz_encode_blocks call (Writer.processBlock batch)."""
+    def encode_blocks(self, transform48, etype, blocks, checksum_bits=0, skip_blocks=None):
+        """blocks: list of byte arrays -> list of (bytes, nbits). One kz_encode_blocks call (Writer.processBlock batch). skip_blocks: see
+        set_skip_blocks (None: the context's setting)."""
         nb = len(blocks)
         arrs = [_u8(b) for b in blocks]
         lens = np.array([a.size for a in arrs], np.uint32)
@@ -269,8 +272,9 @@ class Context:
         out = np.zeros(ostride * max(nb, 1), np.uint8)
         bits = np.zeros(max(nb, 1), np.uint64)
         status = np.zeros(max(nb, 1), np.int32)
-        self._check(self.lib.kz_encode_blocks(self.h, transform48, etype, checksum_bits, slab.ctypes.data, stride, lens.ctypes.data, nb,
-                                              out.ctypes.data, ostride, bits.ctypes.data, status.ctypes.data))
+        with self._skip_blocks(skip_blocks):
+            self._check(self.lib.kz_encode_blocks(self.h, transform48, etype, checksum_bits, slab.ctypes.data, stride, lens.ctypes.data, nb,
+                                                  out.ctypes.data, ostride, bits.ctypes.data, status.ctypes.data))
         return [(out[i * ostride: i * ostride + (int(bits[i]) + 7) // 8].copy(), int(bits[i])) for i in range(nb)]
 
     def decode_blocks(self, transform48, etype, payloads, block_size, checksum_bits=0):
@@ -294,15 +298,16 @@ class Context:
                                               out.ctypes.data, ostride, lens.ctypes.data, status.ctypes.data))
         return [out[i * ostride: i * ostride + int(lens[i])].copy() for i in range(nb)]
 
-    def compress(self, data, transform="NONE", entropy="NONE", block_size=4 << 20, checksum_bits=0, input_size=0, headerless=None):
-        """headerless: True / False sets the headerless writer setting for this call (None: the context's setting)."""
+    def compress(self, data, transform="NONE", entropy="NONE", block_size=4 << 20, checksum_bits=0, input_size=0, headerless=None, skip_blocks=None):
+        """headerless: True / False sets the headerless writer setting for this call (None: the context's setting). skip_blocks: the same
+        for set_skip_blocks."""
         a = _u8(data)
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         cap = self.lib.kz_max_stream_output(a.size, block_size)
         out = np.empty(cap, np.uint8)
         n = C.c_size_t(0)
-        with self._headerless(writer=headerless):
+        with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
             self._check(self.lib.kz_compress_stream(self.h, t48, et, block_size, checksum_bits, input_size, _p(a), a.size, out.ctypes.data, cap, C.byref(n)))
         return out[: n.value].copy()
 
@@ -376,9 +381,30 @@ class Context:
                 else:
                     self.set_headerless_reader(*prev_r)
 
+    # ---- kanzi's skipBlocks option (kz_set_skip_blocks): store incompressible blocks raw ----------------------------------------------
+    def set_skip_blocks(self, on=True):
+        """The encodes that follow (encode_blocks, compress*, compress_streams*, compress_fragment_device, stream_writer when it opens) store
+        every block of more than 15 bytes that starts with a compressed format's magic number or whose order-0 entropy reaches 973 / 1024
+        as a COPY block, as kanzi c --skip does."""
+        self._check(self.lib.kz_set_skip_blocks(self.h, 1 if on else 0))
+        self._skip = bool(on)
+
+    @contextlib.contextmanager
+    def _skip_blocks(self, on):
+        """Sets the skipBlocks setting for one call (on: a bool) and restores the previous one afterwards. None leaves it as it is."""
+        if on is None:
+            yield
+            return
+        prev = self._skip
+        self.set_skip_blocks(on)
+        try:
+            yield
+        finally:
+            self.set_skip_blocks(prev)
+
     # ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams) -----------------------------------
     # Per-stream failures do not raise: status[s] = 0 or -(kanzi error code), and outputs[s] is None for a failed stream.
-    def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None, headerless=None):
+    def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None, headerless=None, skip_blocks=None):
         """One compressed stream per input, each equal to compress(inputs[s], ..., input_size=input_sizes[s]) -> (outputs, status)."""
         arrs = [_u8(x) for x in inputs]
         t48 = transform_type(transform) if isinstance(transform, str) else transform
@@ -391,7 +417,7 @@ class Context:
         dst = np.empty(max(int(cap.sum()), 1), np.uint8)
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
-        with self._headerless(writer=headerless):
+        with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
             self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len),
                                          None if isz is None else _p(isz), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
@@ -415,14 +441,14 @@ class Context:
         return outs, status
 
     def compress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, transform, entropy, block_size, checksum_bits=0,
-                                input_sizes=None, headerless=None):
+                                input_sizes=None, headerless=None, skip_blocks=None):
         """src / dst: CUDA uint8 tensors (or device addresses); offsets (multiples of 16) and lengths: host sequences -> (out_len, status)."""
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
-        with self._headerless(writer=headerless):
+        with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
             self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl),
                                                 None if isz is None else _p(isz), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
@@ -436,9 +462,9 @@ class Context:
         return out_len, status
 
     # ---- device-resident entry points (pointers are CUDA device addresses, e.g. torch tensors' data_ptr()) -------
-    def compress_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, input_size=0, headerless=None):
+    def compress_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, input_size=0, headerless=None, skip_blocks=None):
         out_n = C.c_size_t(0)
-        with self._headerless(writer=headerless):
+        with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
             self._check(self.lib.kz_compress_stream_device(self.h, transform48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap,
                                                            C.byref(out_n)))
         return out_n.value
@@ -460,9 +486,10 @@ class Context:
         return out_n.value
 
     # ---- sharded streams (one stream, blocks spread over ranks; kanzi-go_b200/parallel.py drives these) ---------------------
-    def compress_fragment_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0):
+    def compress_fragment_device(self, d_src, n, d_dst, cap, transform48, etype, block_size, checksum_bits=0, skip_blocks=None):
         bits = C.c_uint64(0)
-        self._check(self.lib.kz_compress_fragment_device(self.h, transform48, etype, block_size, checksum_bits, d_src, n, d_dst, cap, C.byref(bits)))
+        with self._skip_blocks(skip_blocks):
+            self._check(self.lib.kz_compress_fragment_device(self.h, transform48, etype, block_size, checksum_bits, d_src, n, d_dst, cap, C.byref(bits)))
         return bits.value
 
     def stream_header(self, transform48, etype, block_size, checksum_bits=0, input_size=0):
@@ -500,15 +527,16 @@ class Context:
         return self.lib.kz_cuda_stream(self.h)
 
     # ---- streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded memory -------------------------------
-    def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0, headerless=None):
+    def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0, headerless=None, skip_blocks=None):
         """A StreamSession: write(data) -> bytes and finish() -> bytes give the stream compress() writes for the concatenated input.
-        batch_blocks=None: about 256 MiB of input per batch. headerless: as in compress (the session keeps the setting it opened with)."""
+        batch_blocks=None: about 256 MiB of input per batch. headerless, skip_blocks: as in compress (the session keeps the settings it
+        opened with)."""
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         if batch_blocks is None:
             batch_blocks = default_batch_blocks(block_size)
         h = C.c_void_p()
-        with self._headerless(writer=headerless):
+        with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
             self._check(self.lib.kz_writer_open(self.h, t48, et, block_size, checksum_bits, batch_blocks, input_size, C.byref(h)))
         return StreamSession(self, h, self.lib.kz_writer_write, self.lib.kz_writer_finish, self.lib.kz_writer_free)
 
@@ -728,9 +756,11 @@ class Writer:
     """io.Writer (CompressedOutputStream): NewWriter(os, transform, entropy, blockSize, jobs, checksum, fileSize, headerless)
     (io/CompressedStream.go:216). write() buffers, close() compresses everything that was written in one GPU batch
     (the reference cuts batches of `jobs` blocks; batches do not change the bytes) and returns nothing; the stream
-    bytes are in .getvalue(). headerless=True writes no stream header: a HeaderlessReader with the same parameters reads it."""
+    bytes are in .getvalue(). headerless=True writes no stream header: a HeaderlessReader with the same parameters reads it.
+    skip_blocks=True is ctx["skipBlocks"] (kanzi c --skip): incompressible blocks are stored raw (Context.set_skip_blocks)."""
 
-    def __init__(self, transform="NONE", entropy="NONE", block_size=4 << 20, jobs=1, checksum=0, file_size=0, ctx=None, headerless=False):
+    def __init__(self, transform="NONE", entropy="NONE", block_size=4 << 20, jobs=1, checksum=0, file_size=0, ctx=None, headerless=False,
+                 skip_blocks=False):
         if not (1 <= jobs <= 64):
             raise KanziError(18, "The number of jobs must be in [1..64], got %d" % jobs)
         if block_size > (1 << 30):
@@ -745,6 +775,7 @@ class Writer:
         self.checksum = checksum
         self.file_size = file_size
         self.headerless = bool(headerless)
+        self.skip_blocks = bool(skip_blocks)
         self.ctx = ctx or default_context()
         self._chunks = []
         self._out = None
@@ -758,7 +789,8 @@ class Writer:
     def close(self):
         if self._out is None:
             data = np.concatenate(self._chunks) if self._chunks else np.zeros(0, np.uint8)
-            self._out = self.ctx.compress(data, self.t48, self.etype, self.block_size, self.checksum, self.file_size, headerless=self.headerless)
+            self._out = self.ctx.compress(data, self.t48, self.etype, self.block_size, self.checksum, self.file_size, headerless=self.headerless,
+                                          skip_blocks=self.skip_blocks)
 
     def getvalue(self):
         self.close()

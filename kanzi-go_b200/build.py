@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libkanzi_b200.so")
-SOURCES = ["kz_ans.cu", "kz_ans1.cu", "kz_huffman.cu", "kz_range.cu", "kz_hash.cu", "kz_sbrt.cu", "kz_zrlt.cu", "kz_rolz.cu", "kz_alias.cu", "kz_fsd.cu", "kz_text.cu", "kz_text_par.cu", "kz_utf.cu", "kz_exe.cu", "kz_bwt.cu", "kz_lz.cu", "kz_lz_par.cu", "kz_lz_inv.cu", "kz_concat.cu", "kz_api.cu"]
+SOURCES = ["kz_ans.cu", "kz_ans1.cu", "kz_huffman.cu", "kz_range.cu", "kz_hash.cu", "kz_sbrt.cu", "kz_zrlt.cu", "kz_rolz.cu", "kz_alias.cu", "kz_fsd.cu", "kz_text.cu", "kz_text_par.cu", "kz_utf.cu", "kz_exe.cu", "kz_bwt.cu", "kz_lz.cu", "kz_lz_par.cu", "kz_lz_inv.cu", "kz_concat.cu", "kz_skip.cu", "kz_api.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
          "-Xptxas", "-v"]
 

@@ -24,6 +24,8 @@
 #include "kz_text.cuh"
 #include "kz_utf.cuh"
 #include "kz_exe.cuh"
+#include "kz_entropy_core.cuh"
+#include "kz_skip.cuh"
 #include "kz_stream_plan.h"
 
 #include <condition_variable>
@@ -1057,6 +1059,66 @@ int32_t magic_data_type(const uint8_t* p, size_t n) {
     return 0;
 }
 
+// kanzi's skipBlocks option (encodingTask.encode, io/CompressedStream.go:778-800), device half: the order-0 histogram of every block
+// d_base + off[b] (len[b] bytes, any alignment) and its entropy test (kz_skip.cu). The blocks of at most SMALL_BLOCK bytes, stored in any
+// case, are not read. On return the work is queued, and *d_heads points at 4 * nb zero bytes of ctx->d_skip for the caller's block heads,
+// followed by nb flag bytes (1: the order-0 entropy reaches INCOMPRESSIBLE_THRESHOLD), so that one copy brings both back.
+int skip_test(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint8_t** d_heads) {
+    const uint32_t nb = (uint32_t)len.size();
+    std::vector<SkipTile> tiles;
+    for (uint32_t b = 0; b < nb; b++)
+        if (len[b] > SMALL_BLOCK)
+            for (uint32_t o = 0; o < len[b]; o += SKIP_TILE) tiles.push_back(SkipTile{off[b] + o, std::min(SKIP_TILE, len[b] - o), b});
+    const size_t o_heads = (size_t)nb * 256 * 4;  // behind the histograms
+    CK(ctx->d_skip.ensure(o_heads + 5 * (size_t)nb));
+    uint8_t* S = ctx->d_skip.as<uint8_t>();
+    CK(cudaMemsetAsync(S, 0, o_heads + 4 * (size_t)nb, ctx->stream));
+    Packer pk;
+    const size_t o_tiles = pk.add(tiles.data(), tiles.size() * sizeof(SkipTile));
+    const size_t o_len = pk.add(len.data(), (size_t)nb * 4);
+    const size_t o_log2 = pk.add(host_log2_4096(), 257 * 4);
+    int rc = upload(ctx, pk);
+    if (rc) return rc;
+    const uint8_t* T = ctx->d_tables.as<uint8_t>();
+    if (!tiles.empty()) {
+        LaunchScope ls(ctx, "skip_hist");
+        skip_hist_kernel<<<(uint32_t)((tiles.size() + SKIP_HIST_WARPS - 1) / SKIP_HIST_WARPS), 32 * SKIP_HIST_WARPS, 0, ctx->stream>>>(
+            d_base, (const SkipTile*)(T + o_tiles), (uint32_t)tiles.size(), (uint32_t*)S);
+    }
+    {
+        LaunchScope ls(ctx, "skip_decide");
+        skip_decide_kernel<<<(nb + 255) / 256, 256, 0, ctx->stream>>>((const uint32_t*)S, (const uint32_t*)(T + o_len), nb, (const uint32_t*)(T + o_log2),
+                                                                     S + o_heads + 4 * (size_t)nb);
+    }
+    CK(cudaGetLastError());
+    *d_heads = S + o_heads;
+    return 0;
+}
+
+// skipBlocks, host half: block b (len[b] bytes) is stored when it has more than SMALL_BLOCK bytes and its head is the magic number of a
+// compressed format (magic_data_type 7: IsDataCompressed(GetMagicType)) or its entropy flag is set. hf = 4 head bytes per block, then one
+// flag byte per block (skip_test). With profiling on, the blocks and bytes stored for each reason add up under "skip:magic" and
+// "skip:entropy" (bytes_in = blocks, bytes_out = bytes).
+std::vector<uint8_t> stored_blocks(kz_ctx* ctx, const std::vector<uint8_t>& hf, const uint32_t* len, uint32_t nb) {
+    std::vector<uint8_t> store(nb, 0);
+    uint64_t n_magic = 0, b_magic = 0, n_ent = 0, b_ent = 0;
+    for (uint32_t b = 0; b < nb; b++) {
+        if (len[b] <= SMALL_BLOCK) continue;
+        if (magic_data_type(&hf[(size_t)b * 4], len[b]) == 7) {
+            store[b] = 1, n_magic++, b_magic += len[b];
+        } else if (hf[(size_t)nb * 4 + b]) {
+            store[b] = 1, n_ent++, b_ent += len[b];
+        }
+    }
+    if (ctx->profile) {
+        auto& m = ctx->prof["skip:magic"];
+        m.bytes_in += n_magic, m.bytes_out += b_magic, m.launches++;
+        auto& e = ctx->prof["skip:entropy"];
+        e.bytes_in += n_ent, e.bytes_out += b_ent, e.launches++;
+    }
+    return store;
+}
+
 struct TransformPlan {
     int nt = 0;
     uint64_t ids[8];
@@ -1591,8 +1653,11 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
 // Forward transform stage (ByteTransformSequence.Forward, transform/Sequence.go:64-125) of every block of a batch.
 // Block b is d_src[b*stride : +len_b]. On return *d_data is the base of the post-transform data and jobs[] describes
 // every block for the entropy stage. NONE leaves the data in place; the stages alternate between ctx->d_tmp and ctx->d_tmp2.
+// A block with store[b] set (skipBlocks) is a COPY block, like a block of at most SMALL_BLOCK bytes: no stage runs on it, and
+// a batch of nothing but COPY blocks runs no stage at all.
 int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, size_t n, uint32_t block_size, uint64_t stride, const uint32_t* lens,
-                  uint32_t nblocks, const uint8_t** d_data, std::vector<EncJob>& jobs, const std::vector<int32_t>* init_dt = nullptr) {
+                  uint32_t nblocks, const uint8_t** d_data, std::vector<EncJob>& jobs, const std::vector<int32_t>* init_dt = nullptr,
+                  const std::vector<uint8_t>* store = nullptr) {
     jobs.resize(nblocks);
     std::vector<uint32_t> len(nblocks);
     uint32_t max_len = 0;
@@ -1607,20 +1672,25 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
         j.post_len = len[b];
         j.ntransforms = (uint32_t)plan.nt;
         j.skip_flags = 0x7F;  // NullTransform succeeds: bit 7 cleared (Sequence.go:65,107)
-        j.copy = len[b] <= SMALL_BLOCK;  // io/CompressedStream.go:773-776: transform and entropy forced to NONE
+        j.copy = len[b] <= SMALL_BLOCK || (store && (*store)[b]);  // io/CompressedStream.go:773-799: transform and entropy forced to NONE
         j.checksum = 0;
     }
     if (plan.none() || nblocks == 0) return 0;
     // ctx["dataType"] of every block: the caller's value (from the block's magic number, encodingTask.encode :808-816), updated by the stages
     std::vector<int32_t> dts(nblocks, 0);
     if (init_dt) dts = *init_dt;
+    std::vector<uint8_t> active(nblocks), applied;
+    bool any = false;
+    for (uint32_t b = 0; b < nblocks; b++) {
+        active[b] = !jobs[b].copy && len[b] > 0;
+        any = any || active[b];
+    }
+    if (!any) return 0;
     // room for the largest stage output: +33 bytes per BWT / SBRT stage, n/64 + 128 for LZ, n/16 for MM, headers of PACK
     const uint64_t gstride = ((uint64_t)max_len + max_len / 8 + 33ull * plan.nt + 8192 + 1024 + 256 + 15) & ~15ull;
     CK(ctx->d_tmp.ensure(gstride * nblocks + 64));
     if (plan.nt > 1) CK(ctx->d_tmp2.ensure(gstride * nblocks + 64));  // stage i writes to d_tmp (i even) or d_tmp2 (i odd)
-    std::vector<uint8_t> active(nblocks), applied;
     std::vector<uint8_t> flags(nblocks, 0xFF);
-    for (uint32_t b = 0; b < nblocks; b++) active[b] = !jobs[b].copy && len[b] > 0;
     const uint8_t* cur = d_src;
     uint64_t cur_stride = stride;
     for (int i = 0; i < plan.nt; i++) {
@@ -1926,6 +1996,11 @@ int kz_set_block_range(kz_ctx* ctx, int64_t from_block, int64_t to_block) {
     return 0;
 }
 
+int kz_set_skip_blocks(kz_ctx* ctx, int on) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    ctx->skip_blocks = on != 0;
+    return 0;
+}
 int kz_set_headerless_writer(kz_ctx* ctx, int on) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     ctx->headerless_writer = on != 0;
@@ -1995,8 +2070,8 @@ size_t kz_transform_max_encoded_len(uint64_t type, size_t n) {
 // ---- whole stream, device resident ---------------------------------------------------------------------------
 static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size, const void* d_src,
                                 size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits);
-static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src,
-                                size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res);
+static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, bool skip,
+                                const void* d_src, size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res);
 int kz_compress_stream_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size,
                               const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, out_n, false, nullptr);
@@ -2025,7 +2100,7 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     if (fragment || ctx->headerless_writer) hdr_bits = 0;  // an empty leading segment (Writer.writeHeader :430)
     EncResult res;
     ctx->fragment = fragment;
-    rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, d_src, n, hdr, hdr_bits, d_dst, cap, res);
+    rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, ctx->skip_blocks, d_src, n, hdr, hdr_bits, d_dst, cap, res);
     ctx->fragment = false;
     if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
@@ -2035,27 +2110,44 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
 }
 
 // What compress_device_impl runs on the n bytes at d_src, cut into blocks of block_size: the initial dataType of every block from its magic
-// number, the forward transforms, the block checksums and the LAYOUT_STREAM encode behind the leading segment `lead` (lead_bits bits: the
-// stream header, or a writer session's carry). A writer session runs every batch of its stream through it.
-static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src,
-                                size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res) {
+// number, with skip (skipBlocks) the blocks stored raw, the forward transforms, the block checksums and the LAYOUT_STREAM encode behind the
+// leading segment `lead` (lead_bits bits: the stream header, or a writer session's carry). A writer session runs every batch of its stream
+// through it.
+static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, bool skip,
+                                const void* d_src, size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res) {
     const uint32_t nblocks = (uint32_t)((n + block_size - 1) / block_size);
     std::vector<EncJob> jobs;
     int rc = 0;
     const uint8_t* d_data = nullptr;
     std::vector<int32_t> init_dt;
-    if (plan.uses_magic() && nblocks) {  // the first four bytes of every block decide its initial data type
-        std::vector<uint8_t> heads((size_t)nblocks * 4, 0);
+    std::vector<uint8_t> store;
+    if ((plan.uses_magic() || skip) && nblocks) {  // the first four bytes of every block decide its initial data type (and whether it is stored)
         const size_t last = n - (size_t)(nblocks - 1) * block_size;
-        if (nblocks > 1) CK(cudaMemcpy2DAsync(heads.data(), 4, d_src, block_size, 4, nblocks - 1, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(&heads[(size_t)(nblocks - 1) * 4], (const uint8_t*)d_src + (size_t)(nblocks - 1) * block_size, std::min<size_t>(4, last),
-                           cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<uint8_t> heads((size_t)nblocks * (skip ? 5 : 4), 0);  // with skip, the entropy flags follow the heads in the same copy
+        std::vector<uint32_t> blen(nblocks);
+        for (uint32_t b = 0; b < nblocks; b++) blen[b] = b + 1 < nblocks ? block_size : (uint32_t)last;
+        uint8_t* d_heads = nullptr;
+        if (skip) {
+            std::vector<uint64_t> boff(nblocks);
+            for (uint32_t b = 0; b < nblocks; b++) boff[b] = (uint64_t)b * block_size;
+            rc = skip_test(ctx, (const uint8_t*)d_src, boff, blen, &d_heads);
+            if (rc) return rc;
+        }
+        const cudaMemcpyKind kind = d_heads ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+        uint8_t* dst = d_heads ? d_heads : heads.data();
+        if (nblocks > 1) CK(cudaMemcpy2DAsync(dst, 4, d_src, block_size, 4, nblocks - 1, kind, ctx->stream));
+        CK(cudaMemcpyAsync(dst + (size_t)(nblocks - 1) * 4, (const uint8_t*)d_src + (size_t)(nblocks - 1) * block_size, std::min<size_t>(4, last), kind,
+                           ctx->stream));
+        if (d_heads) CK(cudaMemcpyAsync(heads.data(), d_heads, heads.size(), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        init_dt.resize(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++)
-            init_dt[b] = magic_data_type(&heads[(size_t)b * 4], b + 1 < nblocks ? block_size : last);
+        if (plan.uses_magic()) {
+            init_dt.resize(nblocks);
+            for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(&heads[(size_t)b * 4], blen[b]);
+        }
+        if (skip) store = stored_blocks(ctx, heads, blen.data(), nblocks);
     }
-    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, n, block_size, block_size, nullptr, nblocks, &d_data, jobs, init_dt.empty() ? nullptr : &init_dt);
+    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, n, block_size, block_size, nullptr, nblocks, &d_data, jobs, init_dt.empty() ? nullptr : &init_dt,
+                       store.empty() ? nullptr : &store);
     if (rc) return rc;
     if (checksum_bits && nblocks) {  // encodingTask.encode :753-763: hash of the original block
         std::vector<uint64_t> hoff(nblocks), hv;
@@ -2325,19 +2417,31 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
     }
     const uint32_t nb = (uint32_t)blen.size();
     first[nstreams] = nb;
-    // ctx["dataType"] of every block from its first four bytes (encodingTask.encode :806-816), gathered in one copy
+    // ctx["dataType"] of every block from its first four bytes (encodingTask.encode :806-816), gathered in one copy; with skipBlocks the
+    // blocks stored raw, from the same heads and the entropy flags that follow them
     std::vector<int32_t> dts(nb, 0);
-    if (plan.uses_magic() && nb) {
-        CK(ctx->d_asm.ensure((size_t)nb * 4));
-        CK(cudaMemsetAsync(ctx->d_asm.p, 0, (size_t)nb * 4, ctx->stream));
+    std::vector<uint8_t> store;
+    const bool skip = ctx->skip_blocks;
+    if ((plan.uses_magic() || skip) && nb) {
+        uint8_t* d_heads = nullptr;
+        if (skip) {
+            rc = skip_test(ctx, d_src, boff, blen, &d_heads);
+            if (rc) return rc;
+        } else {
+            CK(ctx->d_asm.ensure((size_t)nb * 4));
+            CK(cudaMemsetAsync(ctx->d_asm.p, 0, (size_t)nb * 4, ctx->stream));
+            d_heads = ctx->d_asm.as<uint8_t>();
+        }
         CopyList heads;
-        for (uint32_t b = 0; b < nb; b++) heads.add(d_src + boff[b], ctx->d_asm.as<uint8_t>() + 4 * (size_t)b, std::min<uint32_t>(4, blen[b]));
+        for (uint32_t b = 0; b < nb; b++) heads.add(d_src + boff[b], d_heads + 4 * (size_t)b, std::min<uint32_t>(4, blen[b]));
         rc = run_copies(ctx, heads);
         if (rc) return rc;
-        std::vector<uint8_t> h((size_t)nb * 4);
-        CK(cudaMemcpyAsync(h.data(), ctx->d_asm.p, h.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<uint8_t> h((size_t)nb * (skip ? 5 : 4));
+        CK(cudaMemcpyAsync(h.data(), d_heads, h.size(), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t b = 0; b < nb; b++) dts[b] = magic_data_type(&h[(size_t)b * 4], blen[b]);
+        if (plan.uses_magic())
+            for (uint32_t b = 0; b < nb; b++) dts[b] = magic_data_type(&h[(size_t)b * 4], blen[b]);
+        if (skip) store = stored_blocks(ctx, h, blen.data(), nb);
     }
     std::vector<uint64_t> hv;
     if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
@@ -2356,12 +2460,14 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
         uint8_t* slots = ctx->d_slots.as<uint8_t>();
         std::vector<uint32_t> lens(k);
         std::vector<int32_t> pdt(k);
+        std::vector<uint8_t> pstore(store.empty() ? 0 : k);
         CopyList place;
         uint32_t max_len = 0;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t b = P.order[i0 + j];
             lens[j] = blen[b];
             pdt[j] = dts[b];
+            if (!store.empty()) pstore[j] = store[b];
             max_len = std::max(max_len, blen[b]);
             place.add(d_src + boff[b], slots + j * s, blen[b]);
         }
@@ -2369,7 +2475,7 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
         if (rc) return rc;
         const uint8_t* d_data = nullptr;
         std::vector<EncJob> jobs;
-        rc = forward_stage(ctx, plan, slots, 0, block_size, s, lens.data(), k, &d_data, jobs, &pdt);
+        rc = forward_stage(ctx, plan, slots, 0, block_size, s, lens.data(), k, &d_data, jobs, &pdt, pstore.empty() ? nullptr : &pstore);
         if (rc) return rc;
         if (checksum_bits)
             for (uint32_t j = 0; j < k; j++) jobs[j].checksum = hv[P.order[i0 + j]];
@@ -2716,7 +2822,20 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     const uint8_t* d_data = nullptr;
     std::vector<int32_t> init_dt(nblocks, 0);
     for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(slab + b * block_stride, block_len[b]);
-    rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), 0, 0, dstride, block_len, nblocks, &d_data, jobs, &init_dt);
+    std::vector<uint8_t> store;
+    if (ctx->skip_blocks) {  // skipBlocks: the heads are in host memory, only the entropy flags come back
+        std::vector<uint64_t> boff(nblocks);
+        for (uint32_t b = 0; b < nblocks; b++) boff[b] = b * dstride;
+        uint8_t* d_heads = nullptr;
+        rc = skip_test(ctx, ctx->d_in.as<uint8_t>(), boff, std::vector<uint32_t>(block_len, block_len + nblocks), &d_heads);
+        if (rc) return rc;
+        std::vector<uint8_t> hf((size_t)nblocks * 5, 0);
+        for (uint32_t b = 0; b < nblocks; b++) memcpy(&hf[(size_t)b * 4], slab + b * block_stride, std::min<uint32_t>(4, block_len[b]));
+        CK(cudaMemcpyAsync(&hf[(size_t)nblocks * 4], d_heads + (size_t)nblocks * 4, nblocks, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        store = stored_blocks(ctx, hf, block_len, nblocks);
+    }
+    rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), 0, 0, dstride, block_len, nblocks, &d_data, jobs, &init_dt, store.empty() ? nullptr : &store);
     if (rc) return rc;
     if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
         std::vector<uint64_t> hoff(nblocks), hv;
@@ -3236,6 +3355,7 @@ struct kz_writer : kz::Session {
     uint32_t etype = 0, block_size = 0, checksum_bits = 0;
     int64_t input_size = 0;
     bool headerless = false;  // the context's headerless writer setting when the session opened (kz_set_headerless_writer)
+    bool skip = false;        // and its skipBlocks setting (kz_set_skip_blocks)
     DevBuf d_out;            // the finished bytes of one batch
     size_t out_cap = 0;
     uint64_t batches = 0;    // batches encoded (worker)
@@ -3258,7 +3378,7 @@ struct kz_writer : kz::Session {
         ctx->stream_bs = block_size;
         ctx->fragment = !last;
         ctx->volatile_lead = true;
-        int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, d_in[k].p, in_len[k], lead, lead_bits, d_out.p, out_cap, res);
+        int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, skip, d_in[k].p, in_len[k], lead, lead_bits, d_out.p, out_cap, res);
         ctx->fragment = false;
         ctx->volatile_lead = false;
         if (rc) return rc;
@@ -3482,6 +3602,7 @@ int kz_writer_open(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_siz
     w->checksum_bits = checksum_bits;
     w->input_size = input_size_hint;
     w->headerless = ctx->headerless_writer;
+    w->skip = ctx->skip_blocks;
     const size_t in_bytes = (size_t)batch_blocks * block_size;
     w->out_cap = kz_max_stream_output(in_bytes, block_size) + 64;
     rc = w->alloc_inputs(in_bytes);

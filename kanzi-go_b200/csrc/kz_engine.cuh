@@ -138,6 +138,7 @@ struct kz_ctx {
     uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
     int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)
     bool headerless_writer = false;          // kz_set_headerless_writer: the stream-level encodes write no stream header
+    bool skip_blocks = false;                // kz_set_skip_blocks: the encodes store incompressible blocks raw (ctx["skipBlocks"])
     struct Headerless {                      // kz_set_headerless_reader: the stream-level decodes take these instead of a header
         bool on = false;
         uint64_t t48 = 0;
@@ -156,6 +157,7 @@ struct kz_ctx {
     kz::DevBuf d_in, d_out, d_tmp, d_tmp2, d_seg, d_chunks, d_tables, d_enc_tab, d_hdr, d_pay, d_small, d_dl, d_rcp, d_ws, d_lens, d_hist;
     // many-stream entry points: copy lists, pass slots, pass entropy output, compact block bit strings, stream assembly / staging
     kz::DevBuf d_copy, d_slots, d_enc, d_bits, d_asm;
+    kz::DevBuf d_skip;  // skipBlocks test: block histograms, heads and entropy flags
     kz::PinnedBuf h_stage, h_dl, h_io;  // h_io: packed inputs / outputs of the host-buffer many-stream entry points
     // the open writer / reader session (the end of kz_api.cu), if any; kz_destroy closes it. kz_device_bytes asks it, because its
     // worker thread grows the scratch
@@ -164,7 +166,7 @@ struct kz_ctx {
     template <class F>
     void each_dev_buf(F&& f) {
         kz::DevBuf* bufs[] = {&d_in, &d_out, &d_tmp, &d_tmp2, &d_seg, &d_chunks, &d_tables, &d_enc_tab, &d_hdr, &d_pay, &d_small, &d_dl, &d_rcp, &d_ws, &d_lens,
-                              &d_hist, &d_copy, &d_slots, &d_enc, &d_bits, &d_asm};
+                              &d_hist, &d_copy, &d_slots, &d_enc, &d_bits, &d_asm, &d_skip};
         for (auto b : bufs) f(*b);
     }
     size_t scratch_bytes() {

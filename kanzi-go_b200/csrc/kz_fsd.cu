@@ -14,6 +14,7 @@
 #include "kz_alias.cuh"
 #include <vector>
 
+#include "kz_entropy_core.cuh"
 #include "kz_fsd.cuh"
 
 namespace kz {
@@ -58,39 +59,6 @@ Ws carve(uint8_t* ws, uint32_t nblocks, uint32_t max_len) {
     p += align256((size_t)nblocks * w.ntiles * 4);
     w.tile_off = reinterpret_cast<uint32_t*>(p);
     return w;
-}
-
-// internal/Global.go:60-93 LOG2_4096[i] = round(4096 * log2(i)) (entries 0 and 1 are 0): a data table of the reference, regenerated from
-// its definition (checked entry by entry against the reference's table when this was written)
-const uint32_t* host_log2_4096() {
-    static uint32_t tab[257];
-    static bool init = false;
-    if (!init) {
-        tab[0] = 0;
-        for (int k = 1; k <= 256; k++) tab[k] = (uint32_t)(4096.0 * std::log2((double)k) + 0.5);
-        init = true;
-    }
-    return tab;
-}
-
-// internal/Global.go:175-191 Log2ScaledBy1024
-KZ_D uint32_t log2_scaled_1024(uint32_t x, const uint32_t* T) {
-    if (x < 256) return (T[x] + 2) >> 2;
-    const uint32_t lg = 31u - (uint32_t)__clz((int)x);
-    if ((x & (x - 1)) == 0) return lg << 10;
-    return ((lg - 7) * 1024) + ((T[x >> (lg - 7)] + 2) >> 2);
-}
-// internal/Global.go:196-214 ComputeFirstOrderEntropy1024
-KZ_D int entropy_1024(uint32_t block_len, const uint32_t* histo, const uint32_t* T) {
-    if (block_len == 0) return 0;
-    unsigned long long sum = 0;
-    const uint32_t ll = log2_scaled_1024(block_len, T);
-    for (int i = 0; i < 256; i++) {
-        if (histo[i] == 0) continue;
-        const uint32_t l = log2_scaled_1024(histo[i], T);
-        sum += ((unsigned long long)histo[i] * (unsigned long long)(ll - l)) >> 3;
-    }
-    return (int)(sum / (unsigned long long)block_len);
 }
 
 // internal/Magic.go:73-112 GetMagicType reduced to what FSDCodec.Forward :170-187 asks: no magic, or BMP / RIFF / PBM / PGM / PPM
