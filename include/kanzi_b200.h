@@ -196,7 +196,8 @@ void kz_set_stream_block_size(kz_ctx* ctx, uint64_t block_size);
  * Read by kz_decompress_stream, kz_decompress_stream_device, kz_decompress_streams and kz_decompress_streams_device (the same range for every
  * stream, as BlockDecompressor applies one from / to to every file) and kz_reader_open, which captures the range when the session opens
  * (later calls do not change an open session, and the call is allowed while one is open). kz_decode_blocks, kz_decompress_fragment_device, kz_entropy_* and kz_transform_* ignore it:
- * their block numbers are not stream ids.
+ * their block numbers are not stream ids. So do kz_index_build[_device] and kz_read_ranges[_device]: an index covers every record, and a
+ * read selects blocks by byte offset.
  * Semantics: every record of the stream is still walked to the end marker, so a bad record length, a record past the end or a truncated
  * stream is reported wherever it lies. A skipped block is never parsed, entropy decoded, inverse transformed or checksummed: a defect inside
  * it is not an error. The output is the decoded blocks of the range back to back (out_n / out_len = their length, 0 for an empty range). The
@@ -300,6 +301,67 @@ int kz_reader_read(kz_reader* r, const uint8_t* src, size_t n, size_t* consumed,
 int kz_reader_finish(kz_reader* r, uint8_t* dst, size_t cap, size_t* produced);
 void kz_reader_free(kz_reader* r);
 size_t kz_device_bytes(kz_ctx* ctx);
+
+/* ---- stream index and batched range reads: bytes [off, off + len) of the original data without decoding the stream (an object store
+ *      serving ranges of a compressed object, record-level compression, one file out of a directory stream) -----------------------------
+ * Blocks are independent and every block but the last decodes to exactly block_size bytes, so decoded byte off lives in block
+ * off / block_size. An index records where every block record lies in the stream; it is built once, kept (kz_index_save) beside the
+ * stream, and then serves any number of reads, each of which decodes only the blocks its requests touch, every block once per call.
+ * The index: a host object. It holds the stream's header fields (or the headerless reader setting in force when it is built, as
+ *   kz_reader_open captures it), the stream's byte length and first 32 bytes, and for every record the first bit and the bit length of
+ *   its payload. It does not own the stream and holds no device memory. kz_index_build[_device] parses the header and walks the record
+ *   prefixes (twice: once to count, once to store; no limit on the record count other than the stream's length) and decodes nothing.
+ *   Errors are the codes kz_decompress_stream gives for the same bytes (bad header, version or block size, a record length past the
+ *   end, truncation); a kanzi chain or codec the GPU path lacks is -KZ_ERR_CREATE_CODEC. The stream of an empty input gives an index
+ *   of 0 blocks. kz_index_build_device follows the rule of kz_decompress_stream_device (16-byte aligned, >= 64 readable bytes behind n).
+ *   The block range (kz_set_block_range) is ignored by the index and by the reads: their block numbers come from byte offsets.
+ * Size: the decoded length of the last block is not in its record, and the header's input size is a hint the decoders never trust. So
+ *   *size is -1 until a read has decoded the last block, and exact afterwards; 0 from the start for a stream of 0 blocks.
+ * Blob layout (kz_index_save / kz_index_load), little endian: u32 magic "KZIX" (0x58495A4B) | u32 format version 1 | u64 transform48 |
+ *   u32 entropy | u32 block_size | u32 checksum_bits | u32 header bit length (0 = headerless) | i64 input_size | u64 stream_bytes |
+ *   u64 nblocks | i64 size (-1 = not known) | the stream's first 32 bytes (zero padded) | nblocks x u64 payload start bit | nblocks x
+ *   u64 payload bit length | u64 XXH64 (seed 0) of every byte before it. 104 + 16 x nblocks bytes. kz_index_save returns the bytes
+ *   needed and writes when cap suffices. kz_index_load needs no context and no GPU; a blob is input from outside the program, so every
+ *   field is checked: -KZ_ERR_INVALID_FILE for a short blob, a wrong magic, version, length or hash, fields no stream header or
+ *   headerless setting can hold, records out of order, without room for their prefixes or outside stream_bytes, a size that does not
+ *   fit nblocks.
+ * Reads: request i asks for decoded bytes [off[i], off[i] + len[i]) and gets them at dst + dst_off[i]; out_len[i] = the bytes delivered.
+ *   Nothing is written outside [dst_off[i], dst_off[i] + len[i]). pread semantics: a request that runs past the end of the data is
+ *   short, 0 bytes at or beyond the end, and that is no error. Requests may overlap, repeat, come in any order and have length 0. A
+ *   request that touches the last block decodes it, which sets the index's size. src / n is the stream the index was built from: a
+ *   read whose n or first 32 bytes differ from the index's fails as a whole with -KZ_ERR_INVALID_PARAM before anything is decoded.
+ * Errors: status[i] = 0 or -(kanzi error code). A block that fails (block header, entropy decode, inverse transform, checksum; in that
+ *   order) fails exactly the requests that touch it, with the code kz_decompress_stream gives for that block under
+ *   kz_set_block_range(k, k + 1); a request on several failing blocks gets the code of the first. out_len[i] = 0 and nothing is written
+ *   for a failed request; requests on other blocks succeed. With checksums in the stream every decoded block is verified. A decoded
+ *   block that is not the last and not exactly block_size long (no kanzi writer produces one) makes offsets behind it meaningless: the
+ *   requests that touch it or any later block fail with -KZ_ERR_INVALID_FILE. Call-level failures (a bad argument, a stale index, an
+ *   open session on ctx, a CUDA or allocation error) set every status and are the return value; otherwise the return value is 0 when
+ *   every request succeeded, else the first failing request's code.
+ * Memory: the touched blocks are decoded in passes of at most STREAM_PASS_BUDGET (1 GiB, kanzi-go_b200/csrc/kz_stream_plan.h) of
+ *   scratch, three slots per block; scratch follows a pass, never the number of requests or the stream's length. On top of it the host
+ *   variant holds the requested bytes once on the device (and in pinned memory) and the record windows of one pass; the device variant
+ *   stages only requests whose blocks span passes. The host variant uploads only the byte windows that hold the touched records
+ *   (16-byte aligned starts, 64 bytes of slack, neighbours merged) and brings the requested bytes back in one transfer.
+ * Cost: one decode of each touched block plus one copy launch per pass; no record walk. With kz_profile(ctx,1):
+ *   kz_stage_bytes("read:blocks") = blocks decoded / decoded bytes, ("read:h2d") = windows / bytes uploaded by the host variant,
+ *   ("read:out") = slices / bytes delivered.
+ * Threads: the one-thread-per-context rule; while a session is open on ctx the calls that take ctx fail with -KZ_ERR_INVALID_PARAM.
+ *   An index is used by one thread at a time (a read updates its size). */
+typedef struct kz_index kz_index;
+int kz_index_build(kz_ctx* ctx, const uint8_t* src, size_t n, kz_index** out);
+int kz_index_build_device(kz_ctx* ctx, const void* d_src, size_t n, kz_index** out);
+/* Any out pointer may be NULL. *size: decoded bytes, -1 = not known yet. */
+int kz_index_info(const kz_index* ix, uint64_t* transform48, uint32_t* entropy, uint32_t* block_size, uint32_t* checksum_bits, int64_t* input_size,
+                  uint64_t* nblocks, uint64_t* stream_bytes, int64_t* size);
+size_t kz_index_save(const kz_index* ix, uint8_t* dst, size_t cap);
+int kz_index_load(const uint8_t* blob, size_t n, kz_index** out);
+void kz_index_free(kz_index* ix);
+int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, uint8_t* dst,
+                   const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+/* d_src as for kz_index_build_device; d_dst and dst_off need no alignment; the offset, length and result arrays are host arrays. */
+int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
+                          const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,138 @@
+// Stream index and batched range reads: bytes [off, off+len) of the original data without decoding the stream
+// (kz_index_*, kz_read_ranges in kanzi_b200.h). The reference has no counterpart: its Reader decodes from the first block, and
+// --from / --to (:1858-1871) selects whole blocks after walking every record. Lives at v2/gpu/index.go.
+package gpu
+
+/*
+#include "kanzi_b200.h"
+*/
+import "C"
+
+import (
+	"errors"
+	"io"
+	"unsafe"
+)
+
+// Index says where every block record of one stream lies. It does not own the stream; Save's bytes are kept beside it.
+type Index struct {
+	h *C.kz_index
+}
+
+// BuildIndex parses the header of stream (or takes the headerless reader setting of c) and walks its records. Nothing is decoded.
+func (c *Context) BuildIndex(stream []byte) (*Index, error) {
+	if len(stream) == 0 {
+		return nil, errors.New("gpu: empty stream")
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var h *C.kz_index
+	if rc := C.kz_index_build(c.h, (*C.uint8_t)(unsafe.Pointer(&stream[0])), C.size_t(len(stream)), &h); rc != 0 {
+		return nil, c.err(rc)
+	}
+	return &Index{h: h}, nil
+}
+
+// LoadIndex reads an index from Save's bytes. It needs no GPU; a damaged blob is ERR_INVALID_FILE.
+func LoadIndex(blob []byte) (*Index, error) {
+	if len(blob) == 0 {
+		return nil, errors.New("gpu: empty index blob")
+	}
+	var h *C.kz_index
+	if rc := C.kz_index_load((*C.uint8_t)(unsafe.Pointer(&blob[0])), C.size_t(len(blob)), &h); rc != 0 {
+		return nil, errors.New("gpu: not a stream index blob")
+	}
+	return &Index{h: h}, nil
+}
+
+// Save returns the self-describing blob of the index (layout in kanzi_b200.h).
+func (x *Index) Save() []byte {
+	n := C.kz_index_save(x.h, nil, 0)
+	out := make([]byte, int(n))
+	C.kz_index_save(x.h, (*C.uint8_t)(unsafe.Pointer(&out[0])), n)
+	return out
+}
+
+// Size is the decoded length of the stream, or -1 until a read has decoded the last block.
+func (x *Index) Size() int64 {
+	var size C.int64_t
+	C.kz_index_info(x.h, nil, nil, nil, nil, nil, nil, nil, &size)
+	return int64(size)
+}
+
+// Free releases the index.
+func (x *Index) Free() {
+	C.kz_index_free(x.h)
+	x.h = nil
+}
+
+// Range is one request of ReadRanges: Len decoded bytes from Off, delivered into Dst[:N]. Err is the request's own failure
+// (a StreamError with the block's code); a request that runs past the end of the data is short, not failed.
+type Range struct {
+	Off uint64
+	Dst []byte
+	N   int
+	Err error
+}
+
+// ReadRanges serves every request in one call: each block the requests touch is decoded once. The returned error is a failure of
+// the call as a whole (a stale index, a session open on c, a chain the GPU path lacks); failures of single blocks, and a CUDA error,
+// which sets every request's status, are in the requests' Err.
+func (c *Context) ReadRanges(x *Index, stream []byte, reqs []Range) error {
+	n := len(reqs)
+	if n == 0 {
+		return nil
+	}
+	off := make([]C.uint64_t, n)
+	ln := make([]C.uint64_t, n)
+	dstOff := make([]C.uint64_t, n)
+	outLen := make([]C.uint64_t, n)
+	status := make([]C.int32_t, n)
+	total := uint64(0)
+	for i, r := range reqs {
+		off[i], ln[i], dstOff[i] = C.uint64_t(r.Off), C.uint64_t(len(r.Dst)), C.uint64_t(total)
+		total += uint64(len(r.Dst))
+	}
+	buf := make([]byte, total+1) // cgo must not see pointers into several Go slices: one buffer, then copies
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_read_ranges(c.h, x.h, (*C.uint8_t)(unsafe.Pointer(&stream[0])), C.size_t(len(stream)), C.uint32_t(n), &off[0], &ln[0],
+		(*C.uint8_t)(unsafe.Pointer(&buf[0])), &dstOff[0], &outLen[0], &status[0])
+	if rc == -C.KZ_ERR_INVALID_PARAM || rc == -C.KZ_ERR_CREATE_CODEC { // no block fails with these: the call failed as a whole
+		return c.err(rc)
+	}
+	for i := range reqs {
+		reqs[i].N, reqs[i].Err = int(outLen[i]), nil
+		if status[i] != 0 {
+			reqs[i].Err = &StreamError{Code: int(-status[i])}
+			continue
+		}
+		copy(reqs[i].Dst, buf[uint64(dstOff[i]):uint64(dstOff[i])+uint64(outLen[i])])
+	}
+	return nil
+}
+
+// ReaderAt is an io.ReaderAt over the original data of (stream, index): every ReadAt is one kz_read_ranges call of one request.
+// Callers with many reads in hand use ReadRanges, which decodes each touched block once for all of them.
+type ReaderAt struct {
+	C      *Context
+	Index  *Index
+	Stream []byte
+}
+
+func (r *ReaderAt) ReadAt(p []byte, off int64) (int, error) {
+	if off < 0 {
+		return 0, errors.New("gpu: negative offset")
+	}
+	req := []Range{{Off: uint64(off), Dst: p}}
+	if err := r.C.ReadRanges(r.Index, r.Stream, req); err != nil {
+		return 0, err
+	}
+	if req[0].Err != nil {
+		return 0, req[0].Err
+	}
+	if req[0].N < len(p) {
+		return req[0].N, io.EOF
+	}
+	return req[0].N, nil
+}

@@ -41,6 +41,8 @@ ABI_SYMBOLS = [
     "kz_writer_open", "kz_writer_write", "kz_writer_finish", "kz_writer_free", "kz_reader_open", "kz_reader_read", "kz_reader_finish",
     "kz_reader_free", "kz_device_bytes", "kz_set_block_range", "kz_bwt_profile",
     "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader", "kz_set_skip_blocks",
+    "kz_index_build", "kz_index_build_device", "kz_index_info", "kz_index_save", "kz_index_load", "kz_index_free", "kz_read_ranges",
+    "kz_read_ranges_device",
 ]
 
 
@@ -161,6 +163,17 @@ def load_library(build_if_missing=True):
     L.kz_reader_free.restype = None
     L.kz_device_bytes.argtypes = [vp]
     L.kz_device_bytes.restype = sz
+    L.kz_index_build.argtypes = [vp, vp, sz, C.POINTER(vp)]
+    L.kz_index_build_device.argtypes = [vp, vp, sz, C.POINTER(vp)]
+    L.kz_index_info.argtypes = [vp, C.POINTER(u64), C.POINTER(u32), C.POINTER(u32), C.POINTER(u32), C.POINTER(C.c_int64), C.POINTER(u64), C.POINTER(u64),
+                                C.POINTER(C.c_int64)]
+    L.kz_index_save.argtypes = [vp, vp, sz]
+    L.kz_index_save.restype = sz
+    L.kz_index_load.argtypes = [vp, sz, C.POINTER(vp)]
+    L.kz_index_free.argtypes = [vp]
+    L.kz_index_free.restype = None
+    L.kz_read_ranges.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
+    L.kz_read_ranges_device.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -526,6 +539,22 @@ class Context:
     def cuda_stream(self):
         return self.lib.kz_cuda_stream(self.h)
 
+    # ---- stream index (kz_index_*): built once, then serves batched range reads (StreamIndex.read / read_many) ---------------------
+    def index(self, stream, headerless=None):
+        """The StreamIndex of a host stream: header fields and record positions; decodes nothing. headerless: as in decompress."""
+        s = _u8(stream)
+        h = C.c_void_p()
+        with self._headerless(reader=headerless):
+            self._check(self.lib.kz_index_build(self.h, _p(s), s.size, C.byref(h)))
+        return StreamIndex(h, self)
+
+    def index_device(self, d_src, n, headerless=None):
+        """The StreamIndex of the stream of n bytes at d_src (16-byte aligned, >= 64 readable bytes behind it)."""
+        h = C.c_void_p()
+        with self._headerless(reader=headerless):
+            self._check(self.lib.kz_index_build_device(self.h, _dptr(d_src), n, C.byref(h)))
+        return StreamIndex(h, self)
+
     # ---- streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded memory -------------------------------
     def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0, headerless=None, skip_blocks=None):
         """A StreamSession: write(data) -> bytes and finish() -> bytes give the stream compress() writes for the concatenated input.
@@ -585,6 +614,84 @@ class Context:
 
     def launch_count(self, reset=False):
         return self.lib.kz_launch_count(self.h, 1 if reset else 0)
+
+
+class StreamIndex:
+    """Where every block record of one stream lies (kz_index): a host object, built by Context.index / index_device or loaded from a saved
+    blob. read / read_many / read_many_device return decoded bytes [off, off + length) and decode only the blocks they touch; they take
+    the stream again (the index does not own it) and the context to decode on (ctx=None: the one that built the index)."""
+
+    def __init__(self, h, ctx=None):
+        self.h, self.ctx = h, ctx
+        self.lib = load_library()
+
+    @classmethod
+    def load(cls, blob, ctx=None):
+        """An index from save()'s bytes; needs no GPU. A damaged blob raises KanziError(15)."""
+        b = _u8(blob)
+        h = C.c_void_p()
+        rc = load_library().kz_index_load(_p(b), b.size, C.byref(h))
+        if rc:
+            raise KanziError(-rc, "not a stream index blob")
+        return cls(h, ctx)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.kz_index_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def info(self):
+        t48, ns, nb, isz, size = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_int64(0), C.c_int64(0)
+        et, bs, ck = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        self.lib.kz_index_info(self.h, C.byref(t48), C.byref(et), C.byref(bs), C.byref(ck), C.byref(isz), C.byref(nb), C.byref(ns), C.byref(size))
+        return {"transform48": t48.value, "entropy": et.value, "block_size": bs.value, "checksum_bits": ck.value, "input_size": isz.value,
+                "nblocks": nb.value, "stream_bytes": ns.value, "size": size.value}
+
+    @property
+    def size(self):
+        """Decoded bytes of the stream; -1 until a read has decoded the last block."""
+        return self.info["size"]
+
+    def save(self):
+        n = self.lib.kz_index_save(self.h, None, 0)
+        out = np.zeros(n, np.uint8)
+        self.lib.kz_index_save(self.h, out.ctypes.data, n)
+        return out.tobytes()
+
+    def read_many(self, stream, requests, ctx=None):
+        """requests: [(off, length), ...] -> (list of bytes, status list). Failures do not raise: status[i] = 0 or -(kanzi error code); a
+        short request gives fewer bytes, a failed one b"". A call-level failure (stale index, open session) sets every status."""
+        ctx = ctx or self.ctx
+        s = _u8(stream)
+        off = np.array([r[0] for r in requests], np.uint64)
+        ln = np.array([r[1] for r in requests], np.uint64)
+        dst_off = _offsets(ln)
+        dst = np.empty(max(int(ln.sum()), 1), np.uint8)
+        out_len, status = np.zeros(len(requests), np.uint64), np.zeros(len(requests), np.int32)
+        self.lib.kz_read_ranges(ctx.h, self.h, _p(s), s.size, len(requests), _p(off), _p(ln), dst.ctypes.data, _p(dst_off), _p(out_len), _p(status))
+        return [dst[int(o): int(o) + int(n)].tobytes() for o, n in zip(dst_off, out_len)], status.tolist()
+
+    def read(self, stream, off, length, ctx=None):
+        """Decoded bytes [off, off + length), short at the end of the data; raises when the block fails."""
+        out, st = self.read_many(stream, [(off, length)], ctx)
+        if st[0]:
+            (ctx or self.ctx)._check(st[0])
+        return out[0]
+
+    def read_many_device(self, d_src, n, off, length, d_dst, dst_off, ctx=None):
+        """Device-resident read_many: d_src / d_dst are CUDA tensors or addresses, the rest host sequences -> (out_len, status)."""
+        ctx = ctx or self.ctx
+        o, ln, do = (np.ascontiguousarray(a, np.uint64) for a in (off, length, dst_off))
+        out_len, status = np.zeros(len(o), np.uint64), np.zeros(len(o), np.int32)
+        self.lib.kz_read_ranges_device(ctx.h, self.h, _dptr(d_src), n, len(o), _p(o), _p(ln), _dptr(d_dst), _p(do), _p(out_len), _p(status))
+        return out_len, status
 
 
 def default_batch_blocks(block_size):

@@ -27,6 +27,7 @@
 #include "kz_entropy_core.cuh"
 #include "kz_skip.cuh"
 #include "kz_stream_plan.h"
+#include "kz_read_plan.h"
 
 #include <condition_variable>
 #include <map>
@@ -2239,22 +2240,26 @@ int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uin
 // Parses the header of the stream at d_src and walks its block records: rec_bit[b] = first bit of record b (its 5-bit prefix), rec_bit[nblocks] =
 // first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries. With a headerless reader setting the fields are
 // the setting's and rec_bit[0] = 0.
+// The header of the stream of n bytes at d_src, parsed from its first bytes (head, 64 bytes, receives them), or the headerless reader
+// setting when one is in force: what kz_stream_index_device and kz_index_build_device walk the records from.
+static int device_stream_header(kz_ctx* ctx, const void* d_src, size_t n, uint8_t* head, StreamHeader& sh) {
+    memset(head, 0, 64);
+    if (n) CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (ctx->headerless_reader.on) {
+        sh = headerless_header(ctx);
+        return 0;
+    }
+    return parse_stream_header(ctx, head, n, sh);
+}
 int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t max_blocks, uint64_t* t48, uint32_t* etype, uint32_t* block_size,
                            uint32_t* checksum_bits, int64_t* input_size, uint64_t* rec_bit, uint32_t* nblocks) {
     if (!ctx || !d_src || !rec_bit || !nblocks) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     StreamHeader sh;
-    int rc = 0;
-    if (ctx->headerless_reader.on) {
-        sh = headerless_header(ctx);
-    } else {
-        uint8_t head[64];
-        memset(head, 0, sizeof(head));
-        CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        rc = parse_stream_header(ctx, head, n, sh);
-        if (rc) return rc;
-    }
+    uint8_t head[64];
+    int rc = device_stream_header(ctx, d_src, n, head, sh);
+    if (rc) return rc;
     if (t48) *t48 = sh.t48;
     if (etype) *etype = sh.etype;
     if (block_size) *block_size = sh.block_size;
@@ -2794,6 +2799,337 @@ int kz_decompress_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, co
         return 0;
     }();
     return finish_streams(nstreams, status, out_len, rc);
+}
+
+// ---- stream index and batched range reads (kz_index_*, kz_read_ranges[_device]; plan and blob in kz_read_plan.h) -------------
+}  // extern "C"
+
+struct kz_index : kz::StreamIndex {};
+
+namespace {
+
+StreamHeader index_header(const kz_index& ix) {
+    StreamHeader sh;
+    sh.t48 = ix.t48;
+    sh.etype = ix.etype;
+    sh.block_size = ix.block_size;
+    sh.checksum_bits = ix.checksum_bits;
+    sh.input_size = ix.input_size;
+    sh.bits = ix.header_bits;
+    return sh;
+}
+
+// The stream bytes of one read pass as decode_walked sees them: the device stream itself, or the packed windows of the host variant.
+struct PassInput {
+    const uint32_t* d_words = nullptr;
+    uint64_t words_len = 0;
+    std::vector<uint64_t> bit_off;  // per block of the pass: its record's first payload bit in d_words
+};
+
+// Host variant: uploads only the byte windows that hold the records of blocks ks: each starts at a multiple of 16 and carries the 64
+// bytes the decoders may read behind a record (zeros where the stream ends); windows that meet are merged. One transfer per pass.
+int upload_windows(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const uint64_t* ks, uint32_t nk, PassInput& in) {
+    struct Window {
+        uint64_t lo, hi, at;  // stream bytes [lo, hi) at packed offset `at`
+    };
+    std::vector<Window> win;
+    std::vector<uint32_t> win_of(nk);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < nk; i++) {
+        const uint64_t lo = (ix.start[ks[i]] / 8) & ~15ull, hi = (ix.start[ks[i]] + ix.bits[ks[i]] + 7) / 8 + 64;
+        if (win.empty() || lo > win.back().hi) win.push_back(Window{lo, hi, 0});
+        else win.back().hi = std::max(win.back().hi, hi);
+        win_of[i] = (uint32_t)win.size() - 1;
+    }
+    for (Window& w : win) w.at = total, total += round16(w.hi - w.lo);
+    CK(ctx->h_io.ensure(total + 64));
+    CK(ctx->d_in.ensure(total + 128));
+    memset(ctx->h_io.p, 0, total);
+    for (const Window& w : win) memcpy((uint8_t*)ctx->h_io.p + w.at, src + w.lo, std::min<uint64_t>(w.hi, ix.stream_bytes) - w.lo);
+    CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+    in.d_words = ctx->d_in.as<uint32_t>();
+    in.words_len = (total + 3) / 4 + 16;
+    in.bit_off.resize(nk);
+    for (uint32_t i = 0; i < nk; i++) in.bit_off[i] = ix.start[ks[i]] - 8 * win[win_of[i]].lo + 8 * win[win_of[i]].at;
+    if (ctx->profile) {
+        auto& e = ctx->prof["read:h2d"];
+        e.bytes_in += win.size(), e.bytes_out += total, e.launches++;
+    }
+    return 0;
+}
+
+// One batched read. src is the host stream (host variant: dst is host memory too) or null (d_src is the stream, dst device memory).
+int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nreq, const uint64_t* off,
+                     const uint64_t* len, uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    const bool host = src != nullptr;
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    for (uint32_t i = 0; i < nreq; i++) {
+        if (dst_off[i] + len[i] < dst_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+        if (len[i] && !dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    }
+    if (!host && ((uintptr_t)d_src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    // the stream the index was built from: its length and its leading bytes
+    uint8_t head[INDEX_HEAD] = {0};
+    const size_t nh = std::min<size_t>(n, INDEX_HEAD);
+    if (n != ix->stream_bytes) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from a stream of another length");
+    if (host) memcpy(head, src, nh);
+    else if (nh) {
+        CK(cudaMemcpyAsync(head, d_src, nh, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    if (memcmp(head, ix->head, INDEX_HEAD)) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from another stream");
+    const StreamHeader sh = index_header(*ix);
+    TransformPlan plan;
+    int rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    if (!etype_supported(sh.etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+
+    const uint32_t bs = sh.block_size;
+    const uint64_t nblocks = ix->nblocks();
+    const ReadPlan P = plan_reads(nblocks, bs, ix->size, nreq, off, len);
+    const uint32_t nk = (uint32_t)P.blocks.size();
+    // A request is staged (its slices gathered in ctx->d_asm, delivered when every block it touches has decoded) when it goes to host
+    // memory or its blocks lie in more than one pass: nothing is written for a request that fails.
+    std::vector<uint32_t> pass_of(nk);
+    for (uint32_t p = 0; p < P.npasses(); p++)
+        for (uint32_t k = P.first[p]; k < P.first[p + 1]; k++) pass_of[k] = p;
+    std::vector<uint32_t> first_pass(nreq, 0);
+    std::vector<uint8_t> staged(nreq, host);
+    for (uint32_t k = 0; k < nk; k++)
+        for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++) {
+            const ReadSlice& sl = P.slices[s];
+            if (sl.at == 0) first_pass[sl.req] = pass_of[k];
+        }
+    for (const ReadSlice& sl : P.slices)
+        if (pass_of[sl.block] != first_pass[sl.req]) staged[sl.req] = 1;
+    std::vector<uint64_t> stage_at(nreq, 0);
+    uint64_t stage_total = 0;
+    for (uint32_t i = 0; i < nreq; i++)
+        if (staged[i]) stage_at[i] = stage_total, stage_total += P.want[i];
+    if (stage_total) CK(ctx->d_asm.ensure(stage_total + 64));
+    const uint64_t astride = decompress_slot(bs);
+
+    std::vector<int32_t> blk_status(nk, 0);
+    std::vector<uint32_t> blk_len(nk, 0);
+    std::vector<uint8_t> too_long(nk, 0);
+    for (uint32_t i = 0; i < nreq; i++) status[i] = 0, out_len[i] = 0;
+    uint32_t unseekable = nk;  // the first touched block whose length breaks the block arithmetic
+    uint64_t dec_blocks = 0, dec_bytes = 0, out_slices = 0, out_bytes = 0;
+    for (uint32_t p = 0; p < P.npasses() && unseekable == nk; p++) {
+        const uint32_t a = P.first[p], e = P.first[p + 1];
+        PassInput in;
+        if (host) {
+            rc = upload_windows(ctx, *ix, src, &P.blocks[a], e - a, in);
+            if (rc) return rc;
+        } else {
+            in.d_words = (const uint32_t*)d_src;
+            in.words_len = (n + 3) / 4 + 16;
+            for (uint32_t k = a; k < e; k++) in.bit_off.push_back(ix->start[P.blocks[k]]);
+        }
+        CK(ctx->d_slots.ensure(astride * (e - a) + 64));
+        uint8_t* arena = ctx->d_slots.as<uint8_t>();
+        // decodes blocks ks of the pass into their arena slots, one DecodeFailure per block
+        auto decode = [&](const std::vector<uint32_t>& ks) -> int {
+            std::vector<DecJob> jobs(ks.size(), DecJob());
+            std::vector<uint32_t> owner(ks.size());
+            std::vector<uint8_t> last(ks.size());
+            std::vector<DecodeFailure> fail(ks.size());
+            for (size_t i = 0; i < ks.size(); i++) {
+                jobs[i].bit_off = in.bit_off[ks[i] - a];
+                jobs[i].bits = ix->bits[P.blocks[ks[i]]];
+                owner[i] = (uint32_t)i;
+                last[i] = P.blocks[ks[i]] + 1 == nblocks;
+                too_long[ks[i]] = 0;
+            }
+            auto place = [&](uint32_t i, uint32_t n_out) {
+                blk_len[ks[i]] = n_out;
+                if (n_out > bs) {
+                    too_long[ks[i]] = 1;
+                    return NO_ROOM;
+                }
+                return (uint64_t)(ks[i] - a) * astride;
+            };
+            int r = decode_walked(ctx, sh, plan, in.d_words, in.words_len, jobs, owner, last, place, arena, fail.data());
+            if (r) return r;
+            for (size_t i = 0; i < ks.size(); i++) blk_status[ks[i]] = fail[i].failed() ? fail[i].code : 0;
+            return 0;
+        };
+        std::vector<uint32_t> ks(e - a);
+        std::iota(ks.begin(), ks.end(), a);
+        rc = decode(ks);
+        if (rc) return rc;
+        // A failing stage call cannot name its block, and a failure of one block may hide a later one's: every failed block of a pass
+        // of several is decoded again alone, so that its status is the one a decode of that block alone gives. Only corrupt input pays.
+        if (e - a > 1)
+            for (uint32_t k = a; k < e; k++)
+                if (blk_status[k] && !too_long[k]) {
+                    rc = decode(std::vector<uint32_t>{k});
+                    if (rc) return rc;
+                }
+        for (uint32_t k = a; k < e; k++) {
+            const bool is_last = P.blocks[k] + 1 == nblocks;
+            if (too_long[k] || (!blk_status[k] && (is_last ? blk_len[k] == 0 : blk_len[k] != bs))) unseekable = std::min(unseekable, k);
+            if (!blk_status[k]) dec_blocks++, dec_bytes += blk_len[k];
+            if (is_last && !blk_status[k] && unseekable == nk) ix->size = (int64_t)((nblocks - 1) * bs + blk_len[k]);
+        }
+        for (uint32_t k = a; k < e; k++) {
+            if (k >= unseekable) blk_status[k] = -KZ_ERR_INVALID_FILE;
+            if (blk_status[k])
+                for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
+                    if (!status[P.slices[s].req]) status[P.slices[s].req] = blk_status[k];
+        }
+        CopyList out;
+        for (uint32_t k = a; k < e; k++)
+            for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++) {
+                const ReadSlice& sl = P.slices[s];
+                if (status[sl.req] || sl.in_block >= blk_len[k]) continue;
+                const uint64_t m = std::min<uint64_t>(sl.len, blk_len[k] - sl.in_block);
+                uint8_t* to = staged[sl.req] ? ctx->d_asm.as<uint8_t>() + stage_at[sl.req] + sl.at : dst + dst_off[sl.req] + sl.at;
+                out.add(arena + (uint64_t)(k - a) * astride + sl.in_block, to, m);
+                out_len[sl.req] += m;
+                out_slices++, out_bytes += m;
+            }
+        rc = run_copies(ctx, out);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));  // the arena and the windows are reused by the next pass
+    }
+    if (unseekable != nk) {
+        ctx->err = "Invalid bitstream: a block before the last is not block_size bytes long";
+        for (uint32_t k = unseekable; k < nk; k++)
+            for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
+                if (!status[P.slices[s].req]) status[P.slices[s].req] = -KZ_ERR_INVALID_FILE;
+    }
+    for (uint32_t i = 0; i < nreq; i++)
+        if (status[i]) out_len[i] = 0;
+    // delivery of the staged requests: one transfer to the host, or one copy launch on the device
+    if (host && stage_total) {
+        CK(ctx->h_io.ensure(stage_total));
+        CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.p, stage_total, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t i = 0; i < nreq; i++)
+            if (!status[i] && out_len[i]) memcpy(dst + dst_off[i], (uint8_t*)ctx->h_io.p + stage_at[i], out_len[i]);
+    } else if (stage_total) {
+        CopyList deliver;
+        for (uint32_t i = 0; i < nreq; i++)
+            if (staged[i] && !status[i]) deliver.add(ctx->d_asm.as<uint8_t>() + stage_at[i], dst + dst_off[i], out_len[i]);
+        rc = run_copies(ctx, deliver);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    if (ctx->profile) {
+        auto& b = ctx->prof["read:blocks"];
+        b.bytes_in += dec_blocks, b.bytes_out += dec_bytes, b.launches++;
+        auto& o = ctx->prof["read:out"];
+        o.bytes_in += out_slices, o.bytes_out += out_bytes, o.launches++;
+    }
+    return 0;
+}
+
+int read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len,
+                void* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc;
+    if (!ix || (!src && !d_src) || (nreq && (!off || !len || !dst_off || !out_len || !status))) rc = ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+    else if (cudaSetDevice(ctx->device) != cudaSuccess) rc = ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    else rc = read_ranges_impl(ctx, ix, src, (const uint8_t*)d_src, n, nreq, off, len, (uint8_t*)dst, dst_off, out_len, status);
+    return finish_streams(nreq, status, out_len, rc);
+}
+
+}  // namespace
+
+extern "C" {
+
+int kz_index_build_device(kz_ctx* ctx, const void* d_src, size_t n, kz_index** out) {
+    if (!ctx || !out || (!d_src && n)) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    if ((uintptr_t)d_src & 15) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    StreamHeader sh;
+    uint8_t head[64];
+    int rc = device_stream_header(ctx, d_src, n, head, sh);
+    if (rc) return rc;
+    TransformPlan plan;
+    rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    if (!etype_supported(sh.etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+    // every record is kept, so the walk runs twice: once storing nothing (an empty block range) for the count, once to store them
+    std::vector<Walked> w;
+    for (int store = 0; store < 2; store++) {
+        const uint32_t count = store ? (uint32_t)w[0].n : 0;
+        if (store && count == 0) break;
+        std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, count, 0}};
+        rc = walk_streams(ctx, (const uint32_t*)d_src, wj, store ? -1 : 0, store ? -1 : 1, w);
+        if (rc) return rc;
+        if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
+    }
+    std::unique_ptr<kz_index> ix(new kz_index());
+    ix->t48 = sh.t48;
+    ix->etype = sh.etype;
+    ix->block_size = sh.block_size;
+    ix->checksum_bits = sh.checksum_bits;
+    ix->header_bits = (uint32_t)sh.bits;
+    ix->input_size = sh.input_size;
+    ix->stream_bytes = n;
+    memcpy(ix->head, head, INDEX_HEAD);
+    ix->start = w[0].bit_off;
+    ix->bits = w[0].bits;
+    ix->size = ix->start.empty() ? 0 : -1;
+    if (!index_consistent(*ix)) return ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: the records do not form an index");
+    *out = ix.release();
+    return 0;
+}
+
+int kz_index_build(kz_ctx* ctx, const uint8_t* src, size_t n, kz_index** out) {
+    if (!ctx || !out || !src) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    CK(cudaSetDevice(ctx->device));
+    CK(ctx->d_in.ensure(n + 128));
+    CK(cudaMemsetAsync((uint8_t*)ctx->d_in.p + (n & ~size_t(3)), 0, 128, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
+    return kz_index_build_device(ctx, ctx->d_in.p, n, out);
+}
+
+int kz_index_info(const kz_index* ix, uint64_t* t48, uint32_t* etype, uint32_t* block_size, uint32_t* checksum_bits, int64_t* input_size,
+                  uint64_t* nblocks, uint64_t* stream_bytes, int64_t* size) {
+    if (!ix) return -KZ_ERR_INVALID_PARAM;
+    if (t48) *t48 = ix->t48;
+    if (etype) *etype = ix->etype;
+    if (block_size) *block_size = ix->block_size;
+    if (checksum_bits) *checksum_bits = ix->checksum_bits;
+    if (input_size) *input_size = ix->input_size;
+    if (nblocks) *nblocks = ix->nblocks();
+    if (stream_bytes) *stream_bytes = ix->stream_bytes;
+    if (size) *size = ix->size;
+    return 0;
+}
+
+size_t kz_index_save(const kz_index* ix, uint8_t* dst, size_t cap) {
+    if (!ix) return 0;
+    const size_t need = index_blob_bytes(ix->nblocks());
+    if (dst && cap >= need) index_save(*ix, dst);
+    return need;
+}
+
+int kz_index_load(const uint8_t* blob, size_t n, kz_index** out) {
+    if (!out) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    std::unique_ptr<kz_index> ix(new kz_index());
+    if (!index_load(blob, n, *ix)) return -KZ_ERR_INVALID_FILE;
+    *out = ix.release();
+    return 0;
+}
+
+void kz_index_free(kz_index* ix) { delete ix; }
+
+int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, uint8_t* dst,
+                   const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    return read_ranges(ctx, ix, src, nullptr, n, nreq, off, len, dst, dst_off, out_len, status);
+}
+
+int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
+                          const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    return read_ranges(ctx, ix, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
 }
 
 // ---- block batch, host buffers (Writer.processBlock / Reader.processBlock replacement) -----------------------
