@@ -270,7 +270,7 @@ int kz_set_skip_blocks(kz_ctx* ctx, int on);
  *     min(max(2048, 1.5 x block_size), 2^30)) + 64), rounded up to 16 per block; plus the context's scratch for one batch. The reader sizes
  *     its buffers from the stream header, a headerless reader from its setting when it opens.
  *   kz_device_bytes: the device bytes held by ctx's scratch and an open session's buffers (the sum of their capacities); while a session is
- *   open, the scratch as it was after the worker's last batch.
+ *   open, the scratch as it was after the worker's last batch. The pages of ctx's block caches (kz_cache_create) are added.
  * Errors: the first failure is sticky: every later call returns the same code, and kz_last_error(ctx) gives its message. The reader gives a
  *   stream with a single defect (bad header or version, bad block prefix, bad block header, entropy failure, checksum mismatch, failing
  *   inverse transform, truncation) the code kz_decompress_stream gives for those bytes (given a cap large enough that its record count limit,
@@ -362,6 +362,49 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 /* d_src as for kz_index_build_device; d_dst and dst_off need no alignment; the offset, length and result arrays are host arrays. */
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+
+/* ---- block cache: decoded blocks kept in HBM between range reads, so that repeated reads of the same blocks (an io.ReaderAt reading a
+ *      few KiB at a time, hot objects of an object store) copy instead of decoding -----------------------------------------------------------
+ * A cache is made on one context with a byte budget and is used only with that context. Its device memory is allocated once, when it is
+ *   made: the budget rounded down to whole pages of 64 KiB, in one allocation; nothing is allocated per entry. An entry is one decoded
+ *   block on max(1, ceil(length / 64 KiB)) pages. A budget below one page (0 included) is valid and caches nothing.
+ * Lifetime: free the caches of a context before kz_destroy. kz_destroy releases the pages of any cache still open; its handle then answers
+ *   -KZ_ERR_INVALID_PARAM (kz_cache_stats still answers) and must still be given to kz_cache_free.
+ * Reads: kz_read_ranges_cached[_device] take the arguments of kz_read_ranges[_device] plus the cache, and return exactly what those return
+ *   for the same arguments: the bytes, out_len, status, the return value and the update of the index's size. Only which blocks are decoded
+ *   differs. They are the only calls that read or fill a cache: whole-stream decodes, sessions and kz_read_ranges[_device] never touch one.
+ *   A call hashes every record its requests touch and looks the keys up; the blocks found (hits) are served first, by one copy launch out
+ *   of their pages; the others are decoded in passes as kz_read_ranges decodes them, and every one that decodes without error is inserted
+ *   behind its pass. A block that fails is never inserted, so it is decoded again, and fails with the same code, on every call. A block
+ *   longer than the whole budget is served as without a cache and not inserted. Refused (-KZ_ERR_INVALID_PARAM, every status) like
+ *   kz_read_ranges while a session is open on ctx, and also when the cache belongs to another context or is NULL.
+ * Key: an entry belongs to the content of a record, not to a stream, so one cache serves many streams and indexes (a loaded index, a
+ *   second index of the same stream, identical records in different streams share entries). The key is a 64-bit hash of the record's
+ *   payload bits, the bit length, the fields that change what a record decodes to (transform48, entropy, checksum_bits, block_size) and
+ *   whether the record is the stream's last. The hash: the payload realigned to bit 0 and zero padded to a whole byte, XXH64 (seed 0) of
+ *   every 4 KiB tile, then XXH64 (seed 0) of the tile digests and the bit length as little-endian u64. Two distinct records with the same
+ *   key collide with a probability of about 2^-64 per pair; a collision would serve the other record's bytes.
+ * Eviction: least recently used first, by last use (a hit or an insert); deterministic. Entries used earlier in a call may be evicted by the
+ *   call's own inserts (their bytes have already been copied).
+ * Cost: the device variant hashes the touched records with one launch over 4 KiB tiles plus one for the roots and one copy of the keys
+ *   back; the host variant hashes them on the CPU from src and uploads only the windows of the records it misses, so a call whose blocks
+ *   are all cached uploads nothing. With kz_profile(ctx,1): kz_stage_bytes("read:cache_hit" / "read:cache_miss") = blocks / decoded
+ *   bytes, ("read:cache_insert" / "read:cache_evict") = entries / bytes, kz_kernel_time("record_hash") the device hashing (its two
+ *   launches), "host:record_hash" the host hashing; "read:blocks" counts the blocks actually decoded.
+ * Stats (kz_cache_stats; any pointer may be NULL): entries, resident_bytes (decoded bytes held), budget_bytes (as given), and since the cache
+ *   was made: hits and misses (blocks looked up), inserts, evictions, served_bytes (bytes copied out of the cache to requests).
+ *   kz_cache_clear drops every entry and keeps the counters.
+ * kz_device_bytes(ctx) counts the pages of ctx's caches. */
+typedef struct kz_cache kz_cache;
+int kz_cache_create(kz_ctx* ctx, uint64_t budget_bytes, kz_cache** out);
+void kz_cache_free(kz_cache* cache);
+int kz_cache_clear(kz_cache* cache);
+int kz_cache_stats(const kz_cache* cache, uint64_t* entries, uint64_t* resident_bytes, uint64_t* budget_bytes, uint64_t* hits, uint64_t* misses,
+                   uint64_t* inserts, uint64_t* evictions, uint64_t* served_bytes);
+int kz_read_ranges_cached(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const uint8_t* src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len,
+                          uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+int kz_read_ranges_cached_device(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
+                                 const uint64_t* len, void* d_dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
 
 #ifdef __cplusplus
 }

@@ -79,6 +79,19 @@ type Range struct {
 // the call as a whole (a stale index, a session open on c, a chain the GPU path lacks); failures of single blocks, and a CUDA error,
 // which sets every request's status, are in the requests' Err.
 func (c *Context) ReadRanges(x *Index, stream []byte, reqs []Range) error {
+	return c.readRanges(nil, x, stream, reqs)
+}
+
+// ReadRangesCached is ReadRanges through the block cache k of c (kz_read_ranges_cached): the same results, and the blocks k holds are
+// copied instead of decoded. Blocks decoded here are kept in k for later calls.
+func (c *Context) ReadRangesCached(k *Cache, x *Index, stream []byte, reqs []Range) error {
+	if k == nil {
+		return errors.New("gpu: nil block cache")
+	}
+	return c.readRanges(k, x, stream, reqs)
+}
+
+func (c *Context) readRanges(k *Cache, x *Index, stream []byte, reqs []Range) error {
 	n := len(reqs)
 	if n == 0 {
 		return nil
@@ -96,8 +109,13 @@ func (c *Context) ReadRanges(x *Index, stream []byte, reqs []Range) error {
 	buf := make([]byte, total+1) // cgo must not see pointers into several Go slices: one buffer, then copies
 	c.mu.Lock()
 	defer c.mu.Unlock()
-	rc := C.kz_read_ranges(c.h, x.h, (*C.uint8_t)(unsafe.Pointer(&stream[0])), C.size_t(len(stream)), C.uint32_t(n), &off[0], &ln[0],
-		(*C.uint8_t)(unsafe.Pointer(&buf[0])), &dstOff[0], &outLen[0], &status[0])
+	src, dst := (*C.uint8_t)(unsafe.Pointer(&stream[0])), (*C.uint8_t)(unsafe.Pointer(&buf[0]))
+	var rc C.int
+	if k == nil {
+		rc = C.kz_read_ranges(c.h, x.h, src, C.size_t(len(stream)), C.uint32_t(n), &off[0], &ln[0], dst, &dstOff[0], &outLen[0], &status[0])
+	} else {
+		rc = C.kz_read_ranges_cached(c.h, k.h, x.h, src, C.size_t(len(stream)), C.uint32_t(n), &off[0], &ln[0], dst, &dstOff[0], &outLen[0], &status[0])
+	}
 	if rc == -C.KZ_ERR_INVALID_PARAM || rc == -C.KZ_ERR_CREATE_CODEC { // no block fails with these: the call failed as a whole
 		return c.err(rc)
 	}
@@ -113,11 +131,13 @@ func (c *Context) ReadRanges(x *Index, stream []byte, reqs []Range) error {
 }
 
 // ReaderAt is an io.ReaderAt over the original data of (stream, index): every ReadAt is one kz_read_ranges call of one request.
-// Callers with many reads in hand use ReadRanges, which decodes each touched block once for all of them.
+// Callers with many reads in hand use ReadRanges, which decodes each touched block once for all of them. With Cache set (a cache of
+// C), each ReadAt goes through it: reading a block in small pieces decodes it once instead of once per piece.
 type ReaderAt struct {
 	C      *Context
 	Index  *Index
 	Stream []byte
+	Cache  *Cache
 }
 
 func (r *ReaderAt) ReadAt(p []byte, off int64) (int, error) {
@@ -125,7 +145,7 @@ func (r *ReaderAt) ReadAt(p []byte, off int64) (int, error) {
 		return 0, errors.New("gpu: negative offset")
 	}
 	req := []Range{{Off: uint64(off), Dst: p}}
-	if err := r.C.ReadRanges(r.Index, r.Stream, req); err != nil {
+	if err := r.C.readRanges(r.Cache, r.Index, r.Stream, req); err != nil {
 		return 0, err
 	}
 	if req[0].Err != nil {
@@ -135,4 +155,43 @@ func (r *ReaderAt) ReadAt(p []byte, off int64) (int, error) {
 		return req[0].N, io.EOF
 	}
 	return req[0].N, nil
+}
+
+// Cache keeps decoded blocks in HBM between reads of one Context (kz_cache_*). Entries belong to the content of a block record, so one
+// cache serves every stream and index read through it. Free it before the Context is closed.
+type Cache struct {
+	c *Context // its calls take the context's lock: reads on other goroutines update the counters and the context's cache list
+	h *C.kz_cache
+}
+
+// CacheStats are the counters of a Cache (kz_cache_stats): what it holds, and what it did since it was made.
+type CacheStats struct {
+	Entries, ResidentBytes, BudgetBytes, Hits, Misses, Inserts, Evictions, ServedBytes uint64
+}
+
+// NewBlockCache allocates a cache of budget bytes of HBM (rounded down to 64 KiB pages) on c, once.
+func (c *Context) NewBlockCache(budget uint64) (*Cache, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var h *C.kz_cache
+	if rc := C.kz_cache_create(c.h, C.uint64_t(budget), &h); rc != 0 {
+		return nil, c.err(rc)
+	}
+	return &Cache{c: c, h: h}, nil
+}
+
+func (k *Cache) Stats() CacheStats {
+	k.c.mu.Lock()
+	defer k.c.mu.Unlock()
+	var v [8]C.uint64_t
+	C.kz_cache_stats(k.h, &v[0], &v[1], &v[2], &v[3], &v[4], &v[5], &v[6], &v[7])
+	return CacheStats{uint64(v[0]), uint64(v[1]), uint64(v[2]), uint64(v[3]), uint64(v[4]), uint64(v[5]), uint64(v[6]), uint64(v[7])}
+}
+
+// Free releases the cache and its device memory.
+func (k *Cache) Free() {
+	k.c.mu.Lock()
+	defer k.c.mu.Unlock()
+	C.kz_cache_free(k.h)
+	k.h = nil
 }

@@ -42,7 +42,8 @@ ABI_SYMBOLS = [
     "kz_reader_free", "kz_device_bytes", "kz_set_block_range", "kz_bwt_profile",
     "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader", "kz_set_skip_blocks",
     "kz_index_build", "kz_index_build_device", "kz_index_info", "kz_index_save", "kz_index_load", "kz_index_free", "kz_read_ranges",
-    "kz_read_ranges_device",
+    "kz_read_ranges_device", "kz_cache_create", "kz_cache_free", "kz_cache_clear", "kz_cache_stats", "kz_read_ranges_cached",
+    "kz_read_ranges_cached_device",
 ]
 
 
@@ -174,6 +175,13 @@ def load_library(build_if_missing=True):
     L.kz_index_free.restype = None
     L.kz_read_ranges.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
     L.kz_read_ranges_device.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
+    L.kz_cache_create.argtypes = [vp, u64, C.POINTER(vp)]
+    L.kz_cache_free.argtypes = [vp]
+    L.kz_cache_free.restype = None
+    L.kz_cache_clear.argtypes = [vp]
+    L.kz_cache_stats.argtypes = [vp] + [C.POINTER(u64)] * 8
+    L.kz_read_ranges_cached.argtypes = [vp, vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
+    L.kz_read_ranges_cached_device.argtypes = [vp, vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -555,6 +563,13 @@ class Context:
             self._check(self.lib.kz_index_build_device(self.h, _dptr(d_src), n, C.byref(h)))
         return StreamIndex(h, self)
 
+    def block_cache(self, budget):
+        """A BlockCache of decoded blocks in `budget` bytes of HBM (kz_cache_create), for StreamIndex.read / read_many /
+        read_many_device(cache=...) on this context."""
+        h = C.c_void_p()
+        self._check(self.lib.kz_cache_create(self.h, budget, C.byref(h)))
+        return BlockCache(self, h)
+
     # ---- streaming sessions (kz_writer_* / kz_reader_*): one stream of any length in bounded memory -------------------------------
     def stream_writer(self, transform, entropy, block_size, checksum_bits=0, batch_blocks=None, input_size=0, headerless=None, skip_blocks=None):
         """A StreamSession: write(data) -> bytes and finish() -> bytes give the stream compress() writes for the concatenated input.
@@ -665,9 +680,10 @@ class StreamIndex:
         self.lib.kz_index_save(self.h, out.ctypes.data, n)
         return out.tobytes()
 
-    def read_many(self, stream, requests, ctx=None):
+    def read_many(self, stream, requests, ctx=None, cache=None):
         """requests: [(off, length), ...] -> (list of bytes, status list). Failures do not raise: status[i] = 0 or -(kanzi error code); a
-        short request gives fewer bytes, a failed one b"". A call-level failure (stale index, open session) sets every status."""
+        short request gives fewer bytes, a failed one b"". A call-level failure (stale index, open session) sets every status.
+        cache: a BlockCache of the context (kz_read_ranges_cached): the same results, blocks it holds are copied instead of decoded."""
         ctx = ctx or self.ctx
         s = _u8(stream)
         off = np.array([r[0] for r in requests], np.uint64)
@@ -675,23 +691,69 @@ class StreamIndex:
         dst_off = _offsets(ln)
         dst = np.empty(max(int(ln.sum()), 1), np.uint8)
         out_len, status = np.zeros(len(requests), np.uint64), np.zeros(len(requests), np.int32)
-        self.lib.kz_read_ranges(ctx.h, self.h, _p(s), s.size, len(requests), _p(off), _p(ln), dst.ctypes.data, _p(dst_off), _p(out_len), _p(status))
+        args = (_p(s), s.size, len(requests), _p(off), _p(ln), dst.ctypes.data, _p(dst_off), _p(out_len), _p(status))
+        if cache is None:
+            self.lib.kz_read_ranges(ctx.h, self.h, *args)
+        else:
+            self.lib.kz_read_ranges_cached(ctx.h, cache.h, self.h, *args)
         return [dst[int(o): int(o) + int(n)].tobytes() for o, n in zip(dst_off, out_len)], status.tolist()
 
-    def read(self, stream, off, length, ctx=None):
+    def read(self, stream, off, length, ctx=None, cache=None):
         """Decoded bytes [off, off + length), short at the end of the data; raises when the block fails."""
-        out, st = self.read_many(stream, [(off, length)], ctx)
+        out, st = self.read_many(stream, [(off, length)], ctx, cache)
         if st[0]:
             (ctx or self.ctx)._check(st[0])
         return out[0]
 
-    def read_many_device(self, d_src, n, off, length, d_dst, dst_off, ctx=None):
+    def read_many_device(self, d_src, n, off, length, d_dst, dst_off, ctx=None, cache=None):
         """Device-resident read_many: d_src / d_dst are CUDA tensors or addresses, the rest host sequences -> (out_len, status)."""
         ctx = ctx or self.ctx
         o, ln, do = (np.ascontiguousarray(a, np.uint64) for a in (off, length, dst_off))
         out_len, status = np.zeros(len(o), np.uint64), np.zeros(len(o), np.int32)
-        self.lib.kz_read_ranges_device(ctx.h, self.h, _dptr(d_src), n, len(o), _p(o), _p(ln), _dptr(d_dst), _p(do), _p(out_len), _p(status))
+        args = (_dptr(d_src), n, len(o), _p(o), _p(ln), _dptr(d_dst), _p(do), _p(out_len), _p(status))
+        if cache is None:
+            self.lib.kz_read_ranges_device(ctx.h, self.h, *args)
+        else:
+            self.lib.kz_read_ranges_cached_device(ctx.h, cache.h, self.h, *args)
         return out_len, status
+
+
+class BlockCache:
+    """Decoded blocks kept in HBM between range reads (kz_cache_*), made by Context.block_cache(budget). Entries belong to the content
+    of a record, so one cache serves every stream and index read on its context. A context manager: leaving the block frees the cache."""
+
+    STATS = ("entries", "resident_bytes", "budget_bytes", "hits", "misses", "inserts", "evictions", "served_bytes")
+
+    def __init__(self, ctx, h):
+        self.ctx, self.h = ctx, h
+        self.lib = load_library()
+
+    @property
+    def stats(self):
+        v = [C.c_uint64(0) for _ in self.STATS]
+        self.lib.kz_cache_stats(self.h, *[C.byref(x) for x in v])
+        return {k: x.value for k, x in zip(self.STATS, v)}
+
+    def clear(self):
+        """Drops every entry; the counters stay."""
+        self.ctx._check(self.lib.kz_cache_clear(self.h))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.kz_cache_free(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def default_batch_blocks(block_size):

@@ -28,6 +28,9 @@
 #include "kz_skip.cuh"
 #include "kz_stream_plan.h"
 #include "kz_read_plan.h"
+#include "kz_block_cache.h"
+#include "kz_record_hash.cuh"
+#include "kz_xxh64_core.cuh"
 
 #include <condition_variable>
 #include <map>
@@ -43,6 +46,16 @@ using namespace kz;
         cudaError_t e_ = (x);                                 \
         if (e_ != cudaSuccess) return ctx->cuda_fail(e_, #x); \
     } while (0)
+
+// A block cache (kz_cache_create): the bookkeeping of kz_block_cache.h over one device allocation of pages. ctx is null once kz_destroy has
+// released the pages of a cache its caller did not free first.
+struct kz_cache {
+    kz_ctx* ctx;
+    kz::PageCache pc;
+    void* d_pages = nullptr;
+    kz_cache(kz_ctx* c, uint64_t budget) : ctx(c), pc(budget) {}
+    size_t device_bytes() const { return d_pages ? (size_t)pc.npages() * kz::CACHE_PAGE : 0; }
+};
 
 namespace {
 
@@ -1915,6 +1928,11 @@ void kz_destroy(kz_ctx* ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->session) close_session(ctx->session);
     cudaStreamSynchronize(ctx->stream);
+    for (kz_cache* c : ctx->caches) {  // caches not freed before: their handles stay valid for kz_cache_free
+        cudaFree(c->d_pages);
+        c->d_pages = nullptr;
+        c->ctx = nullptr;
+    }
     drain_profile(ctx);
     for (auto e : ctx->event_pool) cudaEventDestroy(e);
     ctx->each_dev_buf([](DevBuf& b) { b.release(); });
@@ -2858,11 +2876,66 @@ int upload_windows(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const ui
     return 0;
 }
 
+// The keys of the cached read's blocks (P.blocks): the record hash of every record (kz_xxh64_core.cuh) and the header fields a record's
+// decode depends on. Host variant: hashed on the CPU from the caller's stream. Device variant: one record_hash launch over every tile of
+// the records, one thread per record for the roots, one copy of the keys back.
+int cache_keys(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const uint8_t* d_src, const std::vector<uint64_t>& blocks, std::vector<CacheKey>& key) {
+    const uint32_t nk = (uint32_t)blocks.size();
+    key.assign(nk, CacheKey());
+    for (uint32_t k = 0; k < nk; k++) {
+        key[k].bits = ix.bits[blocks[k]];
+        key[k].t48 = ix.t48;
+        key[k].etype = ix.etype;
+        key[k].checksum_bits = ix.checksum_bits;
+        key[k].block_size = ix.block_size;
+        key[k].last = blocks[k] + 1 == ix.nblocks();
+    }
+    if (nk == 0) return 0;
+    if (src) {
+        HostScope hs(ctx, "record_hash");
+        for (uint32_t k = 0; k < nk; k++) key[k].hash = record_hash_host(src, ix.start[blocks[k]], ix.bits[blocks[k]]);
+        return 0;
+    }
+    std::vector<RecordHashJob> jobs(nk);
+    uint64_t ntiles = 0;
+    for (uint32_t k = 0; k < nk; k++) {
+        jobs[k] = RecordHashJob{ix.start[blocks[k]], ix.bits[blocks[k]], ntiles};
+        ntiles += record_tiles(ix.bits[blocks[k]]);
+    }
+    Packer pk;
+    const size_t o_j = pk.add(jobs.data(), jobs.size() * sizeof(RecordHashJob));
+    int rc = upload(ctx, pk);
+    if (rc) return rc;
+    CK(ctx->d_ws.ensure((ntiles + nk) * 8));
+    const RecordHashJob* d_jobs = (const RecordHashJob*)(ctx->d_tables.as<uint8_t>() + o_j);
+    uint64_t* d_dig = ctx->d_ws.as<uint64_t>();
+    uint64_t* d_key = d_dig + ntiles;
+    {
+        LaunchScope ls(ctx, "record_hash");
+        record_hash_tiles_kernel<<<(unsigned)((ntiles + RECORD_HASH_WARPS - 1) / RECORD_HASH_WARPS), 32 * RECORD_HASH_WARPS, 0, ctx->stream>>>(
+            (const uint32_t*)d_src, d_jobs, (int)nk, ntiles, d_dig);
+    }
+    {
+        LaunchScope ls(ctx, "record_hash");
+        record_hash_root_kernel<<<(nk + 127) / 128, 128, 0, ctx->stream>>>(d_jobs, (int)nk, d_dig, d_key);
+    }
+    CK(cudaGetLastError());
+    std::vector<uint64_t> h(nk);
+    CK(cudaMemcpyAsync(h.data(), d_key, (size_t)nk * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (uint32_t k = 0; k < nk; k++) key[k].hash = h[k];
+    return 0;
+}
+
 // One batched read. src is the host stream (host variant: dst is host memory too) or null (d_src is the stream, dst device memory).
-int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nreq, const uint64_t* off,
-                     const uint64_t* len, uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+// cache: null, or the block cache of a cached read. With a cache the blocks found in it form a pass of their own, served first by one
+// copy launch out of its pages; the others (the misses) run through the decode passes as every block does without a cache, and each
+// that decodes is inserted behind its pass.
+int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nreq,
+                     const uint64_t* off, const uint64_t* len, uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
     const bool host = src != nullptr;
     if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    if (cache && cache->ctx != ctx) return ctx->fail(KZ_ERR_INVALID_PARAM, "the block cache belongs to another context");
     for (uint32_t i = 0; i < nreq; i++) {
         if (dst_off[i] + len[i] < dst_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
         if (len[i] && !dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
@@ -2888,11 +2961,30 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
     const uint64_t nblocks = ix->nblocks();
     const ReadPlan P = plan_reads(nblocks, bs, ix->size, nreq, off, len);
     const uint32_t nk = (uint32_t)P.blocks.size();
+    // The blocks to decode, pass after pass: order[first[p] .. first[p + 1]) (ascending). Without a cache every touched block; with
+    // one the blocks it lacks (hit[k] names the entry of the others).
+    std::vector<CacheKey> key;
+    std::vector<const CacheEntry*> hit(cache ? nk : 0, nullptr);
+    std::vector<uint32_t> order, first;
+    if (cache) {
+        rc = cache_keys(ctx, *ix, src, d_src, P.blocks, key);
+        if (rc) return rc;
+        for (uint32_t k = 0; k < nk; k++)
+            if (!(hit[k] = cache->pc.lookup(key[k]))) order.push_back(k);
+        first = plan_decompress_passes((uint32_t)order.size(), decompress_slot(bs), read_block_cost(bs)).first;
+    } else {
+        order.resize(nk);
+        std::iota(order.begin(), order.end(), 0u);
+        first = P.first;
+    }
+    const uint32_t npasses = (uint32_t)first.size() - 1;
+    const uint32_t hp = cache ? 1 : 0;  // the pass number of the first decode pass (the cache's blocks are pass 0)
     // A request is staged (its slices gathered in ctx->d_asm, delivered when every block it touches has decoded) when it goes to host
-    // memory or its blocks lie in more than one pass: nothing is written for a request that fails.
-    std::vector<uint32_t> pass_of(nk);
-    for (uint32_t p = 0; p < P.npasses(); p++)
-        for (uint32_t k = P.first[p]; k < P.first[p + 1]; k++) pass_of[k] = p;
+    // memory or its blocks lie in more than one pass: nothing is written for a request that fails. A request on cached blocks only is
+    // staged too when one of them lies behind a block still to decode, whose length may make it unseekable.
+    std::vector<uint32_t> pass_of(nk, 0), slot_of(nk, 0);
+    for (uint32_t p = 0; p < npasses; p++)
+        for (uint32_t i = first[p]; i < first[p + 1]; i++) pass_of[order[i]] = hp + p, slot_of[order[i]] = i - first[p];
     std::vector<uint32_t> first_pass(nreq, 0);
     std::vector<uint8_t> staged(nreq, host);
     for (uint32_t k = 0; k < nk; k++)
@@ -2901,7 +2993,7 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
             if (sl.at == 0) first_pass[sl.req] = pass_of[k];
         }
     for (const ReadSlice& sl : P.slices)
-        if (pass_of[sl.block] != first_pass[sl.req]) staged[sl.req] = 1;
+        if (pass_of[sl.block] != first_pass[sl.req] || (cache && hit[sl.block] && !order.empty() && sl.block > order[0])) staged[sl.req] = 1;
     std::vector<uint64_t> stage_at(nreq, 0);
     uint64_t stage_total = 0;
     for (uint32_t i = 0; i < nreq; i++)
@@ -2915,16 +3007,60 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
     for (uint32_t i = 0; i < nreq; i++) status[i] = 0, out_len[i] = 0;
     uint32_t unseekable = nk;  // the first touched block whose length breaks the block arithmetic
     uint64_t dec_blocks = 0, dec_bytes = 0, out_slices = 0, out_bytes = 0;
-    for (uint32_t p = 0; p < P.npasses() && unseekable == nk; p++) {
-        const uint32_t a = P.first[p], e = P.first[p + 1];
+    uint8_t* pages = cache ? (uint8_t*)cache->d_pages : nullptr;
+    bool hit_copies = false;  // the copies out of the cache were queued; the call returns only after they ran
+    if (cache) {
+        // the cached blocks: their lengths are known, so is the unseekable rule among them; a request on them alone that is not staged
+        // gets its status now, before its bytes are written
+        uint64_t hits = 0, hit_bytes = 0, served = 0;
+        for (uint32_t k = 0; k < nk; k++)
+            if (hit[k]) {
+                blk_len[k] = hit[k]->len;
+                if (P.blocks[k] + 1 == nblocks ? blk_len[k] == 0 : blk_len[k] != bs) unseekable = std::min(unseekable, k);
+                hits++, hit_bytes += blk_len[k];
+            }
+        for (uint32_t k = unseekable; k < nk; k++)
+            if (hit[k])
+                for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
+                    if (!staged[P.slices[s].req]) status[P.slices[s].req] = -KZ_ERR_INVALID_FILE;
+        CopyList out;
+        for (uint32_t k = 0; k < std::min(unseekable, nk); k++) {
+            if (!hit[k]) continue;
+            for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++) {
+                const ReadSlice& sl = P.slices[s];
+                if (status[sl.req] || sl.in_block >= blk_len[k]) continue;
+                const uint64_t m = std::min<uint64_t>(sl.len, blk_len[k] - sl.in_block);
+                uint8_t* to = staged[sl.req] ? ctx->d_asm.as<uint8_t>() + stage_at[sl.req] + sl.at : dst + dst_off[sl.req] + sl.at;
+                cache_slice_copies(*hit[k], sl.in_block, m, [&](uint32_t page, uint64_t in_page, uint64_t at, uint64_t c) {
+                    out.add(pages + page * CACHE_PAGE + in_page, to + at, c);
+                });
+                out_len[sl.req] += m;
+                out_slices++, out_bytes += m, served += m;
+            }
+        }
+        rc = run_copies(ctx, out);
+        if (rc) return rc;
+        hit_copies = !out.jobs.empty();
+        cache->pc.note_served(served);
+        if (ctx->profile) {
+            auto& h = ctx->prof["read:cache_hit"];
+            h.bytes_in += hits, h.bytes_out += hit_bytes, h.launches++;
+        }
+    }
+    const CacheStats before = cache ? cache->pc.stats() : CacheStats();
+    uint64_t miss_blocks = 0, miss_bytes = 0, ins_bytes = 0;
+    for (uint32_t p = 0; p < npasses && order[first[p]] < unseekable; p++) {
+        const uint32_t a = first[p], e = first[p + 1];
+        std::vector<uint64_t> pass_blocks(e - a);
+        for (uint32_t i = a; i < e; i++) pass_blocks[i - a] = P.blocks[order[i]];
         PassInput in;
         if (host) {
-            rc = upload_windows(ctx, *ix, src, &P.blocks[a], e - a, in);
+            rc = upload_windows(ctx, *ix, src, pass_blocks.data(), e - a, in);
             if (rc) return rc;
         } else {
             in.d_words = (const uint32_t*)d_src;
             in.words_len = (n + 3) / 4 + 16;
-            for (uint32_t k = a; k < e; k++) in.bit_off.push_back(ix->start[P.blocks[k]]);
+            for (uint64_t b : pass_blocks) in.bit_off.push_back(ix->start[b]);
         }
         CK(ctx->d_slots.ensure(astride * (e - a) + 64));
         uint8_t* arena = ctx->d_slots.as<uint8_t>();
@@ -2935,7 +3071,7 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
             std::vector<uint8_t> last(ks.size());
             std::vector<DecodeFailure> fail(ks.size());
             for (size_t i = 0; i < ks.size(); i++) {
-                jobs[i].bit_off = in.bit_off[ks[i] - a];
+                jobs[i].bit_off = in.bit_off[slot_of[ks[i]]];
                 jobs[i].bits = ix->bits[P.blocks[ks[i]]];
                 owner[i] = (uint32_t)i;
                 last[i] = P.blocks[ks[i]] + 1 == nblocks;
@@ -2947,51 +3083,79 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
                     too_long[ks[i]] = 1;
                     return NO_ROOM;
                 }
-                return (uint64_t)(ks[i] - a) * astride;
+                return (uint64_t)slot_of[ks[i]] * astride;
             };
             int r = decode_walked(ctx, sh, plan, in.d_words, in.words_len, jobs, owner, last, place, arena, fail.data());
             if (r) return r;
             for (size_t i = 0; i < ks.size(); i++) blk_status[ks[i]] = fail[i].failed() ? fail[i].code : 0;
             return 0;
         };
-        std::vector<uint32_t> ks(e - a);
-        std::iota(ks.begin(), ks.end(), a);
+        const std::vector<uint32_t> ks(order.begin() + a, order.begin() + e);
         rc = decode(ks);
         if (rc) return rc;
         // A failing stage call cannot name its block, and a failure of one block may hide a later one's: every failed block of a pass
         // of several is decoded again alone, so that its status is the one a decode of that block alone gives. Only corrupt input pays.
         if (e - a > 1)
-            for (uint32_t k = a; k < e; k++)
+            for (uint32_t k : ks)
                 if (blk_status[k] && !too_long[k]) {
                     rc = decode(std::vector<uint32_t>{k});
                     if (rc) return rc;
                 }
-        for (uint32_t k = a; k < e; k++) {
+        for (uint32_t k : ks) {
             const bool is_last = P.blocks[k] + 1 == nblocks;
             if (too_long[k] || (!blk_status[k] && (is_last ? blk_len[k] == 0 : blk_len[k] != bs))) unseekable = std::min(unseekable, k);
             if (!blk_status[k]) dec_blocks++, dec_bytes += blk_len[k];
             if (is_last && !blk_status[k] && unseekable == nk) ix->size = (int64_t)((nblocks - 1) * bs + blk_len[k]);
         }
-        for (uint32_t k = a; k < e; k++) {
+        // every block of the pass that decoded goes into the cache; an entry this pass made and evicted again gets no copy
+        std::vector<std::pair<uint32_t, uint64_t>> fresh;  // (block, serial)
+        if (cache)
+            for (uint32_t k : ks) {
+                miss_blocks++, miss_bytes += blk_status[k] || too_long[k] ? 0 : blk_len[k];
+                if (blk_status[k] || too_long[k]) continue;
+                bool made = false;
+                const CacheEntry* en = cache->pc.insert(key[k], blk_len[k], &made);
+                if (made) fresh.push_back({k, en->serial}), ins_bytes += blk_len[k];
+            }
+        for (uint32_t k : ks) {
             if (k >= unseekable) blk_status[k] = -KZ_ERR_INVALID_FILE;
             if (blk_status[k])
                 for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
                     if (!status[P.slices[s].req]) status[P.slices[s].req] = blk_status[k];
         }
         CopyList out;
-        for (uint32_t k = a; k < e; k++)
+        for (uint32_t k : ks)
             for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++) {
                 const ReadSlice& sl = P.slices[s];
                 if (status[sl.req] || sl.in_block >= blk_len[k]) continue;
                 const uint64_t m = std::min<uint64_t>(sl.len, blk_len[k] - sl.in_block);
                 uint8_t* to = staged[sl.req] ? ctx->d_asm.as<uint8_t>() + stage_at[sl.req] + sl.at : dst + dst_off[sl.req] + sl.at;
-                out.add(arena + (uint64_t)(k - a) * astride + sl.in_block, to, m);
+                out.add(arena + (uint64_t)slot_of[k] * astride + sl.in_block, to, m);
                 out_len[sl.req] += m;
                 out_slices++, out_bytes += m;
             }
+        for (const auto& f : fresh)
+            if (const CacheEntry* en = cache->pc.peek(key[f.first], f.second))
+                cache_slice_copies(*en, 0, en->len, [&](uint32_t page, uint64_t in_page, uint64_t at, uint64_t c) {
+                    out.add(arena + (uint64_t)slot_of[f.first] * astride + at, pages + page * CACHE_PAGE + in_page, c);
+                });
         rc = run_copies(ctx, out);
         if (rc) return rc;
         CK(cudaStreamSynchronize(ctx->stream));  // the arena and the windows are reused by the next pass
+    }
+    if (cache) {
+        // a cached last block sets the size as a decoded one does
+        const uint32_t k = nk ? nk - 1 : 0;
+        if (nk && hit[k] && P.blocks[k] + 1 == nblocks && unseekable == nk) ix->size = (int64_t)((nblocks - 1) * bs + blk_len[k]);
+        if (ctx->profile) {
+            const CacheStats& after = cache->pc.stats();
+            auto& m = ctx->prof["read:cache_miss"];
+            m.bytes_in += miss_blocks, m.bytes_out += miss_bytes, m.launches++;
+            auto& i = ctx->prof["read:cache_insert"];
+            i.bytes_in += after.inserts - before.inserts, i.bytes_out += ins_bytes, i.launches++;
+            auto& v = ctx->prof["read:cache_evict"];
+            v.bytes_in += after.evictions - before.evictions, v.bytes_out += before.resident + ins_bytes - after.resident, v.launches++;
+        }
     }
     if (unseekable != nk) {
         ctx->err = "Invalid bitstream: a block before the last is not block_size bytes long";
@@ -3016,6 +3180,9 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
         if (rc) return rc;
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    // A call whose blocks were all cached (or whose misses lie behind an unseekable block) has no decode pass and may have no staged
+    // delivery: nothing above waited for the copies out of the cache. The bytes are complete, and a failed copy is reported, on return.
+    if (hit_copies) CK(cudaStreamSynchronize(ctx->stream));
     if (ctx->profile) {
         auto& b = ctx->prof["read:blocks"];
         b.bytes_in += dec_blocks, b.bytes_out += dec_bytes, b.launches++;
@@ -3025,13 +3192,13 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_
     return 0;
 }
 
-int read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len,
-                void* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+int read_ranges(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
+                const uint64_t* len, void* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     int rc;
     if (!ix || (!src && !d_src) || (nreq && (!off || !len || !dst_off || !out_len || !status))) rc = ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
     else if (cudaSetDevice(ctx->device) != cudaSuccess) rc = ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
-    else rc = read_ranges_impl(ctx, ix, src, (const uint8_t*)d_src, n, nreq, off, len, (uint8_t*)dst, dst_off, out_len, status);
+    else rc = read_ranges_impl(ctx, ix, cache, src, (const uint8_t*)d_src, n, nreq, off, len, (uint8_t*)dst, dst_off, out_len, status);
     return finish_streams(nreq, status, out_len, rc);
 }
 
@@ -3124,12 +3291,65 @@ void kz_index_free(kz_index* ix) { delete ix; }
 
 int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, uint8_t* dst,
                    const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
-    return read_ranges(ctx, ix, src, nullptr, n, nreq, off, len, dst, dst_off, out_len, status);
+    return read_ranges(ctx, ix, nullptr, src, nullptr, n, nreq, off, len, dst, dst_off, out_len, status);
 }
 
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
-    return read_ranges(ctx, ix, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
+    return read_ranges(ctx, ix, nullptr, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
+}
+
+// ---- block cache (kz_cache_*, kz_read_ranges_cached[_device]; bookkeeping in kz_block_cache.h) ---------------------------------------
+int kz_cache_create(kz_ctx* ctx, uint64_t budget_bytes, kz_cache** out) {
+    if (!ctx || !out) return -KZ_ERR_INVALID_PARAM;
+    *out = nullptr;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    std::unique_ptr<kz_cache> c(new kz_cache(ctx, budget_bytes));
+    if (c->pc.npages()) CK(cudaMalloc(&c->d_pages, (size_t)c->pc.npages() * CACHE_PAGE));
+    ctx->caches.push_back(c.get());
+    *out = c.release();
+    return 0;
+}
+
+void kz_cache_free(kz_cache* c) {
+    if (!c) return;
+    if (kz_ctx* ctx = c->ctx) {
+        cudaSetDevice(ctx->device);
+        cudaStreamSynchronize(ctx->stream);
+        cudaFree(c->d_pages);
+        ctx->caches.erase(std::find(ctx->caches.begin(), ctx->caches.end(), c));
+    }
+    delete c;
+}
+
+int kz_cache_clear(kz_cache* c) {
+    if (!c || !c->ctx) return -KZ_ERR_INVALID_PARAM;
+    c->pc.clear();
+    return 0;
+}
+
+int kz_cache_stats(const kz_cache* c, uint64_t* entries, uint64_t* resident_bytes, uint64_t* budget_bytes, uint64_t* hits, uint64_t* misses, uint64_t* inserts,
+                   uint64_t* evictions, uint64_t* served_bytes) {
+    if (!c) return -KZ_ERR_INVALID_PARAM;
+    const CacheStats& st = c->pc.stats();
+    const std::pair<uint64_t*, uint64_t> f[] = {{entries, st.entries}, {resident_bytes, st.resident}, {budget_bytes, st.budget}, {hits, st.hits},
+                                                {misses, st.misses},   {inserts, st.inserts},         {evictions, st.evictions}, {served_bytes, st.served}};
+    for (const auto& x : f)
+        if (x.first) *x.first = x.second;
+    return 0;
+}
+
+int kz_read_ranges_cached(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const uint8_t* src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len,
+                          uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (ctx && !cache) return finish_streams(nreq, status, out_len, ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument"));
+    return read_ranges(ctx, ix, cache, src, nullptr, n, nreq, off, len, dst, dst_off, out_len, status);
+}
+
+int kz_read_ranges_cached_device(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
+                                 const uint64_t* len, void* d_dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (ctx && !cache) return finish_streams(nreq, status, out_len, ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument"));
+    return read_ranges(ctx, ix, cache, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
 }
 
 // ---- block batch, host buffers (Writer.processBlock / Reader.processBlock replacement) -----------------------
@@ -4024,7 +4244,9 @@ void kz_reader_free(kz_reader* r) {
 
 size_t kz_device_bytes(kz_ctx* ctx) {
     if (!ctx) return 0;
-    return ctx->session ? ctx->session->device_bytes() : ctx->scratch_bytes();
+    size_t caches = 0;
+    for (const kz_cache* c : ctx->caches) caches += c->device_bytes();
+    return (ctx->session ? ctx->session->device_bytes() : ctx->scratch_bytes()) + caches;
 }
 
 }  // extern "C"

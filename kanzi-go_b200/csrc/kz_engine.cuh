@@ -124,6 +124,8 @@ struct DecJob {          // one block handed to the entropy decode stage
 
 }  // namespace kz
 
+struct kz_cache;
+
 struct kz_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -162,6 +164,8 @@ struct kz_ctx {
     // the open writer / reader session (the end of kz_api.cu), if any; kz_destroy closes it. kz_device_bytes asks it, because its
     // worker thread grows the scratch
     kz::Session* session = nullptr;
+    // the block caches made on this context (kz_cache_create) and not freed yet: kz_device_bytes counts their pages, kz_destroy frees them
+    std::vector<kz_cache*> caches;
 
     template <class F>
     void each_dev_buf(F&& f) {

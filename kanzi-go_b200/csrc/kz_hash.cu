@@ -7,13 +7,13 @@
 // The hash is four independent accumulator chains over 16-byte (32-bit variant) or 32-byte (64-bit variant) stripes,
 // v = rotl(v + x * P2, r) * P1: one WARP per block, lane k < 4 owns accumulator k and walks its chain with the loads of
 // the next 16 stripes already in flight (two register batches); blocks are hashed concurrently. The chain is the
-// format's limit: 4 MiB / 16 B = 262144 dependent rounds per block.
+// format's limit: 4 MiB / 16 B = 262144 dependent rounds per block. The XXH64 round functions are kz_xxh64_core.cuh's.
 #include "kz_hash.cuh"
+#include "kz_xxh64_core.cuh"
 
 namespace kz {
 
 KZ_D uint32_t rotl32(uint32_t x, int r) { return __funnelshift_l(x, x, r); }
-KZ_D uint64_t rotl64(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
 
 KZ_D uint32_t ld32le(const uint8_t* p, bool aligned) {
     if (aligned) return *reinterpret_cast<const uint32_t*>(p);
@@ -25,8 +25,6 @@ KZ_D uint64_t ld64le(const uint8_t* p, bool aligned) {
 }
 
 static const uint32_t P32_1 = 2654435761u, P32_2 = 2246822519u, P32_3 = 3266489917u, P32_4 = 668265263u, P32_5 = 374761393u;
-static const uint64_t P64_1 = 11400714785074694791ull, P64_2 = 14029467366897019727ull, P64_3 = 1609587929392839161ull,
-                      P64_4 = 9650029242287828579ull, P64_5 = 2870177450012600261ull;
 
 static const int HB = 16;  // stripes per register batch
 
@@ -78,9 +76,6 @@ KZ_D uint32_t xxh32_block(const uint8_t* __restrict__ p, uint32_t len, uint32_t 
     return h;
 }
 
-KZ_D uint64_t xxh64_round(uint64_t acc, uint64_t v) { return rotl64(acc + v * P64_2, 31) * P64_1; }
-KZ_D uint64_t xxh64_merge(uint64_t h, uint64_t v) { return (h ^ xxh64_round(0, v)) * P64_1 + P64_4; }
-
 KZ_D uint64_t xxh64_block(const uint8_t* __restrict__ p, uint32_t len, uint64_t seed, int lane) {
     const bool al = (reinterpret_cast<uintptr_t>(p) & 7) == 0;
     uint32_t n = 0;
@@ -113,11 +108,7 @@ KZ_D uint64_t xxh64_block(const uint8_t* __restrict__ p, uint32_t len, uint64_t 
         }
         const uint64_t v1 = __shfl_sync(0xFFFFFFFFu, v, 0), v2 = __shfl_sync(0xFFFFFFFFu, v, 1), v3 = __shfl_sync(0xFFFFFFFFu, v, 2),
                        v4 = __shfl_sync(0xFFFFFFFFu, v, 3);
-        h = rotl64(v1, 1) + rotl64(v2, 7) + rotl64(v3, 12) + rotl64(v4, 18);
-        h = xxh64_merge(h, v1);
-        h = xxh64_merge(h, v2);
-        h = xxh64_merge(h, v3);
-        h = xxh64_merge(h, v4);
+        h = xxh64_fold(v1, v2, v3, v4);
         n = stripes << 5;
     } else {
         h = seed + P64_5;
@@ -126,12 +117,7 @@ KZ_D uint64_t xxh64_block(const uint8_t* __restrict__ p, uint32_t len, uint64_t 
     for (; n + 8 <= len; n += 8) h = rotl64(h ^ xxh64_round(0, ld64le(p + n, al)), 27) * P64_1 + P64_4;
     for (; n + 4 <= len; n += 4) h = rotl64(h ^ ((uint64_t)ld32le(p + n, (reinterpret_cast<uintptr_t>(p + n) & 3) == 0) * P64_1), 23) * P64_2 + P64_3;
     for (; n < len; n++) h = rotl64(h ^ ((uint64_t)p[n] * P64_5), 11) * P64_1;
-    h ^= h >> 33;
-    h *= P64_2;
-    h ^= h >> 29;
-    h *= P64_3;
-    h ^= h >> 32;
-    return h;
+    return xxh64_avalanche(h);
 }
 
 // one warp per block; bits = 32 or 64; seed = 0x4B414E5A ("KANZ", io/CompressedStream.go:272-276)

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "kz_stream_plan.h"
+#include "kz_xxh64_core.cuh"
 
 namespace kz {
 
@@ -32,48 +33,8 @@ struct StreamIndex {
     uint64_t nblocks() const { return start.size(); }
 };
 
-// XXH64 (Yann Collet's public algorithm), seed 0, of n bytes: the blob's trailing hash.
-inline uint64_t index_xxh64(const uint8_t* p, size_t n) {
-    const uint64_t P1 = 11400714785074694791ull, P2 = 14029467366897019727ull, P3 = 1609587929392839161ull, P4 = 9650029242287828579ull,
-                   P5 = 2870177450012600261ull;
-    auto rotl = [](uint64_t v, int r) { return (v << r) | (v >> (64 - r)); };
-    auto rd64 = [](const uint8_t* q) {
-        uint64_t v = 0;
-        for (int i = 7; i >= 0; i--) v = (v << 8) | q[i];
-        return v;
-    };
-    auto round = [&](uint64_t acc, uint64_t v) { return rotl(acc + v * P2, 31) * P1; };
-    auto merge = [&](uint64_t h, uint64_t v) { return (h ^ round(0, v)) * P1 + P4; };
-    const uint8_t* end = p + n;
-    uint64_t h;
-    if (n >= 32) {
-        uint64_t v1 = P1 + P2, v2 = P2, v3 = 0, v4 = 0 - P1;
-        for (; end - p >= 32; p += 32) {
-            v1 = round(v1, rd64(p));
-            v2 = round(v2, rd64(p + 8));
-            v3 = round(v3, rd64(p + 16));
-            v4 = round(v4, rd64(p + 24));
-        }
-        h = rotl(v1, 1) + rotl(v2, 7) + rotl(v3, 12) + rotl(v4, 18);
-        h = merge(merge(merge(merge(h, v1), v2), v3), v4);
-    } else {
-        h = P5;
-    }
-    h += (uint64_t)n;
-    for (; end - p >= 8; p += 8) h = rotl(h ^ round(0, rd64(p)), 27) * P1 + P4;
-    if (end - p >= 4) {
-        const uint64_t v = (uint64_t)p[0] | ((uint64_t)p[1] << 8) | ((uint64_t)p[2] << 16) | ((uint64_t)p[3] << 24);
-        h = rotl(h ^ (v * P1), 23) * P2 + P3;
-        p += 4;
-    }
-    for (; p < end; p++) h = rotl(h ^ (*p * P5), 11) * P1;
-    h ^= h >> 33;
-    h *= P2;
-    h ^= h >> 29;
-    h *= P3;
-    h ^= h >> 32;
-    return h;
-}
+// XXH64, seed 0, of n bytes: the blob's trailing hash.
+inline uint64_t index_xxh64(const uint8_t* p, size_t n) { return xxh64_bytes(p, n, 0); }
 
 inline void index_put(uint8_t* p, uint64_t v, int nbytes) {
     for (int i = 0; i < nbytes; i++) p[i] = (uint8_t)(v >> (8 * i));
