@@ -406,6 +406,44 @@ int kz_read_ranges_cached(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const uint
 int kz_read_ranges_cached_device(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
                                  const uint64_t* len, void* d_dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
 
+/* ---- many streams per call: index many compressed objects, and serve a batch of range reads that touches many of them, in one call
+ *      each (an object store answering a batch of GETs over thousands of small objects) ----------------------------------------------------
+ * Streams use the layout of kz_decompress_streams[_device]: stream s is src + src_off[s], src_len[s] bytes. Device variants: d_src and every
+ *   offset of a stream a call reads are multiples of 16, and at least 64 readable bytes follow each stream.
+ * Index build: out[s] and status[s] are what kz_index_build[_device] gives for stream s alone. A failed stream has out[s] = NULL and status[s]
+ *   = kz_index_build's code for those bytes (a bad header, version or block size, a record past the end, truncation, -KZ_ERR_CREATE_CODEC
+ *   for a chain or codec the GPU path lacks). The headerless reader setting applies to every stream. The headers are gathered by one copy
+ *   launch and brought back in one transfer; all streams are walked by the two walk launches of one kz_index_build. Call-level failures
+ *   (a bad argument, misalignment, an open session, CUDA or allocation errors) set every status and every out[s] = NULL. The return value
+ *   is 0, the call-level code, or the first failing stream's code. Free every index that is not NULL with kz_index_free.
+ * Reads: request i reads [off[i], off[i] + len[i]) of stream req_stream[i] with index ix[req_stream[i]]; cache may be NULL (uncached). Its
+ *   bytes at dst + dst_off[i], out_len[i] and status[i] are exactly what kz_read_ranges[_cached][_device] returns for it when called with
+ *   that index, that stream, the same cache and only that stream's requests; each index's size is updated as that call updates it. pread
+ *   semantics, guards around destinations, the unseekable rule and per-block errors apply per stream.
+ *   What fails a whole kz_read_ranges call fails only one stream here: a NULL ix[s], a stale index (length or first 32 bytes differ) and
+ *   a chain or codec the GPU path lacks fail the requests on stream s with the code kz_read_ranges returns; the other streams are served.
+ *   Call-level failures set every status and are the return value: a bad argument, req_stream[i] >= nstreams, misalignment in the device
+ *   variant, an open session, a cache of another context, CUDA and allocation failures. Otherwise the return value is 0 or the first
+ *   failing request's code. Streams no request names are neither checked nor read, so a caller can pass its whole object table. The same
+ *   kz_index* may sit in several slots; each slot is checked against its own bytes.
+ * Work: each distinct (stream slot, block) the requests touch is decoded at most once, and not at all when the cache holds it. Blocks of
+ *   streams with the same transform48, entropy, block_size and checksum_bits share decode passes; blocks of different ones never do. Kernel
+ *   launches and synchronisations follow the passes, not the number of streams: the device variant gathers the first 32 bytes of every
+ *   named stream with one copy launch and one transfer. Cache lookups and inserts run in plan order (group of decode fields in order of
+ *   first appearance, then stream slot, then block). Memory: what a kz_read_ranges pass takes, plus in the host variant the record windows
+ *   of one pass across all of its streams. With kz_profile(ctx,1) the "read:*" counters count the call once, as one kz_read_ranges. */
+int kz_index_build_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out,
+                           int32_t* status);
+int kz_index_build_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out,
+                                  int32_t* status);
+int kz_read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const uint8_t* src, const uint64_t* src_off,
+                           const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, uint8_t* dst,
+                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+/* d_dst and dst_off need no alignment; every array is a host array. */
+int kz_read_ranges_streams_device(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
+                                  const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, void* d_dst,
+                                  const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+
 #ifdef __cplusplus
 }
 #endif

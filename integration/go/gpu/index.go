@@ -195,3 +195,123 @@ func (k *Cache) Free() {
 	C.kz_cache_free(k.h)
 	k.h = nil
 }
+
+// BuildIndexes indexes many streams in one kz_index_build_streams call: index i is what BuildIndex(streams[i]) gives. A stream that
+// fails has a nil index and its error in errs[i]; the returned error is a failure of the call as a whole (a session open on c).
+func (c *Context) BuildIndexes(streams [][]byte) (idx []*Index, errs []error, err error) {
+	n := len(streams)
+	idx, errs = make([]*Index, n), make([]error, n)
+	if n == 0 {
+		return idx, errs, nil
+	}
+	off := make([]C.uint64_t, n)
+	ln := make([]C.uint64_t, n)
+	total := 0
+	for i, s := range streams {
+		off[i], ln[i] = C.uint64_t(total), C.uint64_t(len(s))
+		total += len(s)
+	}
+	buf := make([]byte, total+1) // cgo must not see pointers into several Go slices: one buffer
+	for i, s := range streams {
+		copy(buf[int(off[i]):], s)
+	}
+	hs := make([]*C.kz_index, n)
+	status := make([]C.int32_t, n)
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_index_build_streams(c.h, C.uint32_t(n), (*C.uint8_t)(unsafe.Pointer(&buf[0])), &off[0], &ln[0], &hs[0], &status[0])
+	if rc == -C.KZ_ERR_INVALID_PARAM { // no stream fails with this code: the call failed as a whole
+		return idx, errs, c.err(rc)
+	}
+	for i := range streams {
+		if hs[i] != nil {
+			idx[i] = &Index{h: hs[i]}
+		} else {
+			errs[i] = &StreamError{Code: int(-status[i])}
+		}
+	}
+	return idx, errs, nil
+}
+
+// StreamRange is one request of ReadRangesStreams: a Range of stream Stream, an index into the streams and indexes of the call.
+type StreamRange struct {
+	Stream int
+	Range
+}
+
+// ReadRangesStreams serves requests on many streams in one kz_read_ranges_streams call, through the block cache k when it is not nil.
+// Each request gets what ReadRanges (or ReadRangesCached) gives it on its own stream. A nil or stale index, or a chain the GPU path
+// lacks, fails only the requests on that stream; streams no request names are not read, so callers may pass their whole object table.
+// The returned error is a failure of the call as a whole (a request on a stream out of range, a session open on c, a cache of another
+// context); every request then holds it too.
+func (c *Context) ReadRangesStreams(k *Cache, idx []*Index, streams [][]byte, reqs []StreamRange) error {
+	n, ns := len(reqs), len(streams)
+	if n == 0 {
+		return nil
+	}
+	if len(idx) != ns {
+		return errors.New("gpu: one index per stream")
+	}
+	named := make([]bool, ns)
+	for _, r := range reqs {
+		if r.Stream < 0 || r.Stream >= ns {
+			return errors.New("gpu: request on a stream out of range")
+		}
+		named[r.Stream] = true
+	}
+	srcOff := make([]C.uint64_t, ns)
+	srcLen := make([]C.uint64_t, ns)
+	hs := make([]*C.kz_index, ns)
+	total := 0
+	for s, b := range streams {
+		if idx[s] != nil {
+			hs[s] = idx[s].h
+		}
+		if named[s] { // only the named streams are copied: the others are neither checked nor read
+			srcOff[s], srcLen[s] = C.uint64_t(total), C.uint64_t(len(b))
+			total += len(b)
+		}
+	}
+	src := make([]byte, total+1)
+	for s, b := range streams {
+		if named[s] {
+			copy(src[int(srcOff[s]):], b)
+		}
+	}
+	rs := make([]C.uint32_t, n)
+	off := make([]C.uint64_t, n)
+	ln := make([]C.uint64_t, n)
+	dstOff := make([]C.uint64_t, n)
+	outLen := make([]C.uint64_t, n)
+	status := make([]C.int32_t, n)
+	dtotal := uint64(0)
+	for i, r := range reqs {
+		rs[i], off[i], ln[i], dstOff[i] = C.uint32_t(r.Stream), C.uint64_t(r.Off), C.uint64_t(len(r.Dst)), C.uint64_t(dtotal)
+		dtotal += uint64(len(r.Dst))
+	}
+	dst := make([]byte, dtotal+1)
+	var kh *C.kz_cache
+	if k != nil {
+		kh = k.h
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_read_ranges_streams(c.h, kh, C.uint32_t(ns), &hs[0], (*C.uint8_t)(unsafe.Pointer(&src[0])), &srcOff[0], &srcLen[0], C.uint32_t(n), &rs[0],
+		&off[0], &ln[0], (*C.uint8_t)(unsafe.Pointer(&dst[0])), &dstOff[0], &outLen[0], &status[0])
+	whole := rc != 0
+	for i := range reqs {
+		reqs[i].N, reqs[i].Err = int(outLen[i]), nil
+		if status[i] != rc {
+			whole = false
+		}
+		if status[i] != 0 {
+			reqs[i].Err = &StreamError{Code: int(-status[i])}
+			continue
+		}
+		copy(reqs[i].Dst, dst[uint64(dstOff[i]):uint64(dstOff[i])+uint64(outLen[i])])
+	}
+	if whole && rc == -C.KZ_ERR_INVALID_PARAM {
+		return c.err(rc)
+	}
+	return nil
+}

@@ -43,7 +43,8 @@ ABI_SYMBOLS = [
     "kz_set_headerless_writer", "kz_set_headerless_reader", "kz_clear_headerless_reader", "kz_set_skip_blocks",
     "kz_index_build", "kz_index_build_device", "kz_index_info", "kz_index_save", "kz_index_load", "kz_index_free", "kz_read_ranges",
     "kz_read_ranges_device", "kz_cache_create", "kz_cache_free", "kz_cache_clear", "kz_cache_stats", "kz_read_ranges_cached",
-    "kz_read_ranges_cached_device",
+    "kz_read_ranges_cached_device", "kz_index_build_streams", "kz_index_build_streams_device", "kz_read_ranges_streams",
+    "kz_read_ranges_streams_device",
 ]
 
 
@@ -182,6 +183,10 @@ def load_library(build_if_missing=True):
     L.kz_cache_stats.argtypes = [vp] + [C.POINTER(u64)] * 8
     L.kz_read_ranges_cached.argtypes = [vp, vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
     L.kz_read_ranges_cached_device.argtypes = [vp, vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, vp]
+    L.kz_index_build_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp]
+    L.kz_index_build_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, vp]
+    L.kz_read_ranges_streams.argtypes = [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_read_ranges_streams_device.argtypes = [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -562,6 +567,60 @@ class Context:
         with self._headerless(reader=headerless):
             self._check(self.lib.kz_index_build_device(self.h, _dptr(d_src), n, C.byref(h)))
         return StreamIndex(h, self)
+
+    # ---- many streams per call (kz_index_build_streams / kz_read_ranges_streams): an object store's table of small objects ----------
+    # Per-stream and per-request failures do not raise: status[s] / status[i] = 0 or -(kanzi error code).
+    def index_streams(self, streams, headerless=None):
+        """One StreamIndex per host stream, each what index(streams[s]) gives -> (indexes, status); indexes[s] is None when stream s failed."""
+        arrs = [_u8(x) for x in streams]
+        src_len = np.array([a.size for a in arrs], np.uint64)
+        src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
+        return self._index_streams(self.lib.kz_index_build_streams, _p(src), _offsets(src_len), src_len, headerless)
+
+    def index_streams_device(self, d_src, src_off, src_len, headerless=None):
+        """index_streams of the streams d_src[src_off[s] : + src_len[s]] (16-byte aligned, >= 64 readable bytes behind each)."""
+        so, sl = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len))
+        return self._index_streams(self.lib.kz_index_build_streams_device, _dptr(d_src), so, sl, headerless)
+
+    def _index_streams(self, fn, src, so, sl, headerless):
+        n = len(sl)
+        hs = (C.c_void_p * max(n, 1))()
+        status = np.zeros(n, np.int32)
+        with self._headerless(reader=headerless):
+            fn(self.h, n, src, _p(so), _p(sl), C.addressof(hs), _p(status))
+        return [StreamIndex(hs[s], self) if hs[s] else None for s in range(n)], status
+
+    @staticmethod
+    def _index_slots(indexes):
+        return (C.c_void_p * max(len(indexes), 1))(*[None if x is None else x.h for x in indexes])
+
+    def read_streams(self, streams, indexes, requests, cache=None):
+        """requests: [(stream_no, off, length), ...] on host streams with their indexes (None allowed) -> (list of bytes, status list):
+        each request gets what indexes[stream_no].read_many(streams[stream_no], ...) gives it, in one call over all streams."""
+        arrs = [_u8(x) for x in streams]
+        src_len = np.array([a.size for a in arrs], np.uint64)
+        src_off = _offsets(src_len)
+        src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
+        ix = self._index_slots(indexes)
+        rs = np.array([r[0] for r in requests], np.uint32)
+        off = np.array([r[1] for r in requests], np.uint64)
+        ln = np.array([r[2] for r in requests], np.uint64)
+        dst_off = _offsets(ln)
+        dst = np.empty(max(int(ln.sum()), 1), np.uint8)
+        out_len, status = np.zeros(len(requests), np.uint64), np.zeros(len(requests), np.int32)
+        self.lib.kz_read_ranges_streams(self.h, None if cache is None else cache.h, len(arrs), C.addressof(ix), _p(src), _p(src_off), _p(src_len),
+                                        len(requests), _p(rs), _p(off), _p(ln), dst.ctypes.data, _p(dst_off), _p(out_len), _p(status))
+        return [dst[int(o): int(o) + int(n)].tobytes() for o, n in zip(dst_off, out_len)], status.tolist()
+
+    def read_streams_device(self, d_src, src_off, src_len, indexes, req_stream, off, length, d_dst, dst_off, cache=None):
+        """Device-resident read_streams: d_src / d_dst are CUDA tensors or addresses, the rest host sequences -> (out_len, status)."""
+        so, sl, o, ln, do = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, off, length, dst_off))
+        rs = np.ascontiguousarray(req_stream, np.uint32)
+        ix = self._index_slots(indexes)
+        out_len, status = np.zeros(len(o), np.uint64), np.zeros(len(o), np.int32)
+        self.lib.kz_read_ranges_streams_device(self.h, None if cache is None else cache.h, len(sl), C.addressof(ix), _dptr(d_src), _p(so), _p(sl), len(o),
+                                               _p(rs), _p(o), _p(ln), _dptr(d_dst), _p(do), _p(out_len), _p(status))
+        return out_len, status
 
     def block_cache(self, budget):
         """A BlockCache of decoded blocks in `budget` bytes of HBM (kz_cache_create), for StreamIndex.read / read_many /

@@ -2837,25 +2837,37 @@ StreamHeader index_header(const kz_index& ix) {
     return sh;
 }
 
-// The stream bytes of one read pass as decode_walked sees them: the device stream itself, or the packed windows of the host variant.
+// One stream of a read: its index, where its bytes start (src + at in the host variant, d_src + at, a multiple of 16, in the device
+// variant) and how many there are.
+struct ReadSource {
+    kz_index* ix;
+    uint64_t at, n;
+};
+
+// The stream bytes of one read pass as decode_walked sees them: the device streams themselves, or the packed windows of the host variant.
 struct PassInput {
     const uint32_t* d_words = nullptr;
     uint64_t words_len = 0;
-    std::vector<uint64_t> bit_off;  // per block of the pass: its record's first payload bit in d_words
 };
 
-// Host variant: uploads only the byte windows that hold the records of blocks ks: each starts at a multiple of 16 and carries the 64
-// bytes the decoders may read behind a record (zeros where the stream ends); windows that meet are merged. One transfer per pass.
-int upload_windows(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const uint64_t* ks, uint32_t nk, PassInput& in) {
+// Host variant: uploads only the byte windows that hold the records of pairs ks (plan order: stream after stream, blocks ascending): each
+// starts at a multiple of 16 and carries the 64 bytes the decoders may read behind a record (zeros where its stream ends); windows of one
+// stream that meet are merged. One transfer per pass. bit_off[k]: the first payload bit of pair k's record in the packed buffer.
+int upload_windows(kz_ctx* ctx, const std::vector<ReadSource>& S, const ReadPlan& P, const uint8_t* src, const std::vector<uint32_t>& ks,
+                   std::vector<uint64_t>& bit_off, PassInput& in) {
     struct Window {
-        uint64_t lo, hi, at;  // stream bytes [lo, hi) at packed offset `at`
+        uint32_t s;
+        uint64_t lo, hi, at;  // bytes [lo, hi) of stream s at packed offset `at`
     };
     std::vector<Window> win;
-    std::vector<uint32_t> win_of(nk);
+    std::vector<uint32_t> win_of(ks.size());
     uint64_t total = 0;
-    for (uint32_t i = 0; i < nk; i++) {
-        const uint64_t lo = (ix.start[ks[i]] / 8) & ~15ull, hi = (ix.start[ks[i]] + ix.bits[ks[i]] + 7) / 8 + 64;
-        if (win.empty() || lo > win.back().hi) win.push_back(Window{lo, hi, 0});
+    for (size_t i = 0; i < ks.size(); i++) {
+        const uint32_t s = P.stream[ks[i]];
+        const kz_index& ix = *S[s].ix;
+        const uint64_t b = P.blocks[ks[i]];
+        const uint64_t lo = (ix.start[b] / 8) & ~15ull, hi = (ix.start[b] + ix.bits[b] + 7) / 8 + 64;
+        if (win.empty() || win.back().s != s || lo > win.back().hi) win.push_back(Window{s, lo, hi, 0});
         else win.back().hi = std::max(win.back().hi, hi);
         win_of[i] = (uint32_t)win.size() - 1;
     }
@@ -2863,12 +2875,14 @@ int upload_windows(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const ui
     CK(ctx->h_io.ensure(total + 64));
     CK(ctx->d_in.ensure(total + 128));
     memset(ctx->h_io.p, 0, total);
-    for (const Window& w : win) memcpy((uint8_t*)ctx->h_io.p + w.at, src + w.lo, std::min<uint64_t>(w.hi, ix.stream_bytes) - w.lo);
+    for (const Window& w : win) memcpy((uint8_t*)ctx->h_io.p + w.at, src + S[w.s].at + w.lo, std::min<uint64_t>(w.hi, S[w.s].n) - w.lo);
     CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
     in.d_words = ctx->d_in.as<uint32_t>();
     in.words_len = (total + 3) / 4 + 16;
-    in.bit_off.resize(nk);
-    for (uint32_t i = 0; i < nk; i++) in.bit_off[i] = ix.start[ks[i]] - 8 * win[win_of[i]].lo + 8 * win[win_of[i]].at;
+    for (size_t i = 0; i < ks.size(); i++) {
+        const Window& w = win[win_of[i]];
+        bit_off[ks[i]] = S[w.s].ix->start[P.blocks[ks[i]]] - 8 * w.lo + 8 * w.at;
+    }
     if (ctx->profile) {
         auto& e = ctx->prof["read:h2d"];
         e.bytes_in += win.size(), e.bytes_out += total, e.launches++;
@@ -2876,31 +2890,36 @@ int upload_windows(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const ui
     return 0;
 }
 
-// The keys of the cached read's blocks (P.blocks): the record hash of every record (kz_xxh64_core.cuh) and the header fields a record's
-// decode depends on. Host variant: hashed on the CPU from the caller's stream. Device variant: one record_hash launch over every tile of
-// the records, one thread per record for the roots, one copy of the keys back.
-int cache_keys(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const uint8_t* d_src, const std::vector<uint64_t>& blocks, std::vector<CacheKey>& key) {
-    const uint32_t nk = (uint32_t)blocks.size();
+// The keys of the cached read's pairs: the record hash of every record (kz_xxh64_core.cuh) and the header fields a record's decode
+// depends on. Host variant: hashed on the CPU from the caller's streams. Device variant: one record_hash launch over every tile of the
+// records of every stream, one thread per record for the roots, one copy of the keys back.
+int cache_keys(kz_ctx* ctx, const std::vector<ReadSource>& S, const ReadPlan& P, const uint8_t* src, const uint8_t* d_src, std::vector<CacheKey>& key) {
+    const uint32_t nk = (uint32_t)P.blocks.size();
     key.assign(nk, CacheKey());
     for (uint32_t k = 0; k < nk; k++) {
-        key[k].bits = ix.bits[blocks[k]];
+        const kz_index& ix = *S[P.stream[k]].ix;
+        key[k].bits = ix.bits[P.blocks[k]];
         key[k].t48 = ix.t48;
         key[k].etype = ix.etype;
         key[k].checksum_bits = ix.checksum_bits;
         key[k].block_size = ix.block_size;
-        key[k].last = blocks[k] + 1 == ix.nblocks();
+        key[k].last = P.blocks[k] + 1 == ix.nblocks();
     }
     if (nk == 0) return 0;
     if (src) {
         HostScope hs(ctx, "record_hash");
-        for (uint32_t k = 0; k < nk; k++) key[k].hash = record_hash_host(src, ix.start[blocks[k]], ix.bits[blocks[k]]);
+        for (uint32_t k = 0; k < nk; k++) {
+            const ReadSource& r = S[P.stream[k]];
+            key[k].hash = record_hash_host(src + r.at, r.ix->start[P.blocks[k]], r.ix->bits[P.blocks[k]]);
+        }
         return 0;
     }
     std::vector<RecordHashJob> jobs(nk);
     uint64_t ntiles = 0;
     for (uint32_t k = 0; k < nk; k++) {
-        jobs[k] = RecordHashJob{ix.start[blocks[k]], ix.bits[blocks[k]], ntiles};
-        ntiles += record_tiles(ix.bits[blocks[k]]);
+        const ReadSource& r = S[P.stream[k]];
+        jobs[k] = RecordHashJob{8 * r.at + r.ix->start[P.blocks[k]], r.ix->bits[P.blocks[k]], ntiles};
+        ntiles += record_tiles(r.ix->bits[P.blocks[k]]);
     }
     Packer pk;
     const size_t o_j = pk.add(jobs.data(), jobs.size() * sizeof(RecordHashJob));
@@ -2927,51 +2946,55 @@ int cache_keys(kz_ctx* ctx, const kz_index& ix, const uint8_t* src, const uint8_
     return 0;
 }
 
-// One batched read. src is the host stream (host variant: dst is host memory too) or null (d_src is the stream, dst device memory).
+// One batched read over the streams S, every one already checked against its index (read_stream_check). src is the host buffer the
+// streams lie in (host variant: dst is host memory too) or null (d_src holds them, dst is device memory). Request i reads stream
+// req_src[i] (null: every request reads S[0]).
 // cache: null, or the block cache of a cached read. With a cache the blocks found in it form a pass of their own, served first by one
 // copy launch out of its pages; the others (the misses) run through the decode passes as every block does without a cache, and each
 // that decodes is inserted behind its pass.
-int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nreq,
-                     const uint64_t* off, const uint64_t* len, uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+// Every rule that makes a one-stream read's results holds per stream: a pair's pass is cut from its decode group only, the unseekable rule
+// is kept per stream, and a failed block of a pass of several is decoded again alone. So what a request gets does not depend on which
+// other streams share the call.
+int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uint8_t* d_src, const std::vector<ReadSource>& S, uint32_t nreq,
+                     const uint32_t* req_src, const uint64_t* off, const uint64_t* len, uint8_t* dst, const uint64_t* dst_off, uint64_t* out_len,
+                     int32_t* status) {
     const bool host = src != nullptr;
-    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
-    if (cache && cache->ctx != ctx) return ctx->fail(KZ_ERR_INVALID_PARAM, "the block cache belongs to another context");
-    for (uint32_t i = 0; i < nreq; i++) {
-        if (dst_off[i] + len[i] < dst_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
-        if (len[i] && !dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    const uint32_t ns = (uint32_t)S.size();
+    // decode groups, numbered in the order they first appear: the header and transform plan of each
+    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, uint32_t> group_of;
+    std::vector<StreamHeader> gsh;
+    std::vector<TransformPlan> gplan;
+    std::vector<ReadStream> RS(ns);
+    uint64_t src_end = 0;
+    int rc = 0;
+    for (uint32_t s = 0; s < ns; s++) {
+        const kz_index& ix = *S[s].ix;
+        auto it = group_of.find(std::make_tuple(ix.t48, ix.etype, ix.block_size, ix.checksum_bits));
+        if (it == group_of.end()) {
+            it = group_of.emplace(std::make_tuple(ix.t48, ix.etype, ix.block_size, ix.checksum_bits), (uint32_t)gsh.size()).first;
+            gsh.push_back(index_header(ix));
+            gplan.emplace_back();
+            rc = plan_transforms(ctx, ix.t48, ix.etype, gplan.back(), KZ_ERR_CREATE_CODEC);
+            if (rc) return rc;
+        }
+        RS[s] = ReadStream{ix.nblocks(), ix.block_size, ix.size, it->second};
+        src_end = std::max(src_end, S[s].at + S[s].n);
     }
-    if (!host && ((uintptr_t)d_src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    // the stream the index was built from: its length and its leading bytes
-    uint8_t head[INDEX_HEAD] = {0};
-    const size_t nh = std::min<size_t>(n, INDEX_HEAD);
-    if (n != ix->stream_bytes) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from a stream of another length");
-    if (host) memcpy(head, src, nh);
-    else if (nh) {
-        CK(cudaMemcpyAsync(head, d_src, nh, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    if (memcmp(head, ix->head, INDEX_HEAD)) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from another stream");
-    const StreamHeader sh = index_header(*ix);
-    TransformPlan plan;
-    int rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_CREATE_CODEC);
-    if (rc) return rc;
-    if (!etype_supported(sh.etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
-
-    const uint32_t bs = sh.block_size;
-    const uint64_t nblocks = ix->nblocks();
-    const ReadPlan P = plan_reads(nblocks, bs, ix->size, nreq, off, len);
+    const ReadPlan P = plan_reads_streams(RS, nreq, req_src, off, len);
     const uint32_t nk = (uint32_t)P.blocks.size();
-    // The blocks to decode, pass after pass: order[first[p] .. first[p + 1]) (ascending). Without a cache every touched block; with
-    // one the blocks it lacks (hit[k] names the entry of the others).
+    auto IX = [&](uint32_t k) -> kz_index& { return *S[P.stream[k]].ix; };
+    auto is_last = [&](uint32_t k) { return P.blocks[k] + 1 == IX(k).nblocks(); };
+    // The pairs to decode, pass after pass: order[first[p] .. first[p + 1]) (in plan order). Without a cache every touched pair; with
+    // one the pairs it lacks (hit[k] names the entry of the others).
     std::vector<CacheKey> key;
     std::vector<const CacheEntry*> hit(cache ? nk : 0, nullptr);
     std::vector<uint32_t> order, first;
     if (cache) {
-        rc = cache_keys(ctx, *ix, src, d_src, P.blocks, key);
+        rc = cache_keys(ctx, S, P, src, d_src, key);
         if (rc) return rc;
         for (uint32_t k = 0; k < nk; k++)
             if (!(hit[k] = cache->pc.lookup(key[k]))) order.push_back(k);
-        first = plan_decompress_passes((uint32_t)order.size(), decompress_slot(bs), read_block_cost(bs)).first;
+        first = plan_read_passes(RS, P.stream, order);
     } else {
         order.resize(nk);
         std::iota(order.begin(), order.end(), 0u);
@@ -2981,10 +3004,11 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
     const uint32_t hp = cache ? 1 : 0;  // the pass number of the first decode pass (the cache's blocks are pass 0)
     // A request is staged (its slices gathered in ctx->d_asm, delivered when every block it touches has decoded) when it goes to host
     // memory or its blocks lie in more than one pass: nothing is written for a request that fails. A request on cached blocks only is
-    // staged too when one of them lies behind a block still to decode, whose length may make it unseekable.
-    std::vector<uint32_t> pass_of(nk, 0), slot_of(nk, 0);
+    // staged too when one of them lies behind a block of its stream still to decode, whose length may make it unseekable.
+    std::vector<uint32_t> pass_of(nk, 0), slot_of(nk, 0), first_miss(ns, nk);
     for (uint32_t p = 0; p < npasses; p++)
         for (uint32_t i = first[p]; i < first[p + 1]; i++) pass_of[order[i]] = hp + p, slot_of[order[i]] = i - first[p];
+    for (uint32_t k : order) first_miss[P.stream[k]] = std::min(first_miss[P.stream[k]], k);
     std::vector<uint32_t> first_pass(nreq, 0);
     std::vector<uint8_t> staged(nreq, host);
     for (uint32_t k = 0; k < nk; k++)
@@ -2993,19 +3017,20 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
             if (sl.at == 0) first_pass[sl.req] = pass_of[k];
         }
     for (const ReadSlice& sl : P.slices)
-        if (pass_of[sl.block] != first_pass[sl.req] || (cache && hit[sl.block] && !order.empty() && sl.block > order[0])) staged[sl.req] = 1;
+        if (pass_of[sl.block] != first_pass[sl.req] || (cache && hit[sl.block] && sl.block > first_miss[P.stream[sl.block]])) staged[sl.req] = 1;
     std::vector<uint64_t> stage_at(nreq, 0);
     uint64_t stage_total = 0;
     for (uint32_t i = 0; i < nreq; i++)
         if (staged[i]) stage_at[i] = stage_total, stage_total += P.want[i];
     if (stage_total) CK(ctx->d_asm.ensure(stage_total + 64));
-    const uint64_t astride = decompress_slot(bs);
 
     std::vector<int32_t> blk_status(nk, 0);
     std::vector<uint32_t> blk_len(nk, 0);
     std::vector<uint8_t> too_long(nk, 0);
+    std::vector<uint64_t> bit_off(nk, 0);
     for (uint32_t i = 0; i < nreq; i++) status[i] = 0, out_len[i] = 0;
-    uint32_t unseekable = nk;  // the first touched block whose length breaks the block arithmetic
+    std::vector<uint32_t> uns(ns, nk);  // per stream: its first touched pair whose length breaks the block arithmetic
+    auto broken = [&](uint32_t k) { return k >= uns[P.stream[k]]; };
     uint64_t dec_blocks = 0, dec_bytes = 0, out_slices = 0, out_bytes = 0;
     uint8_t* pages = cache ? (uint8_t*)cache->d_pages : nullptr;
     bool hit_copies = false;  // the copies out of the cache were queued; the call returns only after they ran
@@ -3016,16 +3041,16 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
         for (uint32_t k = 0; k < nk; k++)
             if (hit[k]) {
                 blk_len[k] = hit[k]->len;
-                if (P.blocks[k] + 1 == nblocks ? blk_len[k] == 0 : blk_len[k] != bs) unseekable = std::min(unseekable, k);
+                if (is_last(k) ? blk_len[k] == 0 : blk_len[k] != IX(k).block_size) uns[P.stream[k]] = std::min(uns[P.stream[k]], k);
                 hits++, hit_bytes += blk_len[k];
             }
-        for (uint32_t k = unseekable; k < nk; k++)
-            if (hit[k])
+        for (uint32_t k = 0; k < nk; k++)
+            if (hit[k] && broken(k))
                 for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
                     if (!staged[P.slices[s].req]) status[P.slices[s].req] = -KZ_ERR_INVALID_FILE;
         CopyList out;
-        for (uint32_t k = 0; k < std::min(unseekable, nk); k++) {
-            if (!hit[k]) continue;
+        for (uint32_t k = 0; k < nk; k++) {
+            if (!hit[k] || broken(k)) continue;
             for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++) {
                 const ReadSlice& sl = P.slices[s];
                 if (status[sl.req] || sl.in_block >= blk_len[k]) continue;
@@ -3049,32 +3074,44 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
     }
     const CacheStats before = cache ? cache->pc.stats() : CacheStats();
     uint64_t miss_blocks = 0, miss_bytes = 0, ins_bytes = 0;
-    for (uint32_t p = 0; p < npasses && order[first[p]] < unseekable; p++) {
+    for (uint32_t p = 0; p < npasses; p++) {
         const uint32_t a = first[p], e = first[p + 1];
-        std::vector<uint64_t> pass_blocks(e - a);
-        for (uint32_t i = a; i < e; i++) pass_blocks[i - a] = P.blocks[order[i]];
+        // a stream's blocks of the pass are decoded when its first one there lies before its unseekable block, as a one-stream read
+        // decodes a pass whose first block does
+        std::vector<uint32_t> ks;
+        bool take = false;
+        for (uint32_t i = a; i < e; i++) {
+            const uint32_t k = order[i];
+            if (i == a || P.stream[k] != P.stream[order[i - 1]]) take = !broken(k);
+            if (take) ks.push_back(k);
+        }
+        if (ks.empty()) continue;
+        const StreamHeader& sh = gsh[RS[P.stream[ks[0]]].group];
+        const TransformPlan& plan = gplan[RS[P.stream[ks[0]]].group];
+        const uint32_t bs = sh.block_size;
+        const uint64_t astride = decompress_slot(bs);
         PassInput in;
         if (host) {
-            rc = upload_windows(ctx, *ix, src, pass_blocks.data(), e - a, in);
+            rc = upload_windows(ctx, S, P, src, ks, bit_off, in);
             if (rc) return rc;
         } else {
             in.d_words = (const uint32_t*)d_src;
-            in.words_len = (n + 3) / 4 + 16;
-            for (uint64_t b : pass_blocks) in.bit_off.push_back(ix->start[b]);
+            in.words_len = (src_end + 3) / 4 + 16;
+            for (uint32_t k : ks) bit_off[k] = 8 * S[P.stream[k]].at + IX(k).start[P.blocks[k]];
         }
         CK(ctx->d_slots.ensure(astride * (e - a) + 64));
         uint8_t* arena = ctx->d_slots.as<uint8_t>();
-        // decodes blocks ks of the pass into their arena slots, one DecodeFailure per block
+        // decodes pairs ks of the pass into their arena slots, one DecodeFailure per block
         auto decode = [&](const std::vector<uint32_t>& ks) -> int {
             std::vector<DecJob> jobs(ks.size(), DecJob());
             std::vector<uint32_t> owner(ks.size());
             std::vector<uint8_t> last(ks.size());
             std::vector<DecodeFailure> fail(ks.size());
             for (size_t i = 0; i < ks.size(); i++) {
-                jobs[i].bit_off = in.bit_off[slot_of[ks[i]]];
-                jobs[i].bits = ix->bits[P.blocks[ks[i]]];
+                jobs[i].bit_off = bit_off[ks[i]];
+                jobs[i].bits = IX(ks[i]).bits[P.blocks[ks[i]]];
                 owner[i] = (uint32_t)i;
-                last[i] = P.blocks[ks[i]] + 1 == nblocks;
+                last[i] = is_last(ks[i]);
                 too_long[ks[i]] = 0;
             }
             auto place = [&](uint32_t i, uint32_t n_out) {
@@ -3090,25 +3127,24 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
             for (size_t i = 0; i < ks.size(); i++) blk_status[ks[i]] = fail[i].failed() ? fail[i].code : 0;
             return 0;
         };
-        const std::vector<uint32_t> ks(order.begin() + a, order.begin() + e);
         rc = decode(ks);
         if (rc) return rc;
         // A failing stage call cannot name its block, and a failure of one block may hide a later one's: every failed block of a pass
         // of several is decoded again alone, so that its status is the one a decode of that block alone gives. Only corrupt input pays.
-        if (e - a > 1)
+        if (ks.size() > 1)
             for (uint32_t k : ks)
                 if (blk_status[k] && !too_long[k]) {
                     rc = decode(std::vector<uint32_t>{k});
                     if (rc) return rc;
                 }
         for (uint32_t k : ks) {
-            const bool is_last = P.blocks[k] + 1 == nblocks;
-            if (too_long[k] || (!blk_status[k] && (is_last ? blk_len[k] == 0 : blk_len[k] != bs))) unseekable = std::min(unseekable, k);
+            const uint32_t s = P.stream[k];
+            if (too_long[k] || (!blk_status[k] && (is_last(k) ? blk_len[k] == 0 : blk_len[k] != bs))) uns[s] = std::min(uns[s], k);
             if (!blk_status[k]) dec_blocks++, dec_bytes += blk_len[k];
-            if (is_last && !blk_status[k] && unseekable == nk) ix->size = (int64_t)((nblocks - 1) * bs + blk_len[k]);
+            if (is_last(k) && !blk_status[k] && uns[s] == nk) IX(k).size = (int64_t)((IX(k).nblocks() - 1) * bs + blk_len[k]);
         }
         // every block of the pass that decoded goes into the cache; an entry this pass made and evicted again gets no copy
-        std::vector<std::pair<uint32_t, uint64_t>> fresh;  // (block, serial)
+        std::vector<std::pair<uint32_t, uint64_t>> fresh;  // (pair, serial)
         if (cache)
             for (uint32_t k : ks) {
                 miss_blocks++, miss_bytes += blk_status[k] || too_long[k] ? 0 : blk_len[k];
@@ -3118,7 +3154,7 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
                 if (made) fresh.push_back({k, en->serial}), ins_bytes += blk_len[k];
             }
         for (uint32_t k : ks) {
-            if (k >= unseekable) blk_status[k] = -KZ_ERR_INVALID_FILE;
+            if (broken(k)) blk_status[k] = -KZ_ERR_INVALID_FILE;
             if (blk_status[k])
                 for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
                     if (!status[P.slices[s].req]) status[P.slices[s].req] = blk_status[k];
@@ -3145,8 +3181,8 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
     }
     if (cache) {
         // a cached last block sets the size as a decoded one does
-        const uint32_t k = nk ? nk - 1 : 0;
-        if (nk && hit[k] && P.blocks[k] + 1 == nblocks && unseekable == nk) ix->size = (int64_t)((nblocks - 1) * bs + blk_len[k]);
+        for (uint32_t k = 0; k < nk; k++)
+            if (hit[k] && is_last(k) && uns[P.stream[k]] == nk) IX(k).size = (int64_t)((IX(k).nblocks() - 1) * IX(k).block_size + blk_len[k]);
         if (ctx->profile) {
             const CacheStats& after = cache->pc.stats();
             auto& m = ctx->prof["read:cache_miss"];
@@ -3157,11 +3193,12 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
             v.bytes_in += after.evictions - before.evictions, v.bytes_out += before.resident + ins_bytes - after.resident, v.launches++;
         }
     }
-    if (unseekable != nk) {
+    if (std::any_of(uns.begin(), uns.end(), [&](uint32_t u) { return u != nk; })) {
         ctx->err = "Invalid bitstream: a block before the last is not block_size bytes long";
-        for (uint32_t k = unseekable; k < nk; k++)
-            for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
-                if (!status[P.slices[s].req]) status[P.slices[s].req] = -KZ_ERR_INVALID_FILE;
+        for (uint32_t k = 0; k < nk; k++)
+            if (broken(k))
+                for (uint64_t s = P.slice_of[k]; s < P.slice_of[k + 1]; s++)
+                    if (!status[P.slices[s].req]) status[P.slices[s].req] = -KZ_ERR_INVALID_FILE;
     }
     for (uint32_t i = 0; i < nreq; i++)
         if (status[i]) out_len[i] = 0;
@@ -3192,14 +3229,227 @@ int read_ranges_impl(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* 
     return 0;
 }
 
+// The call-level checks of every read: no open session, the cache (if any) of this context, destinations that do not overflow.
+int read_call_checks(kz_ctx* ctx, kz_cache* cache, uint32_t nreq, const uint64_t* len, const void* dst, const uint64_t* dst_off) {
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    if (cache && cache->ctx != ctx) return ctx->fail(KZ_ERR_INVALID_PARAM, "the block cache belongs to another context");
+    for (uint32_t i = 0; i < nreq; i++) {
+        if (dst_off[i] + len[i] < dst_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+        if (len[i] && !dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    }
+    return 0;
+}
+
+// Whether a stream of n bytes whose first min(n, 32) bytes are head (zero padded) is the one ix was built from, and whether the GPU path
+// has its chain and codec: 0, or the code kz_read_ranges fails a read of it with.
+int read_stream_check(kz_ctx* ctx, const kz_index* ix, uint64_t n, const uint8_t* head) {
+    if (n != ix->stream_bytes) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from a stream of another length");
+    if (memcmp(head, ix->head, INDEX_HEAD)) return ctx->fail(KZ_ERR_INVALID_PARAM, "the index was built from another stream");
+    TransformPlan plan;
+    int rc = plan_transforms(ctx, ix->t48, ix->etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    if (!etype_supported(ix->etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+    return 0;
+}
+
 int read_ranges(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
                 const uint64_t* len, void* dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
-    int rc;
-    if (!ix || (!src && !d_src) || (nreq && (!off || !len || !dst_off || !out_len || !status))) rc = ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
-    else if (cudaSetDevice(ctx->device) != cudaSuccess) rc = ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
-    else rc = read_ranges_impl(ctx, ix, cache, src, (const uint8_t*)d_src, n, nreq, off, len, (uint8_t*)dst, dst_off, out_len, status);
+    const int rc = [&]() -> int {
+        if (!ix || (!src && !d_src) || (nreq && (!off || !len || !dst_off || !out_len || !status))) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+        int r = read_call_checks(ctx, cache, nreq, len, dst, dst_off);
+        if (r) return r;
+        if (!src && ((uintptr_t)d_src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+        // the stream the index was built from: its length and its leading bytes
+        uint8_t head[INDEX_HEAD] = {0};
+        const size_t nh = n == ix->stream_bytes ? std::min<size_t>(n, INDEX_HEAD) : 0;
+        if (src) memcpy(head, src, nh);
+        else if (nh) {
+            CK(cudaMemcpyAsync(head, d_src, nh, cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+        }
+        r = read_stream_check(ctx, ix, n, head);
+        if (r) return r;
+        return read_ranges_impl(ctx, cache, src, (const uint8_t*)d_src, {ReadSource{ix, 0, n}}, nreq, nullptr, off, len, (uint8_t*)dst, dst_off, out_len,
+                                status);
+    }();
     return finish_streams(nreq, status, out_len, rc);
+}
+
+// kz_read_ranges_streams[_device]: the streams the requests name are checked one by one (a failure fails that stream's requests only),
+// then the requests on the streams that pass are served by one read_ranges_impl call.
+int read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const uint8_t* base, bool device, const uint64_t* src_off,
+                        const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, void* dst,
+                        const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    const int rc = [&]() -> int {
+        if (nreq && (!ix || !src_off || !src_len || !req_stream || !off || !len || !dst_off || !out_len || !status))
+            return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+        int r = read_call_checks(ctx, cache, nreq, len, dst, dst_off);
+        if (r) return r;
+        std::vector<uint8_t> named(nstreams, 0);
+        for (uint32_t i = 0; i < nreq; i++) {
+            if (req_stream[i] >= nstreams) return ctx->fail(KZ_ERR_INVALID_PARAM, "a request names a stream past nstreams");
+            named[req_stream[i]] = 1;
+        }
+        std::vector<uint32_t> names;
+        for (uint32_t s = 0; s < nstreams; s++) {
+            if (!named[s]) continue;
+            if (src_off[s] + src_len[s] < src_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+            if (src_len[s] && !base) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+            if (device && (src_off[s] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
+            names.push_back(s);
+        }
+        if (device && ((uintptr_t)base & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+        // the first 32 bytes of every named stream: copied on the host, or gathered by one copy launch and brought back in one transfer
+        // (one stream: copied straight back, as kz_read_ranges_device does)
+        const size_t nn = names.size();
+        std::vector<uint8_t> head(INDEX_HEAD * nn, 0);
+        auto nh = [&](size_t j) { return std::min<uint64_t>(src_len[names[j]], INDEX_HEAD); };
+        if (!device) {
+            for (size_t j = 0; j < nn; j++) memcpy(&head[INDEX_HEAD * j], base + src_off[names[j]], nh(j));
+        } else if (nn == 1 && nh(0)) {
+            CK(cudaMemcpyAsync(head.data(), base + src_off[names[0]], nh(0), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+        } else if (nn > 1) {
+            CK(ctx->d_asm.ensure(INDEX_HEAD * nn + 64));
+            CopyList heads;
+            for (size_t j = 0; j < nn; j++) heads.add(base + src_off[names[j]], ctx->d_asm.as<uint8_t>() + INDEX_HEAD * j, nh(j));
+            r = run_copies(ctx, heads);
+            if (r) return r;
+            CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            for (size_t j = 0; j < nn; j++) memset(&head[INDEX_HEAD * j + nh(j)], 0, INDEX_HEAD - nh(j));
+        }
+        // per stream: a missing or stale index or a chain without a GPU path fails the stream's requests with kz_read_ranges's code
+        std::vector<int32_t> code(nstreams, 0);
+        std::vector<uint32_t> slot(nstreams, 0);
+        std::vector<ReadSource> S;
+        for (size_t j = 0; j < nn; j++) {
+            const uint32_t s = names[j];
+            code[s] = ix[s] ? read_stream_check(ctx, ix[s], src_len[s], &head[INDEX_HEAD * j]) : ctx->fail(KZ_ERR_INVALID_PARAM, "missing index");
+            if (!code[s]) slot[s] = (uint32_t)S.size(), S.push_back(ReadSource{ix[s], src_off[s], src_len[s]});
+        }
+        std::vector<uint32_t> keep, rs;
+        std::vector<uint64_t> o, l, d;
+        for (uint32_t i = 0; i < nreq; i++) {
+            status[i] = code[req_stream[i]], out_len[i] = 0;
+            if (status[i]) continue;
+            keep.push_back(i), rs.push_back(slot[req_stream[i]]), o.push_back(off[i]), l.push_back(len[i]), d.push_back(dst_off[i]);
+        }
+        std::vector<uint64_t> kl(keep.size());
+        std::vector<int32_t> ks(keep.size());
+        r = read_ranges_impl(ctx, cache, device ? nullptr : base, device ? base : nullptr, S, (uint32_t)keep.size(), rs.data(), o.data(), l.data(),
+                             (uint8_t*)dst, d.data(), kl.data(), ks.data());
+        if (r) return r;
+        for (size_t j = 0; j < keep.size(); j++) status[keep[j]] = ks[j], out_len[keep[j]] = kl[j];
+        return 0;
+    }();
+    return finish_streams(nreq, status, out_len, rc);
+}
+
+// kz_index_build_device for the streams d_src + src_off[s] (src_len[s] bytes each, >= 64 readable bytes behind each): every header in
+// one gather launch and one transfer, every stream's records in the two walk_streams launches of one build.
+int index_build_streams(kz_ctx* ctx, uint32_t ns, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out, int32_t* status) {
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    std::vector<uint8_t> head(64 * (size_t)ns, 0);
+    if (ns) {
+        CK(ctx->d_asm.ensure(64 * (size_t)ns + 64));
+        CopyList heads;
+        for (uint32_t s = 0; s < ns; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
+        int rc = run_copies(ctx, heads);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (uint32_t s = 0; s < ns; s++) {
+            const uint64_t nh = std::min<uint64_t>(64, src_len[s]);
+            memset(&head[64 * (size_t)s + nh], 0, 64 - nh);
+        }
+    }
+    std::vector<StreamHeader> sh(ns);
+    std::vector<WalkJob> wj;
+    std::vector<uint32_t> who;
+    for (uint32_t s = 0; s < ns; s++) {
+        status[s] = 0;
+        if (ctx->headerless_reader.on) sh[s] = headerless_header(ctx);
+        else if ((status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]))) continue;
+        TransformPlan plan;
+        if ((status[s] = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan, KZ_ERR_CREATE_CODEC))) continue;
+        if (!etype_supported(sh[s].etype)) {
+            status[s] = ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
+            continue;
+        }
+        who.push_back(s);
+        wj.push_back(WalkJob{8 * src_off[s] + sh[s].bits, 8 * (src_off[s] + src_len[s]), 0, 0, 0});
+    }
+    // every record is kept, so the walk runs twice: once storing nothing (an empty block range) for the count, once to store them
+    std::vector<Walked> w;
+    if (!wj.empty()) {
+        int rc = walk_streams(ctx, (const uint32_t*)d_src, wj, 0, 1, w);
+        if (rc) return rc;
+    }
+    std::vector<WalkJob> wj2;
+    std::vector<uint32_t> who2;
+    std::vector<Walked> w2;
+    for (size_t j = 0; j < who.size(); j++) {
+        const uint32_t s = who[j];
+        if (w[j].status) status[s] = ctx->fail(-w[j].status, "Invalid bitstream: corrupted block length");
+        else if (w[j].n) wj2.push_back(WalkJob{8 * src_off[s] + sh[s].bits, 8 * (src_off[s] + src_len[s]), 0, (uint32_t)w[j].n, 0}), who2.push_back(s);
+    }
+    if (!wj2.empty()) {
+        int rc = walk_streams(ctx, (const uint32_t*)d_src, wj2, -1, -1, w2);
+        if (rc) return rc;
+    }
+    std::vector<std::unique_ptr<kz_index>> built(ns);
+    size_t j2 = 0;
+    for (size_t j = 0; j < who.size(); j++) {
+        const uint32_t s = who[j];
+        if (status[s]) continue;
+        const Walked* ws = nullptr;
+        if (w[j].n) {
+            ws = &w2[j2++];
+            if (ws->status) {
+                status[s] = ctx->fail(-ws->status, "Invalid bitstream: corrupted block length");
+                continue;
+            }
+        }
+        std::unique_ptr<kz_index> ix(new kz_index());
+        ix->t48 = sh[s].t48;
+        ix->etype = sh[s].etype;
+        ix->block_size = sh[s].block_size;
+        ix->checksum_bits = sh[s].checksum_bits;
+        ix->header_bits = (uint32_t)sh[s].bits;
+        ix->input_size = sh[s].input_size;
+        ix->stream_bytes = src_len[s];
+        memcpy(ix->head, &head[64 * (size_t)s], INDEX_HEAD);
+        if (ws) {
+            ix->start = ws->bit_off;
+            ix->bits = ws->bits;
+            for (uint64_t& b : ix->start) b -= 8 * src_off[s];
+        }
+        ix->size = ix->start.empty() ? 0 : -1;
+        if (!index_consistent(*ix)) status[s] = ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: the records do not form an index");
+        else built[s] = std::move(ix);
+    }
+    for (uint32_t s = 0; s < ns; s++) out[s] = built[s].release();
+    return 0;
+}
+
+int check_index_streams_args(kz_ctx* ctx, uint32_t ns, const void* src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out, int32_t* status,
+                             bool device) {
+    for (uint32_t s = 0; out && s < ns; s++) out[s] = nullptr;
+    if (ns && (!src_off || !src_len || !out || !status)) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
+    uint64_t end = 0;
+    for (uint32_t s = 0; s < ns; s++) {
+        if (src_off[s] + src_len[s] < src_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+        end = std::max(end, src_off[s] + src_len[s]);
+        if (device && (src_off[s] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
+    }
+    if (end && !src) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    if (device && ((uintptr_t)src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    return 0;
 }
 
 }  // namespace
@@ -3297,6 +3547,49 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
     return read_ranges(ctx, ix, nullptr, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
+}
+
+// ---- many streams per call (kz_index_build_streams[_device], kz_read_ranges_streams[_device]) ----------------------------------------
+int kz_index_build_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out,
+                                  int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_index_streams_args(ctx, nstreams, d_src, src_off, src_len, out, status, true);
+    if (!rc && cudaSetDevice(ctx->device) != cudaSuccess) rc = ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+    if (!rc) rc = index_build_streams(ctx, nstreams, (const uint8_t*)d_src, src_off, src_len, out, status);
+    return finish_streams(nstreams, status, nullptr, rc);
+}
+
+int kz_index_build_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out,
+                           int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    int rc = check_index_streams_args(ctx, nstreams, src, src_off, src_len, out, status, false);
+    if (!rc) rc = [&]() -> int {
+        CK(cudaSetDevice(ctx->device));
+        // the streams packed at 16-byte aligned offsets with 64 zero bytes behind each, moved in one transfer
+        std::vector<uint64_t> in_off(nstreams);
+        uint64_t total = 0;
+        for (uint32_t s = 0; s < nstreams; s++) in_off[s] = total, total += round16(src_len[s]) + 64;
+        CK(ctx->h_io.ensure(total + 64));
+        CK(ctx->d_in.ensure(total + 64));
+        memset(ctx->h_io.p, 0, total);
+        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
+        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+        return index_build_streams(ctx, nstreams, ctx->d_in.as<uint8_t>(), in_off.data(), src_len, out, status);
+    }();
+    return finish_streams(nstreams, status, nullptr, rc);
+}
+
+int kz_read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const uint8_t* src, const uint64_t* src_off,
+                           const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, uint8_t* dst,
+                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    return read_ranges_streams(ctx, cache, nstreams, ix, src, false, src_off, src_len, nreq, req_stream, off, len, dst, dst_off, out_len, status);
+}
+
+int kz_read_ranges_streams_device(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
+                                  const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, void* d_dst,
+                                  const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    return read_ranges_streams(ctx, cache, nstreams, ix, (const uint8_t*)d_src, true, src_off, src_len, nreq, req_stream, off, len, d_dst, dst_off, out_len,
+                               status);
 }
 
 // ---- block cache (kz_cache_*, kz_read_ranges_cached[_device]; bookkeeping in kz_block_cache.h) ---------------------------------------

@@ -115,7 +115,17 @@ inline bool index_load(const uint8_t* blob, size_t n, StreamIndex& x) {
 }
 
 // ---- the plan of one batched read -----------------------------------------------------------------------------------------------
-// One piece of a request inside one block: bytes [in_block, in_block + len) of block blocks[block] go to byte `at` of the request.
+// A read serves requests on one stream or on many (kz_read_ranges_streams). Each stream has a decode group: streams of one group share the
+// fields a block decode depends on (transform48, entropy, block_size, checksum_bits), so their blocks may share a pass; blocks of different
+// groups never do. The plan orders the touched (stream, block) pairs by group, then stream, then block.
+struct ReadStream {
+    uint64_t nblocks;
+    uint32_t block_size;
+    int64_t size;    // decoded bytes, -1: not known (taken as nblocks x block_size)
+    uint32_t group;  // equal groups have equal block sizes
+};
+
+// One piece of a request inside one block: bytes [in_block, in_block + len) of pair `block` go to byte `at` of the request.
 // The plan takes every block for block_size bytes long; the reader clips the slices of the last block to its decoded length.
 struct ReadSlice {
     uint32_t req, block, in_block, len;
@@ -123,10 +133,11 @@ struct ReadSlice {
 };
 
 struct ReadPlan {
-    std::vector<uint64_t> blocks;    // the distinct blocks the requests touch, ascending
-    std::vector<uint32_t> first;     // pass p decodes blocks[first[p] .. first[p + 1])
-    std::vector<ReadSlice> slices;   // ordered by block, so a pass's slices are contiguous ...
-    std::vector<uint64_t> slice_of;  // ... slices[slice_of[k] .. slice_of[k + 1]) read blocks[k]
+    std::vector<uint32_t> stream;    // per touched pair: its stream ...
+    std::vector<uint64_t> blocks;    // ... and its block; the distinct pairs the requests touch, in plan order
+    std::vector<uint32_t> first;     // pass p decodes pairs first[p] .. first[p + 1] - 1
+    std::vector<ReadSlice> slices;   // ordered by pair, so a pass's slices are contiguous ...
+    std::vector<uint64_t> slice_of;  // ... slices[slice_of[k] .. slice_of[k + 1]) read pair k
     std::vector<uint64_t> want;      // per request: its length clipped to the data
     uint32_t npasses() const { return first.empty() ? 0 : (uint32_t)first.size() - 1; }
 };
@@ -135,32 +146,61 @@ struct ReadPlan {
 // the slices are copied from.
 inline uint64_t read_block_cost(uint32_t block_size) { return decompress_block_cost(block_size) + decompress_slot(block_size); }
 
-// Requests [off[i], off[i] + len[i]) on a stream of nblocks blocks of block_size bytes whose decoded size is `size` (-1: not known,
-// taken as nblocks x block_size). A request is clipped to the data (pread); clipped to nothing it touches no block.
-inline ReadPlan plan_reads(uint64_t nblocks, uint32_t block_size, int64_t size, uint32_t nreq, const uint64_t* off, const uint64_t* len,
-                           uint64_t budget = STREAM_PASS_BUDGET) {
+// The passes over pairs order[0 ..] (plan order, e.g. the pairs a cache lacks): runs of one group, each cut by plan_decompress_passes.
+// Returns first: pass p holds order[first[p] .. first[p + 1]).
+inline std::vector<uint32_t> plan_read_passes(const std::vector<ReadStream>& S, const std::vector<uint32_t>& stream_of, const std::vector<uint32_t>& order,
+                                              uint64_t budget = STREAM_PASS_BUDGET) {
+    std::vector<uint32_t> first;
+    const uint32_t n = (uint32_t)order.size();
+    for (uint32_t a = 0, e; a < n; a = e) {
+        const ReadStream& g = S[stream_of[order[a]]];
+        for (e = a + 1; e < n && S[stream_of[order[e]]].group == g.group;) e++;
+        const PassPlan pp = plan_decompress_passes(e - a, decompress_slot(g.block_size), read_block_cost(g.block_size), budget);
+        for (uint32_t p = 0; p < pp.npasses(); p++) first.push_back(a + pp.first[p]);
+    }
+    first.push_back(n);
+    return first;
+}
+
+// Requests [off[i], off[i] + len[i]) on stream req_stream[i] (null: every request on stream 0). A request is clipped to its stream's
+// data (pread); clipped to nothing it touches no block.
+inline ReadPlan plan_reads_streams(const std::vector<ReadStream>& S, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len,
+                                   uint64_t budget = STREAM_PASS_BUDGET) {
     ReadPlan P;
-    const uint64_t total = size >= 0 ? (uint64_t)size : nblocks * block_size;
+    struct Pair {
+        uint32_t group, stream;
+        uint64_t block;
+        bool operator<(const Pair& o) const { return group != o.group ? group < o.group : stream != o.stream ? stream < o.stream : block < o.block; }
+        bool operator==(const Pair& o) const { return group == o.group && stream == o.stream && block == o.block; }
+    };
+    auto stream_of = [&](uint32_t i) { return req_stream ? req_stream[i] : 0u; };
+    std::vector<Pair> pairs;
     P.want.resize(nreq);
     for (uint32_t i = 0; i < nreq; i++) {
+        const ReadStream& s = S[stream_of(i)];
+        const uint64_t total = s.size >= 0 ? (uint64_t)s.size : s.nblocks * s.block_size;
         P.want[i] = off[i] < total ? std::min(len[i], total - off[i]) : 0;
         if (P.want[i]) {
-            const uint64_t lo = off[i] / block_size, hi = (off[i] + P.want[i] - 1) / block_size;
-            for (uint64_t b = lo; b <= hi; b++) P.blocks.push_back(b);
+            const uint64_t lo = off[i] / s.block_size, hi = (off[i] + P.want[i] - 1) / s.block_size;
+            for (uint64_t b = lo; b <= hi; b++) pairs.push_back(Pair{s.group, stream_of(i), b});
         }
     }
-    std::sort(P.blocks.begin(), P.blocks.end());
-    P.blocks.erase(std::unique(P.blocks.begin(), P.blocks.end()), P.blocks.end());
-    // slices counted per block, then placed: a counting sort by block that keeps the requests' order inside a block
-    P.slice_of.assign(P.blocks.size() + 1, 0);
+    std::sort(pairs.begin(), pairs.end());
+    pairs.erase(std::unique(pairs.begin(), pairs.end()), pairs.end());
+    P.stream.resize(pairs.size());
+    P.blocks.resize(pairs.size());
+    for (size_t k = 0; k < pairs.size(); k++) P.stream[k] = pairs[k].stream, P.blocks[k] = pairs[k].block;
+    // slices counted per pair, then placed: a counting sort by pair that keeps the requests' order inside a pair
+    P.slice_of.assign(pairs.size() + 1, 0);
     auto each_slice = [&](auto&& f) {
         for (uint32_t i = 0; i < nreq; i++) {
             uint64_t pos = off[i], left = P.want[i];
             if (!left) continue;
-            size_t k = std::lower_bound(P.blocks.begin(), P.blocks.end(), pos / block_size) - P.blocks.begin();
+            const uint32_t st = stream_of(i), bs = S[st].block_size;
+            size_t k = std::lower_bound(pairs.begin(), pairs.end(), Pair{S[st].group, st, pos / bs}) - pairs.begin();
             for (; left; k++) {
-                const uint32_t in_block = (uint32_t)(pos % block_size);
-                const uint32_t n = (uint32_t)std::min<uint64_t>(left, block_size - in_block);
+                const uint32_t in_block = (uint32_t)(pos % bs);
+                const uint32_t n = (uint32_t)std::min<uint64_t>(left, bs - in_block);
                 f(ReadSlice{i, (uint32_t)k, in_block, n, pos - off[i]});
                 pos += n;
                 left -= n;
@@ -168,13 +208,20 @@ inline ReadPlan plan_reads(uint64_t nblocks, uint32_t block_size, int64_t size, 
         }
     };
     each_slice([&](const ReadSlice& s) { P.slice_of[s.block + 1]++; });
-    for (size_t k = 0; k < P.blocks.size(); k++) P.slice_of[k + 1] += P.slice_of[k];
+    for (size_t k = 0; k < pairs.size(); k++) P.slice_of[k + 1] += P.slice_of[k];
     P.slices.resize((size_t)P.slice_of.back());
     std::vector<uint64_t> fill(P.slice_of.begin(), P.slice_of.end() - 1);
     each_slice([&](const ReadSlice& s) { P.slices[(size_t)fill[s.block]++] = s; });
-    const PassPlan passes = plan_decompress_passes((uint32_t)P.blocks.size(), decompress_slot(block_size), read_block_cost(block_size), budget);
-    P.first = passes.first;
+    std::vector<uint32_t> order(pairs.size());
+    for (uint32_t k = 0; k < (uint32_t)order.size(); k++) order[k] = k;
+    P.first = plan_read_passes(S, P.stream, order, budget);
     return P;
+}
+
+// The one-stream plan: requests on a stream of nblocks blocks of block_size bytes whose decoded size is `size` (-1: not known).
+inline ReadPlan plan_reads(uint64_t nblocks, uint32_t block_size, int64_t size, uint32_t nreq, const uint64_t* off, const uint64_t* len,
+                           uint64_t budget = STREAM_PASS_BUDGET) {
+    return plan_reads_streams({ReadStream{nblocks, block_size, size, 0}}, nreq, nullptr, off, len, budget);
 }
 
 }  // namespace kz
