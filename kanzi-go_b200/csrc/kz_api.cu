@@ -61,7 +61,6 @@ namespace {
 
 const uint32_t BS_TYPE = 0x4B414E5A;  // io/CompressedStream.go:43
 const uint32_t BS_VERSION = 6;        // :44
-const size_t SMALL_BLOCK = 15;        // :51
 const size_t RAW_PIECE = 64 * 1024;   // raw segments are cut so that one CTA never copies more than this
 
 cudaEvent_t get_event(kz_ctx* ctx) {
@@ -232,6 +231,39 @@ int run_copies(kz_ctx* ctx, const CopyList& cl) {
     return 0;
 }
 
+// The first w bytes of n device ranges (range i: len[i] bytes at d_base + off[i]) to out, w bytes per range and zero padded, and the
+// n_extra bytes at d_extra to extra, behind one synchronisation (none when there is nothing to copy). One range is one copy. Evenly
+// spaced ranges, such as the blocks of one stream, are one cudaMemcpy2DAsync and one copy of a short last range. Other ranges are
+// gathered into ctx->d_asm by one copy launch and come back in one transfer.
+template <class Len>
+int gather_heads(kz_ctx* ctx, const uint8_t* d_base, const uint64_t* off, const Len* len, size_t n, uint32_t w, uint8_t* out,
+                 const uint8_t* d_extra = nullptr, size_t n_extra = 0, uint8_t* extra = nullptr) {
+    const uint64_t MAX_PITCH = 1u << 30;  // the largest block size: a source pitch cudaMemcpy2DAsync takes
+    auto head = [&](size_t i) { return (size_t)std::min<uint64_t>(len[i], w); };
+    memset(out, 0, n * w);
+    bool any = n_extra > 0;
+    for (size_t i = 0; i < n && !any; i++) any = head(i) > 0;
+    if (!any) return 0;
+    const uint64_t pitch = n > 1 ? off[1] - off[0] : 0;
+    bool even = n > 1 && off[1] > off[0] && pitch >= w && pitch <= MAX_PITCH;
+    for (size_t i = 0; i < n && even; i++) even = off[i] == off[0] + i * pitch && (i + 1 == n || len[i] >= w);
+    if (n == 1 || even) {
+        if (n > 1) CK(cudaMemcpy2DAsync(out, w, d_base + off[0], pitch, w, n - 1, cudaMemcpyDeviceToHost, ctx->stream));
+        if (head(n - 1)) CK(cudaMemcpyAsync(out + (n - 1) * w, d_base + off[n - 1], head(n - 1), cudaMemcpyDeviceToHost, ctx->stream));
+    } else if (n) {
+        CK(ctx->d_asm.ensure(n * w));
+        CopyList cl;
+        for (size_t i = 0; i < n; i++) cl.add(d_base + off[i], ctx->d_asm.as<uint8_t>() + i * w, head(i));
+        int rc = run_copies(ctx, cl);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(out, ctx->d_asm.p, n * w, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    if (n_extra) CK(cudaMemcpyAsync(extra, d_extra, n_extra, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (size_t i = 0; i < n; i++) memset(out + i * w + head(i), 0, w - head(i));  // a gather leaves the bytes behind a short head as they were
+    return 0;
+}
+
 // XXHash32/64 of a set of blocks (hash/XXHash32.go, XXHash64.go; seed "KANZ", io/CompressedStream.go:354-356). Synchronous.
 int hash_blocks(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint32_t bits,
                 std::vector<uint64_t>& out) {
@@ -281,6 +313,13 @@ int verify_checksums(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint6
 
 bool etype_supported(uint32_t e) { return e == KZ_E_NONE || e == KZ_E_ANS0 || e == KZ_E_HUFFMAN || e == KZ_E_ANS1 || e == KZ_E_RANGE; }
 
+// The block size and checksum width of every stream-level encode (whole stream, many streams, writer session)
+int check_encode_args(kz_ctx* ctx, uint32_t block_size, uint32_t checksum_bits) {
+    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
+    return 0;
+}
+
 // The gather of every bit-granular output (kz_concat.cu): segment i, seg_bits[i] bits at address seg_src[i], lands at bit seg_dst[i] of
 // d_out. The three tables are device arrays. encode_batch, the many-stream assembly and kz_concat_bits_device all write through it.
 int concat_segments(kz_ctx* ctx, const uint64_t* d_seg_src, const uint64_t* d_seg_bits, const uint64_t* d_seg_dst, int nsegs, uint8_t* d_out) {
@@ -316,8 +355,11 @@ struct EncResult {
     std::vector<int32_t> status;      // per block 0 / -(error code)
 };
 
+// LAYOUT_STREAM: stream_hdr (stream_hdr_bits bits) leads, and the end marker closes the stream unless `fragment` (the records of one rank of
+// a sharded compression, or a writer session's batch before its last). volatile_lead: the leading segment is a writer session's header or
+// carry, which changes from batch to batch.
 int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksum_bits, const uint8_t* d_data, const std::vector<EncJob>& jobs,
-                 const std::vector<uint8_t>& stream_hdr, uint64_t stream_hdr_bits, uint8_t* d_dst, size_t dst_cap,
+                 const std::vector<uint8_t>& stream_hdr, uint64_t stream_hdr_bits, bool fragment, bool volatile_lead, uint8_t* d_dst, size_t dst_cap,
                  const std::vector<uint64_t>& blk_base_bits, EncResult& res) {
     const int nblocks = (int)jobs.size();
     if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
@@ -338,13 +380,13 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
     std::vector<uint8_t> key;
     // a streaming writer's leading segment (header, then the carry) changes from batch to batch: it stays out of the key and is
     // written into the kept tables below
-    const bool lead = ctx->volatile_lead && layout == LAYOUT_STREAM;
+    const bool lead = volatile_lead && layout == LAYOUT_STREAM;
     {
         auto put = [&](const void* p, size_t n) {
             const uint8_t* q = (const uint8_t*)p;
             key.insert(key.end(), q, q + n);
         };
-        const uint64_t scal[8] = {(uint64_t)layout | (ctx->fragment ? 0x100u : 0u) | (lead ? 0x200u : 0u), etype, checksum_bits, (uint64_t)(uintptr_t)d_data,
+        const uint64_t scal[8] = {(uint64_t)layout | (fragment ? 0x100u : 0u) | (lead ? 0x200u : 0u), etype, checksum_bits, (uint64_t)(uintptr_t)d_data,
                                   (uint64_t)(uintptr_t)d_small, (uint64_t)nblocks, lead ? 0 : stream_hdr_bits, (uint64_t)stream_hdr.size()};
         key.reserve(sizeof(scal) + stream_hdr.size() + jobs.size() * 40 + blk_base_bits.size() * 8);
         put(scal, sizeof(scal));
@@ -438,7 +480,7 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
                 }
             }
             if (layout == LAYOUT_STREAM) {
-                add_seg((uint64_t)(uintptr_t)(d_small + small_zero_off), ctx->fragment ? 0 : END_MARKER_BITS);  // end marker (Close :593-594); none behind a fragment
+                add_seg((uint64_t)(uintptr_t)(d_small + small_zero_off), fragment ? 0 : END_MARKER_BITS);  // end marker (Close :593-594); none behind a fragment
                 blk_first[nblocks] = (uint32_t)seg_src.size();
             } else {
                 blk_first[nblocks] = (uint32_t)seg_src.size();
@@ -1033,6 +1075,16 @@ StreamHeader headerless_header(const kz_ctx* ctx) {
     return h;
 }
 
+// The header of a stream of n bytes whose first min(n, 64) bytes are head (zero padded): the headerless reader setting when one is in
+// force, else the header parsed from head.
+int stream_header(kz_ctx* ctx, const uint8_t* head, size_t n, StreamHeader& sh) {
+    if (ctx->headerless_reader.on) {
+        sh = headerless_header(ctx);
+        return 0;
+    }
+    return parse_stream_header(ctx, head, n, sh);
+}
+
 int count_transforms(uint64_t t48, uint64_t* ids) {
     int n = 0;
     for (int i = 0; i < 8; i++) {
@@ -1043,50 +1095,20 @@ int count_transforms(uint64_t t48, uint64_t* ids) {
     return n;
 }
 
-// The data type encodingTask.encode derives from the first four bytes of a block before the transforms run
-// (io/CompressedStream.go:806-816 over internal/Magic.go:73-112 GetMagicType and :116-206 IsDataCompressed / IsDataMultimedia /
-// IsDataExecutable): 7 = DT_BIN for compressed containers, 2 = DT_MULTIMEDIA, 3 = DT_EXE, 0 = DT_UNDEFINED otherwise.
-int32_t magic_data_type(const uint8_t* p, size_t n) {
-    if (n < 4) return 0;
-    const uint32_t key = ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];
-    const uint32_t k24 = key >> 8, k16 = key >> 16;
-    // compressed: JPEG (APP0 marker only: the other FFD8FFEx keys match no class), GIF, PNG, 7z, zstd, brotli, CAB, ZIP, FLAC, xz, KANZ, RAR,
-    // bzip2 / ID3 (24 bits), gzip (16 bits)
-    switch (key) {
-        case 0xFFD8FFE0u: case 0x47494638u: case 0x89504E47u: case 0x377ABCAFu: case 0x28B52FFDu: case 0x81CFB2CEu: case 0x4D534346u:
-        case 0x504B0304u: case 0x664C6143u: case 0xFD377A58u: case 0x4B414E5Au: case 0x52617221u:
-            return 7;
-        default: break;
-    }
-    if ((key & ~0x0Fu) == 0xFFD8FFE0u) return 0;  // GetMagicType returns the key itself: no class matches
-    if (k24 == 0x425A68u || k24 == 0x494433u) return 7;
-    if (key == 0x25504446u) return 0;  // PDF: recognised, in no class
-    if (key == 0x52494646u) return 2;  // RIFF
-    if (key == 0x7F454C46u || key == 0xFEEDFACEu || key == 0xCEFAEDFEu || key == 0xFEEDFACFu || key == 0xCFFAEDFEu) return 3;  // ELF, Mach-O
-    if (k16 == 0x1F8Bu) return 7;  // gzip
-    if (k16 == 0x424Du) return 2;  // BMP
-    if (k16 == 0x4D5Au) return 3;  // MZ
-    if (k16 == 0x5034u || k16 == 0x5035u || k16 == 0x5036u) {  // binary PBM / PGM / PPM: "P4".."P6" followed by white space
-        const uint32_t sub = (key >> 8) & 0xFF;
-        if (sub == 0x07 || sub == 0x0A || sub == 0x0D || sub == 0x20) return 2;
-    }
-    return 0;
-}
-
 // kanzi's skipBlocks option (encodingTask.encode, io/CompressedStream.go:778-800), device half: the order-0 histogram of every block
 // d_base + off[b] (len[b] bytes, any alignment) and its entropy test (kz_skip.cu). The blocks of at most SMALL_BLOCK bytes, stored in any
-// case, are not read. On return the work is queued, and *d_heads points at 4 * nb zero bytes of ctx->d_skip for the caller's block heads,
-// followed by nb flag bytes (1: the order-0 entropy reaches INCOMPRESSIBLE_THRESHOLD), so that one copy brings both back.
-int skip_test(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint8_t** d_heads) {
+// case, are not read. On return the work is queued, and *d_flags points at nb flag bytes of ctx->d_skip (1: the order-0 entropy reaches
+// INCOMPRESSIBLE_THRESHOLD) for stored_blocks (kz_stream_plan.h).
+int skip_test(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, const uint8_t** d_flags) {
     const uint32_t nb = (uint32_t)len.size();
     std::vector<SkipTile> tiles;
     for (uint32_t b = 0; b < nb; b++)
         if (len[b] > SMALL_BLOCK)
             for (uint32_t o = 0; o < len[b]; o += SKIP_TILE) tiles.push_back(SkipTile{off[b] + o, std::min(SKIP_TILE, len[b] - o), b});
-    const size_t o_heads = (size_t)nb * 256 * 4;  // behind the histograms
-    CK(ctx->d_skip.ensure(o_heads + 5 * (size_t)nb));
+    const size_t o_flags = (size_t)nb * 256 * 4;  // behind the histograms
+    CK(ctx->d_skip.ensure(o_flags + nb));
     uint8_t* S = ctx->d_skip.as<uint8_t>();
-    CK(cudaMemsetAsync(S, 0, o_heads + 4 * (size_t)nb, ctx->stream));
+    CK(cudaMemsetAsync(S, 0, o_flags, ctx->stream));
     Packer pk;
     const size_t o_tiles = pk.add(tiles.data(), tiles.size() * sizeof(SkipTile));
     const size_t o_len = pk.add(len.data(), (size_t)nb * 4);
@@ -1102,35 +1124,11 @@ int skip_test(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& o
     {
         LaunchScope ls(ctx, "skip_decide");
         skip_decide_kernel<<<(nb + 255) / 256, 256, 0, ctx->stream>>>((const uint32_t*)S, (const uint32_t*)(T + o_len), nb, (const uint32_t*)(T + o_log2),
-                                                                     S + o_heads + 4 * (size_t)nb);
+                                                                     S + o_flags);
     }
     CK(cudaGetLastError());
-    *d_heads = S + o_heads;
+    *d_flags = S + o_flags;
     return 0;
-}
-
-// skipBlocks, host half: block b (len[b] bytes) is stored when it has more than SMALL_BLOCK bytes and its head is the magic number of a
-// compressed format (magic_data_type 7: IsDataCompressed(GetMagicType)) or its entropy flag is set. hf = 4 head bytes per block, then one
-// flag byte per block (skip_test). With profiling on, the blocks and bytes stored for each reason add up under "skip:magic" and
-// "skip:entropy" (bytes_in = blocks, bytes_out = bytes).
-std::vector<uint8_t> stored_blocks(kz_ctx* ctx, const std::vector<uint8_t>& hf, const uint32_t* len, uint32_t nb) {
-    std::vector<uint8_t> store(nb, 0);
-    uint64_t n_magic = 0, b_magic = 0, n_ent = 0, b_ent = 0;
-    for (uint32_t b = 0; b < nb; b++) {
-        if (len[b] <= SMALL_BLOCK) continue;
-        if (magic_data_type(&hf[(size_t)b * 4], len[b]) == 7) {
-            store[b] = 1, n_magic++, b_magic += len[b];
-        } else if (hf[(size_t)nb * 4 + b]) {
-            store[b] = 1, n_ent++, b_ent += len[b];
-        }
-    }
-    if (ctx->profile) {
-        auto& m = ctx->prof["skip:magic"];
-        m.bytes_in += n_magic, m.bytes_out += b_magic, m.launches++;
-        auto& e = ctx->prof["skip:entropy"];
-        e.bytes_in += n_ent, e.bytes_out += b_ent, e.launches++;
-    }
-    return store;
 }
 
 struct TransformPlan {
@@ -1664,21 +1662,71 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
     return 0;
 }
 
+// What encodingTask.encode (io/CompressedStream.go:753-816) finds out about the blocks of a batch before the transforms run. An empty
+// vector stands for its default on every block.
+struct BlockPrep {
+    std::vector<int32_t> dt;         // the initial ctx["dataType"], from the block's magic number (default 0)
+    std::vector<uint8_t> store;      // skipBlocks: 1 = the block is stored raw (default 0)
+    std::vector<uint64_t> checksum;  // the hash of the original block (default: no checksums)
+    // the entries of blocks idx[0 .. k - 1]
+    BlockPrep pick(const uint32_t* idx, uint32_t k) const {
+        BlockPrep p;
+        auto take = [&](const auto& from, auto& to) {
+            for (uint32_t j = 0; j < k && !from.empty(); j++) to.push_back(from[idx[j]]);
+        };
+        take(dt, p.dt);
+        take(store, p.store);
+        take(checksum, p.checksum);
+        return p;
+    }
+};
+
+// The BlockPrep of the blocks bl over d_base for a plan, the skipBlocks setting and a checksum width: their first four bytes (from
+// host_heads, 4 zero-padded bytes per block, when the caller has them in host memory) decide the data types when the plan reads them
+// (uses_magic) and, with skip, which blocks are stored; checksum_bits != 0 hashes the blocks.
+int prepare_blocks(kz_ctx* ctx, const TransformPlan& plan, bool skip, uint32_t checksum_bits, const uint8_t* d_base, const BlockList& bl, BlockPrep& prep,
+                   const std::vector<uint8_t>* host_heads = nullptr) {
+    const uint32_t nb = bl.size();
+    prep = BlockPrep();
+    if (nb == 0) return 0;
+    if (plan.uses_magic() || skip) {
+        const uint8_t* d_flags = nullptr;
+        if (skip) {
+            int rc = skip_test(ctx, d_base, bl.off, bl.len, &d_flags);
+            if (rc) return rc;
+        }
+        std::vector<uint8_t> heads = host_heads ? *host_heads : std::vector<uint8_t>(4 * (size_t)nb), flags(skip ? nb : 0);
+        int rc = gather_heads(ctx, d_base, bl.off.data(), bl.len.data(), host_heads ? 0 : nb, 4, heads.data(), d_flags, flags.size(), flags.data());
+        if (rc) return rc;
+        if (plan.uses_magic()) {
+            prep.dt.resize(nb);
+            for (uint32_t b = 0; b < nb; b++) prep.dt[b] = magic_data_type(&heads[(size_t)b * 4], bl.len[b]);
+        }
+        if (skip) {
+            const StoreCounts c = stored_blocks(heads.data(), flags.data(), bl.len.data(), nb, prep.store);
+            if (ctx->profile) {  // bytes_in = blocks, bytes_out = bytes
+                auto& m = ctx->prof["skip:magic"];
+                m.bytes_in += c.magic_blocks, m.bytes_out += c.magic_bytes, m.launches++;
+                auto& e = ctx->prof["skip:entropy"];
+                e.bytes_in += c.entropy_blocks, e.bytes_out += c.entropy_bytes, e.launches++;
+            }
+        }
+    }
+    if (checksum_bits) return hash_blocks(ctx, d_base, bl.off, bl.len, checksum_bits, prep.checksum);
+    return 0;
+}
+
 // Forward transform stage (ByteTransformSequence.Forward, transform/Sequence.go:64-125) of every block of a batch.
 // Block b is d_src[b*stride : +len_b]. On return *d_data is the base of the post-transform data and jobs[] describes
 // every block for the entropy stage. NONE leaves the data in place; the stages alternate between ctx->d_tmp and ctx->d_tmp2.
-// A block with store[b] set (skipBlocks) is a COPY block, like a block of at most SMALL_BLOCK bytes: no stage runs on it, and
+// A block that prep stores (skipBlocks) is a COPY block, like a block of at most SMALL_BLOCK bytes: no stage runs on it, and
 // a batch of nothing but COPY blocks runs no stage at all.
-int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, size_t n, uint32_t block_size, uint64_t stride, const uint32_t* lens,
-                  uint32_t nblocks, const uint8_t** d_data, std::vector<EncJob>& jobs, const std::vector<int32_t>* init_dt = nullptr,
-                  const std::vector<uint8_t>* store = nullptr) {
+int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, uint64_t stride, std::vector<uint32_t> len, const BlockPrep& prep,
+                  const uint8_t** d_data, std::vector<EncJob>& jobs) {
+    const uint32_t nblocks = (uint32_t)len.size();
     jobs.resize(nblocks);
-    std::vector<uint32_t> len(nblocks);
     uint32_t max_len = 0;
-    for (uint32_t b = 0; b < nblocks; b++) {
-        len[b] = lens ? lens[b] : (uint32_t)std::min<uint64_t>(block_size, n - (uint64_t)b * block_size);
-        max_len = std::max(max_len, len[b]);
-    }
+    for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, len[b]);
     *d_data = d_src;
     for (uint32_t b = 0; b < nblocks; b++) {
         EncJob& j = jobs[b];
@@ -1686,13 +1734,13 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
         j.post_len = len[b];
         j.ntransforms = (uint32_t)plan.nt;
         j.skip_flags = 0x7F;  // NullTransform succeeds: bit 7 cleared (Sequence.go:65,107)
-        j.copy = len[b] <= SMALL_BLOCK || (store && (*store)[b]);  // io/CompressedStream.go:773-799: transform and entropy forced to NONE
-        j.checksum = 0;
+        j.copy = len[b] <= SMALL_BLOCK || (!prep.store.empty() && prep.store[b]);  // io/CompressedStream.go:773-799: transform and entropy forced to NONE
+        j.checksum = prep.checksum.empty() ? 0 : prep.checksum[b];
     }
     if (plan.none() || nblocks == 0) return 0;
-    // ctx["dataType"] of every block: the caller's value (from the block's magic number, encodingTask.encode :808-816), updated by the stages
-    std::vector<int32_t> dts(nblocks, 0);
-    if (init_dt) dts = *init_dt;
+    // ctx["dataType"] of every block: the value from the block's magic number (encodingTask.encode :808-816), updated by the stages
+    std::vector<int32_t> dts = prep.dt;
+    dts.resize(nblocks, 0);
     std::vector<uint8_t> active(nblocks), applied;
     bool any = false;
     for (uint32_t b = 0; b < nblocks; b++) {
@@ -2087,10 +2135,47 @@ size_t kz_transform_max_encoded_len(uint64_t type, size_t n) {
 }
 
 // ---- whole stream, device resident ---------------------------------------------------------------------------
-static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size, const void* d_src,
-                                size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits);
+// What compress_device_impl runs on the n bytes at d_src, cut into blocks of block_size: prepare_blocks, the forward transforms and the
+// LAYOUT_STREAM encode behind the leading segment `lead` (lead_bits bits: the stream header, or a writer session's carry), with the end
+// marker unless `fragment`. A writer session runs every batch of its stream through it, its leading segment volatile.
 static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, bool skip,
-                                const void* d_src, size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res);
+                                const void* d_src, size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, bool fragment, bool volatile_lead,
+                                void* d_dst, size_t cap, EncResult& res) {
+    const uint64_t off = 0, len = n;
+    const BlockList bl = cut_blocks(&off, &len, 1, block_size);
+    BlockPrep prep;
+    int rc = prepare_blocks(ctx, plan, skip, checksum_bits, (const uint8_t*)d_src, bl, prep);
+    if (rc) return rc;
+    const uint8_t* d_data = nullptr;
+    std::vector<EncJob> jobs;
+    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, block_size, bl.len, prep, &d_data, jobs);
+    if (rc) return rc;
+    return encode_batch(ctx, LAYOUT_STREAM, etype, checksum_bits, d_data, jobs, lead, lead_bits, fragment, volatile_lead, (uint8_t*)d_dst, cap, {}, res);
+}
+
+static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size, const void* d_src,
+                                size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits) {
+    if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
+    CK(cudaSetDevice(ctx->device));
+    ctx->stream_bs = block_size;
+    int rc = check_encode_args(ctx, block_size, checksum_bits);
+    if (rc) return rc;
+    if (((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    TransformPlan plan;
+    rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    if (rc) return rc;
+    std::vector<uint8_t> hdr;
+    uint32_t hdr_bits = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size);
+    if (fragment || ctx->headerless_writer) hdr_bits = 0;  // an empty leading segment (Writer.writeHeader :430)
+    EncResult res;
+    rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, ctx->skip_blocks, d_src, n, hdr, hdr_bits, fragment, false, d_dst, cap, res);
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    *out_n = (size_t)((res.total_bits + 7) / 8);
+    if (out_bits) *out_bits = res.total_bits;
+    return 0;
+}
+
 int kz_compress_stream_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size,
                               const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, out_n, false, nullptr);
@@ -2102,84 +2187,6 @@ int kz_compress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     size_t bytes = 0;
     if (!out_bits) return -KZ_ERR_INVALID_PARAM;
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, 0, d_src, n, d_dst, cap, &bytes, true, out_bits);
-}
-static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size, const void* d_src,
-                                size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits) {
-    if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
-    CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = block_size;
-    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
-    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
-    if (((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    TransformPlan plan;
-    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
-    if (rc) return rc;
-    std::vector<uint8_t> hdr;
-    uint32_t hdr_bits = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size);
-    if (fragment || ctx->headerless_writer) hdr_bits = 0;  // an empty leading segment (Writer.writeHeader :430)
-    EncResult res;
-    ctx->fragment = fragment;
-    rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, ctx->skip_blocks, d_src, n, hdr, hdr_bits, d_dst, cap, res);
-    ctx->fragment = false;
-    if (rc) return rc;
-    CK(cudaStreamSynchronize(ctx->stream));
-    *out_n = (size_t)((res.total_bits + 7) / 8);
-    if (out_bits) *out_bits = res.total_bits;
-    return 0;
-}
-
-// What compress_device_impl runs on the n bytes at d_src, cut into blocks of block_size: the initial dataType of every block from its magic
-// number, with skip (skipBlocks) the blocks stored raw, the forward transforms, the block checksums and the LAYOUT_STREAM encode behind the
-// leading segment `lead` (lead_bits bits: the stream header, or a writer session's carry). A writer session runs every batch of its stream
-// through it.
-static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, bool skip,
-                                const void* d_src, size_t n, const std::vector<uint8_t>& lead, uint32_t lead_bits, void* d_dst, size_t cap, EncResult& res) {
-    const uint32_t nblocks = (uint32_t)((n + block_size - 1) / block_size);
-    std::vector<EncJob> jobs;
-    int rc = 0;
-    const uint8_t* d_data = nullptr;
-    std::vector<int32_t> init_dt;
-    std::vector<uint8_t> store;
-    if ((plan.uses_magic() || skip) && nblocks) {  // the first four bytes of every block decide its initial data type (and whether it is stored)
-        const size_t last = n - (size_t)(nblocks - 1) * block_size;
-        std::vector<uint8_t> heads((size_t)nblocks * (skip ? 5 : 4), 0);  // with skip, the entropy flags follow the heads in the same copy
-        std::vector<uint32_t> blen(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) blen[b] = b + 1 < nblocks ? block_size : (uint32_t)last;
-        uint8_t* d_heads = nullptr;
-        if (skip) {
-            std::vector<uint64_t> boff(nblocks);
-            for (uint32_t b = 0; b < nblocks; b++) boff[b] = (uint64_t)b * block_size;
-            rc = skip_test(ctx, (const uint8_t*)d_src, boff, blen, &d_heads);
-            if (rc) return rc;
-        }
-        const cudaMemcpyKind kind = d_heads ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-        uint8_t* dst = d_heads ? d_heads : heads.data();
-        if (nblocks > 1) CK(cudaMemcpy2DAsync(dst, 4, d_src, block_size, 4, nblocks - 1, kind, ctx->stream));
-        CK(cudaMemcpyAsync(dst + (size_t)(nblocks - 1) * 4, (const uint8_t*)d_src + (size_t)(nblocks - 1) * block_size, std::min<size_t>(4, last), kind,
-                           ctx->stream));
-        if (d_heads) CK(cudaMemcpyAsync(heads.data(), d_heads, heads.size(), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        if (plan.uses_magic()) {
-            init_dt.resize(nblocks);
-            for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(&heads[(size_t)b * 4], blen[b]);
-        }
-        if (skip) store = stored_blocks(ctx, heads, blen.data(), nblocks);
-    }
-    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, n, block_size, block_size, nullptr, nblocks, &d_data, jobs, init_dt.empty() ? nullptr : &init_dt,
-                       store.empty() ? nullptr : &store);
-    if (rc) return rc;
-    if (checksum_bits && nblocks) {  // encodingTask.encode :753-763: hash of the original block
-        std::vector<uint64_t> hoff(nblocks), hv;
-        std::vector<uint32_t> hlen(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            hoff[b] = (uint64_t)b * block_size;
-            hlen[b] = (uint32_t)std::min<uint64_t>(block_size, n - (uint64_t)b * block_size);
-        }
-        rc = hash_blocks(ctx, (const uint8_t*)d_src, hoff, hlen, checksum_bits, hv);
-        if (rc) return rc;
-        for (uint32_t b = 0; b < nblocks; b++) jobs[b].checksum = hv[b];
-    }
-    return encode_batch(ctx, LAYOUT_STREAM, etype, checksum_bits, d_data, jobs, lead, lead_bits, (uint8_t*)d_dst, cap, {}, res);
 }
 
 // Stream header bytes (Writer.writeHeader, io/CompressedStream.go:429-519) for the rank that commits a sharded stream. out: >= 32 bytes.
@@ -2230,69 +2237,8 @@ int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, 
     return 0;
 }
 
-static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
-                                  size_t n, void* d_dst, size_t cap, size_t* out_n);
-int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
-    if (ctx && ctx->headerless_reader.on) {
-        const StreamHeader sh = headerless_header(ctx);
-        return decompress_device_impl(ctx, &sh, 0, 0, ctx->range_from, ctx->range_to, d_src, n, d_dst, cap, out_n);
-    }
-    return decompress_device_impl(ctx, nullptr, 0, 0, ctx ? ctx->range_from : -1, ctx ? ctx->range_to : -1, d_src, n, d_dst, cap, out_n);
-}
-// Decodes `nblocks` block records that start at bit `start_bit` of the fragment at d_src (frag_bytes bytes, >= 64 readable bytes behind them):
-// what one rank of a sharded decompression does with its part of the stream. The stream parameters come from the header rank 0 parsed.
-int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src, size_t frag_bytes,
-                                  uint64_t start_bit, uint32_t nblocks, void* d_dst, size_t cap, size_t* out_n) {
-    if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
-    *out_n = 0;
-    if (nblocks == 0) return 0;
-    StreamHeader sh;
-    sh.t48 = t48;
-    sh.etype = etype;
-    sh.block_size = block_size;
-    sh.checksum_bits = checksum_bits;
-    sh.input_size = 0;
-    sh.bits = 0;
-    return decompress_device_impl(ctx, &sh, start_bit, nblocks, -1, -1, d_src, frag_bytes, d_dst, cap, out_n);
-}
-// Parses the header of the stream at d_src and walks its block records: rec_bit[b] = first bit of record b (its 5-bit prefix), rec_bit[nblocks] =
-// first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries. With a headerless reader setting the fields are
-// the setting's and rec_bit[0] = 0.
-// The header of the stream of n bytes at d_src, parsed from its first bytes (head, 64 bytes, receives them), or the headerless reader
-// setting when one is in force: what kz_stream_index_device and kz_index_build_device walk the records from.
-static int device_stream_header(kz_ctx* ctx, const void* d_src, size_t n, uint8_t* head, StreamHeader& sh) {
-    memset(head, 0, 64);
-    if (n) CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (ctx->headerless_reader.on) {
-        sh = headerless_header(ctx);
-        return 0;
-    }
-    return parse_stream_header(ctx, head, n, sh);
-}
-int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t max_blocks, uint64_t* t48, uint32_t* etype, uint32_t* block_size,
-                           uint32_t* checksum_bits, int64_t* input_size, uint64_t* rec_bit, uint32_t* nblocks) {
-    if (!ctx || !d_src || !rec_bit || !nblocks) return -KZ_ERR_INVALID_PARAM;
-    CK(cudaSetDevice(ctx->device));
-    StreamHeader sh;
-    uint8_t head[64];
-    int rc = device_stream_header(ctx, d_src, n, head, sh);
-    if (rc) return rc;
-    if (t48) *t48 = sh.t48;
-    if (etype) *etype = sh.etype;
-    if (block_size) *block_size = sh.block_size;
-    if (checksum_bits) *checksum_bits = sh.checksum_bits;
-    if (input_size) *input_size = sh.input_size;
-    std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, max_blocks, 0}};
-    std::vector<Walked> w;
-    rc = walk_streams(ctx, (const uint32_t*)d_src, wj, -1, -1, w);
-    if (rc) return rc;
-    if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
-    rec_bit[0] = sh.bits;
-    for (size_t b = 0; b < w[0].bit_off.size(); b++) rec_bit[b + 1] = w[0].bit_off[b] + w[0].bits[b];
-    *nblocks = (uint32_t)w[0].n;
-    return 0;
-}
+// A stream's blocks decoded to d_dst (cap bytes). given: the header fields (as sharded decompression gets them from rank 0) and the first
+// record at start_bit, stop_after records (0: up to the end marker); else the stream's header or the headerless reader setting.
 static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
                                   size_t n, void* d_dst, size_t cap, size_t* out_n) {
     if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
@@ -2303,12 +2249,11 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     if (given) {
         sh = *given;
         sh.bits = start_bit;
-    } else {
+    } else {  // the stream's header, or the headerless reader setting (a headerless stream has no header to read)
         uint8_t head[64];
-        memset(head, 0, sizeof(head));
-        CK(cudaMemcpyAsync(head, d_src, std::min<size_t>(n, 64), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        rc = parse_stream_header(ctx, head, n, sh);
+        const uint64_t off = 0, len = ctx->headerless_reader.on ? 0 : n;
+        rc = gather_heads(ctx, (const uint8_t*)d_src, &off, &len, 1, 64, head);
+        if (rc == 0) rc = stream_header(ctx, head, n, sh);
         if (rc) return rc;
     }
     TransformPlan plan;
@@ -2335,6 +2280,53 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     return 0;
 }
 
+int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
+    return decompress_device_impl(ctx, nullptr, 0, 0, ctx ? ctx->range_from : -1, ctx ? ctx->range_to : -1, d_src, n, d_dst, cap, out_n);
+}
+// Decodes `nblocks` block records that start at bit `start_bit` of the fragment at d_src (frag_bytes bytes, >= 64 readable bytes behind them):
+// what one rank of a sharded decompression does with its part of the stream. The stream parameters come from the header rank 0 parsed.
+int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src, size_t frag_bytes,
+                                  uint64_t start_bit, uint32_t nblocks, void* d_dst, size_t cap, size_t* out_n) {
+    if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
+    *out_n = 0;
+    if (nblocks == 0) return 0;
+    StreamHeader sh;
+    sh.t48 = t48;
+    sh.etype = etype;
+    sh.block_size = block_size;
+    sh.checksum_bits = checksum_bits;
+    sh.input_size = 0;
+    sh.bits = 0;
+    return decompress_device_impl(ctx, &sh, start_bit, nblocks, -1, -1, d_src, frag_bytes, d_dst, cap, out_n);
+}
+// Parses the header of the stream at d_src and walks its block records: rec_bit[b] = first bit of record b (its 5-bit prefix), rec_bit[nblocks] =
+// first bit behind the last record (the end marker). rec_bit must hold max_blocks + 1 entries. With a headerless reader setting the fields are
+// the setting's and rec_bit[0] = 0.
+int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t max_blocks, uint64_t* t48, uint32_t* etype, uint32_t* block_size,
+                           uint32_t* checksum_bits, int64_t* input_size, uint64_t* rec_bit, uint32_t* nblocks) {
+    if (!ctx || !d_src || !rec_bit || !nblocks) return -KZ_ERR_INVALID_PARAM;
+    CK(cudaSetDevice(ctx->device));
+    StreamHeader sh;
+    uint8_t head[64];
+    const uint64_t off = 0, len = n;
+    int rc = gather_heads(ctx, (const uint8_t*)d_src, &off, &len, 1, 64, head);
+    if (rc == 0) rc = stream_header(ctx, head, n, sh);
+    if (rc) return rc;
+    if (t48) *t48 = sh.t48;
+    if (etype) *etype = sh.etype;
+    if (block_size) *block_size = sh.block_size;
+    if (checksum_bits) *checksum_bits = sh.checksum_bits;
+    if (input_size) *input_size = sh.input_size;
+    std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, max_blocks, 0}};
+    std::vector<Walked> w;
+    rc = walk_streams(ctx, (const uint32_t*)d_src, wj, -1, -1, w);
+    if (rc) return rc;
+    if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
+    rec_bit[0] = sh.bits;
+    for (size_t b = 0; b < w[0].bit_off.size(); b++) rec_bit[b + 1] = w[0].bit_off[b] + w[0].bits[b];
+    *nblocks = (uint32_t)w[0].n;
+    return 0;
+}
 // ---- whole stream, host buffers ------------------------------------------------------------------------------
 int kz_compress_stream(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size,
                        const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
@@ -2422,58 +2414,21 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
                                  const uint64_t* dst_cap, uint64_t* out_len, int32_t* status, std::vector<uint64_t>& stage_off, uint64_t* stage_base,
                                  uint64_t* stage_total) {
     ctx->stream_bs = block_size;
-    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
-    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
+    int rc = check_encode_args(ctx, block_size, checksum_bits);
+    if (rc) return rc;
     if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
     TransformPlan plan;
-    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
     if (rc) return rc;
-    // the blocks of every stream, stream after stream (Writer.Write cuts the input into blockSize pieces)
-    std::vector<uint64_t> boff;
-    std::vector<uint32_t> blen, first(nstreams + 1);
-    for (uint32_t s = 0; s < nstreams; s++) {
-        first[s] = (uint32_t)blen.size();
-        for (uint64_t o = 0; o < src_len[s]; o += block_size) {
-            boff.push_back(src_off[s] + o);
-            blen.push_back((uint32_t)std::min<uint64_t>(block_size, src_len[s] - o));
-        }
-    }
-    const uint32_t nb = (uint32_t)blen.size();
-    first[nstreams] = nb;
-    // ctx["dataType"] of every block from its first four bytes (encodingTask.encode :806-816), gathered in one copy; with skipBlocks the
-    // blocks stored raw, from the same heads and the entropy flags that follow them
-    std::vector<int32_t> dts(nb, 0);
-    std::vector<uint8_t> store;
-    const bool skip = ctx->skip_blocks;
-    if ((plan.uses_magic() || skip) && nb) {
-        uint8_t* d_heads = nullptr;
-        if (skip) {
-            rc = skip_test(ctx, d_src, boff, blen, &d_heads);
-            if (rc) return rc;
-        } else {
-            CK(ctx->d_asm.ensure((size_t)nb * 4));
-            CK(cudaMemsetAsync(ctx->d_asm.p, 0, (size_t)nb * 4, ctx->stream));
-            d_heads = ctx->d_asm.as<uint8_t>();
-        }
-        CopyList heads;
-        for (uint32_t b = 0; b < nb; b++) heads.add(d_src + boff[b], d_heads + 4 * (size_t)b, std::min<uint32_t>(4, blen[b]));
-        rc = run_copies(ctx, heads);
-        if (rc) return rc;
-        std::vector<uint8_t> h((size_t)nb * (skip ? 5 : 4));
-        CK(cudaMemcpyAsync(h.data(), d_heads, h.size(), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        if (plan.uses_magic())
-            for (uint32_t b = 0; b < nb; b++) dts[b] = magic_data_type(&h[(size_t)b * 4], blen[b]);
-        if (skip) store = stored_blocks(ctx, h, blen.data(), nb);
-    }
-    std::vector<uint64_t> hv;
-    if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
-        rc = hash_blocks(ctx, d_src, boff, blen, checksum_bits, hv);
-        if (rc) return rc;
-    }
+    // the blocks of every stream, stream after stream, prepared together before the passes
+    const BlockList bl = cut_blocks(src_off, src_len, nstreams, block_size);
+    const uint32_t nb = bl.size();
+    BlockPrep prep;
+    rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, d_src, bl, prep);
+    if (rc) return rc;
     // passes: transforms and entropy coding of the blocks of a pass, then their bit strings packed into ctx->d_bits
     const EntropyScratch es = entropy_scratch(etype);
-    const PassPlan P = plan_compress_passes(blen, [&](uint64_t s) { return compress_block_cost(s, es); });
+    const PassPlan P = plan_compress_passes(bl.len, [&](uint64_t s) { return compress_block_cost(s, es); });
     std::vector<uint64_t> bbits(nb), barena(nb);
     uint64_t arena = 0;
     for (uint32_t p = 0; p < P.npasses(); p++) {
@@ -2482,32 +2437,26 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
         CK(ctx->d_slots.ensure(s * k + 64));
         uint8_t* slots = ctx->d_slots.as<uint8_t>();
         std::vector<uint32_t> lens(k);
-        std::vector<int32_t> pdt(k);
-        std::vector<uint8_t> pstore(store.empty() ? 0 : k);
         CopyList place;
         uint32_t max_len = 0;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t b = P.order[i0 + j];
-            lens[j] = blen[b];
-            pdt[j] = dts[b];
-            if (!store.empty()) pstore[j] = store[b];
-            max_len = std::max(max_len, blen[b]);
-            place.add(d_src + boff[b], slots + j * s, blen[b]);
+            lens[j] = bl.len[b];
+            max_len = std::max(max_len, bl.len[b]);
+            place.add(d_src + bl.off[b], slots + j * s, bl.len[b]);
         }
         rc = run_copies(ctx, place);
         if (rc) return rc;
         const uint8_t* d_data = nullptr;
         std::vector<EncJob> jobs;
-        rc = forward_stage(ctx, plan, slots, 0, block_size, s, lens.data(), k, &d_data, jobs, &pdt, pstore.empty() ? nullptr : &pstore);
+        rc = forward_stage(ctx, plan, slots, s, lens, prep.pick(&P.order[i0], k), &d_data, jobs);
         if (rc) return rc;
-        if (checksum_bits)
-            for (uint32_t j = 0; j < k; j++) jobs[j].checksum = hv[P.order[i0 + j]];
         const uint64_t ostride = round16(kz_max_block_output(max_len));
         CK(ctx->d_enc.ensure(ostride * k + 64));
         std::vector<uint64_t> base(k);
         for (uint32_t j = 0; j < k; j++) base[j] = 8 * (uint64_t)j * ostride;
         EncResult res;
-        rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, ctx->d_enc.as<uint8_t>(), ostride * k, base, res);
+        rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, false, false, ctx->d_enc.as<uint8_t>(), ostride * k, base, res);
         if (rc) return rc;
         uint64_t need = arena;
         for (uint32_t j = 0; j < k; j++) need += round16((res.blk_bits[j] + 7) / 8);
@@ -2541,7 +2490,7 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
             memcpy(&small[64 * (size_t)s], hdr.data(), 64);
         }
         uint64_t bits = hdr_bits[s] + END_MARKER_BITS;
-        for (uint32_t b = first[s]; b < first[s + 1]; b++) {
+        for (uint32_t b = bl.first[s]; b < bl.first[s + 1]; b++) {
             pre_bits[b] = write_block_prefix(&small[64 * (size_t)nstreams + 8 * (size_t)b], bbits[b]);
             bits += pre_bits[b] + bbits[b];
             nsegs += 1 + (bbits[b] + 8 * RAW_PIECE - 1) / (8 * RAW_PIECE);
@@ -2569,7 +2518,7 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
             d += nbits;
         };
         if (hdr_bits[s]) add(A + 64 * (size_t)s, hdr_bits[s]);
-        for (uint32_t b = first[s]; b < first[s + 1]; b++) {
+        for (uint32_t b = bl.first[s]; b < bl.first[s + 1]; b++) {
             add(A + 64 * (size_t)nstreams + 8 * (size_t)b, pre_bits[b]);
             for (uint64_t o = 0; o < bbits[b]; o += 8 * RAW_PIECE) add(ctx->d_bits.as<uint8_t>() + barena[b] + o / 8, std::min<uint64_t>(8 * RAW_PIECE, bbits[b] - o));
         }
@@ -2647,62 +2596,40 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     return 0;
 }
 
-static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64_t start_bit, uint32_t stop_after, int64_t from, int64_t to, const void* d_src,
-                                  size_t n, void* d_dst, size_t cap, size_t* out_n);
-
 // Decodes stream s = d_src[src_off[s] : + src_len[s]] (>= 64 readable bytes behind it) to d_dst + dst_off[s]. src_bytes: readable bytes at d_src.
 static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off, const uint64_t* src_len,
                                    uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
     for (uint32_t s = 0; s < nstreams; s++) status[s] = 0, out_len[s] = 0;
     if (nstreams == 0) return 0;
-    int rc = 0;
+    // headers: the first 64 bytes of every stream in one gather (a headerless stream has none to read), then each stream's header or the
+    // headerless reader setting; the streams with the same header fields form a group
+    std::vector<uint8_t> head(64 * (size_t)nstreams);
+    std::vector<uint64_t> head_len(nstreams, 0);
+    if (!ctx->headerless_reader.on) head_len.assign(src_len, src_len + nstreams);
+    int rc = gather_heads(ctx, d_src, src_off, head_len.data(), nstreams, 64, head.data());
+    if (rc) return rc;
+    std::vector<StreamHeader> sh(nstreams);
+    std::vector<TransformPlan> plan(nstreams);
+    std::vector<uint64_t> hdr_bits(nstreams, 0);
+    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
+    for (uint32_t s = 0; s < nstreams; s++) {
+        status[s] = stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
+        if (status[s]) continue;
+        rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
+        if (rc) return rc;
+        if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
+        hdr_bits[s] = sh[s].bits;
+        groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
+    }
     std::vector<uint32_t> alone;
-    const bool headerless = ctx->headerless_reader.on;
-    const StreamHeader hl = headerless ? headerless_header(ctx) : StreamHeader();
-    if (headerless) {  // no headers to gather: every stream has the setting's fields, so all of them form one group
-        TransformPlan plan;
-        rc = plan_transforms(ctx, hl.t48, hl.etype, plan, KZ_ERR_INVALID_CODEC);
+    for (auto& kv : groups) {
+        const uint32_t s0 = kv.second[0];
+        rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
         if (rc) return rc;
-        std::vector<uint32_t> all(nstreams);
-        for (uint32_t s = 0; s < nstreams; s++) all[s] = s;
-        rc = decode_stream_group(ctx, hl, plan, all, std::vector<uint64_t>(nstreams, 0), d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len,
-                                 status, alone);
-        if (rc) return rc;
-    } else {
-        // headers: the first 64 bytes of every stream in one gather and one transfer, parsed by parse_stream_header
-        CK(ctx->d_asm.ensure(64 * (size_t)nstreams));
-        CK(cudaMemsetAsync(ctx->d_asm.p, 0, 64 * (size_t)nstreams, ctx->stream));
-        CopyList heads;
-        for (uint32_t s = 0; s < nstreams; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
-        rc = run_copies(ctx, heads);
-        if (rc) return rc;
-        std::vector<uint8_t> head(64 * (size_t)nstreams);
-        CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        std::vector<StreamHeader> sh(nstreams);
-        std::vector<TransformPlan> plan(nstreams);
-        std::vector<uint64_t> hdr_bits(nstreams, 0);
-        std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
-        for (uint32_t s = 0; s < nstreams; s++) {
-            status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
-            if (status[s]) continue;
-            rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
-            if (rc) return rc;
-            if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
-            hdr_bits[s] = sh[s].bits;
-            groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
-        }
-        for (auto& kv : groups) {
-            const uint32_t s0 = kv.second[0];
-            rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status,
-                                     alone);
-            if (rc) return rc;
-        }
     }
     for (uint32_t s : alone) {  // only corrupt input, too little room or a failing stage call gets here
         size_t n = 0;
-        status[s] = decompress_device_impl(ctx, headerless ? &hl : nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s],
-                                           d_dst + dst_off[s], dst_cap[s], &n);
+        status[s] = decompress_device_impl(ctx, nullptr, 0, 0, ctx->range_from, ctx->range_to, d_src + src_off[s], src_len[s], d_dst + dst_off[s], dst_cap[s], &n);
         out_len[s] = status[s] ? 0 : n;
     }
     return 0;
@@ -3263,12 +3190,9 @@ int read_ranges(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, 
         if (!src && ((uintptr_t)d_src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
         // the stream the index was built from: its length and its leading bytes
         uint8_t head[INDEX_HEAD] = {0};
-        const size_t nh = n == ix->stream_bytes ? std::min<size_t>(n, INDEX_HEAD) : 0;
-        if (src) memcpy(head, src, nh);
-        else if (nh) {
-            CK(cudaMemcpyAsync(head, d_src, nh, cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-        }
+        const uint64_t at = 0, nh = n == ix->stream_bytes ? n : 0;
+        if (src) memcpy(head, src, std::min<uint64_t>(nh, INDEX_HEAD));
+        else if ((r = gather_heads(ctx, (const uint8_t*)d_src, &at, &nh, 1, INDEX_HEAD, head))) return r;
         r = read_stream_check(ctx, ix, n, head);
         if (r) return r;
         return read_ranges_impl(ctx, cache, src, (const uint8_t*)d_src, {ReadSource{ix, 0, n}}, nreq, nullptr, off, len, (uint8_t*)dst, dst_off, out_len,
@@ -3303,25 +3227,16 @@ int read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_inde
             names.push_back(s);
         }
         if (device && ((uintptr_t)base & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-        // the first 32 bytes of every named stream: copied on the host, or gathered by one copy launch and brought back in one transfer
-        // (one stream: copied straight back, as kz_read_ranges_device does)
+        // the first 32 bytes of every named stream: copied on the host, or gathered on the device (one stream: copied straight back, as
+        // kz_read_ranges_device does)
         const size_t nn = names.size();
         std::vector<uint8_t> head(INDEX_HEAD * nn, 0);
-        auto nh = [&](size_t j) { return std::min<uint64_t>(src_len[names[j]], INDEX_HEAD); };
+        std::vector<uint64_t> hoff(nn), hlen(nn);
+        for (size_t j = 0; j < nn; j++) hoff[j] = src_off[names[j]], hlen[j] = src_len[names[j]];
         if (!device) {
-            for (size_t j = 0; j < nn; j++) memcpy(&head[INDEX_HEAD * j], base + src_off[names[j]], nh(j));
-        } else if (nn == 1 && nh(0)) {
-            CK(cudaMemcpyAsync(head.data(), base + src_off[names[0]], nh(0), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-        } else if (nn > 1) {
-            CK(ctx->d_asm.ensure(INDEX_HEAD * nn + 64));
-            CopyList heads;
-            for (size_t j = 0; j < nn; j++) heads.add(base + src_off[names[j]], ctx->d_asm.as<uint8_t>() + INDEX_HEAD * j, nh(j));
-            r = run_copies(ctx, heads);
-            if (r) return r;
-            CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            for (size_t j = 0; j < nn; j++) memset(&head[INDEX_HEAD * j + nh(j)], 0, INDEX_HEAD - nh(j));
+            for (size_t j = 0; j < nn; j++) memcpy(&head[INDEX_HEAD * j], base + hoff[j], std::min<uint64_t>(hlen[j], INDEX_HEAD));
+        } else if ((r = gather_heads(ctx, base, hoff.data(), hlen.data(), nn, INDEX_HEAD, head.data()))) {
+            return r;
         }
         // per stream: a missing or stale index or a chain without a GPU path fails the stream's requests with kz_read_ranges's code
         std::vector<int32_t> code(nstreams, 0);
@@ -3350,31 +3265,18 @@ int read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_inde
     return finish_streams(nreq, status, out_len, rc);
 }
 
-// kz_index_build_device for the streams d_src + src_off[s] (src_len[s] bytes each, >= 64 readable bytes behind each): every header in
-// one gather launch and one transfer, every stream's records in the two walk_streams launches of one build.
+// The indexes of the streams d_src + src_off[s] (src_len[s] bytes each, >= 64 readable bytes behind each), kz_index_build_device being
+// the one-stream case: every header in one gather_heads, every stream's records in the two walk_streams launches of one build.
 int index_build_streams(kz_ctx* ctx, uint32_t ns, const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out, int32_t* status) {
     if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
-    std::vector<uint8_t> head(64 * (size_t)ns, 0);
-    if (ns) {
-        CK(ctx->d_asm.ensure(64 * (size_t)ns + 64));
-        CopyList heads;
-        for (uint32_t s = 0; s < ns; s++) heads.add(d_src + src_off[s], ctx->d_asm.as<uint8_t>() + 64 * (size_t)s, std::min<uint64_t>(64, src_len[s]));
-        int rc = run_copies(ctx, heads);
-        if (rc) return rc;
-        CK(cudaMemcpyAsync(head.data(), ctx->d_asm.p, head.size(), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (uint32_t s = 0; s < ns; s++) {
-            const uint64_t nh = std::min<uint64_t>(64, src_len[s]);
-            memset(&head[64 * (size_t)s + nh], 0, 64 - nh);
-        }
-    }
+    std::vector<uint8_t> head(64 * (size_t)ns);
+    int rc = gather_heads(ctx, d_src, src_off, src_len, ns, 64, head.data());
+    if (rc) return rc;
     std::vector<StreamHeader> sh(ns);
     std::vector<WalkJob> wj;
     std::vector<uint32_t> who;
     for (uint32_t s = 0; s < ns; s++) {
-        status[s] = 0;
-        if (ctx->headerless_reader.on) sh[s] = headerless_header(ctx);
-        else if ((status[s] = parse_stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]))) continue;
+        if ((status[s] = stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]))) continue;
         TransformPlan plan;
         if ((status[s] = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan, KZ_ERR_CREATE_CODEC))) continue;
         if (!etype_supported(sh[s].etype)) {
@@ -3387,7 +3289,7 @@ int index_build_streams(kz_ctx* ctx, uint32_t ns, const uint8_t* d_src, const ui
     // every record is kept, so the walk runs twice: once storing nothing (an empty block range) for the count, once to store them
     std::vector<Walked> w;
     if (!wj.empty()) {
-        int rc = walk_streams(ctx, (const uint32_t*)d_src, wj, 0, 1, w);
+        rc = walk_streams(ctx, (const uint32_t*)d_src, wj, 0, 1, w);
         if (rc) return rc;
     }
     std::vector<WalkJob> wj2;
@@ -3399,7 +3301,7 @@ int index_build_streams(kz_ctx* ctx, uint32_t ns, const uint8_t* d_src, const ui
         else if (w[j].n) wj2.push_back(WalkJob{8 * src_off[s] + sh[s].bits, 8 * (src_off[s] + src_len[s]), 0, (uint32_t)w[j].n, 0}), who2.push_back(s);
     }
     if (!wj2.empty()) {
-        int rc = walk_streams(ctx, (const uint32_t*)d_src, wj2, -1, -1, w2);
+        rc = walk_streams(ctx, (const uint32_t*)d_src, wj2, -1, -1, w2);
         if (rc) return rc;
     }
     std::vector<std::unique_ptr<kz_index>> built(ns);
@@ -3462,39 +3364,10 @@ int kz_index_build_device(kz_ctx* ctx, const void* d_src, size_t n, kz_index** o
     CK(cudaSetDevice(ctx->device));
     if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
     if ((uintptr_t)d_src & 15) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    StreamHeader sh;
-    uint8_t head[64];
-    int rc = device_stream_header(ctx, d_src, n, head, sh);
-    if (rc) return rc;
-    TransformPlan plan;
-    rc = plan_transforms(ctx, sh.t48, sh.etype, plan, KZ_ERR_CREATE_CODEC);
-    if (rc) return rc;
-    if (!etype_supported(sh.etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
-    // every record is kept, so the walk runs twice: once storing nothing (an empty block range) for the count, once to store them
-    std::vector<Walked> w;
-    for (int store = 0; store < 2; store++) {
-        const uint32_t count = store ? (uint32_t)w[0].n : 0;
-        if (store && count == 0) break;
-        std::vector<WalkJob> wj{WalkJob{sh.bits, 8ull * n, 0, count, 0}};
-        rc = walk_streams(ctx, (const uint32_t*)d_src, wj, store ? -1 : 0, store ? -1 : 1, w);
-        if (rc) return rc;
-        if (w[0].status) return ctx->fail(-w[0].status, "Invalid bitstream: corrupted block length");
-    }
-    std::unique_ptr<kz_index> ix(new kz_index());
-    ix->t48 = sh.t48;
-    ix->etype = sh.etype;
-    ix->block_size = sh.block_size;
-    ix->checksum_bits = sh.checksum_bits;
-    ix->header_bits = (uint32_t)sh.bits;
-    ix->input_size = sh.input_size;
-    ix->stream_bytes = n;
-    memcpy(ix->head, head, INDEX_HEAD);
-    ix->start = w[0].bit_off;
-    ix->bits = w[0].bits;
-    ix->size = ix->start.empty() ? 0 : -1;
-    if (!index_consistent(*ix)) return ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: the records do not form an index");
-    *out = ix.release();
-    return 0;
+    const uint64_t off = 0, len = n;
+    int32_t status = 0;
+    const int rc = index_build_streams(ctx, 1, (const uint8_t*)d_src, &off, &len, out, &status);
+    return rc ? rc : status;
 }
 
 int kz_index_build(kz_ctx* ctx, const uint8_t* src, size_t n, kz_index** out) {
@@ -3664,40 +3537,29 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     for (uint32_t b = 0; b < nblocks; b++)
         if (block_len[b])
             CK(cudaMemcpyAsync((uint8_t*)ctx->d_in.p + b * dstride, slab + b * block_stride, block_len[b], cudaMemcpyHostToDevice, ctx->stream));
-    std::vector<EncJob> jobs;
     TransformPlan plan;
     int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
     if (rc) return rc;
-    const uint8_t* d_data = nullptr;
-    std::vector<int32_t> init_dt(nblocks, 0);
-    for (uint32_t b = 0; b < nblocks; b++) init_dt[b] = magic_data_type(slab + b * block_stride, block_len[b]);
-    std::vector<uint8_t> store;
-    if (ctx->skip_blocks) {  // skipBlocks: the heads are in host memory, only the entropy flags come back
-        std::vector<uint64_t> boff(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) boff[b] = b * dstride;
-        uint8_t* d_heads = nullptr;
-        rc = skip_test(ctx, ctx->d_in.as<uint8_t>(), boff, std::vector<uint32_t>(block_len, block_len + nblocks), &d_heads);
-        if (rc) return rc;
-        std::vector<uint8_t> hf((size_t)nblocks * 5, 0);
-        for (uint32_t b = 0; b < nblocks; b++) memcpy(&hf[(size_t)b * 4], slab + b * block_stride, std::min<uint32_t>(4, block_len[b]));
-        CK(cudaMemcpyAsync(&hf[(size_t)nblocks * 4], d_heads + (size_t)nblocks * 4, nblocks, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        store = stored_blocks(ctx, hf, block_len, nblocks);
+    // the blocks' heads are in host memory: preparing them costs no round trip
+    BlockList bl;
+    bl.len.assign(block_len, block_len + nblocks);
+    bl.first = {0, nblocks};
+    std::vector<uint8_t> heads(4 * (size_t)nblocks, 0);
+    for (uint32_t b = 0; b < nblocks; b++) {
+        bl.off.push_back(b * dstride);
+        memcpy(&heads[(size_t)b * 4], slab + b * block_stride, std::min<uint32_t>(4, block_len[b]));
     }
-    rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), 0, 0, dstride, block_len, nblocks, &d_data, jobs, &init_dt, store.empty() ? nullptr : &store);
+    BlockPrep prep;
+    rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, ctx->d_in.as<uint8_t>(), bl, prep, &heads);
     if (rc) return rc;
-    if (checksum_bits) {  // encodingTask.encode :753-763: hash of the original block
-        std::vector<uint64_t> hoff(nblocks), hv;
-        std::vector<uint32_t> hlen(block_len, block_len + nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) hoff[b] = (uint64_t)b * dstride;
-        rc = hash_blocks(ctx, ctx->d_in.as<uint8_t>(), hoff, hlen, checksum_bits, hv);
-        if (rc) return rc;
-        for (uint32_t b = 0; b < nblocks; b++) jobs[b].checksum = hv[b];
-    }
+    const uint8_t* d_data = nullptr;
+    std::vector<EncJob> jobs;
+    rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), dstride, bl.len, prep, &d_data, jobs);
+    if (rc) return rc;
     std::vector<uint64_t> base(nblocks);
     for (uint32_t b = 0; b < nblocks; b++) base[b] = 8 * (uint64_t)b * ostride;
     EncResult res;
-    rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, ctx->d_out.as<uint8_t>(), ostride * nblocks, base, res);
+    rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, false, false, ctx->d_out.as<uint8_t>(), ostride * nblocks, base, res);
     if (rc) return rc;
     for (uint32_t b = 0; b < nblocks; b++) {
         out_bits[b] = res.blk_bits[b];
@@ -3816,7 +3678,7 @@ int kz_entropy_encode(kz_ctx* ctx, uint32_t type, const uint8_t* src, size_t n, 
     jobs[0].copy = false;
     jobs[0].checksum = 0;
     EncResult res;
-    int rc = encode_batch(ctx, LAYOUT_RAW, type, 0, ctx->d_in.as<uint8_t>(), jobs, {}, 0, ctx->d_out.as<uint8_t>(), dcap, {0}, res);
+    int rc = encode_batch(ctx, LAYOUT_RAW, type, 0, ctx->d_in.as<uint8_t>(), jobs, {}, 0, false, false, ctx->d_out.as<uint8_t>(), dcap, {0}, res);
     if (rc) return rc;
     const size_t nbytes = (size_t)((res.blk_bits[0] + 7) / 8);
     if (nbytes > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
@@ -4173,8 +4035,6 @@ struct Session {
         cudaSetDevice(ctx->device);
         if (copy) cudaStreamSynchronize(copy);
         cudaStreamSynchronize(ctx->stream);
-        ctx->fragment = false;
-        ctx->volatile_lead = false;
         for (auto& e : ev)
             if (e) cudaEventDestroy(e);
         if (copy) cudaStreamDestroy(copy);
@@ -4225,11 +4085,8 @@ struct kz_writer : kz::Session {
         else lead[0] = carry;
         EncResult res;
         ctx->stream_bs = block_size;
-        ctx->fragment = !last;
-        ctx->volatile_lead = true;
-        int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, skip, d_in[k].p, in_len[k], lead, lead_bits, d_out.p, out_cap, res);
-        ctx->fragment = false;
-        ctx->volatile_lead = false;
+        int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, skip, d_in[k].p, in_len[k], lead, lead_bits, !last, true, d_out.p, out_cap,
+                                      res);
         if (rc) return rc;
         CK(cudaStreamSynchronize(ctx->stream));
         batches++;
@@ -4436,12 +4293,12 @@ int kz_writer_open(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_siz
     *out = nullptr;
     CK(cudaSetDevice(ctx->device));
     if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is already open on this context");
-    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
-    if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
+    int rc = check_encode_args(ctx, block_size, checksum_bits);
+    if (rc) return rc;
     if (batch_blocks < 1 || batch_blocks > 1024) return ctx->fail(KZ_ERR_INVALID_PARAM, "batch_blocks must be in [1..1024]");
     if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
     TransformPlan plan;
-    int rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
+    rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
     if (rc) return rc;
     kz_writer* w = new kz_writer(ctx, batch_blocks);
     w->plan = plan;

@@ -134,8 +134,6 @@ struct kz_ctx {
     bool profile = false;
     int bwt_profile = 0;  // kz_bwt_profile: bit 0 times the BWT forward rounds (with profile), bit 1 forces the 56-bit rounds
     kz::EncPlan enc_plan;
-    bool fragment = false;        // encode_batch: LAYOUT_STREAM without the end marker (kz_compress_fragment_device, a writer session)
-    bool volatile_lead = false;   // encode_batch: the leading segment is a writer session's header or carry, kept out of the plan key
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
     uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
     int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)

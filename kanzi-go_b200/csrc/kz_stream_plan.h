@@ -1,6 +1,6 @@
-// Pass planner of the many-stream entry points (kz_compress_streams / kz_decompress_streams, kz_api.cu), and the slot and error-order
-// rules of every stream-level decode. Pure host code: no CUDA types, so that tests/host/stream_plan_host.cpp compiles it with g++ and
-// checks it on the CPU.
+// Pass planner of the many-stream entry points (kz_compress_streams / kz_decompress_streams, kz_api.cu), the block cutting and
+// per-block decisions of every encode path, and the slot and error-order rules of every stream-level decode. Pure host code: no CUDA
+// types, so that tests/host/stream_plan_host.cpp compiles it with g++ and checks it on the CPU.
 //
 // A pass is a set of blocks that run through the transform and entropy stages together. Every block of a pass gets a slot of the
 // pass's stride in the device scratch buffers, so the scratch of a pass is (number of blocks) x cost(stride). The planner keeps that
@@ -28,6 +28,86 @@ struct PassPlan {
 };
 
 inline uint64_t round16(uint64_t n) { return (n + 15) & ~15ull; }
+
+const size_t SMALL_BLOCK = 15;  // io/CompressedStream.go:51: blocks of at most this many bytes are stored, whatever the options
+
+// Blocks over a base address: block b is len[b] bytes at off[b]. Cut from streams (cut_blocks), stream s holds blocks
+// first[s] .. first[s + 1] - 1; a list that was not cut from streams has first = {0, size()}.
+struct BlockList {
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> len;
+    std::vector<uint32_t> first;
+    uint32_t size() const { return (uint32_t)len.size(); }
+};
+
+// Writer.Write cuts its input into blockSize pieces: stream s (src_len[s] bytes at src_off[s]) becomes blocks of block_size bytes and a
+// shorter last one; an empty stream has no blocks.
+inline BlockList cut_blocks(const uint64_t* src_off, const uint64_t* src_len, uint32_t nstreams, uint32_t block_size) {
+    BlockList L;
+    L.first.resize(nstreams + 1);
+    for (uint32_t s = 0; s < nstreams; s++) {
+        L.first[s] = L.size();
+        for (uint64_t o = 0; o < src_len[s]; o += block_size) {
+            L.off.push_back(src_off[s] + o);
+            L.len.push_back((uint32_t)std::min<uint64_t>(block_size, src_len[s] - o));
+        }
+    }
+    L.first[nstreams] = L.size();
+    return L;
+}
+
+// The data type encodingTask.encode derives from the first four bytes of a block before the transforms run
+// (io/CompressedStream.go:806-816 over internal/Magic.go:73-112 GetMagicType and :116-206 IsDataCompressed / IsDataMultimedia /
+// IsDataExecutable): 7 = DT_BIN for compressed containers, 2 = DT_MULTIMEDIA, 3 = DT_EXE, 0 = DT_UNDEFINED otherwise.
+inline int32_t magic_data_type(const uint8_t* p, size_t n) {
+    if (n < 4) return 0;
+    const uint32_t key = ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];
+    const uint32_t k24 = key >> 8, k16 = key >> 16;
+    // compressed: JPEG (APP0 marker only: the other FFD8FFEx keys match no class), GIF, PNG, 7z, zstd, brotli, CAB, ZIP, FLAC, xz, KANZ, RAR,
+    // bzip2 / ID3 (24 bits), gzip (16 bits)
+    switch (key) {
+        case 0xFFD8FFE0u: case 0x47494638u: case 0x89504E47u: case 0x377ABCAFu: case 0x28B52FFDu: case 0x81CFB2CEu: case 0x4D534346u:
+        case 0x504B0304u: case 0x664C6143u: case 0xFD377A58u: case 0x4B414E5Au: case 0x52617221u:
+            return 7;
+        default: break;
+    }
+    if ((key & ~0x0Fu) == 0xFFD8FFE0u) return 0;  // GetMagicType returns the key itself: no class matches
+    if (k24 == 0x425A68u || k24 == 0x494433u) return 7;
+    if (key == 0x25504446u) return 0;  // PDF: recognised, in no class
+    if (key == 0x52494646u) return 2;  // RIFF
+    if (key == 0x7F454C46u || key == 0xFEEDFACEu || key == 0xCEFAEDFEu || key == 0xFEEDFACFu || key == 0xCFFAEDFEu) return 3;  // ELF, Mach-O
+    if (k16 == 0x1F8Bu) return 7;  // gzip
+    if (k16 == 0x424Du) return 2;  // BMP
+    if (k16 == 0x4D5Au) return 3;  // MZ
+    if (k16 == 0x5034u || k16 == 0x5035u || k16 == 0x5036u) {  // binary PBM / PGM / PPM: "P4".."P6" followed by white space
+        const uint32_t sub = (key >> 8) & 0xFF;
+        if (sub == 0x07 || sub == 0x0A || sub == 0x0D || sub == 0x20) return 2;
+    }
+    return 0;
+}
+
+// The blocks and bytes stored_blocks stores for each reason
+struct StoreCounts {
+    uint64_t magic_blocks = 0, magic_bytes = 0, entropy_blocks = 0, entropy_bytes = 0;
+};
+
+// kanzi's skipBlocks option (encodingTask.encode, io/CompressedStream.go:778-800), host half: block b (len[b] bytes, heads[4b ..] its
+// first four bytes, zero padded) is stored when it has more than SMALL_BLOCK bytes and its head is the magic number of a compressed
+// format (magic_data_type 7: IsDataCompressed(GetMagicType)) or its entropy flag (flags[b], the device half's test) is set. Blocks of at
+// most SMALL_BLOCK bytes are stored in any case, by the COPY rule of the forward stage: store[b] stays 0 for them.
+inline StoreCounts stored_blocks(const uint8_t* heads, const uint8_t* flags, const uint32_t* len, uint32_t nb, std::vector<uint8_t>& store) {
+    StoreCounts c;
+    store.assign(nb, 0);
+    for (uint32_t b = 0; b < nb; b++) {
+        if (len[b] <= SMALL_BLOCK) continue;
+        if (magic_data_type(&heads[(size_t)b * 4], len[b]) == 7) {
+            store[b] = 1, c.magic_blocks++, c.magic_bytes += len[b];
+        } else if (flags[b]) {
+            store[b] = 1, c.entropy_blocks++, c.entropy_bytes += len[b];
+        }
+    }
+    return c;
+}
 
 // Scratch the entropy stage (encode_batch) takes per chunk of a codec: its chunk size, and fixed + per_byte x (chunk bytes) bytes of
 // tables, headers, payload and histograms per chunk. NONE has no chunks (chunk = 0).
