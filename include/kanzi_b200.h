@@ -91,7 +91,11 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32
                      uint64_t* out_bits, int32_t* status);
 /* Replaces the concurrent part of decodingTask.decode (io/CompressedStream.go:1873-2011). Block b's bit string is
  * in[in_off[b] : in_off[b] + ceil(in_bits[b]/8)] (byte aligned, as extracted by the serial section :1816-1852).
- * Decoded bytes go to out[b*out_stride ...], out_len[b] = decoded length. block_size = stream block size (:1896). */
+ * Decoded bytes go to out[b*out_stride ...], out_len[b] = decoded length. block_size = stream block size (:1896).
+ * Every block is decoded as if it were alone in the call: status[b] = 0 or the code of decoding block b alone (a bad block header, a
+ * failed entropy decode or inverse transform, a checksum mismatch, or -KZ_ERR_WRITE_FILE when its decoded length exceeds out_stride).
+ * status[] and out_len[] are written for every block; a failed block gets out_len[b] = 0, and every other block its decoded bytes.
+ * Returns 0, or the code (kz_last_error: the message) of the first failing block in index order. */
 int kz_decode_blocks(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t checksum_bits, const uint8_t* in,
                      const uint64_t* in_off, const uint64_t* in_bits, uint32_t nblocks, uint32_t block_size, uint8_t* out,
                      uint64_t out_stride, uint32_t* out_len, int32_t* status);

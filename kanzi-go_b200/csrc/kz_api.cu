@@ -296,20 +296,6 @@ int hash_blocks(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>&
 
 // decodingTask.decode :1990-2006: hash of the decoded block against the transmitted checksum
 const char* const CHECKSUM_MISMATCH = "Corrupted bitstream: block checksum mismatch";
-int verify_checksums(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint32_t bits,
-                     std::vector<DecJob>& jobs) {
-    std::vector<uint64_t> hv;
-    int rc = hash_blocks(ctx, d_base, off, len, bits, hv);
-    if (rc) return rc;
-    for (size_t b = 0; b < jobs.size(); b++) {
-        const uint64_t want = bits == 32 ? (jobs[b].checksum & 0xFFFFFFFFull) : jobs[b].checksum;
-        if (hv[b] != want) {
-            jobs[b].status = -KZ_ERR_CRC_CHECK;
-            return ctx->fail(KZ_ERR_CRC_CHECK, CHECKSUM_MISMATCH);
-        }
-    }
-    return 0;
-}
 
 bool etype_supported(uint32_t e) { return e == KZ_E_NONE || e == KZ_E_ANS0 || e == KZ_E_HUFFMAN || e == KZ_E_ANS1 || e == KZ_E_RANGE; }
 
@@ -1783,6 +1769,26 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
     return 0;
 }
 
+// Transforms and entropy codes the blocks of a batch laid out in slots of one stride (block j: len[j] bytes at d_slots + j * stride). Block
+// j's bit string goes to ctx->d_enc + j * *ostride (ostride: kz_max_block_output of the longest block, rounded to 16) and is bits[j] long.
+int encode_slots(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t checksum_bits, const uint8_t* d_slots, uint64_t stride,
+                 const std::vector<uint32_t>& len, const BlockPrep& prep, uint64_t* ostride, std::vector<uint64_t>& bits) {
+    const uint32_t k = (uint32_t)len.size();
+    const uint8_t* d_data = nullptr;
+    std::vector<EncJob> jobs;
+    int rc = forward_stage(ctx, plan, d_slots, stride, len, prep, &d_data, jobs);
+    if (rc) return rc;
+    *ostride = round16(kz_max_block_output(*std::max_element(len.begin(), len.end())));
+    CK(ctx->d_enc.ensure(*ostride * k + 64));
+    std::vector<uint64_t> base(k);
+    for (uint32_t j = 0; j < k; j++) base[j] = 8 * (uint64_t)j * *ostride;
+    EncResult res;
+    rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, false, false, ctx->d_enc.as<uint8_t>(), *ostride * k, base, res);
+    if (rc) return rc;
+    bits = res.blk_bits;
+    return 0;
+}
+
 // Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186) of every block of a batch. The entropy
 // stage left block b's pre_len bytes at d_pre + b*pstride, a scratch buffer of this context with room for pstride - 64 bytes per
 // block; the stages alternate between it and ctx->d_tmp2. out_len[b] = decoded length of block b. Once the lengths are known,
@@ -1936,6 +1942,44 @@ int decode_walked(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan
         if (hv[i] != want) fail[owner[idx[i]]].note(STAGE_CHECKSUM, -KZ_ERR_CRC_CHECK, CHECKSUM_MISMATCH);
     }
     return 0;
+}
+
+// The block stages of block records of one header, each block on its own: decode_walked with one DecodeFailure per block, then every
+// failed block of a batch of several is decoded again alone, so that fail[i] is what decoding block i alone gives. A failing stage call
+// cannot name its block, and one block's failure may hide a later one's; only corrupt input pays. A block that place refused is not
+// decoded again. jobs (bit_off / bits set), last and place are decode_walked's; len[i] is the decoded length place was last given for
+// block i (0 when it never was).
+template <class Place>
+int decode_isolated(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan, const uint32_t* d_words, uint64_t words_len, const std::vector<DecJob>& jobs,
+                    const std::vector<uint8_t>& last, Place&& place, uint8_t* d_dst, std::vector<DecodeFailure>& fail, std::vector<uint32_t>& len) {
+    const uint32_t nb = (uint32_t)jobs.size();
+    fail.assign(nb, DecodeFailure());
+    len.assign(nb, 0);
+    std::vector<uint8_t> refused(nb, 0);
+    auto decode = [&](const std::vector<uint32_t>& ids) {
+        std::vector<DecJob> run;
+        std::vector<uint32_t> owner;
+        std::vector<uint8_t> run_last;
+        for (uint32_t b : ids) run.push_back(jobs[b]), owner.push_back((uint32_t)owner.size()), run_last.push_back(last[b]);
+        std::vector<DecodeFailure> f(ids.size());
+        auto put = [&](uint32_t i, uint32_t n) {
+            const uint32_t b = ids[i];
+            const uint64_t at = place(b, n);
+            len[b] = n;
+            refused[b] = at == NO_ROOM;
+            return at;
+        };
+        int rc = decode_walked(ctx, sh, plan, d_words, words_len, run, owner, run_last, put, d_dst, f.data());
+        for (size_t i = 0; i < ids.size(); i++) fail[ids[i]] = f[i];
+        return rc;
+    };
+    std::vector<uint32_t> all(nb);
+    std::iota(all.begin(), all.end(), 0u);
+    int rc = decode(all);
+    if (rc || nb == 1) return rc;
+    for (uint32_t b = 0; b < nb && !rc; b++)
+        if (fail[b].failed() && !refused[b]) rc = decode({b});
+    return rc;
 }
 
 
@@ -2438,35 +2482,26 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
         uint8_t* slots = ctx->d_slots.as<uint8_t>();
         std::vector<uint32_t> lens(k);
         CopyList place;
-        uint32_t max_len = 0;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t b = P.order[i0 + j];
             lens[j] = bl.len[b];
-            max_len = std::max(max_len, bl.len[b]);
             place.add(d_src + bl.off[b], slots + j * s, bl.len[b]);
         }
         rc = run_copies(ctx, place);
         if (rc) return rc;
-        const uint8_t* d_data = nullptr;
-        std::vector<EncJob> jobs;
-        rc = forward_stage(ctx, plan, slots, s, lens, prep.pick(&P.order[i0], k), &d_data, jobs);
-        if (rc) return rc;
-        const uint64_t ostride = round16(kz_max_block_output(max_len));
-        CK(ctx->d_enc.ensure(ostride * k + 64));
-        std::vector<uint64_t> base(k);
-        for (uint32_t j = 0; j < k; j++) base[j] = 8 * (uint64_t)j * ostride;
-        EncResult res;
-        rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, false, false, ctx->d_enc.as<uint8_t>(), ostride * k, base, res);
+        uint64_t ostride = 0;
+        std::vector<uint64_t> bits;
+        rc = encode_slots(ctx, plan, etype, checksum_bits, slots, s, lens, prep.pick(&P.order[i0], k), &ostride, bits);
         if (rc) return rc;
         uint64_t need = arena;
-        for (uint32_t j = 0; j < k; j++) need += round16((res.blk_bits[j] + 7) / 8);
+        for (uint32_t j = 0; j < k; j++) need += round16((bits[j] + 7) / 8);
         rc = ensure_keep(ctx, ctx->d_bits, arena, need + 64);
         if (rc) return rc;
         CopyList pack;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t b = P.order[i0 + j];
-            const uint64_t nbytes = (res.blk_bits[j] + 7) / 8;
-            bbits[b] = res.blk_bits[j];
+            const uint64_t nbytes = (bits[j] + 7) / 8;
+            bbits[b] = bits[j];
             barena[b] = arena;
             pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + arena, nbytes);
             arena += round16(nbytes);
@@ -2953,7 +2988,6 @@ int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uin
 
     std::vector<int32_t> blk_status(nk, 0);
     std::vector<uint32_t> blk_len(nk, 0);
-    std::vector<uint8_t> too_long(nk, 0);
     std::vector<uint64_t> bit_off(nk, 0);
     for (uint32_t i = 0; i < nreq; i++) status[i] = 0, out_len[i] = 0;
     std::vector<uint32_t> uns(ns, nk);  // per stream: its first touched pair whose length breaks the block arithmetic
@@ -3028,45 +3062,23 @@ int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uin
         }
         CK(ctx->d_slots.ensure(astride * (e - a) + 64));
         uint8_t* arena = ctx->d_slots.as<uint8_t>();
-        // decodes pairs ks of the pass into their arena slots, one DecodeFailure per block
-        auto decode = [&](const std::vector<uint32_t>& ks) -> int {
-            std::vector<DecJob> jobs(ks.size(), DecJob());
-            std::vector<uint32_t> owner(ks.size());
-            std::vector<uint8_t> last(ks.size());
-            std::vector<DecodeFailure> fail(ks.size());
-            for (size_t i = 0; i < ks.size(); i++) {
-                jobs[i].bit_off = bit_off[ks[i]];
-                jobs[i].bits = IX(ks[i]).bits[P.blocks[ks[i]]];
-                owner[i] = (uint32_t)i;
-                last[i] = is_last(ks[i]);
-                too_long[ks[i]] = 0;
-            }
-            auto place = [&](uint32_t i, uint32_t n_out) {
-                blk_len[ks[i]] = n_out;
-                if (n_out > bs) {
-                    too_long[ks[i]] = 1;
-                    return NO_ROOM;
-                }
-                return (uint64_t)slot_of[ks[i]] * astride;
-            };
-            int r = decode_walked(ctx, sh, plan, in.d_words, in.words_len, jobs, owner, last, place, arena, fail.data());
-            if (r) return r;
-            for (size_t i = 0; i < ks.size(); i++) blk_status[ks[i]] = fail[i].failed() ? fail[i].code : 0;
-            return 0;
-        };
-        rc = decode(ks);
+        // the pairs ks of the pass into their arena slots; a block longer than block_size has no slot and fails
+        std::vector<DecJob> jobs(ks.size(), DecJob());
+        std::vector<uint8_t> last(ks.size());
+        for (size_t i = 0; i < ks.size(); i++) {
+            jobs[i].bit_off = bit_off[ks[i]];
+            jobs[i].bits = IX(ks[i]).bits[P.blocks[ks[i]]];
+            last[i] = is_last(ks[i]);
+        }
+        std::vector<DecodeFailure> fail;
+        std::vector<uint32_t> olen;
+        rc = decode_isolated(ctx, sh, plan, in.d_words, in.words_len, jobs, last,
+                             [&](uint32_t i, uint32_t n) { return n > bs ? NO_ROOM : (uint64_t)slot_of[ks[i]] * astride; }, arena, fail, olen);
         if (rc) return rc;
-        // A failing stage call cannot name its block, and a failure of one block may hide a later one's: every failed block of a pass
-        // of several is decoded again alone, so that its status is the one a decode of that block alone gives. Only corrupt input pays.
-        if (ks.size() > 1)
-            for (uint32_t k : ks)
-                if (blk_status[k] && !too_long[k]) {
-                    rc = decode(std::vector<uint32_t>{k});
-                    if (rc) return rc;
-                }
+        for (size_t i = 0; i < ks.size(); i++) blk_status[ks[i]] = fail[i].code, blk_len[ks[i]] = olen[i];
         for (uint32_t k : ks) {
             const uint32_t s = P.stream[k];
-            if (too_long[k] || (!blk_status[k] && (is_last(k) ? blk_len[k] == 0 : blk_len[k] != bs))) uns[s] = std::min(uns[s], k);
+            if (blk_len[k] > bs || (!blk_status[k] && (is_last(k) ? blk_len[k] == 0 : blk_len[k] != bs))) uns[s] = std::min(uns[s], k);
             if (!blk_status[k]) dec_blocks++, dec_bytes += blk_len[k];
             if (is_last(k) && !blk_status[k] && uns[s] == nk) IX(k).size = (int64_t)((IX(k).nblocks() - 1) * bs + blk_len[k]);
         }
@@ -3074,8 +3086,8 @@ int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uin
         std::vector<std::pair<uint32_t, uint64_t>> fresh;  // (pair, serial)
         if (cache)
             for (uint32_t k : ks) {
-                miss_blocks++, miss_bytes += blk_status[k] || too_long[k] ? 0 : blk_len[k];
-                if (blk_status[k] || too_long[k]) continue;
+                miss_blocks++, miss_bytes += blk_status[k] ? 0 : blk_len[k];
+                if (blk_status[k]) continue;
                 bool made = false;
                 const CacheEntry* en = cache->pc.insert(key[k], blk_len[k], &made);
                 if (made) fresh.push_back({k, en->serial}), ins_bytes += blk_len[k];
@@ -3530,10 +3542,9 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     uint32_t max_len = 0;
     for (uint32_t b = 0; b < nblocks; b++) max_len = std::max(max_len, block_len[b]);
     const uint64_t dstride = ((uint64_t)max_len + 15) & ~15ull;
-    const uint64_t ostride = (kz_max_block_output(max_len) + 15) & ~size_t(15);
+    uint64_t ostride = round16(kz_max_block_output(max_len));  // encode_slots' stride
     if (out_stride < ostride) return ctx->fail(KZ_ERR_INVALID_PARAM, "out_stride must be >= kz_max_block_output(max block length)");
     CK(ctx->d_in.ensure(dstride * nblocks + 64));
-    CK(ctx->d_out.ensure(ostride * nblocks + 64));
     for (uint32_t b = 0; b < nblocks; b++)
         if (block_len[b])
             CK(cudaMemcpyAsync((uint8_t*)ctx->d_in.p + b * dstride, slab + b * block_stride, block_len[b], cudaMemcpyHostToDevice, ctx->stream));
@@ -3552,20 +3563,14 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     BlockPrep prep;
     rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, ctx->d_in.as<uint8_t>(), bl, prep, &heads);
     if (rc) return rc;
-    const uint8_t* d_data = nullptr;
-    std::vector<EncJob> jobs;
-    rc = forward_stage(ctx, plan, ctx->d_in.as<uint8_t>(), dstride, bl.len, prep, &d_data, jobs);
-    if (rc) return rc;
-    std::vector<uint64_t> base(nblocks);
-    for (uint32_t b = 0; b < nblocks; b++) base[b] = 8 * (uint64_t)b * ostride;
-    EncResult res;
-    rc = encode_batch(ctx, LAYOUT_BLOCKS, etype, checksum_bits, d_data, jobs, {}, 0, false, false, ctx->d_out.as<uint8_t>(), ostride * nblocks, base, res);
+    std::vector<uint64_t> bits;
+    rc = encode_slots(ctx, plan, etype, checksum_bits, ctx->d_in.as<uint8_t>(), dstride, bl.len, prep, &ostride, bits);
     if (rc) return rc;
     for (uint32_t b = 0; b < nblocks; b++) {
-        out_bits[b] = res.blk_bits[b];
+        out_bits[b] = bits[b];
         if (status) status[b] = 0;
-        size_t nbytes = (size_t)((res.blk_bits[b] + 7) / 8);
-        CK(cudaMemcpyAsync(out + b * out_stride, (uint8_t*)ctx->d_out.p + b * ostride, nbytes, cudaMemcpyDeviceToHost, ctx->stream));
+        size_t nbytes = (size_t)((bits[b] + 7) / 8);
+        CK(cudaMemcpyAsync(out + b * out_stride, ctx->d_enc.as<uint8_t>() + b * ostride, nbytes, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaStreamSynchronize(ctx->stream));
     return 0;
@@ -3598,64 +3603,26 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     CK(cudaMemsetAsync(ctx->d_in.p, 0, dsz + 128, ctx->stream));
     for (uint32_t b = 0; b < nblocks; b++)
         CK(cudaMemcpyAsync((uint8_t*)ctx->d_in.p + jobs[b].bit_off / 8, in + in_off[b], (size_t)((in_bits[b] + 7) / 8), cudaMemcpyHostToDevice, ctx->stream));
-    const uint32_t* d_words = ctx->d_in.as<uint32_t>();
-    int rc = decode_parse_headers(ctx, d_words, jobs, checksum_bits, block_size);
+    const StreamHeader sh = {t48, etype, block_size, checksum_bits, 0, 0};
+    // block b is staged at b * slot: a block header claims at most max(2048, 1.5 x block_size) bytes (parse_block_header), and no stage
+    // writes more than decode_walked's stride for that claim allows
+    const uint32_t claim = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(2048, (uint64_t)block_size + block_size / 2), 1u << 30);
+    const uint64_t slot = decode_stride(block_size, claim);
+    CK(ctx->d_out.ensure(slot * nblocks + 64));
+    std::vector<DecodeFailure> fail;
+    std::vector<uint32_t> len;
+    // every block may be its stream's last: NONE's multiple-of-16 rule does not apply to a batch of blocks
+    int rc = decode_isolated(ctx, sh, plan, ctx->d_in.as<uint32_t>(), dsz / 4 + 16, jobs, std::vector<uint8_t>(nblocks, 1),
+                             [&](uint32_t b, uint32_t n) { return n <= out_stride ? b * slot : NO_ROOM; }, ctx->d_out.as<uint8_t>(), fail, len);
     if (rc) return rc;
-    const uint64_t ostride = (((uint64_t)block_size + block_size / 2 + 2048) + 15) & ~15ull;
-    CK(ctx->d_out.ensure(ostride * nblocks + 64));
     for (uint32_t b = 0; b < nblocks; b++) {
-        jobs[b].out_off = b * ostride;
-        if (jobs[b].status == 0 && jobs[b].pre_len > out_stride) jobs[b].status = -KZ_ERR_WRITE_FILE;
-    }
-    rc = decode_batch(ctx, etype, d_words, dsz / 4 + 16, jobs, ctx->d_out.as<uint8_t>());
-    if (rc) return rc;
-    int worst = 0;
-    for (uint32_t b = 0; b < nblocks; b++)
-        if (jobs[b].status && !worst) worst = jobs[b].status;
-    if (checksum_bits && plan.none() && !worst) {
-        std::vector<uint64_t> hoff(nblocks);
-        std::vector<uint32_t> hlen(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) {
-            hoff[b] = b * ostride;
-            hlen[b] = jobs[b].pre_len;
-        }
-        int vrc = verify_checksums(ctx, ctx->d_out.as<uint8_t>(), hoff, hlen, checksum_bits, jobs);
-        if (vrc) return vrc;
-    }
-    if (plan.none() || worst) {
-        for (uint32_t b = 0; b < nblocks; b++) {
-            if (status) status[b] = jobs[b].status;
-            if (jobs[b].status) {
-                out_len[b] = 0;
-                continue;
-            }
-            out_len[b] = jobs[b].pre_len;
-            CK(cudaMemcpyAsync(out + b * out_stride, (uint8_t*)ctx->d_out.p + b * ostride, jobs[b].pre_len, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        CK(cudaStreamSynchronize(ctx->stream));
-        if (worst) return ctx->fail(-worst, "block decoding failed");
-        return 0;
-    }
-    // inverse transforms into a scratch area (block b at b * ostride), then out
-    CK(ctx->d_tmp.ensure(ostride * nblocks + 64));
-    std::vector<uint32_t> olen;
-    // block b fits its slot at b * ostride: the block header bounds pre_len below ostride, and the stages cap their output at ostride - 64
-    rc = inverse_stage(ctx, plan, jobs, ctx->d_out.as<uint8_t>(), ostride, ctx->d_tmp.as<uint8_t>(), [&](uint32_t b, uint32_t) { return (uint64_t)b * ostride; },
-                       olen);
-    if (rc) return rc;
-    if (checksum_bits) {
-        std::vector<uint64_t> hoff(nblocks);
-        for (uint32_t b = 0; b < nblocks; b++) hoff[b] = (uint64_t)b * ostride;
-        int vrc = verify_checksums(ctx, ctx->d_tmp.as<uint8_t>(), hoff, olen, checksum_bits, jobs);
-        if (vrc) return vrc;
-    }
-    for (uint32_t b = 0; b < nblocks; b++) {
-        if (status) status[b] = 0;
-        out_len[b] = olen[b];
-        if (olen[b] > out_stride) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-        CK(cudaMemcpyAsync(out + b * out_stride, ctx->d_tmp.as<uint8_t>() + (uint64_t)b * ostride, olen[b], cudaMemcpyDeviceToHost, ctx->stream));
+        if (status) status[b] = fail[b].code;
+        out_len[b] = fail[b].failed() ? 0 : len[b];
+        if (out_len[b]) CK(cudaMemcpyAsync(out + b * out_stride, ctx->d_out.as<uint8_t>() + b * slot, out_len[b], cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaStreamSynchronize(ctx->stream));
+    for (uint32_t b = 0; b < nblocks; b++)
+        if (fail[b].failed()) return ctx->fail(-fail[b].code, fail[b].msg);
     return 0;
 }
 
