@@ -124,11 +124,17 @@ int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* 
  * written. Nothing is written outside [dst_off[s], dst_off[s] + dst_cap[s]).
  * Compress: stream s is byte for byte what kz_compress_stream(ctx, transform48, entropy, block_size, checksum_bits, input_size[s],
  *   src + src_off[s], src_len[s], ...) writes (input_size NULL = 0 for every stream). Empty streams are allowed (header and end marker), as
- *   are streams shorter than 16 bytes (COPY blocks). One call uses one block size: with `-b auto` every file has its own block size, and the
- *   caller groups files by block size. When stream s needs more than dst_cap[s] bytes, status[s] = -KZ_ERR_WRITE_FILE, nothing is written
- *   for it and out_len[s] = the bytes it needs.
- * Decompress: streams may have different headers (transform, entropy, block size, checksum); the library groups them. Stream s decodes to
- *   dst + dst_off[s]; out_len[s] = its length.
+ *   are streams shorter than 16 bytes (COPY blocks). When stream s needs more than dst_cap[s] bytes, status[s] = -KZ_ERR_WRITE_FILE,
+ *   nothing is written for it and out_len[s] = the bytes it needs.
+ * Compress with a block size per stream (kz_compress_streams_bs[_device]; BlockCompressor's `-b auto`, where every file gets the block
+ *   size size / jobs): block_size is an array of nstreams entries, and stream s is byte for byte what kz_compress_stream writes with
+ *   block_size[s]. The blocks of all streams share every pass, whatever their block sizes. A block size kz_compress_stream refuses
+ *   (outside [1024, 2^30], or not a multiple of 16) fails only its own stream: status[s] = -KZ_ERR_INVALID_PARAM, out_len[s] = 0, nothing
+ *   written. A NULL block_size is a call-level error. kz_compress_streams[_device] is the same call with one block size, which is
+ *   checked at call level.
+ * Decompress: streams may have different headers (transform, entropy, block size, checksum). Streams whose headers differ at most in block
+ *   size share their walk and decode passes; each other combination of transform, entropy and checksum runs passes of its own. Stream s
+ *   decodes to dst + dst_off[s]; out_len[s] = its length.
  * Status: status[s] = 0 or -(kanzi error code). A stream with status 0 is complete and correct whatever happened to the others. These errors
  *   belong to one stream: a bad header or version, a bad block prefix or block header, an entropy-decode failure, a checksum mismatch, a
  *   failing inverse transform, and dst_cap[s] too small (-KZ_ERR_WRITE_FILE); each gets the code kz_decompress_stream gives for the same
@@ -153,6 +159,12 @@ int kz_compress_streams_device(kz_ctx* ctx, uint64_t transform48, uint32_t entro
                                const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
 int kz_decompress_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, void* d_dst,
                                  const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+int kz_compress_streams_bs(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams,
+                           const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst,
+                           const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
+int kz_compress_streams_bs_device(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, const uint32_t* block_size, uint32_t checksum_bits,
+                                  uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size,
+                                  void* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status);
 
 /* ---- sharded streams (io.Writer / io.Reader with the blocks of ONE stream spread over several GPUs; the NCCL scatter / gather of the
  *      byte ranges is the host side's business, kanzi-go_b200/parallel.py; blocks are independent: io/CompressedStream.go:896-898) ---------- */

@@ -121,8 +121,8 @@ type StreamResult struct {
 
 // CompressStreams compresses every input as a stream of its own in one call, as BlockCompressor's multi-file path
 // (app/BlockCompressor.go:543-613) would use it instead of one Writer per file. Stream i is byte for byte what a Writer with
-// the same parameters and fileSize = inputSizes[i] writes for inputs[i]. All inputs share one block size: with `-b auto` the
-// caller groups its files by block size and makes one call per group. A file whose output does not fit fails alone; a transform or
+// the same parameters and fileSize = inputSizes[i] writes for inputs[i]. All inputs share one block size; with `-b auto`, where every
+// file has its own, use CompressStreamsBlockSizes. A file whose output does not fit fails alone; a transform or
 // entropy failure on one file's data (the reference fails that file with ERR_PROCESS_BLOCK) fails the whole call, and the caller
 // then compresses the files one by one. The call holds all inputs, encoded blocks and streams in device memory at once: split a
 // large directory into calls of a size the GPU holds. After c.SetHeaderlessWriter(true) no stream carries a header (the Writer's
@@ -157,9 +157,56 @@ func (c *Context) CompressStreams(transformType uint64, entropyType uint32, bloc
 	return c.streamResults(rc, dst, dstOff, outLen, status, n)
 }
 
+// CompressStreamsBlockSizes is CompressStreams with one block size per file: blockSizes[i] for inputs[i], as BlockCompressor's `-b auto`
+// gives every file (app/BlockCompressor.go:574-580, AutoBlockSize). All files still share one call and its passes. A block size that a
+// Writer refuses (outside [1 KiB, 1 GiB] or not a multiple of 16) fails only its own file, with ERR_INVALID_PARAM.
+func (c *Context) CompressStreamsBlockSizes(transformType uint64, entropyType uint32, blockSizes []uint32, ckBits uint, inputs [][]byte,
+	inputSizes []int64) ([]StreamResult, error) {
+	n := len(inputs)
+	if len(blockSizes) != n {
+		return nil, fmt.Errorf("kanzi gpu: %d block sizes for %d inputs", len(blockSizes), n)
+	}
+	srcOff, srcLen := make([]uint64, n), make([]uint64, n)
+	dstOff, dstCap := make([]uint64, n), make([]uint64, n)
+	var srcTotal, dstTotal uint64
+	for i, in := range inputs {
+		srcOff[i], srcLen[i] = srcTotal, uint64(len(in))
+		srcTotal += uint64(len(in))
+		dstOff[i], dstCap[i] = dstTotal, uint64(C.kz_max_stream_output(C.size_t(len(in)), C.uint32_t(blockSizes[i])))
+		dstTotal += dstCap[i]
+	}
+	src := make([]byte, srcTotal+1)
+	for i, in := range inputs {
+		copy(src[srcOff[i]:], in)
+	}
+	dst := make([]byte, dstTotal+1)
+	outLen, status := make([]uint64, n+1), make([]C.int32_t, n+1)
+	bs := make([]uint32, n+1)
+	copy(bs, blockSizes)
+	var isz *C.int64_t
+	if len(inputSizes) == n && n > 0 {
+		isz = (*C.int64_t)(unsafe.Pointer(&inputSizes[0]))
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.kz_compress_streams_bs(c.h, C.uint64_t(transformType), C.uint32_t(entropyType), (*C.uint32_t)(unsafe.Pointer(&bs[0])), C.uint32_t(ckBits),
+		C.uint32_t(n), (*C.uint8_t)(unsafe.Pointer(&src[0])), u64p(srcOff), u64p(srcLen), isz, (*C.uint8_t)(unsafe.Pointer(&dst[0])), u64p(dstOff),
+		u64p(dstCap), u64p(outLen), &status[0])
+	return c.streamResults(rc, dst, dstOff, outLen, status, n)
+}
+
+// AutoBlockSize is the block size BlockCompressor's `-b auto` gives a file of size bytes with jobs jobs (app/BlockCompressor.go:574-580).
+func AutoBlockSize(size int64, jobs uint) uint32 {
+	bl := size / int64(jobs)
+	bl = (bl + 63) &^ 63
+	bl = min(bl, 1<<30)
+	bl = max(bl, 1024)
+	return uint32(bl)
+}
+
 // DecompressStreams decodes many streams in one call, as BlockDecompressor's multi-file path would: the streams may have different
-// headers (transform, entropy, block size, checksum). caps[i] bounds the decoded size of stream i (the file size its header records,
-// or the caller's limit). A corrupt stream gets the error code a Reader would report for it; every other stream decodes normally.
+// headers (transform, entropy, block size, checksum), and streams that differ only in block size share one set of passes. caps[i]
+// bounds the decoded size of stream i (the file size its header records, or the caller's limit). A corrupt stream gets the error code a Reader would report for it; every other stream decodes normally.
 // A stream whose transform or entropy codec the GPU path lacks fails the whole call with ERR_INVALID_CODEC: the caller then keeps
 // the reference's Reader for the files of that call. The device holds every input and sum(caps) bytes of output at once.
 // After c.SetHeaderlessReader(...) the streams have no header and all share its parameters (NewHeaderlessReader for every file).

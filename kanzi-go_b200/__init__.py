@@ -44,7 +44,7 @@ ABI_SYMBOLS = [
     "kz_index_build", "kz_index_build_device", "kz_index_info", "kz_index_save", "kz_index_load", "kz_index_free", "kz_read_ranges",
     "kz_read_ranges_device", "kz_cache_create", "kz_cache_free", "kz_cache_clear", "kz_cache_stats", "kz_read_ranges_cached",
     "kz_read_ranges_cached_device", "kz_index_build_streams", "kz_index_build_streams_device", "kz_read_ranges_streams",
-    "kz_read_ranges_streams_device",
+    "kz_read_ranges_streams_device", "kz_compress_streams_bs", "kz_compress_streams_bs_device",
 ]
 
 
@@ -151,6 +151,8 @@ def load_library(build_if_missing=True):
     L.kz_set_skip_blocks.argtypes = [vp, i32]
     L.kz_compress_streams.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_compress_streams_device.argtypes = [vp, u64, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_compress_streams_bs.argtypes = [vp, u64, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_compress_streams_bs_device.argtypes = [vp, u64, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_decompress_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
     L.kz_writer_open.argtypes = [vp, u64, u32, u32, u32, u32, C.c_int64, C.POINTER(vp)]
@@ -431,21 +433,29 @@ class Context:
     # ---- many independent streams in one call (kz_compress_streams / kz_decompress_streams) -----------------------------------
     # Per-stream failures do not raise: status[s] = 0 or -(kanzi error code), and outputs[s] is None for a failed stream.
     def compress_streams(self, inputs, transform, entropy, block_size, checksum_bits=0, input_sizes=None, headerless=None, skip_blocks=None):
-        """One compressed stream per input, each equal to compress(inputs[s], ..., input_size=input_sizes[s]) -> (outputs, status)."""
+        """One compressed stream per input, each equal to compress(inputs[s], ..., input_size=input_sizes[s]) -> (outputs, status).
+        block_size: one int for every stream, or a sequence with one block size per stream (kanzi's `-b auto`: see auto_block_size); a
+        stream whose block size compress refuses then fails alone with status -KZ_ERR_INVALID_PARAM."""
         arrs = [_u8(x) for x in inputs]
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         src_len = np.array([a.size for a in arrs], np.uint64)
         src_off = _offsets(src_len)
         src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
-        cap = np.array([self.lib.kz_max_stream_output(a.size, block_size) for a in arrs], np.uint64)
+        bs = _block_sizes(block_size, len(arrs))
+        sizes = [block_size] * len(arrs) if bs is None else [int(b) for b in bs]
+        cap = np.array([self.lib.kz_max_stream_output(a.size, b) for a, b in zip(arrs, sizes)], np.uint64)
         dst_off = _offsets(cap)
         dst = np.empty(max(int(cap.sum()), 1), np.uint8)
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(arrs), np.uint64), np.zeros(len(arrs), np.int32)
         with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
-            self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len),
-                                         None if isz is None else _p(isz), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
+            if bs is None:
+                self.lib.kz_compress_streams(self.h, t48, et, block_size, checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len),
+                                             None if isz is None else _p(isz), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
+            else:
+                self.lib.kz_compress_streams_bs(self.h, t48, et, _p(bs), checksum_bits, len(arrs), _p(src), _p(src_off), _p(src_len),
+                                                None if isz is None else _p(isz), dst.ctypes.data, _p(dst_off), _p(cap), _p(out_len), _p(status))
         outs = [dst[int(o): int(o) + int(n)].copy() if st == 0 else None for o, n, st in zip(dst_off, out_len, status)]
         return outs, status
 
@@ -468,15 +478,21 @@ class Context:
 
     def compress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, transform, entropy, block_size, checksum_bits=0,
                                 input_sizes=None, headerless=None, skip_blocks=None):
-        """src / dst: CUDA uint8 tensors (or device addresses); offsets (multiples of 16) and lengths: host sequences -> (out_len, status)."""
+        """src / dst: CUDA uint8 tensors (or device addresses); offsets (multiples of 16) and lengths: host sequences -> (out_len, status).
+        block_size: an int, or one block size per stream (as compress_streams)."""
         t48 = transform_type(transform) if isinstance(transform, str) else transform
         et = entropy_type(entropy) if isinstance(entropy, str) else entropy
         so, sl, do, dc = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, dst_off, dst_cap))
         isz = None if input_sizes is None else np.ascontiguousarray(input_sizes, np.int64)
         out_len, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
+        bs = _block_sizes(block_size, len(sl))
         with self._headerless(writer=headerless), self._skip_blocks(skip_blocks):
-            self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl),
-                                                None if isz is None else _p(isz), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+            if bs is None:
+                self.lib.kz_compress_streams_device(self.h, t48, et, block_size, checksum_bits, len(sl), _dptr(src), _p(so), _p(sl),
+                                                    None if isz is None else _p(isz), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
+            else:
+                self.lib.kz_compress_streams_bs_device(self.h, t48, et, _p(bs), checksum_bits, len(sl), _dptr(src), _p(so), _p(sl),
+                                                       None if isz is None else _p(isz), _dptr(dst), _p(do), _p(dc), _p(out_len), _p(status))
         return out_len, status
 
     def decompress_streams_device(self, src, src_off, src_len, dst, dst_off, dst_cap, from_block=None, to_block=None, headerless=None):
@@ -813,6 +829,25 @@ class BlockCache:
             self.close()
         except Exception:
             pass
+
+
+def auto_block_size(size, jobs):
+    """The block size BlockCompressor's `-b auto` gives a file of `size` bytes compressed with `jobs` jobs (app/BlockCompressor.go:574-580):
+    size / jobs, rounded up to a multiple of 64, clamped to [1 KiB, 1 GiB]."""
+    bs = size // jobs
+    bs = (bs + 63) & ~63
+    return max(1024, min(bs, 1 << 30))
+
+
+def _block_sizes(block_size, n):
+    """None for one int block size; else the per-stream sizes as a uint32 array of n entries (values that do not fit go as 0, which every
+    stream refuses)."""
+    if isinstance(block_size, (int, np.integer)):
+        return None
+    sizes = [int(b) for b in block_size]
+    if len(sizes) != n:
+        raise KanziError(18, "block_size has %d entries for %d streams" % (len(sizes), n))
+    return np.array([b if 0 <= b < (1 << 32) else 0 for b in sizes], np.uint32)
 
 
 def default_batch_blocks(block_size):

@@ -299,11 +299,16 @@ const char* const CHECKSUM_MISMATCH = "Corrupted bitstream: block checksum misma
 
 bool etype_supported(uint32_t e) { return e == KZ_E_NONE || e == KZ_E_ANS0 || e == KZ_E_HUFFMAN || e == KZ_E_ANS1 || e == KZ_E_RANGE; }
 
-// The block size and checksum width of every stream-level encode (whole stream, many streams, writer session)
-int check_encode_args(kz_ctx* ctx, uint32_t block_size, uint32_t checksum_bits) {
-    if (block_size < 1024 || block_size > (1u << 30) || (block_size & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+// The block sizes a stream-level encode accepts
+bool block_size_ok(uint32_t block_size) { return block_size >= 1024 && block_size <= (1u << 30) && !(block_size & 15); }
+int check_checksum_bits(kz_ctx* ctx, uint32_t checksum_bits) {
     if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
     return 0;
+}
+// The block size and checksum width of every stream-level encode (whole stream, many streams, writer session)
+int check_encode_args(kz_ctx* ctx, uint32_t block_size, uint32_t checksum_bits) {
+    if (!block_size_ok(block_size)) return ctx->fail(KZ_ERR_INVALID_PARAM, "Invalid block size");
+    return check_checksum_bits(ctx, checksum_bits);
 }
 
 // The gather of every bit-granular output (kz_concat.cu): segment i, seg_bits[i] bits at address seg_src[i], lands at bit seg_dst[i] of
@@ -648,10 +653,10 @@ int encode_batch(kz_ctx* ctx, EncLayout layout, uint32_t etype, uint32_t checksu
 // entropy decode of a batch of blocks
 // ------------------------------------------------------------------------------------------------------------
 __global__ void block_header_kernel(const uint32_t* __restrict__ words, const uint64_t* __restrict__ bit_off, const uint64_t* __restrict__ bits, int nblocks,
-                                    uint32_t checksum_bits, uint32_t block_size, BlockHeader* __restrict__ out) {
+                                    uint32_t checksum_bits, const uint32_t* __restrict__ block_size, BlockHeader* __restrict__ out) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nblocks) return;
-    out[b] = parse_block_header(words, bit_off[b], bits[b], checksum_bits, block_size);
+    out[b] = parse_block_header(words, bit_off[b], bits[b], checksum_bits, block_size[b]);
 }
 
 // The block records of one stream for stream_walk_kernel: bits [start_bit, end_bit) of the word buffer, found records go to entries
@@ -721,12 +726,13 @@ struct Walked {
     int32_t status = 0;
     bool overflow = false;
     std::vector<uint64_t> bit_off, bits;
-    // appends the stored records as DecJobs of `own`; last[b]: the record is the stream's last
-    void append(uint32_t own, std::vector<DecJob>& jobs, std::vector<uint32_t>& owner, std::vector<uint8_t>& last) const {
+    // appends the stored records as DecJobs of `own`, a stream of block_size; last[b]: the record is the stream's last
+    void append(uint32_t own, uint32_t block_size, std::vector<DecJob>& jobs, std::vector<uint32_t>& owner, std::vector<uint8_t>& last) const {
         for (size_t r = 0; r < bit_off.size(); r++) {
             DecJob j = DecJob();
             j.bit_off = bit_off[r];
             j.bits = bits[r];
+            j.block_size = block_size;
             jobs.push_back(j);
             owner.push_back(own);
             last.push_back(first + r + 1 == n);
@@ -809,18 +815,21 @@ int walk_streams(kz_ctx* ctx, const uint32_t* d_words, std::vector<WalkJob>& job
     return 0;
 }
 
-// jobs[b].bit_off / bits / out_off must be set; fills pre_len, mode, ..., status. d_words = device stream buffer.
-int decode_parse_headers(kz_ctx* ctx, const uint32_t* d_words, std::vector<DecJob>& jobs, uint32_t checksum_bits, uint32_t block_size) {
+// jobs[b].bit_off / bits / block_size must be set; fills pre_len, mode, ..., status. d_words = device stream buffer.
+int decode_parse_headers(kz_ctx* ctx, const uint32_t* d_words, std::vector<DecJob>& jobs, uint32_t checksum_bits) {
     const int nblocks = (int)jobs.size();
     if (nblocks == 0) return 0;
     std::vector<uint64_t> off(nblocks), bits(nblocks);
+    std::vector<uint32_t> bs(nblocks);
     for (int b = 0; b < nblocks; b++) {
         off[b] = jobs[b].bit_off;
         bits[b] = jobs[b].bits;
+        bs[b] = jobs[b].block_size;
     }
     Packer pk;
     const size_t o_off = pk.add(off.data(), off.size() * 8);
     const size_t o_bits = pk.add(bits.data(), bits.size() * 8);
+    const size_t o_bs = pk.add(bs.data(), bs.size() * 4);
     const size_t o_out = pk.reserve(sizeof(BlockHeader) * (size_t)nblocks);
     int rc = upload(ctx, pk);
     if (rc) return rc;
@@ -828,7 +837,7 @@ int decode_parse_headers(kz_ctx* ctx, const uint32_t* d_words, std::vector<DecJo
     {
         LaunchScope ls(ctx, "block_header");
         block_header_kernel<<<(nblocks + 127) / 128, 128, 0, ctx->stream>>>(d_words, (uint64_t*)(T + o_off), (uint64_t*)(T + o_bits), nblocks, checksum_bits,
-                                                                            block_size, (BlockHeader*)(T + o_out));
+                                                                            (const uint32_t*)(T + o_bs), (BlockHeader*)(T + o_out));
     }
     CK(ctx->h_dl.ensure(sizeof(BlockHeader) * (size_t)nblocks));
     CK(cudaMemcpyAsync(ctx->h_dl.p, T + o_out, sizeof(BlockHeader) * (size_t)nblocks, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1171,8 +1180,9 @@ struct StageIo {
 
 // A stage with one descriptor and one StageResult per block (ROLZ, TEXT, UTF, EXE, MM, PACK / DNA; Block is RolzBlock for ROLZ, which
 // carries a scratch offset, StageBlock otherwise). Every sub-batch of `sub` blocks (0: the whole batch) that holds an active block gets
-// its descriptors (offsets, len, data_type; `desc` sets cap and the stage's own fields), ws(nb, max_len) bytes of workspace, one upload
-// of the descriptors with room for the results, one `launch` (the stage's kernels) under a LaunchScope named `scope`, and the results
+// its descriptors (offsets, len, data_type; `desc` sets cap and the stage's own fields), ws(b0, nb, max_len) bytes of workspace for blocks
+// b0 .. b0 + nb - 1, one upload of the descriptors with room for the results, one `launch` (the stage's kernels, given b0 as well) under a
+// LaunchScope named `scope`, and the results
 // copied back. Forward: status 0 = transformed, anything else = declined, ctx["dataType"] after the call is kept for every active block;
 // a negative status fails with `bad` when one is given (EXE: a block the reference panics on). Inverse: any status but 0 fails with `bad`.
 template <class Block, class Desc, class Ws, class Launch>
@@ -1194,7 +1204,7 @@ int run_desc_stage(kz_ctx* ctx, const StageIo& io, const char* scope, uint32_t s
             hb[k].data_type = io.dts ? (*io.dts)[b] : 0;
             desc(hb[k], b);
         }
-        CK(ctx->d_ws.ensure(ws(nb, max_len)));
+        CK(ctx->d_ws.ensure(ws(b0, nb, max_len)));
         Packer pk;
         const size_t o_blk = pk.add(hb.data(), hb.size() * sizeof(Block));
         const size_t o_res = pk.reserve((size_t)nb * sizeof(StageResult));
@@ -1203,7 +1213,7 @@ int run_desc_stage(kz_ctx* ctx, const StageIo& io, const char* scope, uint32_t s
         uint8_t* T = ctx->d_tables.as<uint8_t>();
         {
             LaunchScope ls(ctx, scope);
-            cudaError_t e = launch((const Block*)(T + o_blk), hb.data(), nb, max_len, (StageResult*)(T + o_res));
+            cudaError_t e = launch(b0, (const Block*)(T + o_blk), hb.data(), nb, max_len, (StageResult*)(T + o_res));
             if (e != cudaSuccess) return ctx->cuda_fail(e, scope);
         }
         std::vector<StageResult> hr(nb);
@@ -1229,8 +1239,9 @@ int run_desc_stage(kz_ctx* ctx, const StageIo& io, const char* scope, uint32_t s
 }
 
 // One forward stage. Block b: d_in + b*istride (len[b] bytes) -> d_out + b*ostride. applied[b] = 1 and len[b] updated on success.
+// bs[b]: ctx["blockSize"] of block b's stream, 0 when the caller has none (TEXT then takes the longest block of the call).
 int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride, uint8_t* d_out, uint64_t ostride, std::vector<uint32_t>& len,
-                  const std::vector<uint8_t>& active, std::vector<uint8_t>& applied, std::vector<int32_t>* dts = nullptr) {
+                  const std::vector<uint8_t>& active, std::vector<uint8_t>& applied, const std::vector<uint64_t>& bs, std::vector<int32_t>* dts = nullptr) {
     const uint32_t nblocks = (uint32_t)len.size();
     applied.assign(nblocks, 0);
     const StageIo io{istride, ostride, len, active, &applied, dts};
@@ -1297,8 +1308,8 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
                 d.scratch_off = b * sstride;
                 d.cap = (uint32_t)std::min<uint64_t>(ostride, 0xFFFFFFF0u);
             },
-            [&](uint32_t nb, uint32_t) { return sstride * nb + 256; },
-            [&](const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            [&](uint32_t, uint32_t nb, uint32_t) { return sstride * nb + 256; },
+            [&](uint32_t, const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 rolz_forward_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, ctx->d_ws.as<uint8_t>(), d_out, res);
                 return cudaGetLastError();
             });
@@ -1330,20 +1341,26 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             }
     } else if (t == KZ_T_TEXT) {  // TextCodec (encoding 2): declines unless the block looks like text
         if (!text_available()) return ctx->fail(KZ_ERR_CREATE_CODEC, "TEXT: the library was built without the static dictionary");
-        const uint64_t sbs = ctx->stream_bs ? ctx->stream_bs : *std::max_element(len.begin(), len.end());
-        return run_desc_stage<StageBlock>(
+        std::vector<uint64_t> sbs(bs);
+        const uint64_t longest = *std::max_element(len.begin(), len.end());
+        for (uint64_t& v : sbs) v = v ? v : longest;
+        uint64_t serial = 0;
+        const int rc = run_desc_stage<StageBlock>(
             ctx, io, "text_forward", 64,                          // ~9 MB of dictionary per block
             [&](StageBlock& d, uint32_t b) { d.cap = len[b]; },  // MaxEncodedLen = srcLen (:1720-1724)
-            [&](uint32_t nb, uint32_t max_len) { return text_workspace(nb, sbs, max_len); },
-            [&](const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t max_len, StageResult* res) {
-                return text_forward_batch(d_in, d_out, db, hb, nb, max_len, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+            [&](uint32_t b0, uint32_t nb, uint32_t max_len) { return text_workspace(&sbs[b0], nb, max_len); },
+            [&](uint32_t b0, const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t max_len, StageResult* res) {
+                return text_forward_batch(d_in, d_out, db, hb, nb, max_len, &sbs[b0], ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches,
+                                          &serial);
             });
+        if (ctx->profile && serial) ctx->prof["text_forward_serial"].launches += serial;  // blocks the serial walk did (kz_kernel_time count)
+        return rc;
     } else if (t == KZ_T_UTF) {  // UTFCodec.Forward: declines unless the block is UTF-8 with enough multi-byte sequences
         return run_desc_stage<StageBlock>(
             ctx, io, "utf_forward", 32,  // 16 MB of code point counters per block
             [&](StageBlock& d, uint32_t b) { d.cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 8192, 0xFFFFFFF0u); },  // MaxEncodedLen (:386-388)
-            [](uint32_t nb, uint32_t) { return utf_workspace(nb); },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            [](uint32_t, uint32_t nb, uint32_t) { return utf_workspace(nb); },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 return utf_forward_batch(d_in, d_out, db, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             });
     } else if (t == KZ_T_EXE) {  // EXECodec.Forward: declines unless the block is x86 / ARM64 code
@@ -1352,8 +1369,8 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
             if (active[b] && mel(len[b]) > ostride) return ctx->fail(KZ_ERR_UNKNOWN, "internal: stage buffer too small for EXE");
         return run_desc_stage<StageBlock>(
             ctx, io, "exe_forward", 0, [&](StageBlock& d, uint32_t b) { d.cap = (uint32_t)std::min<uint64_t>(mel(len[b]), 0xFFFFFFF0u); },
-            [](uint32_t, uint32_t) { return (size_t)0; },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            [](uint32_t, uint32_t, uint32_t) { return (size_t)0; },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 exe_forward_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, d_out, res);
                 return cudaGetLastError();
             },
@@ -1364,8 +1381,8 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
         return run_desc_stage<StageBlock>(
             ctx, io, "fsd_forward", 1024,
             [&](StageBlock& d, uint32_t b) { d.cap = fsd_max_encoded_len(len[b]); },  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
-            [](uint32_t nb, uint32_t max_len) { return fsd_workspace(nb, max_len); },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
+            [](uint32_t, uint32_t nb, uint32_t max_len) { return fsd_workspace(nb, max_len); },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
                 return fsd_forward_batch(d_in, d_out, db, nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             });
     } else if (t == KZ_T_PACK || t == KZ_T_DNA) {  // AliasCodec.Forward: bit packing of small alphabets / digram aliases; often declines
@@ -1375,8 +1392,8 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
                 d.cap = (uint32_t)std::min<uint64_t>((uint64_t)len[b] + 1024, 0xFFFFFFF0u);  // the sequence sizes dst with MaxEncodedLen (Sequence.go:81-93)
                 d.flags = t == KZ_T_DNA ? 1u : 0u;
             },
-            [](uint32_t nb, uint32_t max_len) { return alias_workspace(nb, max_len); },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
+            [](uint32_t, uint32_t nb, uint32_t max_len) { return alias_workspace(nb, max_len); },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t max_len, StageResult* res) {
                 return alias_forward_batch(d_in, d_out, db, nb, max_len, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             });
     } else if (t == KZ_T_RANK || t == KZ_T_MTFT) {  // SBRT.Forward never declines (buffers are sized for MaxEncodedLen)
@@ -1462,9 +1479,9 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
     return 0;
 }
 
-// One inverse stage, mirror of apply_forward. cap = capacity of a destination block.
+// One inverse stage, mirror of apply_forward. cap = capacity of a destination block; bs[b] = 0: TEXT takes cap as ctx["blockSize"].
 int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, uint64_t stride, uint32_t cap, std::vector<uint32_t>& len,
-                  const std::vector<uint8_t>& active) {
+                  const std::vector<uint8_t>& active, const std::vector<uint64_t>& bs) {
     const uint32_t nblocks = (uint32_t)len.size();
     const StageIo io{stride, stride, len, active, nullptr, nullptr};
     auto cap_all = [&](StageBlock& d, uint32_t) { d.cap = cap; };
@@ -1515,8 +1532,8 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
                 d.scratch_off = b * sstride;
                 d.cap = cap;
             },
-            [&](uint32_t nb, uint32_t) { return sstride * nb + 256; },
-            [&](const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            [&](uint32_t, uint32_t nb, uint32_t) { return sstride * nb + 256; },
+            [&](uint32_t, const RolzBlock* db, const RolzBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 rolz_inverse_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, ctx->d_ws.as<uint8_t>(), d_out, res);
                 return cudaGetLastError();
             },
@@ -1547,24 +1564,29 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         }
     } else if (t == KZ_T_TEXT) {
         if (!text_available()) return ctx->fail(KZ_ERR_CREATE_CODEC, "TEXT: the library was built without the static dictionary");
-        const uint64_t sbs = ctx->stream_bs ? ctx->stream_bs : cap;
-        return run_desc_stage<StageBlock>(
-            ctx, io, "text_inverse", 64, cap_all, [&](uint32_t nb, uint32_t max_len) { return text_workspace_inverse(nb, sbs, max_len); },
-            [&](const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
-                return text_inverse_batch(d_in, d_out, db, hb, nb, sbs, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
+        std::vector<uint64_t> sbs(bs);
+        for (uint64_t& v : sbs) v = v ? v : cap;
+        uint64_t serial = 0;
+        const int rc = run_desc_stage<StageBlock>(
+            ctx, io, "text_inverse", 64, cap_all, [&](uint32_t b0, uint32_t nb, uint32_t max_len) { return text_workspace_inverse(&sbs[b0], nb, max_len); },
+            [&](uint32_t b0, const StageBlock* db, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
+                return text_inverse_batch(d_in, d_out, db, hb, nb, &sbs[b0], ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches,
+                                          &serial);
             },
             "Text transform failed: invalid data");
+        if (ctx->profile && serial) ctx->prof["text_inverse_serial"].launches += serial;
+        return rc;
     } else if (t == KZ_T_UTF) {
         return run_desc_stage<StageBlock>(
-            ctx, io, "utf_inverse", 32, cap_all, [](uint32_t nb, uint32_t) { return utf_workspace(nb); },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            ctx, io, "utf_inverse", 32, cap_all, [](uint32_t, uint32_t nb, uint32_t) { return utf_workspace(nb); },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 return utf_inverse_batch(d_in, d_out, db, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             },
             "UTF inverse transform failed: invalid data");
     } else if (t == KZ_T_EXE) {
         return run_desc_stage<StageBlock>(
-            ctx, io, "exe_inverse", 0, cap_all, [](uint32_t, uint32_t) { return (size_t)0; },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            ctx, io, "exe_inverse", 0, cap_all, [](uint32_t, uint32_t, uint32_t) { return (size_t)0; },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 exe_inverse_kernel<<<nb, 32, 0, ctx->stream>>>(d_in, db, (int)nb, d_out, res);
                 return cudaGetLastError();
             },
@@ -1573,15 +1595,15 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
         uint64_t total_len = 0;
         for (uint32_t b = 0; b < nblocks; b++) total_len += active[b] ? len[b] : 0;
         return run_desc_stage<StageBlock>(
-            ctx, io, "fsd_inverse", 0, cap_all, [&](uint32_t nb, uint32_t) { return fsd_inverse_workspace(nb, total_len); },
-            [&](const StageBlock*, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
+            ctx, io, "fsd_inverse", 0, cap_all, [&](uint32_t, uint32_t nb, uint32_t) { return fsd_inverse_workspace(nb, total_len); },
+            [&](uint32_t, const StageBlock*, const StageBlock* hb, uint32_t nb, uint32_t, StageResult* res) {
                 return fsd_inverse_tiles(d_in, d_out, hb, nb, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             },
             "FSD inverse transform failed: invalid data");
     } else if (t == KZ_T_PACK || t == KZ_T_DNA) {
         return run_desc_stage<StageBlock>(
-            ctx, io, "alias_inverse", 256, cap_all, [&](uint32_t nb, uint32_t) { return alias_workspace(nb, cap); },
-            [&](const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
+            ctx, io, "alias_inverse", 256, cap_all, [&](uint32_t, uint32_t nb, uint32_t) { return alias_workspace(nb, cap); },
+            [&](uint32_t, const StageBlock* db, const StageBlock*, uint32_t nb, uint32_t, StageResult* res) {
                 return alias_inverse_batch(d_in, d_out, db, nb, cap, ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, res, ctx->stream, &ctx->launches);
             },
             "Alias codec inverse transform failed: invalid data");
@@ -1706,9 +1728,9 @@ int prepare_blocks(kz_ctx* ctx, const TransformPlan& plan, bool skip, uint32_t c
 // Block b is d_src[b*stride : +len_b]. On return *d_data is the base of the post-transform data and jobs[] describes
 // every block for the entropy stage. NONE leaves the data in place; the stages alternate between ctx->d_tmp and ctx->d_tmp2.
 // A block that prep stores (skipBlocks) is a COPY block, like a block of at most SMALL_BLOCK bytes: no stage runs on it, and
-// a batch of nothing but COPY blocks runs no stage at all.
-int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, uint64_t stride, std::vector<uint32_t> len, const BlockPrep& prep,
-                  const uint8_t** d_data, std::vector<EncJob>& jobs) {
+// a batch of nothing but COPY blocks runs no stage at all. bs[b]: ctx["blockSize"] of block b's stream (apply_forward).
+int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, uint64_t stride, std::vector<uint32_t> len, const std::vector<uint64_t>& bs,
+                  const BlockPrep& prep, const uint8_t** d_data, std::vector<EncJob>& jobs) {
     const uint32_t nblocks = (uint32_t)len.size();
     jobs.resize(nblocks);
     uint32_t max_len = 0;
@@ -1745,7 +1767,7 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
         uint8_t* outb = (i & 1) ? ctx->d_tmp2.as<uint8_t>() : ctx->d_tmp.as<uint8_t>();
         uint64_t bytes_in = 0, bytes_out = 0;
         for (uint32_t b = 0; b < nblocks; b++) bytes_in += active[b] ? len[b] : 0;
-        int rc = apply_forward(ctx, plan.ids[i], cur, cur_stride, outb, gstride, len, active, applied, &dts);
+        int rc = apply_forward(ctx, plan.ids[i], cur, cur_stride, outb, gstride, len, active, applied, bs, &dts);
         if (rc) return rc;
         for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
         note_stage_bytes(ctx, "fwd", plan.ids[i], bytes_in, bytes_out);
@@ -1771,12 +1793,13 @@ int forward_stage(kz_ctx* ctx, const TransformPlan& plan, const uint8_t* d_src, 
 
 // Transforms and entropy codes the blocks of a batch laid out in slots of one stride (block j: len[j] bytes at d_slots + j * stride). Block
 // j's bit string goes to ctx->d_enc + j * *ostride (ostride: kz_max_block_output of the longest block, rounded to 16) and is bits[j] long.
+// bs[j]: ctx["blockSize"] of block j's stream.
 int encode_slots(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t checksum_bits, const uint8_t* d_slots, uint64_t stride,
-                 const std::vector<uint32_t>& len, const BlockPrep& prep, uint64_t* ostride, std::vector<uint64_t>& bits) {
+                 const std::vector<uint32_t>& len, const std::vector<uint64_t>& bs, const BlockPrep& prep, uint64_t* ostride, std::vector<uint64_t>& bits) {
     const uint32_t k = (uint32_t)len.size();
     const uint8_t* d_data = nullptr;
     std::vector<EncJob> jobs;
-    int rc = forward_stage(ctx, plan, d_slots, stride, len, prep, &d_data, jobs);
+    int rc = forward_stage(ctx, plan, d_slots, stride, len, bs, prep, &d_data, jobs);
     if (rc) return rc;
     *ostride = round16(kz_max_block_output(*std::max_element(len.begin(), len.end())));
     CK(ctx->d_enc.ensure(*ostride * k + 64));
@@ -1803,7 +1826,8 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
     if (nblocks == 0) return 0;
     const uint32_t blk_cap = (uint32_t)std::min<uint64_t>(pstride - 64, 0xFFFFFFF0u);
     std::vector<uint32_t> len(nblocks);
-    for (uint32_t b = 0; b < nblocks; b++) len[b] = jobs[b].pre_len;
+    std::vector<uint64_t> bs(nblocks);
+    for (uint32_t b = 0; b < nblocks; b++) len[b] = jobs[b].pre_len, bs[b] = jobs[b].block_size;
     CK(ctx->d_tmp2.ensure(pstride * nblocks + 64));
     uint8_t* cur = d_pre;
     uint8_t* other = ctx->d_tmp2.as<uint8_t>();
@@ -1818,7 +1842,7 @@ int inverse_stage(kz_ctx* ctx, const TransformPlan& plan, std::vector<DecJob>& j
         if (!any) continue;
         uint64_t bytes_in = 0, bytes_out = 0;
         for (uint32_t b = 0; b < nblocks; b++) bytes_in += active[b] ? len[b] : 0;
-        int rc = apply_inverse(ctx, plan.ids[i], cur, other, pstride, blk_cap, len, active);
+        int rc = apply_inverse(ctx, plan.ids[i], cur, other, pstride, blk_cap, len, active, bs);
         if (rc) return rc;
         for (uint32_t b = 0; b < nblocks; b++) bytes_out += active[b] ? len[b] : 0;
         note_stage_bytes(ctx, "inv", plan.ids[i], bytes_in, bytes_out);
@@ -1881,9 +1905,8 @@ int decode_walked(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan
     auto note_all = [&](int s, int rc) {
         for (uint32_t b : idx) fail[owner[b]].note(s, rc, ctx->err);
     };
-    ctx->stream_bs = sh.block_size;
     if (!stage(STAGE_HEADER)) return 0;
-    int rc = decode_parse_headers(ctx, d_words, run, sh.checksum_bits, sh.block_size);
+    int rc = decode_parse_headers(ctx, d_words, run, sh.checksum_bits);
     if (rc) return rc;
     done();
     for (uint32_t b = 0; b < nb; b++) {
@@ -1901,9 +1924,7 @@ int decode_walked(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan
     if (!stage(STAGE_DECODE)) return 0;
     uint64_t stride = 0;
     if (!plan.none()) {
-        uint32_t max_pre = 0;
-        for (const DecJob& j : run) max_pre = std::max(max_pre, j.pre_len);
-        stride = decode_stride(sh.block_size, max_pre);
+        for (const DecJob& j : run) stride = std::max(stride, decode_stride(j.block_size, j.pre_len));
         CK(ctx->d_tmp.ensure(stride * run.size() + 64));
         for (size_t i = 0; i < run.size(); i++) run[i].out_off = i * stride;
     }
@@ -2192,7 +2213,7 @@ static int encode_stream_blocks(kz_ctx* ctx, const TransformPlan& plan, uint32_t
     if (rc) return rc;
     const uint8_t* d_data = nullptr;
     std::vector<EncJob> jobs;
-    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, block_size, bl.len, prep, &d_data, jobs);
+    rc = forward_stage(ctx, plan, (const uint8_t*)d_src, block_size, bl.len, std::vector<uint64_t>(bl.size(), block_size), prep, &d_data, jobs);
     if (rc) return rc;
     return encode_batch(ctx, LAYOUT_STREAM, etype, checksum_bits, d_data, jobs, lead, lead_bits, fragment, volatile_lead, (uint8_t*)d_dst, cap, {}, res);
 }
@@ -2201,7 +2222,6 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
                                 size_t n, void* d_dst, size_t cap, size_t* out_n, bool fragment, uint64_t* out_bits) {
     if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = block_size;
     int rc = check_encode_args(ctx, block_size, checksum_bits);
     if (rc) return rc;
     if (((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
@@ -2314,7 +2334,7 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
     std::vector<DecJob> jobs;
     std::vector<uint32_t> owner;
     std::vector<uint8_t> last;
-    w[0].append(0, jobs, owner, last);
+    w[0].append(0, sh.block_size, jobs, owner, last);
     BackToBack place{cap};
     DecodeFailure f;
     rc = decode_walked(ctx, sh, plan, d_words, (n + 3) / 4 + 16, jobs, owner, last, place, (uint8_t*)d_dst, &f);  // >= 64 readable bytes past n
@@ -2451,22 +2471,29 @@ static int finish_streams(uint32_t nstreams, int32_t* status, uint64_t* out_len,
     return 0;
 }
 
-// Compresses stream s = d_src[src_off[s] : + src_len[s]]. Stream s is assembled in ctx->d_asm at 8 * stage_off[s] (16-byte aligned, behind
-// the header / prefix table of `small_bytes`); its length is out_len[s], status[s] = -KZ_ERR_WRITE_FILE when it exceeds dst_cap[s].
-static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams,
+// Compresses stream s = d_src[src_off[s] : + src_len[s]] with blocks of block_size[s] bytes. Stream s is assembled in ctx->d_asm at
+// 8 * stage_off[s] (16-byte aligned, behind the header / prefix table of `small_bytes`); its length is out_len[s], status[s] =
+// -KZ_ERR_WRITE_FILE when it exceeds dst_cap[s]. A stream whose block size kz_compress_stream refuses gets -KZ_ERR_INVALID_PARAM and no
+// blocks; the other streams' blocks share every pass, whatever their block sizes.
+static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams,
                                  const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size,
                                  const uint64_t* dst_cap, uint64_t* out_len, int32_t* status, std::vector<uint64_t>& stage_off, uint64_t* stage_base,
                                  uint64_t* stage_total) {
-    ctx->stream_bs = block_size;
-    int rc = check_encode_args(ctx, block_size, checksum_bits);
+    int rc = check_checksum_bits(ctx, checksum_bits);
     if (rc) return rc;
     if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
     TransformPlan plan;
     rc = plan_transforms(ctx, t48, etype, plan, KZ_ERR_CREATE_CODEC);
     if (rc) return rc;
-    // the blocks of every stream, stream after stream, prepared together before the passes
-    const BlockList bl = cut_blocks(src_off, src_len, nstreams, block_size);
+    // the blocks of every stream, stream after stream, prepared together before the passes; a refused stream has none
+    std::vector<uint64_t> cut_len(src_len, src_len + nstreams);
+    for (uint32_t s = 0; s < nstreams; s++)
+        if (!block_size_ok(block_size[s])) cut_len[s] = 0;
+    const BlockList bl = cut_blocks(src_off, cut_len.data(), nstreams, block_size);
     const uint32_t nb = bl.size();
+    std::vector<uint64_t> bbs(nb);  // ctx["blockSize"] of every block
+    for (uint32_t s = 0; s < nstreams; s++)
+        for (uint32_t b = bl.first[s]; b < bl.first[s + 1]; b++) bbs[b] = block_size[s];
     BlockPrep prep;
     rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, d_src, bl, prep);
     if (rc) return rc;
@@ -2481,17 +2508,19 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
         CK(ctx->d_slots.ensure(s * k + 64));
         uint8_t* slots = ctx->d_slots.as<uint8_t>();
         std::vector<uint32_t> lens(k);
+        std::vector<uint64_t> pbs(k);
         CopyList place;
         for (uint32_t j = 0; j < k; j++) {
             const uint32_t b = P.order[i0 + j];
             lens[j] = bl.len[b];
+            pbs[j] = bbs[b];
             place.add(d_src + bl.off[b], slots + j * s, bl.len[b]);
         }
         rc = run_copies(ctx, place);
         if (rc) return rc;
         uint64_t ostride = 0;
         std::vector<uint64_t> bits;
-        rc = encode_slots(ctx, plan, etype, checksum_bits, slots, s, lens, prep.pick(&P.order[i0], k), &ostride, bits);
+        rc = encode_slots(ctx, plan, etype, checksum_bits, slots, s, lens, pbs, prep.pick(&P.order[i0], k), &ostride, bits);
         if (rc) return rc;
         uint64_t need = arena;
         for (uint32_t j = 0; j < k; j++) need += round16((bits[j] + 7) / 8);
@@ -2519,9 +2548,14 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
     uint64_t stage = 0, nsegs = 0;
     for (uint32_t s = 0; s < nstreams; s++) {
         hdr_bits[s] = 0;
+        if (!block_size_ok(block_size[s])) {
+            out_len[s] = 0;
+            status[s] = -KZ_ERR_INVALID_PARAM;
+            continue;
+        }
         if (!ctx->headerless_writer) {  // Writer.writeHeader :430
             std::vector<uint8_t> hdr;
-            hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size, checksum_bits, input_size ? input_size[s] : 0);
+            hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size[s], checksum_bits, input_size ? input_size[s] : 0);
             memcpy(&small[64 * (size_t)s], hdr.data(), 64);
         }
         uint64_t bits = hdr_bits[s] + END_MARKER_BITS;
@@ -2575,12 +2609,13 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint
     return 0;
 }
 
-// One group of streams with the same header fields: walk, then decode_walked pass by pass, each block written behind the previous one of
-// its stream at d_dst + dst_off[s]. A stream on which anything goes wrong (a bad record, block header, entropy payload or checksum, too
+// One group of streams whose headers differ at most in block size (sh: the first one's; shs[s]: stream s's, which gives its first record's
+// bit and its block size): walk, then decode_walked pass by pass (plan_decompress_passes by block size), each block written behind the
+// previous one of its stream at d_dst + dst_off[s]. A stream on which anything goes wrong (a bad record, block header, entropy payload or checksum, too
 // little room, or a failing stage call of a pass it has blocks in) is put on `alone`; the caller decodes it again on its own with the
 // single-stream path, so that its status is the code kz_decompress_stream_device gives for the same bytes.
 static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const TransformPlan& plan, const std::vector<uint32_t>& grp,
-                               const std::vector<uint64_t>& hdr_bits, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off,
+                               const std::vector<StreamHeader>& shs, const uint8_t* d_src, uint64_t src_bytes, const uint64_t* src_off,
                                const uint64_t* src_len, uint8_t* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len,
                                int32_t* status, std::vector<uint32_t>& alone) {
     const uint32_t ng = (uint32_t)grp.size();
@@ -2590,7 +2625,7 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     for (uint32_t g = 0; g < ng; g++) {
         const uint32_t s = grp[g];
         const uint64_t by_cap = std::min<uint64_t>(dst_cap[s] / 1024 + 16, 1u << 22);
-        wj[g] = WalkJob{8 * src_off[s] + hdr_bits[s], 8 * (src_off[s] + src_len[s]), 0, (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1), 0};
+        wj[g] = WalkJob{8 * src_off[s] + shs[s].bits, 8 * (src_off[s] + src_len[s]), 0, (uint32_t)std::min<uint64_t>(by_cap, 8 * src_len[s] / 9 + 1), 0};
     }
     std::vector<Walked> w;
     int rc = walk_streams(ctx, d_words, wj, ctx->range_from, ctx->range_to, w);
@@ -2601,7 +2636,7 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
     std::vector<uint8_t> last;
     for (uint32_t g = 0; g < ng; g++) {
         if (w[g].status || w[g].overflow) fail[g].note(STAGE_WALK, w[g].status ? w[g].status : -KZ_ERR_BLOCK_SIZE, "");
-        else w[g].append(g, all, own, last);
+        else w[g].append(g, shs[grp[g]].block_size, all, own, last);
     }
     std::vector<uint64_t> written(ng, 0);
     auto place = [&](uint32_t g, uint32_t len) {  // behind the stream's earlier blocks, within its dst_cap
@@ -2610,12 +2645,19 @@ static int decode_stream_group(kz_ctx* ctx, const StreamHeader& sh, const Transf
         written[g] += len;
         return dst_off[s] + written[g] - len;
     };
-    const PassPlan P = plan_decompress_passes((uint32_t)all.size(), decompress_slot(sh.block_size), decompress_block_cost(sh.block_size));
+    std::vector<uint32_t> bs(all.size());
+    for (size_t b = 0; b < all.size(); b++) bs[b] = all[b].block_size;
+    // the blocks of a stream have one block size, so they stay in order within and across passes, and place() sees them in order
+    const PassPlan P = plan_decompress_passes(bs);
     for (uint32_t p = 0; p < P.npasses(); p++) {
-        const uint32_t a = P.first[p], e = P.first[p + 1];
-        std::vector<DecJob> jobs(all.begin() + a, all.begin() + e);
-        const std::vector<uint32_t> owner(own.begin() + a, own.begin() + e);
-        rc = decode_walked(ctx, sh, plan, d_words, (src_bytes + 3) / 4 + 16, jobs, owner, std::vector<uint8_t>(last.begin() + a, last.begin() + e),
+        std::vector<DecJob> jobs;
+        std::vector<uint32_t> owner;
+        std::vector<uint8_t> run_last;
+        for (uint32_t i = P.first[p]; i < P.first[p + 1]; i++) {
+            const uint32_t b = P.order[i];
+            jobs.push_back(all[b]), owner.push_back(own[b]), run_last.push_back(last[b]);
+        }
+        rc = decode_walked(ctx, sh, plan, d_words, (src_bytes + 3) / 4 + 16, jobs, owner, run_last,
                            [&](uint32_t b, uint32_t len) { return place(owner[b], len); }, d_dst, fail.data());
         if (rc) return rc;
     }
@@ -2637,7 +2679,7 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     for (uint32_t s = 0; s < nstreams; s++) status[s] = 0, out_len[s] = 0;
     if (nstreams == 0) return 0;
     // headers: the first 64 bytes of every stream in one gather (a headerless stream has none to read), then each stream's header or the
-    // headerless reader setting; the streams with the same header fields form a group
+    // headerless reader setting; the streams whose header fields differ at most in block size form a group and share its passes
     std::vector<uint8_t> head(64 * (size_t)nstreams);
     std::vector<uint64_t> head_len(nstreams, 0);
     if (!ctx->headerless_reader.on) head_len.assign(src_len, src_len + nstreams);
@@ -2645,21 +2687,19 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     if (rc) return rc;
     std::vector<StreamHeader> sh(nstreams);
     std::vector<TransformPlan> plan(nstreams);
-    std::vector<uint64_t> hdr_bits(nstreams, 0);
-    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
+    std::map<std::tuple<uint64_t, uint32_t, uint32_t>, std::vector<uint32_t>> groups;
     for (uint32_t s = 0; s < nstreams; s++) {
         status[s] = stream_header(ctx, &head[64 * (size_t)s], src_len[s], sh[s]);
         if (status[s]) continue;
         rc = plan_transforms(ctx, sh[s].t48, sh[s].etype, plan[s], KZ_ERR_INVALID_CODEC);
         if (rc) return rc;
         if (!etype_supported(sh[s].etype)) return ctx->fail(KZ_ERR_INVALID_CODEC, "entropy codec not available on the GPU path");
-        hdr_bits[s] = sh[s].bits;
-        groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].block_size, sh[s].checksum_bits)].push_back(s);
+        groups[std::make_tuple(sh[s].t48, sh[s].etype, sh[s].checksum_bits)].push_back(s);
     }
     std::vector<uint32_t> alone;
     for (auto& kv : groups) {
         const uint32_t s0 = kv.second[0];
-        rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, hdr_bits, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
+        rc = decode_stream_group(ctx, sh[s0], plan[s0], kv.second, sh, d_src, src_bytes, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, alone);
         if (rc) return rc;
     }
     for (uint32_t s : alone) {  // only corrupt input, too little room or a failing stage call gets here
@@ -2670,13 +2710,17 @@ static int decompress_streams_impl(kz_ctx* ctx, uint32_t nstreams, const uint8_t
     return 0;
 }
 
-int kz_compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const void* d_src,
-                               const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst, const uint64_t* dst_off,
-                               const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+// kz_compress_streams[_bs][_device]: block_size has nstreams entries. one_size != nullptr: the call has one block size, *one_size, which is
+// checked at call level as kz_compress_stream checks it.
+static int compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, const uint32_t* one_size, uint32_t checksum_bits,
+                                   uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst,
+                                   const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     int rc = check_stream_args(ctx, nstreams, d_src, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, true);
+    if (!rc && !block_size) rc = ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
     if (rc) return finish_streams(nstreams, status, out_len, rc);
     if (cudaSetDevice(ctx->device) != cudaSuccess) return finish_streams(nstreams, status, out_len, -KZ_ERR_PROCESS_BLOCK);
+    if (one_size && (rc = check_encode_args(ctx, *one_size, checksum_bits)) != 0) return finish_streams(nstreams, status, out_len, rc);
     std::vector<uint64_t> stage_off;
     uint64_t stage_base = 0, stage_total = 0;
     rc = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, (const uint8_t*)d_src, src_off, src_len, input_size, dst_cap, out_len,
@@ -2691,14 +2735,19 @@ int kz_compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32
     return finish_streams(nstreams, status, out_len, rc);
 }
 
-int kz_compress_streams(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const uint8_t* src,
-                        const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap,
-                        uint64_t* out_len, int32_t* status) {
+static int compress_streams_host(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, const uint32_t* one_size, uint32_t checksum_bits,
+                                 uint32_t nstreams, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst,
+                                 const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     int rc = check_stream_args(ctx, nstreams, src, src_off, src_len, dst, dst_off, dst_cap, out_len, status, false);
+    if (!rc && !block_size) rc = ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
     if (rc) return finish_streams(nstreams, status, out_len, rc);
     rc = [&]() -> int {
         CK(cudaSetDevice(ctx->device));
+        if (one_size) {
+            int r = check_encode_args(ctx, *one_size, checksum_bits);
+            if (r) return r;
+        }
         // the inputs packed at 16-byte aligned offsets and moved in one transfer
         std::vector<uint64_t> in_off(nstreams);
         uint64_t total = 0;
@@ -2720,6 +2769,36 @@ int kz_compress_streams(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t bloc
         return 0;
     }();
     return finish_streams(nstreams, status, out_len, rc);
+}
+
+int kz_compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const void* d_src,
+                               const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst, const uint64_t* dst_off,
+                               const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    const std::vector<uint32_t> bs(std::max(nstreams, 1u), block_size);
+    return compress_streams_device(ctx, t48, etype, bs.data(), &block_size, checksum_bits, nstreams, d_src, src_off, src_len, input_size, d_dst, dst_off, dst_cap,
+                                   out_len, status);
+}
+
+int kz_compress_streams(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const uint8_t* src,
+                        const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                        uint64_t* out_len, int32_t* status) {
+    const std::vector<uint32_t> bs(std::max(nstreams, 1u), block_size);
+    return compress_streams_host(ctx, t48, etype, bs.data(), &block_size, checksum_bits, nstreams, src, src_off, src_len, input_size, dst, dst_off, dst_cap,
+                                 out_len, status);
+}
+
+int kz_compress_streams_bs_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams,
+                                  const void* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst,
+                                  const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    return compress_streams_device(ctx, t48, etype, block_size, nullptr, checksum_bits, nstreams, d_src, src_off, src_len, input_size, d_dst, dst_off, dst_cap,
+                                   out_len, status);
+}
+
+int kz_compress_streams_bs(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams, const uint8_t* src,
+                           const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, uint8_t* dst, const uint64_t* dst_off,
+                           const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    return compress_streams_host(ctx, t48, etype, block_size, nullptr, checksum_bits, nstreams, src, src_off, src_len, input_size, dst, dst_off, dst_cap,
+                                 out_len, status);
 }
 
 int kz_decompress_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, void* d_dst,
@@ -3068,6 +3147,7 @@ int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uin
         for (size_t i = 0; i < ks.size(); i++) {
             jobs[i].bit_off = bit_off[ks[i]];
             jobs[i].bits = IX(ks[i]).bits[P.blocks[ks[i]]];
+            jobs[i].block_size = sh.block_size;
             last[i] = is_last(ks[i]);
         }
         std::vector<DecodeFailure> fail;
@@ -3535,7 +3615,6 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
                      const uint32_t* block_len, uint32_t nblocks, uint8_t* out, uint64_t out_stride, uint64_t* out_bits, int32_t* status) {
     if (!ctx || !slab || !block_len || !out || !out_bits) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = ctx->user_stream_bs;
     if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
     if (nblocks == 0) return 0;
     // device layout: block b at b * dstride (16-byte aligned)
@@ -3564,7 +3643,8 @@ int kz_encode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
     rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, ctx->d_in.as<uint8_t>(), bl, prep, &heads);
     if (rc) return rc;
     std::vector<uint64_t> bits;
-    rc = encode_slots(ctx, plan, etype, checksum_bits, ctx->d_in.as<uint8_t>(), dstride, bl.len, prep, &ostride, bits);
+    rc = encode_slots(ctx, plan, etype, checksum_bits, ctx->d_in.as<uint8_t>(), dstride, bl.len, std::vector<uint64_t>(nblocks, ctx->user_stream_bs), prep,
+                      &ostride, bits);
     if (rc) return rc;
     for (uint32_t b = 0; b < nblocks; b++) {
         out_bits[b] = bits[b];
@@ -3581,7 +3661,6 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
                      int32_t* status) {
     if (!ctx || !in || !in_off || !in_bits || !out || !out_len) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = block_size;
     if (checksum_bits != 0 && checksum_bits != 32 && checksum_bits != 64) return ctx->fail(KZ_ERR_INVALID_PARAM, "checksum must be 0, 32 or 64 bits");
     TransformPlan plan;
     {
@@ -3596,6 +3675,7 @@ int kz_decode_blocks(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t checksu
         jobs[b] = DecJob();
         jobs[b].bit_off = 8 * doff;
         jobs[b].bits = in_bits[b];
+        jobs[b].block_size = block_size;
         doff += (((in_bits[b] + 7) / 8) + 8 + 15) & ~15ull;
     }
     const uint64_t dsz = doff;
@@ -3687,7 +3767,6 @@ int kz_entropy_decode(kz_ctx* ctx, uint32_t type, const uint8_t* src, size_t src
 int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = ctx->user_stream_bs;
     *out_n = 0;
     if (!TransformPlan::seq_id(type)) return ctx->fail(KZ_ERR_CREATE_CODEC, NO_GPU_TRANSFORM);
     if (n == 0) return 0;
@@ -3705,7 +3784,8 @@ int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8
     std::vector<uint32_t> len(1, (uint32_t)n);
     std::vector<uint8_t> active(1, 1), applied;
     std::vector<int32_t> dt1(1, data_type ? *data_type : 0);  // ctx["dataType"]; BWT / BWTS / LZ / LZX / RANK / MTFT / ZRLT leave it as it is
-    int rc = apply_forward(ctx, type, ctx->d_in.as<uint8_t>(), stride, ctx->d_out.as<uint8_t>(), stride, len, active, applied, &dt1);
+    int rc = apply_forward(ctx, type, ctx->d_in.as<uint8_t>(), stride, ctx->d_out.as<uint8_t>(), stride, len, active, applied,
+                           std::vector<uint64_t>(1, ctx->user_stream_bs), &dt1);
     if (rc) return rc;
     if (data_type) *data_type = dt1[0];
     if (!applied[0]) return 1;
@@ -3719,7 +3799,6 @@ int kz_transform_forward(kz_ctx* ctx, uint64_t type, int* data_type, const uint8
 int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
     if (!ctx || (!src && n) || !dst || !out_n) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    ctx->stream_bs = ctx->user_stream_bs;
     *out_n = 0;
     if (!TransformPlan::seq_id(type)) return ctx->fail(KZ_ERR_CREATE_CODEC, NO_GPU_TRANSFORM);
     if (n == 0) return 0;
@@ -3739,7 +3818,8 @@ int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t 
     CK(cudaMemcpyAsync(ctx->d_in.p, src, n, cudaMemcpyHostToDevice, ctx->stream));
     std::vector<uint32_t> len(1, (uint32_t)n);
     std::vector<uint8_t> active(1, 1);
-    int rc = apply_inverse(ctx, type, ctx->d_in.as<uint8_t>(), ctx->d_out.as<uint8_t>(), stride, (uint32_t)cap, len, active);
+    int rc = apply_inverse(ctx, type, ctx->d_in.as<uint8_t>(), ctx->d_out.as<uint8_t>(), stride, (uint32_t)cap, len, active,
+                           std::vector<uint64_t>(1, ctx->user_stream_bs));
     if (rc) return rc;
     if (len[0]) CK(cudaMemcpyAsync(dst, ctx->d_out.p, len[0], cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -4051,7 +4131,6 @@ struct kz_writer : kz::Session {
         if (batches == 0) lead_bits = headerless ? 0 : build_stream_header(lead, t48, etype, block_size, checksum_bits, input_size);
         else lead[0] = carry;
         EncResult res;
-        ctx->stream_bs = block_size;
         int rc = encode_stream_blocks(ctx, plan, etype, block_size, checksum_bits, skip, d_in[k].p, in_len[k], lead, lead_bits, !last, true, d_out.p, out_cap,
                                       res);
         if (rc) return rc;
@@ -4240,6 +4319,7 @@ struct kz_reader : kz::Session {
             jobs[b] = DecJob();
             jobs[b].bit_off = boff[b];
             jobs[b].bits = bbits[b];
+            jobs[b].block_size = sh.block_size;
         }
         std::vector<uint8_t> last(nb, 0);
         last[nb - 1] = ends_batch;

@@ -120,6 +120,7 @@ struct DecJob {          // one block handed to the entropy decode stage
     uint64_t data_bit;
     uint64_t end_pos;    // bit position after the entropy data (filled for ANS/Huffman by the walk kernels)
     int32_t status;
+    uint32_t block_size; // blockSize of the block's stream: bounds its header's length claim and its decode slot; TEXT sizes its hash map by it
 };
 
 }  // namespace kz
@@ -135,7 +136,6 @@ struct kz_ctx {
     int bwt_profile = 0;  // kz_bwt_profile: bit 0 times the BWT forward rounds (with profile), bit 1 forces the 56-bit rounds
     kz::EncPlan enc_plan;
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
-    uint64_t stream_bs = 0;       // ctx["blockSize"] of the call in progress (TEXT sizes its hash map from it)
     int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)
     bool headerless_writer = false;          // kz_set_headerless_writer: the stream-level encodes write no stream header
     bool skip_blocks = false;                // kz_set_skip_blocks: the encodes store incompressible blocks raw (ctx["skipBlocks"])

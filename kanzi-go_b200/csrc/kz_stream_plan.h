@@ -17,6 +17,10 @@ namespace kz {
 
 // Device scratch bytes one pass may take (the block costs below). A block whose own cost is larger runs alone in a pass of its own.
 const uint64_t STREAM_PASS_BUDGET = 1ull << 30;
+// Blocks one decompression pass may hold: the inverse stages launch one row of CTAs per block (LZ inverse, MM, PACK, UTF: grid.y = the
+// blocks of the call), and a grid has at most 65,535 rows. A pass over more blocks would fail its stage call, and every stream with blocks
+// in it would be decoded again on its own.
+const uint32_t MAX_PASS_BLOCKS = 65535;
 
 struct PassPlan {
     std::vector<uint32_t> first;       // pass p holds the blocks order[first[p] .. first[p + 1])
@@ -40,20 +44,24 @@ struct BlockList {
     uint32_t size() const { return (uint32_t)len.size(); }
 };
 
-// Writer.Write cuts its input into blockSize pieces: stream s (src_len[s] bytes at src_off[s]) becomes blocks of block_size bytes and a
+// Writer.Write cuts its input into blockSize pieces: stream s (src_len[s] bytes at src_off[s]) becomes blocks of block_size[s] bytes and a
 // shorter last one; an empty stream has no blocks.
-inline BlockList cut_blocks(const uint64_t* src_off, const uint64_t* src_len, uint32_t nstreams, uint32_t block_size) {
+inline BlockList cut_blocks(const uint64_t* src_off, const uint64_t* src_len, uint32_t nstreams, const uint32_t* block_size) {
     BlockList L;
     L.first.resize(nstreams + 1);
     for (uint32_t s = 0; s < nstreams; s++) {
         L.first[s] = L.size();
-        for (uint64_t o = 0; o < src_len[s]; o += block_size) {
+        for (uint64_t o = 0; o < src_len[s]; o += block_size[s]) {
             L.off.push_back(src_off[s] + o);
-            L.len.push_back((uint32_t)std::min<uint64_t>(block_size, src_len[s] - o));
+            L.len.push_back((uint32_t)std::min<uint64_t>(block_size[s], src_len[s] - o));
         }
     }
     L.first[nstreams] = L.size();
     return L;
+}
+// every stream with the same block size
+inline BlockList cut_blocks(const uint64_t* src_off, const uint64_t* src_len, uint32_t nstreams, uint32_t block_size) {
+    return cut_blocks(src_off, src_len, nstreams, std::vector<uint32_t>(nstreams, block_size).data());
 }
 
 // The data type encodingTask.encode derives from the first four bytes of a block before the transforms run
@@ -202,6 +210,37 @@ inline PassPlan plan_decompress_passes(uint32_t n, uint64_t stride, uint64_t cos
             P.slot[i + j] = j;
         }
         P.scratch = std::max(P.scratch, (uint64_t)k * cost);
+    }
+    P.first.push_back(n);
+    return P;
+}
+
+// Decompression of blocks that each carry their stream's block size (a group of streams that differ only in block size): block b gets
+// decompress_slot(block_size[b]) and costs decompress_block_cost(block_size[b]). Blocks are taken by slot, largest first (stable, so the
+// blocks of a stream stay in order); a pass opens with the largest slot left, which is its stride, and admits blocks while that stride is
+// at most twice theirs plus 16, the pass's blocks x cost(stride) stays within the budget, and the pass holds at most MAX_PASS_BLOCKS
+// blocks. So small blocks do not get the slots of large ones, and with one block size the plan is the uniform one above, cut into passes
+// of at most MAX_PASS_BLOCKS blocks.
+inline PassPlan plan_decompress_passes(const std::vector<uint32_t>& block_size, uint64_t budget = STREAM_PASS_BUDGET) {
+    PassPlan P;
+    const uint32_t n = (uint32_t)block_size.size();
+    P.order.resize(n);
+    std::iota(P.order.begin(), P.order.end(), 0u);
+    std::stable_sort(P.order.begin(), P.order.end(), [&](uint32_t a, uint32_t b) { return block_size[a] > block_size[b]; });
+    P.pass.assign(n, 0);
+    P.slot.assign(n, 0);
+    for (uint32_t i = 0; i < n;) {
+        const uint32_t p = P.npasses(), bs = block_size[P.order[i]];
+        const uint64_t s = decompress_slot(bs), c = decompress_block_cost(bs);
+        P.first.push_back(i);
+        P.stride.push_back(s);
+        uint32_t k = 0;
+        while (i < n && k < MAX_PASS_BLOCKS && s <= 2 * decompress_slot(block_size[P.order[i]]) + 16 && (k == 0 || (uint64_t)(k + 1) * c <= budget)) {
+            P.pass[P.order[i]] = p;
+            P.slot[P.order[i]] = k++;
+            i++;
+        }
+        P.scratch = std::max(P.scratch, (uint64_t)k * c);
     }
     P.first.push_back(n);
     return P;

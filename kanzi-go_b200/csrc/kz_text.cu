@@ -30,19 +30,30 @@ const uint32_t SWORDS_BYTES = 8192;  // room for the letters of the static dicti
 
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// block b's hash map: 1 << log slots at map + off (text_map_layout)
+struct MapSlice {
+    uint64_t off;
+    uint32_t log, pad;
+};
+
 struct Ws {
     Entry* sdict;      // [1024] static entries
     uint8_t* swords;   // lower-cased letters
     uint32_t* hist0;   // [nblocks][256]
     uint32_t* hist1;   // [nblocks][65536]
     uint32_t* go;      // [nblocks] mode byte | 0x100 when the walk has to run
-    int32_t* map;      // [nblocks][1 << log]
+    MapSlice* slice;   // [nblocks] where each block's map lies (uploaded only when a serial walk runs)
+    int32_t* map;      // the maps of all blocks, back to back
     Entry* list;       // [nblocks][MAX_DICT_SIZE]
-    uint32_t log;
+    std::vector<MapSlice> h_slice;
 };
-Ws carve(uint8_t* ws, uint32_t nblocks, uint64_t stream_block_size) {
+Ws carve(uint8_t* ws, uint32_t nblocks, const uint64_t* bs) {
     Ws w;
-    w.log = log_hash_size(stream_block_size);
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> lg;
+    const uint64_t slots = text_map_layout(bs, nblocks, off, lg);
+    w.h_slice.resize(nblocks);
+    for (uint32_t b = 0; b < nblocks; b++) w.h_slice[b] = MapSlice{off[b], lg[b], 0};
     uint8_t* p = ws;
     w.sdict = reinterpret_cast<Entry*>(p);
     p += align256(sizeof(Entry) * STATIC_WORDS);
@@ -54,8 +65,10 @@ Ws carve(uint8_t* ws, uint32_t nblocks, uint64_t stream_block_size) {
     p += align256((size_t)nblocks * 65536 * 4);
     w.go = reinterpret_cast<uint32_t*>(p);
     p += align256((size_t)nblocks * 4);
+    w.slice = reinterpret_cast<MapSlice*>(p);
+    p += align256((size_t)nblocks * sizeof(MapSlice));
     w.map = reinterpret_cast<int32_t*>(p);
-    p += align256(((size_t)nblocks << w.log) * 4);
+    p += align256((size_t)slots * 4);
     w.list = reinterpret_cast<Entry*>(p);
     return w;
 }
@@ -155,10 +168,11 @@ __global__ void __launch_bounds__(32) text_plan_kernel(const uint8_t* __restrict
 
 // dictionary set-up of the blocks that go on: empty map, list = static entries followed by {hash 0, data i, no word} (reset :1190-1223)
 __global__ void __launch_bounds__(256) text_init_kernel(const uint32_t* __restrict__ go, const Entry* __restrict__ sdict, int static_n, int32_t* __restrict__ map_all,
-                                                         uint32_t log, Entry* __restrict__ list_all) {
+                                                         const MapSlice* __restrict__ slice, Entry* __restrict__ list_all) {
     const int b = blockIdx.y;
     if (go && !(go[b] & 0x100u)) return;
-    int32_t* map = map_all + ((size_t)b << log);
+    int32_t* map = map_all + slice[b].off;
+    const uint32_t log = slice[b].log;
     Entry* list = list_all + (size_t)b * MAX_DICT_SIZE;
     const uint32_t stride = gridDim.x * 256, t0 = blockIdx.x * 256 + threadIdx.x;
     for (uint32_t i = t0; i < (1u << log); i += stride) map[i] = -1;
@@ -189,13 +203,13 @@ KZ_D Dict make_dict(int32_t* map, uint32_t log, Entry* list, int static_n, const
 
 __global__ void __launch_bounds__(32) text_forward_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks,
                                                                 const uint32_t* __restrict__ go, int static_n, const uint8_t* __restrict__ swords,
-                                                                int32_t* __restrict__ map_all, uint32_t log, Entry* __restrict__ list_all,
+                                                                int32_t* __restrict__ map_all, const MapSlice* __restrict__ slice, Entry* __restrict__ list_all,
                                                                 uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
     if (!(go[b] & 0x100u)) return;
     const StageBlock blk = blocks[b];
-    Dict D = make_dict(map_all + ((size_t)b << log), log, list_all + (size_t)b * MAX_DICT_SIZE, static_n, swords, (int)blk.len);
+    Dict D = make_dict(map_all + slice[b].off, slice[b].log, list_all + (size_t)b * MAX_DICT_SIZE, static_n, swords, (int)blk.len);
     const int n = forward_walk(in + blk.src_off, (int)blk.len, out + blk.dst_off, (uint8_t)(go[b] & 0xFF), D);
     if (n >= 0) {
         StageResult r = res[b];
@@ -206,7 +220,7 @@ __global__ void __launch_bounds__(32) text_forward_walk_kernel(const uint8_t* __
 }
 
 __global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __restrict__ in, const StageBlock* __restrict__ blocks, int nblocks, int static_n,
-                                                                const uint8_t* __restrict__ swords, int32_t* __restrict__ map_all, uint32_t log,
+                                                                const uint8_t* __restrict__ swords, int32_t* __restrict__ map_all, const MapSlice* __restrict__ slice,
                                                                 Entry* __restrict__ list_all, uint8_t* __restrict__ out, StageResult* __restrict__ res) {
     const int b = blockIdx.x;
     if (b >= nblocks || threadIdx.x != 0) return;
@@ -220,7 +234,7 @@ __global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __
     if (blk.len != 0 && blk.cap != 0) {  // wrapper :573-575
         int64_t n = -1;
         if (blk.len >= 2 && blk.len <= (1u << 30)) {
-            Dict D = make_dict(map_all + ((size_t)b << log), log, list_all + (size_t)b * MAX_DICT_SIZE, static_n, swords, (int)min(blk.cap, 0x7FFFFFFFu));
+            Dict D = make_dict(map_all + slice[b].off, slice[b].log, list_all + (size_t)b * MAX_DICT_SIZE, static_n, swords, (int)min(blk.cap, 0x7FFFFFFFu));
             n = inverse_walk(in + blk.src_off, (int)blk.len, out + blk.dst_off, (int64_t)blk.cap, D);
         }
         if (n < 0) r.status = -KZ_E_PROCESS_BLOCK;
@@ -231,27 +245,43 @@ __global__ void __launch_bounds__(32) text_inverse_walk_kernel(const uint8_t* __
 
 }  // namespace
 
-size_t text_workspace_serial(uint32_t nblocks, uint64_t stream_block_size) {
-    const uint32_t lg = log_hash_size(stream_block_size);
+uint64_t text_map_layout(const uint64_t* bs, uint32_t nblocks, std::vector<uint64_t>& off, std::vector<uint32_t>& lg) {
+    off.resize(nblocks);
+    lg.resize(nblocks);
+    uint64_t slots = 0;
+    for (uint32_t b = 0; b < nblocks; b++) {
+        lg[b] = log_hash_size(bs[b]);
+        off[b] = slots;
+        slots += 1ull << lg[b];
+    }
+    return slots;
+}
+
+size_t text_workspace_serial(const uint64_t* bs, uint32_t nblocks) {
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> lg;
+    const uint64_t slots = text_map_layout(bs, nblocks, off, lg);
     return align256(sizeof(Entry) * STATIC_WORDS) + align256(SWORDS_BYTES) + align256((size_t)nblocks * 256 * 4) + align256((size_t)nblocks * 65536 * 4) +
-           align256((size_t)nblocks * 4) + align256(((size_t)nblocks << lg) * 4) + align256((size_t)nblocks * MAX_DICT_SIZE * sizeof(Entry)) + 256;
+           align256((size_t)nblocks * 4) + align256((size_t)nblocks * sizeof(MapSlice)) + align256((size_t)slots * 4) +
+           align256((size_t)nblocks * MAX_DICT_SIZE * sizeof(Entry)) + 256;
 }
-size_t text_workspace(uint32_t nblocks, uint64_t stream_block_size, uint32_t max_len) {
-    return align256(text_workspace_serial(nblocks, stream_block_size)) + text_parallel_workspace(nblocks, max_len, stream_block_size) + 256;
+size_t text_workspace(const uint64_t* bs, uint32_t nblocks, uint32_t max_len) {
+    return align256(text_workspace_serial(bs, nblocks)) + text_parallel_workspace(bs, nblocks, max_len) + 256;
 }
-size_t text_workspace_inverse(uint32_t nblocks, uint64_t stream_block_size, uint32_t max_len) {
-    return align256(text_workspace_serial(nblocks, stream_block_size)) + text_inverse_parallel_workspace(nblocks, max_len, stream_block_size) + 256;
+size_t text_workspace_inverse(const uint64_t* bs, uint32_t nblocks, uint32_t max_len) {
+    return align256(text_workspace_serial(bs, nblocks)) + text_inverse_parallel_workspace(bs, nblocks, max_len) + 256;
 }
 
 cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint32_t max_len,
-                               uint64_t stream_block_size, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
+                               const uint64_t* bs, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches,
+                               uint64_t* serial) {
 #if !KZ_HAVE_TEXT_DICT
-    (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)max_len; (void)stream_block_size; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
+    (void)serial; (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)max_len; (void)bs; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
     return cudaErrorNotSupported;
 #else
     if (nblocks == 0) return cudaSuccess;
-    if (ws_bytes < text_workspace(nblocks, stream_block_size, max_len)) return cudaErrorInvalidValue;
-    const Ws w = carve(ws, nblocks, stream_block_size);
+    if (ws_bytes < text_workspace(bs, nblocks, max_len)) return cudaErrorInvalidValue;
+    const Ws w = carve(ws, nblocks, bs);
     const HostStatic& S = host_static();
     cudaError_t e;
     if ((e = cudaMemcpyAsync(w.sdict, S.entries.data(), sizeof(Entry) * STATIC_WORDS, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
@@ -261,14 +291,17 @@ cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageB
     text_hist_kernel<<<dim3(HIST_SLICES, nblocks), 256, 0, stream>>>(d_in, d_blocks, w.hist0, w.hist1);
     text_plan_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, w.hist0, w.hist1, w.go, d_res);
     // data-parallel path (kz_text_par.cu); blocks it does not cover come back in `fallback` and take the serial walk below
-    uint8_t* pws = ws + align256(text_workspace_serial(nblocks, stream_block_size));
-    const size_t pws_bytes = ws_bytes - align256(text_workspace_serial(nblocks, stream_block_size));
+    uint8_t* pws = ws + align256(text_workspace_serial(bs, nblocks));
+    const size_t pws_bytes = ws_bytes - align256(text_workspace_serial(bs, nblocks));
     std::vector<StageBlock> tb(h_blocks, h_blocks + nblocks);
     std::vector<uint32_t> fallback;
-    if ((e = text_forward_parallel(d_in, d_out, tb, w.go, stream_block_size, w.sdict, w.swords, S.n, pws, pws_bytes, d_res, stream, fallback, launches)) != cudaSuccess)
+    if ((e = text_forward_parallel(d_in, d_out, tb, w.go, bs, w.sdict, w.swords, S.n, pws, pws_bytes, d_res, stream, fallback, launches)) != cudaSuccess)
         return e;
     bool any = false;
-    for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
+    for (uint32_t b = 0; b < nblocks; b++) {
+        any = any || fallback[b];
+        if (serial && fallback[b] && h_blocks[b].len) ++*serial;  // a block of data the serial walk decodes
+    }
     if (!any) return cudaGetLastError();
     std::vector<uint32_t> go(nblocks);
     // on the context's own (non-blocking) stream: a plain cudaMemcpy would neither wait for it nor leave other contexts alone
@@ -277,44 +310,49 @@ cudaError_t text_forward_batch(const uint8_t* d_in, uint8_t* d_out, const StageB
     for (uint32_t b = 0; b < nblocks; b++)
         if (!fallback[b]) go[b] = 0;
     if ((e = cudaMemcpyAsync(w.go, go.data(), nblocks * 4, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;  // `go` is a local
-    text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(w.go, w.sdict, S.n, w.map, w.log, w.list);
-    text_forward_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, w.go, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);
+    if ((e = cudaMemcpyAsync(w.slice, w.h_slice.data(), nblocks * sizeof(MapSlice), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;  // `go` and the slices are locals
+    text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(w.go, w.sdict, S.n, w.map, w.slice, w.list);
+    text_forward_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_blocks, (int)nblocks, w.go, S.n, w.swords, w.map, w.slice, w.list, d_out, d_res);
     if (launches) *launches += 4;
     return cudaGetLastError();
 #endif
 }
 
-cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, uint64_t stream_block_size,
-                               uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches) {
+cudaError_t text_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const StageBlock* d_blocks, const StageBlock* h_blocks, uint32_t nblocks, const uint64_t* bs,
+                               uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream, uint64_t* launches, uint64_t* serial) {
 #if !KZ_HAVE_TEXT_DICT
-    (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)stream_block_size; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
+    (void)serial; (void)d_in; (void)d_out; (void)d_blocks; (void)h_blocks; (void)nblocks; (void)bs; (void)ws; (void)ws_bytes; (void)d_res; (void)stream; (void)launches;
     return cudaErrorNotSupported;
 #else
     if (nblocks == 0) return cudaSuccess;
-    if (ws_bytes < text_workspace_serial(nblocks, stream_block_size)) return cudaErrorInvalidValue;
-    const Ws w = carve(ws, nblocks, stream_block_size);
+    if (ws_bytes < text_workspace_serial(bs, nblocks)) return cudaErrorInvalidValue;
+    const Ws w = carve(ws, nblocks, bs);
     const HostStatic& S = host_static();
     cudaError_t e;
     if ((e = cudaMemcpyAsync(w.sdict, S.entries.data(), sizeof(Entry) * STATIC_WORDS, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     if ((e = cudaMemcpyAsync(w.swords, S.words.data(), SWORDS_BYTES, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     // data-parallel path (kz_text_par.cu); trivial blocks and every anomaly come back in `fallback` and take the serial walk below
-    const size_t used = align256(text_workspace_serial(nblocks, stream_block_size));
+    const size_t used = align256(text_workspace_serial(bs, nblocks));
     std::vector<StageBlock> tb(h_blocks, h_blocks + nblocks);
     std::vector<uint32_t> fallback;
-    if ((e = text_inverse_parallel(d_in, d_out, tb, stream_block_size, w.sdict, w.swords, S.n, ws + used, ws_bytes - used, d_res, stream, fallback, launches)) != cudaSuccess)
+    if ((e = text_inverse_parallel(d_in, d_out, tb, bs, w.sdict, w.swords, S.n, ws + used, ws_bytes - used, d_res, stream, fallback, launches)) != cudaSuccess)
         return e;
     bool any = false;
-    for (uint32_t b = 0; b < nblocks; b++) any = any || fallback[b];
+    for (uint32_t b = 0; b < nblocks; b++) {
+        any = any || fallback[b];
+        if (serial && fallback[b] && h_blocks[b].len) ++*serial;  // a block of data the serial walk decodes
+    }
     if (!any) return cudaGetLastError();
     // the serial kernel writes res[b] for every block: give it a descriptor list in which the finished blocks are marked
     for (uint32_t b = 0; b < nblocks; b++)
         if (!fallback[b]) tb[b].flags = 1;
     StageBlock* d_tmp = reinterpret_cast<StageBlock*>(w.hist1);  // the forward-only histogram area is free here
     if ((e = cudaMemcpyAsync(d_tmp, tb.data(), nblocks * sizeof(StageBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(w.slice, w.h_slice.data(), nblocks * sizeof(MapSlice), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
-    text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(nullptr, w.sdict, S.n, w.map, w.log, w.list);
-    text_inverse_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_tmp, (int)nblocks, S.n, w.swords, w.map, w.log, w.list, d_out, d_res);
+    text_init_kernel<<<dim3(INIT_SLICES, nblocks), 256, 0, stream>>>(nullptr, w.sdict, S.n, w.map, w.slice, w.list);
+    text_inverse_walk_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_tmp, (int)nblocks, S.n, w.swords, w.map, w.slice, w.list, d_out, d_res);
     if (launches) *launches += 2;
     return cudaGetLastError();
 #endif

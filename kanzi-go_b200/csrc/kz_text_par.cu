@@ -29,10 +29,12 @@ struct TpBlock {
     uint64_t src_off, dst_off;
     uint64_t cand_off;  // first entry in the candidate-indexed arrays
     uint64_t cp_off;    // first entry in cp[]
-    uint64_t owner_off;
+    uint64_t owner_off; // first slot of the block's hash map (text_map_layout)
     uint32_t len, go;   // go = mode | 0x100 when the block is text (text_plan_kernel), 0 otherwise
     uint32_t pt_base, npt;
     uint32_t ct_base, nct_cap;
+    uint32_t mask;       // slots of the block's map - 1 (its stream's block size decides)
+    uint32_t owner0_off; // first slot of the static words' map for that size
 };
 struct TpState {
     uint32_t ncand, nf, lead, nins;
@@ -200,12 +202,13 @@ __global__ void __launch_bounds__(256) tp_init_ins_kernel(const TpBlock* __restr
 }
 
 // ---- phase B: one dictionary round ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) tp_round_begin_kernel(const TpBlock* __restrict__ blocks, TpState* __restrict__ st, const int32_t* __restrict__ owner0, uint32_t slots,
+__global__ void __launch_bounds__(256) tp_round_begin_kernel(const TpBlock* __restrict__ blocks, TpState* __restrict__ st, const int32_t* __restrict__ owner0,
                                                               int32_t* __restrict__ owner) {
     const TpBlock B = blocks[blockIdx.y];
     if (!(B.go & 0x100u)) return;
     int32_t* o = owner + B.owner_off;
-    for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < slots; i += gridDim.x * 256) o[i] = owner0[i];
+    const int32_t* o0 = owner0 + B.owner0_off;
+    for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i <= B.mask; i += gridDim.x * 256) o[i] = o0[i];
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         TpState& S = st[blockIdx.y];
         S.changed = 0;
@@ -215,7 +218,7 @@ __global__ void __launch_bounds__(256) tp_round_begin_kernel(const TpBlock* __re
     }
 }
 __global__ void __launch_bounds__(256) tp_round_owners_kernel(const TpBlock* __restrict__ blocks, TpState* __restrict__ st, const Candidate* __restrict__ cand_all,
-                                                               const uint8_t* __restrict__ ins, uint32_t mask, int32_t* __restrict__ owner, uint32_t* __restrict__ ct_cnt) {
+                                                               const uint8_t* __restrict__ ins, int32_t* __restrict__ owner, uint32_t* __restrict__ ct_cnt) {
     __shared__ uint32_t s_a[8];
     const int b = blockIdx.y;
     const TpBlock B = blocks[b];
@@ -231,7 +234,7 @@ __global__ void __launch_bounds__(256) tp_round_owners_kernel(const TpBlock* __r
         if (k >= nc || !ins[B.cand_off + k]) continue;
         mine++;
         first = min(first, (int)k);
-        const uint32_t s1 = cand_all[B.cand_off + k].h1 & mask;
+        const uint32_t s1 = cand_all[B.cand_off + k].h1 & B.mask;
         if (s1 == 0) {
             const int z = atomicAdd(&S.z0.n, 1);
             if (z < Z0_MAX) {
@@ -265,7 +268,7 @@ __global__ void __launch_bounds__(256) tp_round_nx_kernel(const TpBlock* __restr
 }
 __global__ void __launch_bounds__(256) tp_round_eval_kernel(const uint8_t* __restrict__ in, const TpBlock* __restrict__ blocks, TpState* __restrict__ st,
                                                              const Candidate* __restrict__ cand_all, const uint8_t* __restrict__ ins, uint8_t* __restrict__ ins_new,
-                                                             uint32_t mask, const int32_t* __restrict__ owner, const Entry* __restrict__ sdict,
+                                                             const int32_t* __restrict__ owner, const Entry* __restrict__ sdict,
                                                              const uint8_t* __restrict__ swords, const uint32_t* __restrict__ ct_base_cnt, uint32_t* __restrict__ rank,
                                                              int32_t* __restrict__ focc, uint8_t* __restrict__ fflip, int inverse) {
     __shared__ uint32_t s_a[8];
@@ -292,7 +295,7 @@ __global__ void __launch_bounds__(256) tp_round_eval_kernel(const uint8_t* __res
     V.src = in + B.src_off;
     V.cand = cand_all + B.cand_off;
     V.owner = owner + B.owner_off;
-    V.mask = mask;
+    V.mask = B.mask;
     V.sdict = sdict;
     V.swords = swords;
     V.z0 = &s_z0;
@@ -540,10 +543,34 @@ __global__ void tp_set_counts_kernel(const TpBlock* __restrict__ blocks, int nbl
         st[b].fail = 0;
     }
 }
-__global__ void tp_owner0_kernel(const Entry* __restrict__ sdict, int static_n, uint32_t mask, int32_t* __restrict__ owner0) {
-    // later static words win a shared slot (textCodec2.reset :1212-1215): one thread, 1024 stores
-    if (blockIdx.x == 0 && threadIdx.x == 0)
-        for (int i = 0; i < static_n; i++) owner0[(uint32_t)sdict[i].hash & mask] = -(i + 1);
+// The static words' maps of every hash size a batch uses (lg 13 .. 24), back to back: CTA k fills the map of lg[k] at slot off[k].
+struct Owner0Maps {
+    uint32_t n;
+    uint32_t lg[12], off[12];
+};
+// lg of every block -> the maps of its distinct sizes (owner0_off of each block); returns the slots of all of them
+uint64_t owner0_maps(const std::vector<uint32_t>& lg, Owner0Maps& m, std::vector<uint32_t>& owner0_off) {
+    m.n = 0;
+    uint64_t slots = 0;
+    owner0_off.resize(lg.size());
+    for (size_t b = 0; b < lg.size(); b++) {
+        uint32_t k = 0;
+        while (k < m.n && m.lg[k] != lg[b]) k++;
+        if (k == m.n) {
+            m.lg[m.n] = lg[b], m.off[m.n] = (uint32_t)slots, m.n++;
+            slots += 1ull << lg[b];
+        }
+        owner0_off[b] = m.off[k];
+    }
+    return slots;
+}
+__global__ void tp_owner0_kernel(const Entry* __restrict__ sdict, int static_n, Owner0Maps m, int32_t* __restrict__ owner0) {
+    // later static words win a shared slot (textCodec2.reset :1212-1215): one thread per map, 1024 stores
+    if (blockIdx.x < m.n && threadIdx.x == 0) {
+        const uint32_t mask = (1u << m.lg[blockIdx.x]) - 1;
+        int32_t* o = owner0 + m.off[blockIdx.x];
+        for (int i = 0; i < static_n; i++) o[(uint32_t)sdict[i].hash & mask] = -(i + 1);
+    }
 }
 __global__ void __launch_bounds__(256) tp_fill_kernel(int32_t* __restrict__ p, int32_t v, size_t n) {
     for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) p[i] = v;
@@ -895,7 +922,7 @@ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 // the dictionary rounds of kz_text_par_core.cuh for every block with go & 0x100; h_st[b].changed != 0 afterwards: no fixed point within MAX_ROUNDS
 cudaError_t dictionary_rounds(const uint8_t* d_in, const TpBlock* d_pb, const std::vector<TpBlock>& pb, TpState* d_st, std::vector<TpState>& h_st,
-                              const Candidate* d_cand, uint8_t* d_ins, uint8_t* d_ins2, uint32_t mask, uint32_t slots, int32_t* d_owner, const int32_t* d_owner0,
+                              const Candidate* d_cand, uint8_t* d_ins, uint8_t* d_ins2, int32_t* d_owner, const int32_t* d_owner0,
                               const Entry* sd, const uint8_t* d_swords, uint32_t* d_ct, uint32_t* d_tot, uint32_t* d_rank, int32_t* d_focc, uint8_t* d_fflip,
                               uint32_t max_nct, int inverse, size_t ins_bytes /* size of d_ins / d_ins2 */, cudaStream_t stream, uint64_t* launches) {
     const uint32_t nblocks = (uint32_t)pb.size();
@@ -904,11 +931,11 @@ cudaError_t dictionary_rounds(const uint8_t* d_in, const TpBlock* d_pb, const st
     bool converged = false;
     cudaError_t e;
     for (int rounds = 0; rounds < MAX_ROUNDS && !converged; rounds++) {
-        tp_round_begin_kernel<<<gs, 256, 0, stream>>>(d_pb, d_st, d_owner0, slots, d_owner);
-        tp_round_owners_kernel<<<gc, 256, 0, stream>>>(d_pb, d_st, d_cand, cur, mask, d_owner, d_ct);
+        tp_round_begin_kernel<<<gs, 256, 0, stream>>>(d_pb, d_st, d_owner0, d_owner);
+        tp_round_owners_kernel<<<gc, 256, 0, stream>>>(d_pb, d_st, d_cand, cur, d_owner, d_ct);
         tp_round_nx_kernel<<<gs, 256, 0, stream>>>(d_pb, d_st, cur);
         tp_scan_tiles_kernel<<<nblocks, 32, 0, stream>>>(d_pb, (int)nblocks, 1, d_ct, d_tot, CT, d_tot, 8, 1);
-        tp_round_eval_kernel<<<gc, 256, 0, stream>>>(d_in, d_pb, d_st, d_cand, cur, nxt, mask, d_owner, sd, d_swords, d_ct, d_rank, d_focc, d_fflip, inverse);
+        tp_round_eval_kernel<<<gc, 256, 0, stream>>>(d_in, d_pb, d_st, d_cand, cur, nxt, d_owner, sd, d_swords, d_ct, d_rank, d_focc, d_fflip, inverse);
         if (launches) *launches += 5;
         if ((e = cudaMemcpyAsync(h_st.data(), d_st, nblocks * sizeof(TpState), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
         if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
@@ -924,19 +951,31 @@ cudaError_t dictionary_rounds(const uint8_t* d_in, const TpBlock* d_pb, const st
     return cudaGetLastError();
 }
 
+// the hash maps of a batch: every block's (text_map_layout), then the static words' map of each distinct size (owner0_maps)
+struct HashMaps {
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> lg, owner0_off;
+    Owner0Maps o0;
+    uint64_t slots = 0, o0_slots = 0;
+    HashMaps(const uint64_t* bs, uint32_t nblocks) {
+        slots = text_map_layout(bs, nblocks, off, lg);
+        o0_slots = owner0_maps(lg, o0, owner0_off);
+    }
+};
+
 }  // namespace
 
-size_t text_parallel_workspace(uint32_t nblocks, uint32_t max_len, uint64_t stream_block_size) {
-    const uint32_t lg = log_hash_size(stream_block_size);
+size_t text_parallel_workspace(const uint64_t* bs, uint32_t nblocks, uint32_t max_len) {
+    const HashMaps H(bs, nblocks);
     const size_t nb = nblocks;
     const size_t cands = nb * ((size_t)max_len / 3 + 16), cps = nb * ((size_t)max_len + 8), pts = nb * ((size_t)max_len / PT + 2), cts = nb * (((size_t)max_len / 3 + 16 + CT - 1) / CT + 1);
     return align256(nb * sizeof(TpBlock)) + align256(nb * sizeof(TpState)) + align256(nb * 32) + align256(nb * 4) + 2 * align256(pts * 4) + 2 * align256(cts * 4) +
            align256(cands * sizeof(Candidate)) + 3 * align256(cands) + 3 * align256(cands * 4) + align256(cands * sizeof(FoundW)) + align256(cps * 4) +
-           align256((nb << lg) * 4) + align256((size_t(1) << lg) * 4) + 8192;
+           align256(H.slots * 4) + align256(H.o0_slots * 4) + 8192;
 }
 
 // d_go: the plan kernel's verdict per block (mode | 0x100 for text blocks). On return h_fallback[b] != 0 marks the text blocks the serial walk must do.
-cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, const uint32_t* d_go, uint64_t stream_block_size,
+cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, const uint32_t* d_go, const uint64_t* bs,
                                   const void* d_sdict, const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream,
                                   std::vector<uint32_t>& h_fallback, uint64_t* launches) {
     const uint32_t nblocks = (uint32_t)tb.size();
@@ -949,8 +988,7 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     bool any = false;
     for (uint32_t b = 0; b < nblocks; b++) any = any || (h_go[b] & 0x100u);
     if (!any) return cudaSuccess;
-    const uint32_t lg = log_hash_size(stream_block_size);
-    const uint32_t slots = 1u << lg, mask = slots - 1;
+    const HashMaps H(bs, nblocks);
     std::vector<TpBlock> pb(nblocks);
     uint64_t cands = 0, cps = 0;
     uint32_t pts = 0, cts = 0, max_npt = 1, max_nct = 1;
@@ -964,7 +1002,9 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
         cands += (uint64_t)B.len / 3 + 16;
         B.cp_off = cps;
         cps += (uint64_t)B.len + 8;
-        B.owner_off = (uint64_t)b << lg;
+        B.owner_off = H.off[b];
+        B.mask = (1u << H.lg[b]) - 1;
+        B.owner0_off = H.owner0_off[b];
         B.pt_base = pts;
         B.npt = B.len / PT + 1;  // the tile of position `len` included (cp[len] = total cost)
         pts += B.npt + 1;
@@ -999,8 +1039,8 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     uint8_t* d_fflip = take(cands);
     FoundW* d_found = (FoundW*)take(cands * sizeof(FoundW));
     uint32_t* d_cp = (uint32_t*)take(cps * 4);
-    int32_t* d_owner = (int32_t*)take(((size_t)nblocks << lg) * 4);
-    int32_t* d_owner0 = (int32_t*)take((size_t)slots * 4);
+    int32_t* d_owner = (int32_t*)take((size_t)H.slots * 4);
+    int32_t* d_owner0 = (int32_t*)take((size_t)H.o0_slots * 4);
     if (off > ws_bytes) return cudaErrorInvalidValue;
     const Entry* sd = (const Entry*)d_sdict;
     if ((e = cudaMemcpyAsync(d_pb, pb.data(), nblocks * sizeof(TpBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
@@ -1008,8 +1048,8 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     if ((e = cudaMemsetAsync(d_tot, 0, nblocks * 32, stream)) != cudaSuccess) return e;
     const dim3 gp(max_npt, nblocks), gc(max_nct, nblocks), gs(32, nblocks);
     // ---- A
-    tp_fill_kernel<<<64, 256, 0, stream>>>(d_owner0, OCC_EMPTY, slots);
-    tp_owner0_kernel<<<1, 32, 0, stream>>>(sd, static_n, mask, d_owner0);
+    tp_fill_kernel<<<64, 256, 0, stream>>>(d_owner0, OCC_EMPTY, H.o0_slots);
+    tp_owner0_kernel<<<H.o0.n, 32, 0, stream>>>(sd, static_n, H.o0, d_owner0);
     tp_last_nontext_kernel<<<gp, 256, 0, stream>>>(d_in, d_pb, d_tile_last);
     tp_carry_kernel<<<nblocks, 32, 0, stream>>>(d_in, d_pb, (int)nblocks, d_tile_last, d_st);
     tp_candidates_kernel<<<gp, 256, 0, stream>>>(d_in, d_pb, d_tile_last, d_pt, 0, d_cand);
@@ -1020,7 +1060,7 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     tp_init_ins_kernel<<<gs, 256, 0, stream>>>(d_pb, d_st, d_cand, d_ins);
     // ---- B
     std::vector<TpState> h_st(nblocks);
-    if ((e = dictionary_rounds(d_in, d_pb, pb, d_st, h_st, d_cand, d_ins, d_ins2, mask, slots, d_owner, d_owner0, sd, d_swords, d_ct, d_tot, d_rank, d_focc, d_fflip, max_nct,
+    if ((e = dictionary_rounds(d_in, d_pb, pb, d_st, h_st, d_cand, d_ins, d_ins2, d_owner, d_owner0, sd, d_swords, d_ct, d_tot, d_rank, d_focc, d_fflip, max_nct,
                                0, (size_t)cands, stream, launches)) != cudaSuccess)
         return e;
     // the last round confirmed `nxt` (== cur bytewise for converged blocks); rank / focc / fflip belong to it
@@ -1050,14 +1090,13 @@ cudaError_t text_forward_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     return cudaGetLastError();
 }
 
-cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, uint64_t stream_block_size, const void* d_sdict,
+cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std::vector<StageBlock>& tb, const uint64_t* bs, const void* d_sdict,
                                   const uint8_t* d_swords, int static_n, uint8_t* ws, size_t ws_bytes, StageResult* d_res, cudaStream_t stream,
                                   std::vector<uint32_t>& h_fallback, uint64_t* launches) {
     const uint32_t nblocks = (uint32_t)tb.size();
     h_fallback.assign(nblocks, 1);
     if (nblocks == 0) return cudaSuccess;
-    const uint32_t lg = log_hash_size(stream_block_size);
-    const uint32_t slots = 1u << lg, mask = slots - 1;
+    const HashMaps H(bs, nblocks);
     std::vector<TiBlock> ib(nblocks);
     std::vector<TpBlock> pb(nblocks);
     uint64_t cands = 0, poss = 0;
@@ -1074,7 +1113,7 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
         cands += (uint64_t)B.len / 4 + 16;
         B.pos_off = poss;
         poss += (uint64_t)B.len + 16;
-        B.owner_off = (uint64_t)b << lg;
+        B.owner_off = H.off[b];
         B.pt_base = pts;
         B.npt = B.len / PT + 1;
         pts += B.npt + 1;
@@ -1084,6 +1123,7 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
         TpBlock& P = pb[b];
         P.src_off = B.src_off, P.dst_off = B.dst_off, P.cand_off = B.cand_off, P.cp_off = 0, P.owner_off = B.owner_off;
         P.len = B.len, P.go = B.go, P.pt_base = B.pt_base, P.npt = B.npt, P.ct_base = B.ct_base, P.nct_cap = B.nct_cap;
+        P.mask = (1u << H.lg[b]) - 1, P.owner0_off = H.owner0_off[b];
         if (B.go) {
             any = true;
             max_npt = std::max(max_npt, B.npt);
@@ -1115,8 +1155,8 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     int32_t* d_focc = (int32_t*)take(cands * 4);
     uint32_t* d_ins_list = (uint32_t*)take(cands * 4);
     uint8_t* d_fflip = take(cands);
-    int32_t* d_owner = (int32_t*)take(((size_t)nblocks << lg) * 4);
-    int32_t* d_owner0 = (int32_t*)take((size_t)slots * 4);
+    int32_t* d_owner = (int32_t*)take((size_t)H.slots * 4);
+    int32_t* d_owner0 = (int32_t*)take((size_t)H.o0_slots * 4);
     if (off > ws_bytes) return cudaErrorInvalidValue;
     const Entry* sd = (const Entry*)d_sdict;
     cudaError_t e;
@@ -1125,8 +1165,8 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     if ((e = cudaMemsetAsync(d_tot, 0, nblocks * 32, stream)) != cudaSuccess) return e;
     const dim3 gp(max_npt, nblocks), gs(32, nblocks);
     const uint32_t gb = (nblocks + 255) / 256;
-    tp_fill_kernel<<<64, 256, 0, stream>>>(d_owner0, OCC_EMPTY, slots);
-    tp_owner0_kernel<<<1, 32, 0, stream>>>(sd, static_n, mask, d_owner0);
+    tp_fill_kernel<<<64, 256, 0, stream>>>(d_owner0, OCC_EMPTY, H.o0_slots);
+    tp_owner0_kernel<<<H.o0.n, 32, 0, stream>>>(sd, static_n, H.o0, d_owner0);
     ti_token_tiles_kernel<<<gp, 256, 0, stream>>>(d_in, d_ib, d_fn);
     ti_token_carry_kernel<<<nblocks, 32, 0, stream>>>(d_ib, (int)nblocks, d_fn, d_ist);
     ti_token_mark_kernel<<<gp, 256, 0, stream>>>(d_in, d_ib, d_fn, d_start, d_lastq);
@@ -1138,7 +1178,7 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     ti_init_ins_kernel<<<gs, 256, 0, stream>>>(d_pb, d_tst, d_ins);
     if (launches) *launches += 11;
     std::vector<TpState> h_st(nblocks);
-    if ((e = dictionary_rounds(d_in, d_pb, pb, d_tst, h_st, d_cand, d_ins, d_ins2, mask, slots, d_owner, d_owner0, sd, d_swords, d_ct, d_tot, d_rank, d_focc, d_fflip, max_nct, 1,
+    if ((e = dictionary_rounds(d_in, d_pb, pb, d_tst, h_st, d_cand, d_ins, d_ins2, d_owner, d_owner0, sd, d_swords, d_ct, d_tot, d_rank, d_focc, d_fflip, max_nct, 1,
                                (size_t)cands, stream, launches)) != cudaSuccess)
         return e;
     ti_ins_list_kernel<<<gs, 256, 0, stream>>>(d_pb, d_tst, d_ins, d_rank, d_ins_list);
@@ -1164,13 +1204,13 @@ cudaError_t text_inverse_parallel(const uint8_t* d_in, uint8_t* d_out, const std
     return cudaGetLastError();
 }
 
-size_t text_inverse_parallel_workspace(uint32_t nblocks, uint32_t max_len, uint64_t stream_block_size) {
-    const uint32_t lg = log_hash_size(stream_block_size);
+size_t text_inverse_parallel_workspace(const uint64_t* bs, uint32_t nblocks, uint32_t max_len) {
+    const HashMaps H(bs, nblocks);
     const size_t nb = nblocks;
     const size_t cands = nb * ((size_t)max_len / 4 + 16), poss = nb * ((size_t)max_len + 16), pts = nb * ((size_t)max_len / PT + 2), cts = nb * (((size_t)max_len / 4 + 16 + CT - 1) / CT + 1);
     return align256(nb * sizeof(TiBlock)) + align256(nb * sizeof(TpBlock)) + align256(nb * sizeof(TpState)) + align256(nb * sizeof(TiState)) + align256(nb * 32) +
            3 * align256(pts * 4) + align256(cts * 4) + align256(poss) + align256(poss * 4) + align256(cands * sizeof(Candidate)) + 3 * align256(cands) + 3 * align256(cands * 4) +
-           align256((nb << lg) * 4) + align256((size_t(1) << lg) * 4) + 8192;
+           align256(H.slots * 4) + align256(H.o0_slots * 4) + 8192;
 }
 
 }  // namespace kz
