@@ -379,6 +379,51 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
 
+/* ---- writes: byte ranges written into a compressed stream, and appends, re-encoding only the blocks they touch ------------------------
+ * Blocks are independent, every block but the last decodes to exactly block_size bytes, and nothing in a record depends on its position,
+ *   so a write that touches blocks k .. m re-encodes only those; everything before record k stays as it is and the records behind m are
+ *   copied, moved by the change in bit length. The caller rewrites only the stream's tail: for an append, the last record and the end marker.
+ * Writes: write i puts data[data_off[i] .. + len[i]) at decoded offset off[i], in array order (a later write wins where writes overlap).
+ *   pwrite semantics: a write that ends past the current end grows the data, and a gap between the end and a write's offset reads as zero
+ *   bytes. A zero-length write changes nothing, wherever it points. off[i] == KZ_WRITE_APPEND means the current end of the data, counting
+ *   the call's earlier writes.
+ * Result: the new stream is src[0 .. *keep) followed by dst[0 .. *out_n). *keep = floor(cut / 8), cut being the first bit of the prefix of
+ *   the first record that changes, or the end marker's first bit when the writes only add blocks behind a full last block; dst starts with
+ *   the cut % 8 bits of src[*keep] that lie before the cut. A call that changes nothing returns *keep = n and *out_n = 0.
+ *   The new stream is byte for byte what kz_compress_stream writes for the new data with the stream's own transform, entropy, block size,
+ *   checksum bits and header input-size hint (left as it is: readers never trust it); a headerless index gives a headerless stream whatever
+ *   the headerless-writer setting. This holds when the old stream is what kz_compress_stream writes for the old data under ctx's current
+ *   kz_set_skip_blocks setting. Records behind the cut that are not re-encoded are copied as they are and never verified.
+ * Work: a block is re-encoded when a write of length > 0 overlaps it, a zero gap covers it, or it is the old last block and the data grows
+ *   past its end. Only the re-encoded old blocks the writes do not cover completely are decoded. When the index does not know the size
+ *   (kz_index_info), the old last block is decoded first if the result depends on its length: a KZ_WRITE_APPEND before the writes reach
+ *   past the last block's range, or a write into that range or beyond while the writes do not cover all of it. Blocks the writes cover and
+ *   new blocks are never decoded. Decode and encode run in passes within the budget of the reads.
+ * Index: on success ix describes the new stream: record starts and lengths, stream_bytes, the first 32 bytes, and the size, which becomes
+ *   exact once the last block has been decoded or fully written (else it keeps its value). kz_index_save gives the blob kz_index_build
+ *   gives for the new stream, apart from the size where the build does not know it. On any failure ix, src and the caller's bytes are
+ *   unchanged.
+ * Errors: a stale index (n or the first 32 bytes differ) -KZ_ERR_INVALID_PARAM, as kz_read_ranges; a chain or codec the GPU path lacks
+ *   -KZ_ERR_CREATE_CODEC; an open session on ctx, len[i] > 0 with a NULL data or data_off, or a new size whose blocks x block_size pass 2^62
+ *   -KZ_ERR_INVALID_PARAM. A block that must be decoded and fails returns the code kz_read_ranges gives for that block (block header,
+ *   entropy, inverse transform or checksum); a decoded block before the last that is not block_size bytes long -KZ_ERR_INVALID_FILE; an
+ *   encode failure its code. cap too small: -KZ_ERR_WRITE_FILE with *out_n set to the capacity the call needs, the tail's length rounded up
+ *   to a multiple of 4 bytes (the tail is written in whole 32-bit words). (n - keep) + k * kz_max_block_output(block_size) + 16 bytes, k
+ *   blocks re-encoded or added, always suffice.
+ * Memory: one pass's scratch, the uploaded tail (host variant: src from the first record the call reads or moves, n - keep bytes or
+ *   slightly more) and write bytes, the new records and the output. Appends of unbounded length through a session opened on an index are
+ *   not offered.
+ * With kz_profile(ctx,1): kz_stage_bytes("write:decoded") = blocks / decoded bytes, ("write:encoded") = blocks / their input bytes,
+ *   ("write:moved") = runs of old records / bits re-emitted behind the re-encoded blocks, ("write:h2d") = uploads / bytes (host variant).
+ * Threads: the one-thread-per-context rule; an index is used by one thread at a time. */
+#define KZ_WRITE_APPEND UINT64_MAX
+int kz_write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len, const uint8_t* data,
+                    const uint64_t* data_off, uint8_t* dst, size_t cap, uint64_t* keep, size_t* out_n);
+/* d_src as for kz_index_build_device (16-byte aligned, at least 64 readable bytes behind it); d_dst 16-byte aligned and not overlapping
+ *   d_src; d_data + data_off[i] are device bytes with no alignment rule; off, len, data_off, keep and out_n are host memory. */
+int kz_write_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len,
+                           const void* d_data, const uint64_t* data_off, void* d_dst, size_t cap, uint64_t* keep, size_t* out_n);
+
 /* ---- block cache: decoded blocks kept in HBM between range reads, so that repeated reads of the same blocks (an io.ReaderAt reading a
  *      few KiB at a time, hot objects of an object store) copy instead of decoding -----------------------------------------------------------
  * A cache is made on one context with a byte budget and is used only with that context. Its device memory is allocated once, when it is

@@ -315,3 +315,67 @@ func (c *Context) ReadRangesStreams(k *Cache, idx []*Index, streams [][]byte, re
 	}
 	return nil
 }
+
+// Write is one write of WriteRanges: Data at decoded offset Off, or at the current end of the data when Append is set.
+type Write struct {
+	Off    uint64
+	Append bool
+	Data   []byte
+}
+
+// WriteRanges applies writes in order to the data of (stream, x) with pwrite semantics (a later write wins where writes overlap, a
+// write past the end grows the data and the gap reads as zeros) and re-encodes only the blocks they touch (kz_write_ranges). The new
+// stream is stream[:keep] followed by tail, what a Writer with the stream's parameters writes for the new data; x then describes it.
+// On error x and stream are unchanged.
+func (c *Context) WriteRanges(x *Index, stream []byte, writes []Write) (keep int, tail []byte, err error) {
+	if len(stream) == 0 {
+		return 0, nil, errors.New("gpu: empty stream")
+	}
+	n := len(writes)
+	off := make([]C.uint64_t, n+1)
+	ln := make([]C.uint64_t, n+1)
+	dataOff := make([]C.uint64_t, n+1)
+	total := 0
+	for i, w := range writes {
+		off[i], ln[i], dataOff[i] = C.uint64_t(w.Off), C.uint64_t(len(w.Data)), C.uint64_t(total)
+		if w.Append {
+			off[i] = C.KZ_WRITE_APPEND
+		}
+		total += len(w.Data)
+	}
+	data := make([]byte, total+1) // one buffer for cgo, as in readRanges
+	for i, w := range writes {
+		copy(data[int(dataOff[i]):], w.Data)
+	}
+	var bs C.uint32_t
+	C.kz_index_info(x.h, nil, nil, &bs, nil, nil, nil, nil, nil)
+	blocks := 0
+	for _, w := range writes {
+		if len(w.Data) > 0 {
+			blocks += len(w.Data)/int(bs) + 2
+		}
+	}
+	capacity := len(stream) + blocks*int(C.kz_max_block_output(C.size_t(bs))) + 16
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	for {
+		dst := make([]byte, capacity+1)
+		var k C.uint64_t
+		var outN C.size_t
+		rc := C.kz_write_ranges(c.h, x.h, (*C.uint8_t)(unsafe.Pointer(&stream[0])), C.size_t(len(stream)), C.uint32_t(n), &off[0], &ln[0],
+			(*C.uint8_t)(unsafe.Pointer(&data[0])), &dataOff[0], (*C.uint8_t)(unsafe.Pointer(&dst[0])), C.size_t(capacity), &k, &outN)
+		if rc == -C.KZ_ERR_WRITE_FILE && int(outN) > capacity { // a zero gap added blocks: the call names the capacity it needs
+			capacity = int(outN)
+			continue
+		}
+		if rc != 0 {
+			return 0, nil, c.err(rc)
+		}
+		return int(k), dst[:int(outN)], nil
+	}
+}
+
+// Append writes p behind the end of the data of (stream, x): WriteRanges with one appending write.
+func (c *Context) Append(x *Index, stream []byte, p []byte) (keep int, tail []byte, err error) {
+	return c.WriteRanges(x, stream, []Write{{Append: true, Data: p}})
+}

@@ -44,8 +44,10 @@ ABI_SYMBOLS = [
     "kz_index_build", "kz_index_build_device", "kz_index_info", "kz_index_save", "kz_index_load", "kz_index_free", "kz_read_ranges",
     "kz_read_ranges_device", "kz_cache_create", "kz_cache_free", "kz_cache_clear", "kz_cache_stats", "kz_read_ranges_cached",
     "kz_read_ranges_cached_device", "kz_index_build_streams", "kz_index_build_streams_device", "kz_read_ranges_streams",
-    "kz_read_ranges_streams_device", "kz_compress_streams_bs", "kz_compress_streams_bs_device",
+    "kz_read_ranges_streams_device", "kz_compress_streams_bs", "kz_compress_streams_bs_device", "kz_write_ranges", "kz_write_ranges_device",
 ]
+
+WRITE_APPEND = (1 << 64) - 1  # KZ_WRITE_APPEND: a write's offset that means the end of the data as the call's earlier writes left it
 
 
 class KanziError(RuntimeError):
@@ -189,6 +191,8 @@ def load_library(build_if_missing=True):
     L.kz_index_build_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, vp]
     L.kz_read_ranges_streams.argtypes = [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
     L.kz_read_ranges_streams_device.argtypes = [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_write_ranges.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, sz, C.POINTER(u64), C.POINTER(sz)]
+    L.kz_write_ranges_device.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, sz, C.POINTER(u64), C.POINTER(sz)]
     _lib = L
     return L
 
@@ -791,6 +795,56 @@ class StreamIndex:
         else:
             self.lib.kz_read_ranges_cached_device(ctx.h, cache.h, self.h, *args)
         return out_len, status
+
+    def write_many(self, stream, writes, ctx=None):
+        """writes: [(off, data), ...] in order (off = WRITE_APPEND: the current end) -> (keep, tail): the new stream is stream[:keep] + tail,
+        what compress gives for the new data, and the index now describes it (kz_write_ranges). Only the blocks the writes touch are
+        re-encoded. Raises KanziError, leaving the index as it was."""
+        ctx = ctx or self.ctx
+        s = _u8(stream)
+        bufs = [_u8(d) for _, d in writes]
+        off = np.array([int(o) for o, _ in writes], np.uint64)
+        ln = np.array([b.size for b in bufs], np.uint64)
+        data = np.concatenate(bufs) if bufs else np.zeros(0, np.uint8)
+        bs = self.info["block_size"]
+        # (n - keep) + k * kz_max_block_output(block_size) + 16 with k bounded by the blocks the writes span; a zero gap may add more, and
+        # the call then names the capacity it needs
+        k = sum(int(n) // bs + 2 for n in ln if n)
+        cap = s.size + k * self.lib.kz_max_block_output(bs) + 16
+        keep, out_n = C.c_uint64(0), C.c_size_t(0)
+        while True:
+            dst = np.empty(max(cap, 1), np.uint8)
+            rc = self.lib.kz_write_ranges(ctx.h, self.h, _p(s), s.size, len(writes), _p(off), _p(ln), _p(data), _p(_offsets(ln)), dst.ctypes.data, cap,
+                                          C.byref(keep), C.byref(out_n))
+            if rc == -12 and out_n.value > cap:  # KZ_ERR_WRITE_FILE
+                cap = out_n.value
+                continue
+            ctx._check(rc)
+            return keep.value, dst[: out_n.value].tobytes()
+
+    def write(self, stream, off, data, ctx=None):
+        """data at decoded offset off (pwrite: past the end grows the data, a gap reads as zeros) -> (keep, tail), as write_many."""
+        return self.write_many(stream, [(off, data)], ctx)
+
+    def append(self, stream, data, ctx=None):
+        """data behind the end of the data -> (keep, tail), as write_many."""
+        return self.write_many(stream, [(WRITE_APPEND, data)], ctx)
+
+    def write_many_device(self, d_src, n, off, length, d_data, data_off, d_dst, cap, ctx=None):
+        """Device-resident write_many (kz_write_ranges_device): d_src / d_data / d_dst are CUDA tensors or addresses, off / length /
+        data_off host sequences -> (keep, out_n). Raises KanziError; on -KZ_ERR_WRITE_FILE (code 12) its `needed` is the capacity the
+        call needs."""
+        ctx = ctx or self.ctx
+        o, ln, do = (np.ascontiguousarray(a, np.uint64) for a in (off, length, data_off))
+        keep, out_n = C.c_uint64(0), C.c_size_t(0)
+        rc = self.lib.kz_write_ranges_device(ctx.h, self.h, _dptr(d_src), n, len(o), _p(o), _p(ln), _dptr(d_data), _p(do), _dptr(d_dst), cap,
+                                             C.byref(keep), C.byref(out_n))
+        try:
+            ctx._check(rc)
+        except KanziError as e:
+            e.needed = out_n.value
+            raise
+        return keep.value, out_n.value
 
 
 class BlockCache:

@@ -64,7 +64,11 @@ __global__ void ans0_decode_kernel(const uint32_t* words, uint64_t words_len, co
                                    const uint64_t* chunk_hdr_bit, uint8_t* out, int32_t* status);
 
 // ---- bit-granular concatenation (kz_concat.cu)
-// seg_dst[i] = absolute destination bit of segment i; copies seg_bits[i] bits from seg_src[i] (byte address, any alignment)
+// seg_dst[i] = absolute destination bit of segment i; copies seg_bits[i] bits from seg_src[i]: a byte address (any alignment), and in the
+// top bits the bit of that byte the segment starts at (seg_source)
+static const uint32_t SEG_BIT_SHIFT = 61;
+static const uint64_t SEG_ADDR_MASK = (1ull << SEG_BIT_SHIFT) - 1;
+inline uint64_t seg_source(const void* p, uint64_t bit) { return (uint64_t)(uintptr_t)((const uint8_t*)p + bit / 8) | ((bit % 8) << SEG_BIT_SHIFT); }
 __global__ void concat_copy_kernel(const uint64_t* seg_src, const uint64_t* seg_bits, const uint64_t* seg_dst, int nsegs, uint32_t* dst_words);
 // exclusive scan of seg_bits (one CTA): seg_dst[i] = base + sum_{k<i} bits[k]; total[0] = base + sum
 __global__ void scan_bits_kernel(const uint64_t* seg_bits, uint64_t* seg_dst, int nsegs, uint64_t base, uint64_t* total);

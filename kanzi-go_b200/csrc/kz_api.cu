@@ -28,6 +28,7 @@
 #include "kz_skip.cuh"
 #include "kz_stream_plan.h"
 #include "kz_read_plan.h"
+#include "kz_write_plan.h"
 #include "kz_block_cache.h"
 #include "kz_record_hash.cuh"
 #include "kz_xxh64_core.cuh"
@@ -3446,6 +3447,253 @@ int check_index_streams_args(kz_ctx* ctx, uint32_t ns, const void* src, const ui
     return 0;
 }
 
+// ---- writes into a compressed stream (kz_write_ranges[_device]; plan in kz_write_plan.h) -------------------------------------------
+// The blocks plan_writes re-encodes go through the stages in passes: the ones whose old bytes survive are decoded into their slots, the
+// write slices are copied over them and the gaps zeroed, and the slots are encoded; every pass's records are packed into ctx->d_bits.
+// One concat then lays out the tail of the new stream: the carry, the new records behind their prefixes, the old records behind them
+// moved to their new bit (read where they lie, at any bit), and the end marker. The index is updated only when everything succeeded.
+// Host variant (src set): the old stream from the first byte a record the call may read or move lies in is uploaded once, the write bytes
+// once, and the tail comes back in one copy. Device variant: d_src, d_data and d_dst are device memory.
+int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len,
+                 const uint8_t* data, const uint64_t* data_off, uint8_t* dst, size_t cap, uint64_t* keep, size_t* out_n) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    if (!ix || !keep || !out_n || (!src && !d_src) || (nw && (!off || !len))) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+    *keep = n;
+    *out_n = 0;
+    const bool host = src != nullptr;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+    for (uint32_t i = 0; i < nw; i++) {
+        if (!len[i]) continue;
+        if (!data || !data_off) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+        if (data_off[i] + len[i] < data_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+    }
+    if (!host && (((uintptr_t)d_src & 15) || ((uintptr_t)dst & 15))) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    if (!host && dst && dst < d_src + n && d_src < dst + cap) return ctx->fail(KZ_ERR_INVALID_PARAM, "the output overlaps the stream");
+    uint8_t head[INDEX_HEAD] = {0};
+    const uint64_t at0 = 0, nh = n == ix->stream_bytes ? n : 0;
+    int rc = 0;
+    if (host) memcpy(head, src, std::min<uint64_t>(nh, INDEX_HEAD));
+    else if ((rc = gather_heads(ctx, d_src, &at0, &nh, 1, INDEX_HEAD, head))) return rc;
+    if ((rc = read_stream_check(ctx, ix, n, head))) return rc;
+    TransformPlan plan;
+    if ((rc = plan_transforms(ctx, ix->t48, ix->etype, plan, KZ_ERR_CREATE_CODEC))) return rc;
+    const StreamHeader sh = index_header(*ix);
+    const uint32_t bs = ix->block_size;
+    const uint64_t nb = ix->nblocks();
+    const uint64_t enc_cost = compress_block_cost(round16(bs), entropy_scratch(ix->etype));
+    StreamIndex x = *ix;  // what the plan knows; ix changes only on success
+    WritePlan P = plan_writes(x, nw, off, len, enc_cost);
+    if (P.status == WRITE_TOO_LARGE) return ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds");
+    // the lowest record the call reads or moves: the cut, or with the size to learn the first block a write names or the last block
+    uint64_t low = nb ? nb - 1 : 0;
+    if (P.status == WRITE_NEED_SIZE) {
+        for (uint32_t i = 0; i < nw; i++)
+            if (len[i] && off[i] != WRITE_APPEND) low = std::min<uint64_t>(low, off[i] / bs);
+    } else if (P.nothing()) {
+        return 0;
+    }
+    const uint64_t ubase = host ? ((P.status == WRITE_NEED_SIZE ? record_prefix_bit(x, low) : P.cut) / 8) & ~15ull : 0;  // first stream byte on the device
+    const uint64_t base_bit = 8 * ubase;
+    const uint8_t* d_base = d_src;
+    const uint8_t* d_wdata = data;  // device bytes of write i at d_wdata + w_at[i]
+    std::vector<uint64_t> w_at(nw, 0);
+    if (host) {
+        uint64_t wtotal = 0;
+        for (uint32_t i = 0; i < nw; i++) w_at[i] = wtotal, wtotal += len[i];
+        const uint64_t tail = n - ubase, wpos = round16(tail) + 128;
+        CK(ctx->d_in.ensure(wpos + wtotal + 64));
+        uint8_t* din = ctx->d_in.as<uint8_t>();
+        CK(cudaMemsetAsync(din + (tail & ~3ull), 0, 128, ctx->stream));
+        if (tail) CK(cudaMemcpyAsync(din, src + ubase, tail, cudaMemcpyHostToDevice, ctx->stream));
+        if (wtotal) {
+            std::vector<uint8_t> wbytes(wtotal);
+            for (uint32_t i = 0; i < nw; i++)
+                if (len[i]) memcpy(&wbytes[w_at[i]], data + data_off[i], len[i]);
+            CK(cudaMemcpyAsync(din + wpos, wbytes.data(), wtotal, cudaMemcpyHostToDevice, ctx->stream));
+        }
+        d_base = din;
+        d_wdata = din + wpos;
+        if (ctx->profile) {
+            auto& e = ctx->prof["write:h2d"];
+            e.bytes_in += (tail ? 1 : 0) + (wtotal ? 1 : 0), e.bytes_out += tail + wtotal, e.launches++;
+        }
+    } else {
+        for (uint32_t i = 0; i < nw; i++) w_at[i] = len[i] ? data_off[i] : 0;
+    }
+    const uint32_t* d_words = (const uint32_t*)d_base;
+    const uint64_t words_len = (n - ubase + 3) / 4 + 16;
+    auto job_of = [&](uint64_t b) {
+        DecJob j = DecJob();
+        j.bit_off = x.start[b] - base_bit;
+        j.bits = x.bits[b];
+        j.block_size = bs;
+        return j;
+    };
+    // the first failure among decoded blocks, in block order: the block's own code, or a length that breaks the block arithmetic
+    auto check_decoded = [&](const std::vector<uint64_t>& blocks, const std::vector<DecodeFailure>& fail, const std::vector<uint32_t>& olen) {
+        for (size_t i = 0; i < blocks.size(); i++) {
+            const bool last = blocks[i] + 1 == nb;
+            if (olen[i] > bs || (!fail[i].failed() && (last ? olen[i] == 0 || (x.size >= 0 && olen[i] != (uint64_t)x.size - (nb - 1) * bs) : olen[i] != bs)))
+                return ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: a block before the last is not block_size bytes long");
+            if (fail[i].failed()) return ctx->fail(-fail[i].code, fail[i].msg);
+        }
+        return 0;
+    };
+    uint64_t dec_blocks = 0, dec_bytes = 0;
+    bool have_last = false;  // the old last block sits decoded in ctx->d_out
+    if (P.status == WRITE_NEED_SIZE) {
+        CK(ctx->d_out.ensure(decompress_slot(bs) + 64));
+        std::vector<DecodeFailure> fail;
+        std::vector<uint32_t> olen;
+        rc = decode_isolated(ctx, sh, plan, d_words, words_len, {job_of(nb - 1)}, {1}, [&](uint32_t, uint32_t m) { return m > bs ? NO_ROOM : 0; },
+                             ctx->d_out.as<uint8_t>(), fail, olen);
+        if (rc || (rc = check_decoded({nb - 1}, fail, olen))) return rc;
+        x.size = (int64_t)((nb - 1) * bs + olen[0]);
+        have_last = true;
+        dec_blocks++, dec_bytes += olen[0];
+        P = plan_writes(x, nw, off, len, enc_cost);
+        if (P.status != WRITE_OK) return ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds");
+        if (P.nothing()) return 0;
+    }
+    // passes: decode, apply the writes, encode; each pass's records packed into ctx->d_bits
+    const uint32_t ne = (uint32_t)P.enc.size();
+    const uint64_t astride = decompress_slot(bs);
+    std::vector<uint64_t> rbits(ne), rarena(ne);
+    uint64_t arena = 0, enc_bytes = 0;
+    for (uint32_t p = 0; p < P.npasses(); p++) {
+        const uint32_t a = P.first[p], k = P.first[p + 1] - a;
+        CK(ctx->d_slots.ensure(astride * k + 64));
+        uint8_t* slots = ctx->d_slots.as<uint8_t>();
+        std::vector<uint64_t> blocks;
+        std::vector<DecJob> jobs;
+        std::vector<uint8_t> last;
+        std::vector<uint32_t> slot;
+        CopyList fill;
+        for (uint32_t j = a; j < a + k; j++) {
+            const uint64_t b = P.enc[j];
+            if (!P.decode[j]) continue;
+            if (have_last && b + 1 == nb) {
+                fill.add(ctx->d_out.p, slots + (j - a) * astride, (uint64_t)x.size - (nb - 1) * bs);
+                continue;
+            }
+            blocks.push_back(b), jobs.push_back(job_of(b)), last.push_back(b + 1 == nb), slot.push_back(j - a);
+        }
+        if (!jobs.empty()) {
+            std::vector<DecodeFailure> fail;
+            std::vector<uint32_t> olen;
+            rc = decode_isolated(ctx, sh, plan, d_words, words_len, jobs, last,
+                                 [&](uint32_t i, uint32_t m) { return m > bs ? NO_ROOM : (uint64_t)slot[i] * astride; }, slots, fail, olen);
+            if (rc || (rc = check_decoded(blocks, fail, olen))) return rc;
+            for (uint32_t m : olen) dec_blocks++, dec_bytes += m;
+        }
+        for (uint32_t j = a; j < a + k; j++)
+            for (uint64_t q = P.piece_of[j]; q < P.piece_of[j + 1]; q++) {
+                const WritePiece& pc = P.pieces[q];
+                uint8_t* to = slots + (uint64_t)(j - a) * astride + pc.at;
+                if (pc.kind == PIECE_WRITE) fill.add(d_wdata + w_at[pc.write] + pc.from, to, pc.len);
+                else if (pc.kind == PIECE_ZERO) CK(cudaMemsetAsync(to, 0, pc.len, ctx->stream));
+            }
+        if ((rc = run_copies(ctx, fill))) return rc;
+        BlockList bl;
+        std::vector<uint32_t> lens(P.enc_len.begin() + a, P.enc_len.begin() + a + k);
+        for (uint32_t j = 0; j < k; j++) bl.off.push_back((uint64_t)j * astride), bl.len.push_back(lens[j]), enc_bytes += lens[j];
+        bl.first = {0, k};
+        BlockPrep prep;
+        if ((rc = prepare_blocks(ctx, plan, ctx->skip_blocks, sh.checksum_bits, slots, bl, prep))) return rc;
+        uint64_t ostride = 0;
+        std::vector<uint64_t> bits;
+        rc = encode_slots(ctx, plan, ix->etype, sh.checksum_bits, slots, astride, lens, std::vector<uint64_t>(k, bs), prep, &ostride, bits);
+        if (rc) return rc;
+        uint64_t need = arena;
+        for (uint32_t j = 0; j < k; j++) need += round16((bits[j] + 7) / 8);
+        if ((rc = ensure_keep(ctx, ctx->d_bits, arena, need + 64))) return rc;
+        CopyList pack;
+        for (uint32_t j = 0; j < k; j++) {
+            rbits[a + j] = bits[j];
+            rarena[a + j] = arena;
+            pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + arena, (bits[j] + 7) / 8);
+            arena += round16((bits[j] + 7) / 8);
+        }
+        if ((rc = run_copies(ctx, pack))) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));  // the slots and the copy lists are reused by the next pass
+    }
+    // the new record table, then the tail: one concat of every segment behind byte floor(cut / 8)
+    const uint64_t zero_off = 8 * (uint64_t)ne;
+    std::vector<uint8_t> small(zero_off + 16, 0);
+    std::vector<uint32_t> pre(ne);
+    for (uint32_t j = 0; j < ne; j++) pre[j] = write_block_prefix(&small[8 * (size_t)j], rbits[j]);
+    StreamIndex y;
+    const uint64_t total_bits = splice_records(x, P, rbits, pre, END_MARKER_BITS, y);
+    const uint64_t kp = P.cut / 8, tail_bits = total_bits - 8 * kp, tail_bytes = (tail_bits + 7) / 8;
+    const uint64_t need_cap = (tail_bits + 31) / 32 * 4;  // the concat writes whole 32-bit words
+    if (need_cap > cap) {
+        *out_n = (size_t)need_cap;
+        return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
+    }
+    if (!dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    CK(ctx->d_asm.ensure(small.size()));
+    uint8_t* A = ctx->d_asm.as<uint8_t>();
+    CK(cudaMemcpyAsync(A, small.data(), small.size(), cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<uint64_t> seg_src, seg_bits, seg_dst;
+    uint64_t d = 0, moved_runs = 0, moved_bits = 0;
+    auto add = [&](uint64_t word, uint64_t nbits) {
+        seg_src.push_back(word), seg_bits.push_back(nbits), seg_dst.push_back(d);
+        d += nbits;
+    };
+    for (const WriteSeg& sg : P.segs) {
+        if (sg.kind == SEG_CARRY) {
+            add(seg_source(d_base, sg.bit - base_bit), sg.bits);
+        } else if (sg.kind == SEG_NEW) {
+            for (uint64_t j = sg.first; j < sg.first + sg.count; j++) {
+                add(seg_source(A + 8 * j, 0), pre[j]);
+                for (uint64_t o = 0; o < rbits[j]; o += 8 * RAW_PIECE)
+                    add(seg_source(ctx->d_bits.as<uint8_t>() + rarena[j], o), std::min<uint64_t>(8 * RAW_PIECE, rbits[j] - o));
+            }
+        } else if (sg.kind == SEG_OLD) {
+            for (uint64_t o = 0; o < sg.bits; o += 8 * RAW_PIECE) add(seg_source(d_base, sg.bit - base_bit + o), std::min<uint64_t>(8 * RAW_PIECE, sg.bits - o));
+            moved_runs++, moved_bits += sg.bits;
+        } else {
+            add(seg_source(A + zero_off, 0), END_MARKER_BITS);
+        }
+    }
+    uint8_t* d_out = dst;
+    if (host) {
+        CK(ctx->d_out.ensure(need_cap + 64));
+        d_out = ctx->d_out.as<uint8_t>();
+    }
+    Packer pk;
+    const size_t o_src = pk.add(seg_src.data(), seg_src.size() * 8);
+    const size_t o_bits = pk.add(seg_bits.data(), seg_bits.size() * 8);
+    const size_t o_dst = pk.add(seg_dst.data(), seg_dst.size() * 8);
+    if ((rc = upload(ctx, pk))) return rc;
+    uint8_t* T = ctx->d_tables.as<uint8_t>();
+    rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), (int)seg_src.size(), d_out);
+    if (rc) return rc;
+    // the new stream's first 32 bytes: the old ones before floor(cut / 8), the tail's behind it
+    uint8_t lead[INDEX_HEAD] = {0};
+    const uint64_t nlead = kp < INDEX_HEAD ? std::min<uint64_t>(INDEX_HEAD - kp, tail_bytes) : 0;
+    if (host) CK(cudaMemcpyAsync(dst, d_out, tail_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    else if (nlead) CK(cudaMemcpyAsync(lead, d_out, nlead, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (host && nlead) memcpy(lead, dst, nlead);
+    memset(y.head + std::min<uint64_t>(kp, INDEX_HEAD), 0, INDEX_HEAD - std::min<uint64_t>(kp, INDEX_HEAD));
+    memcpy(y.head + std::min<uint64_t>(kp, INDEX_HEAD), lead, nlead);
+    static_cast<StreamIndex&>(*ix) = y;
+    *keep = kp;
+    *out_n = (size_t)tail_bytes;
+    if (ctx->profile) {
+        auto note = [&](const char* name, uint64_t a, uint64_t b) {
+            auto& e = ctx->prof[name];
+            e.bytes_in += a, e.bytes_out += b, e.launches++;
+        };
+        note("write:decoded", dec_blocks, dec_bytes);
+        note("write:encoded", ne, enc_bytes);
+        note("write:moved", moved_runs, moved_bits);
+    }
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -3512,6 +3760,18 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
     return read_ranges(ctx, ix, nullptr, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
+}
+
+int kz_write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len, const uint8_t* data,
+                    const uint64_t* data_off, uint8_t* dst, size_t cap, uint64_t* keep, size_t* out_n) {
+    if (!src) return ctx ? ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument") : -KZ_ERR_INVALID_PARAM;
+    return write_ranges(ctx, ix, src, nullptr, n, nw, off, len, data, data_off, dst, cap, keep, out_n);
+}
+
+int kz_write_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len,
+                           const void* d_data, const uint64_t* data_off, void* d_dst, size_t cap, uint64_t* keep, size_t* out_n) {
+    if (!d_src) return ctx ? ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument") : -KZ_ERR_INVALID_PARAM;
+    return write_ranges(ctx, ix, nullptr, (const uint8_t*)d_src, n, nw, off, len, (const uint8_t*)d_data, data_off, (uint8_t*)d_dst, cap, keep, out_n);
 }
 
 // ---- many streams per call (kz_index_build_streams[_device], kz_read_ranges_streams[_device]) ----------------------------------------

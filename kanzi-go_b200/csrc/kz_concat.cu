@@ -91,7 +91,9 @@ __global__ void concat_zero_kernel(const uint64_t* __restrict__ seg_bits, const 
     dst_words[(d + n - 1) >> 5] = 0;
 }
 
-// one CTA per segment (segments are at most a few thousand words; large raw copies are pre-split by the host)
+// one CTA per segment (segments are at most a few thousand words; large raw copies are pre-split by the host). A segment word is the
+// address of the segment's first byte, with the bit of that byte the segment starts at (0 .. 7, MSB first) in bits SEG_BIT_SHIFT and
+// up (seg_source): a segment of whole bytes is its address as it is.
 __global__ void __launch_bounds__(128) concat_copy_kernel(const uint64_t* __restrict__ seg_src, const uint64_t* __restrict__ seg_bits,
                                                            const uint64_t* __restrict__ seg_dst, int nsegs, uint32_t* __restrict__ dst_words) {
     const int i = blockIdx.x;
@@ -99,9 +101,10 @@ __global__ void __launch_bounds__(128) concat_copy_kernel(const uint64_t* __rest
     const uint64_t n = seg_bits[i];
     if (n == 0) return;
     const uint64_t d = seg_dst[i];
-    const uintptr_t sp = (uintptr_t)seg_src[i];
+    const uint64_t word = seg_src[i];
+    const uintptr_t sp = (uintptr_t)(word & SEG_ADDR_MASK);
     const uint32_t* sw = reinterpret_cast<const uint32_t*>(sp & ~(uintptr_t)3);
-    const uint64_t s0 = (uint64_t)(sp & 3) * 8;  // bit offset of the segment's first bit inside sw
+    const uint64_t s0 = (uint64_t)(sp & 3) * 8 + (word >> SEG_BIT_SHIFT);  // bit offset of the segment's first bit inside sw
     const uint64_t w0 = d >> 5, w1 = (d + n - 1) >> 5;
     const uint32_t o = (uint32_t)(d & 31);
     for (uint64_t w = w0 + threadIdx.x; w <= w1; w += blockDim.x) {
