@@ -387,24 +387,25 @@ __global__ void __launch_bounds__(32) sbrt_inverse_warp_kernel(const uint8_t* __
     }
 }
 
-// ---- inverse for blocks <= 16 MiB: the list in the registers of W = 4 warps, mirrored in shared memory ---------------------------------------
+// ---- inverse for blocks <= 16 MiB: the list in the registers of 4 warps, mirrored in shared memory ---------------------------------------------
 // With the list only in registers, every instruction of a step sits on the dependent chain: look-up of the entry of rank r -> qc -> move-up
 // -> next step's look-up. Here the registers keep the list for the move-up, and a copy in shared memory serves the look-ups: after step j - 1
 // has stored its entries, the candidates for the rank r2 of step j + 1 are loaded from the state BEFORE step j — entry r2 and entry r2 - 1 —
 // and step j decides with two compares which one (or its own fresh entry) stands at rank r2 afterwards (the move-up rule applied to that one
 // position). The chain per rank is qc -> 2 compares -> 2 selects -> next qc; the move-up, the stores and the loads for the step after next
 // overlap it. On one warp this is bound by the ALU pipe of its scheduler (~50 integer / predicate instructions per rank), and with every
-// look-up served by the mirror nothing but the lane boundary ties the lanes together, so the 256 entries are spread over W warps (8 / W
-// entries per lane) that sit on different schedulers: every warp takes the same decision about the next entry from the same shared-memory
-// candidates, moves its own part of the list, stores it, and one CTA barrier per rank publishes the stores; the entry that crosses a warp
-// boundary is read from the mirror instead of a shuffle.
-template <bool RANK_MODE, int W>
-__global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
-                                                                     uint8_t* __restrict__ out) {
-    constexpr int S = 8 / W;  // entries per lane
+// look-up served by the mirror nothing but the lane boundary ties the lanes together, so the 256 entries are spread over 4 warps (2 entries
+// per lane) that sit on different schedulers: every warp takes the same decision about the next entry from the same shared-memory
+// candidates, moves its own part of the list, stores it, and one CTA barrier per rank publishes the stores.
+// The entry that crosses a warp boundary is read from the mirror instead of a shuffle. With one warp per scheduler nothing hides a step's
+// latency, and its time follows its instruction count (DESIGN.md §4.3): an entry is (q, x = p << 8 | symbol) in one 8-byte word of the
+// mirror, so that one load fetches a candidate or the boundary entry and one 16-byte store publishes a lane's two entries.
+template <bool RANK_MODE>
+__global__ void __launch_bounds__(128) sbrt_inverse_multi_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
+                                                                 uint8_t* __restrict__ out) {
+    constexpr int S = 2;  // entries per lane
     // two copies, written alternately: a warp that runs ahead stores step j + 1 while another still reads the state after step j - 1 / j
-    __shared__ __align__(16) uint32_t s_q[2][256];
-    __shared__ __align__(16) uint32_t s_x[2][256];
+    __shared__ __align__(16) uint2 s_e[2][256];
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (b >= nblocks) return;
     const SbrtBlock blk = blocks[b];
@@ -419,27 +420,28 @@ __global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_
     for (int k = 0; k < S; k++) {
         Q[k] = 0;
         X[k] = base + k;
-        s_q[0][base + k] = s_q[1][base + k] = 0;
-        s_x[0][base + k] = s_x[1][base + k] = base + k;
+        s_e[0][base + k] = s_e[1][base + k] = make_uint2(0u, base + k);
     }
     __syncthreads();
-    uint32_t a_q, a_x, b_q, b_x;
+    uint2 ca, cb;  // candidates: entries r2 and r2 - 1 of the state before the current step
     auto load_candidates = [&](uint32_t r2, int par) {  // from the copy step `par` wrote
-        const uint32_t r1 = r2 ? r2 - 1 : 0;
-        a_q = s_q[par][r2], a_x = s_x[par][r2], b_q = s_q[par][r1], b_x = s_x[par][r1];
+        ca = s_e[par][r2];
+        cb = r2 ? s_e[par][r2 - 1] : make_uint2(0xFFFFFFFFu, 0u);  // above position 0: a q larger than any qc
     };
     // par = parity of the step: it reads the copy of parity par ^ 1 (the state before it) and writes the copy of parity par
     auto step = [&](uint32_t r, uint32_t r2, uint32_t i, int par, uint32_t& x) -> uint32_t {
         // the entry above this lane's first one (state before the step): a shuffle inside the warp, the mirror across a warp boundary
         uint32_t up_q = __shfl_up_sync(0xFFFFFFFFu, Q[S - 1], 1), up_x = __shfl_up_sync(0xFFFFFFFFu, X[S - 1], 1);
-        if (lane == 0 && warp > 0) up_q = s_q[par ^ 1][base - 1], up_x = s_x[par ^ 1][base - 1];
+        if (lane == 0 && warp > 0) {
+            const uint2 e = s_e[par ^ 1][base - 1];
+            up_q = e.x, up_x = e.y;
+        }
         const uint32_t sym = x & 0xFFu;
         const uint32_t qc = RANK_MODE ? (i + (x >> 8)) >> 1 : i;  // i, p < 2^24
         const uint32_t fresh = (i << 8) | sym;
         {  // the entry at rank r2 after this step (every warp computes the same)
-            const bool mv = r2 <= r && !(a_q > qc);
-            const bool gb = r2 == 0 || b_q > qc;
-            x = mv ? (gb ? fresh : b_x) : a_x;
+            const bool mv = r2 <= r && !(ca.x > qc);
+            x = mv ? (cb.x > qc ? fresh : cb.y) : ca.y;
         }
         const int d = (int)r - (int)base;
         bool gk = Q[S - 1] > qc;
@@ -458,22 +460,13 @@ __global__ void __launch_bounds__(32 * W) sbrt_inverse_multi_kernel(const uint8_
             Q[0] = mv ? (g_up ? qc : up_q) : Q[0];
             X[0] = mv ? (g_up ? fresh : up_x) : X[0];
         }
-        if (S == 4) {
-            reinterpret_cast<uint4*>(s_q[par])[tid] = make_uint4(Q[0], Q[1], Q[S > 2 ? 2 : 0], Q[S > 3 ? 3 : 0]);
-            reinterpret_cast<uint4*>(s_x[par])[tid] = make_uint4(X[0], X[1], X[S > 2 ? 2 : 0], X[S > 3 ? 3 : 0]);
-        } else if (S == 2) {
-            reinterpret_cast<uint2*>(s_q[par])[tid] = make_uint2(Q[0], Q[S > 1 ? 1 : 0]);
-            reinterpret_cast<uint2*>(s_x[par])[tid] = make_uint2(X[0], X[S > 1 ? 1 : 0]);
-        } else {
-            s_q[par][tid] = Q[0];
-            s_x[par][tid] = X[0];
-        }
+        reinterpret_cast<uint4*>(s_e[par])[tid] = make_uint4(Q[0], X[0], Q[1], X[1]);
         __syncthreads();
         return sym;
     };
     uint32_t mine = (uint32_t)lane < n ? src[lane] : 0u;
     uint32_t nxt = 32u + lane < n ? src[32 + lane] : 0u;
-    uint32_t x = s_x[1][__shfl_sync(0xFFFFFFFFu, mine, 0)];
+    uint32_t x = s_e[1][__shfl_sync(0xFFFFFFFFu, mine, 0)].y;
     load_candidates(__shfl_sync(0xFFFFFFFFu, mine, 1), 1);
     uint32_t i0 = 0;
     for (; i0 + 32 <= n; i0 += 32) {
@@ -546,8 +539,8 @@ void sbrt_rank_launch(const uint8_t* data, const SbrtBlock* d_blocks, int mode, 
 
 void sbrt_inverse_launch_len(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, uint32_t max_len, cudaStream_t stream) {
     if (max_len > (1u << 24)) sbrt_inverse_warp_kernel<uint64_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-    else if (mode == 2) sbrt_inverse_multi_kernel<true, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<true, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-    else sbrt_inverse_multi_kernel<false, 4><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<false, 4>, nblocks), stream>>>(data, d_blocks, nblocks, out);
+    else if (mode == 2) sbrt_inverse_multi_kernel<true><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<true>, nblocks), stream>>>(data, d_blocks, nblocks, out);
+    else sbrt_inverse_multi_kernel<false><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<false>, nblocks), stream>>>(data, d_blocks, nblocks, out);
 }
 
 }  // namespace kz
