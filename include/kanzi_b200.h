@@ -110,7 +110,10 @@ int kz_decompress_stream(kz_ctx* ctx, const uint8_t* src, size_t n, uint8_t* dst
 size_t kz_max_stream_output(size_t n, uint32_t block_size);
 
 /* ---- device-resident variants (inputs and outputs already in HBM; used by multi-GPU pipelines and bench.py's
- *      kernel-only `value`). Pointers are CUDA device pointers on ctx's device. Lengths / offsets are host arrays. */
+ *      kernel-only `value`). Pointers are CUDA device pointers on ctx's device. Lengths / offsets are host arrays.
+ *      Every device variant runs after the work already queued on the device's legacy default stream (PyTorch's default stream), and
+ *      so after the blocking streams: buffers written or allocated there need no synchronisation first. Work on a non-blocking stream
+ *      of the caller's must be finished by the caller. */
 /* Compresses n bytes at d_src into the complete stream at d_dst (header, blocks, end marker). *out_n = stream bytes. */
 int kz_compress_stream_device(kz_ctx* ctx, uint64_t transform48, uint32_t entropy, uint32_t block_size, uint32_t checksum_bits,
                               int64_t input_size_hint, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n);

@@ -2030,6 +2030,11 @@ int kz_init(int device, kz_ctx** out) {
         delete ctx;
         return -KZ_ERR_CREATE_COMPRESSOR;
     }
+    if (cudaEventCreateWithFlags(&ctx->caller_done, cudaEventDisableTiming) != cudaSuccess) {
+        cudaStreamDestroy(ctx->stream);
+        delete ctx;
+        return -KZ_ERR_CREATE_COMPRESSOR;
+    }
     cudaFuncSetAttribute(ans0_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENC_SMEM);
     cudaFuncSetAttribute(ans0_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DEC_SMEM);
     cudaFuncSetAttribute(huf_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)HUF_DEC_SMEM);
@@ -2053,6 +2058,7 @@ void kz_destroy(kz_ctx* ctx) {
     ctx->h_stage.release();
     ctx->h_dl.release();
     ctx->h_io.release();
+    cudaEventDestroy(ctx->caller_done);
     cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -2241,14 +2247,27 @@ static int compress_device_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint3
     return 0;
 }
 
+// The device variants read and write buffers that the caller filled or allocated with work of its own, typically PyTorch's on the legacy
+// default stream. The context's stream is non-blocking and would not wait for that work: each device variant first orders it after
+// everything already queued on the legacy default stream (which itself follows every blocking stream), on the device, without a host wait.
+static int after_caller_work(kz_ctx* ctx) {
+    if (!ctx) return 0;  // the entry point's own argument check reports it
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventRecord(ctx->caller_done, cudaStreamLegacy));
+    CK(cudaStreamWaitEvent(ctx->stream, ctx->caller_done, 0));
+    return 0;
+}
+
 int kz_compress_stream_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, int64_t input_size,
                               const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
+    if (int rc = after_caller_work(ctx)) return rc;
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, input_size, d_src, n, d_dst, cap, out_n, false, nullptr);
 }
 // The block records (5 b | lw b | payload each) of n bytes at d_src, without stream header and without end marker: what one rank of a sharded
 // compression contributes (blocks are independent, io/CompressedStream.go:896-898). *out_bits = exact bit length.
 int kz_compress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src, size_t n, void* d_dst,
                                 size_t cap, uint64_t* out_bits) {
+    if (int rc = after_caller_work(ctx)) return rc;
     size_t bytes = 0;
     if (!out_bits) return -KZ_ERR_INVALID_PARAM;
     return compress_device_impl(ctx, t48, etype, block_size, checksum_bits, 0, d_src, n, d_dst, cap, &bytes, true, out_bits);
@@ -2267,6 +2286,7 @@ int kz_stream_header(uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t
 // Bit-granular concatenation of nseg device bit strings (MSB first) into d_dst: the ordered commit of Writer.processBlock (:951-976) for
 // fragments gathered from other ranks. Segments are cut into 64 KiB pieces, one CTA each. *total_bits = length of the result.
 int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, const uint64_t* seg_bits, void* d_dst, size_t cap, uint64_t* total_bits) {
+    if (int rc = after_caller_work(ctx)) return rc;
     if (!ctx || !total_bits || (nseg && (!d_seg || !seg_bits)) || !d_dst) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     std::vector<uint64_t> src, bits;
@@ -2346,12 +2366,14 @@ static int decompress_device_impl(kz_ctx* ctx, const StreamHeader* given, uint64
 }
 
 int kz_decompress_stream_device(kz_ctx* ctx, const void* d_src, size_t n, void* d_dst, size_t cap, size_t* out_n) {
+    if (int rc = after_caller_work(ctx)) return rc;
     return decompress_device_impl(ctx, nullptr, 0, 0, ctx ? ctx->range_from : -1, ctx ? ctx->range_to : -1, d_src, n, d_dst, cap, out_n);
 }
 // Decodes `nblocks` block records that start at bit `start_bit` of the fragment at d_src (frag_bytes bytes, >= 64 readable bytes behind them):
 // what one rank of a sharded decompression does with its part of the stream. The stream parameters come from the header rank 0 parsed.
 int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, const void* d_src, size_t frag_bytes,
                                   uint64_t start_bit, uint32_t nblocks, void* d_dst, size_t cap, size_t* out_n) {
+    if (int rc = after_caller_work(ctx)) return rc;
     if (!ctx || !out_n) return -KZ_ERR_INVALID_PARAM;
     *out_n = 0;
     if (nblocks == 0) return 0;
@@ -2369,6 +2391,7 @@ int kz_decompress_fragment_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uin
 // the setting's and rec_bit[0] = 0.
 int kz_stream_index_device(kz_ctx* ctx, const void* d_src, size_t n, uint32_t max_blocks, uint64_t* t48, uint32_t* etype, uint32_t* block_size,
                            uint32_t* checksum_bits, int64_t* input_size, uint64_t* rec_bit, uint32_t* nblocks) {
+    if (int rc = after_caller_work(ctx)) return rc;
     if (!ctx || !d_src || !rec_bit || !nblocks) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
     StreamHeader sh;
@@ -2775,6 +2798,7 @@ static int compress_streams_host(kz_ctx* ctx, uint64_t t48, uint32_t etype, cons
 int kz_compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t block_size, uint32_t checksum_bits, uint32_t nstreams, const void* d_src,
                                const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst, const uint64_t* dst_off,
                                const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nstreams, status, out_len, rc);
     const std::vector<uint32_t> bs(std::max(nstreams, 1u), block_size);
     return compress_streams_device(ctx, t48, etype, bs.data(), &block_size, checksum_bits, nstreams, d_src, src_off, src_len, input_size, d_dst, dst_off, dst_cap,
                                    out_len, status);
@@ -2791,6 +2815,7 @@ int kz_compress_streams(kz_ctx* ctx, uint64_t t48, uint32_t etype, uint32_t bloc
 int kz_compress_streams_bs_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams,
                                   const void* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size, void* d_dst,
                                   const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nstreams, status, out_len, rc);
     return compress_streams_device(ctx, t48, etype, block_size, nullptr, checksum_bits, nstreams, d_src, src_off, src_len, input_size, d_dst, dst_off, dst_cap,
                                    out_len, status);
 }
@@ -2804,6 +2829,7 @@ int kz_compress_streams_bs(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint
 
 int kz_decompress_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, void* d_dst,
                                  const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nstreams, status, out_len, rc);
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     int rc = check_stream_args(ctx, nstreams, d_src, src_off, src_len, d_dst, dst_off, dst_cap, out_len, status, true);
     if (rc) return finish_streams(nstreams, status, out_len, rc);
@@ -3699,6 +3725,7 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
 extern "C" {
 
 int kz_index_build_device(kz_ctx* ctx, const void* d_src, size_t n, kz_index** out) {
+    if (int rc = after_caller_work(ctx)) return rc;
     if (!ctx || !out || (!d_src && n)) return -KZ_ERR_INVALID_PARAM;
     *out = nullptr;
     CK(cudaSetDevice(ctx->device));
@@ -3759,6 +3786,7 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nreq, status, out_len, rc);
     return read_ranges(ctx, ix, nullptr, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
 }
 
@@ -3770,6 +3798,7 @@ int kz_write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uin
 
 int kz_write_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len,
                            const void* d_data, const uint64_t* data_off, void* d_dst, size_t cap, uint64_t* keep, size_t* out_n) {
+    if (int rc = after_caller_work(ctx)) return rc;
     if (!d_src) return ctx ? ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument") : -KZ_ERR_INVALID_PARAM;
     return write_ranges(ctx, ix, nullptr, (const uint8_t*)d_src, n, nw, off, len, (const uint8_t*)d_data, data_off, (uint8_t*)d_dst, cap, keep, out_n);
 }
@@ -3777,6 +3806,7 @@ int kz_write_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t 
 // ---- many streams per call (kz_index_build_streams[_device], kz_read_ranges_streams[_device]) ----------------------------------------
 int kz_index_build_streams_device(kz_ctx* ctx, uint32_t nstreams, const void* d_src, const uint64_t* src_off, const uint64_t* src_len, kz_index** out,
                                   int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nstreams, status, nullptr, rc);
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
     int rc = check_index_streams_args(ctx, nstreams, d_src, src_off, src_len, out, status, true);
     if (!rc && cudaSetDevice(ctx->device) != cudaSuccess) rc = ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
@@ -3813,6 +3843,7 @@ int kz_read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_i
 int kz_read_ranges_streams_device(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
                                   const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, void* d_dst,
                                   const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nreq, status, out_len, rc);
     return read_ranges_streams(ctx, cache, nstreams, ix, (const uint8_t*)d_src, true, src_off, src_len, nreq, req_stream, off, len, d_dst, dst_off, out_len,
                                status);
 }
@@ -3866,6 +3897,7 @@ int kz_read_ranges_cached(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const uint
 
 int kz_read_ranges_cached_device(kz_ctx* ctx, kz_cache* cache, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off,
                                  const uint64_t* len, void* d_dst, const uint64_t* dst_off, uint64_t* out_len, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nreq, status, out_len, rc);
     if (ctx && !cache) return finish_streams(nreq, status, out_len, ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument"));
     return read_ranges(ctx, ix, cache, nullptr, d_src, n, nreq, off, len, d_dst, dst_off, out_len, status);
 }

@@ -130,6 +130,7 @@ struct kz_cache;
 struct kz_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
+    cudaEvent_t caller_done = nullptr;  // after_caller_work: recorded on the legacy default stream, waited on by `stream`
     std::string err;
     uint64_t launches = 0;
     bool profile = false;

@@ -20,6 +20,8 @@
 // Inverse: the list itself is the decoder state (r -> c needs the list, which needs all earlier symbols), so a block is
 // one serial chain: one CTA per block walks it with the list in registers (blocks run concurrently).
 #include <algorithm>
+#include <mutex>
+#include <vector>
 
 #include "kz_sbrt.cuh"
 #include "kz_sbrt_core.cuh"
@@ -504,8 +506,11 @@ __global__ void __launch_bounds__(128) sbrt_inverse_multi_kernel(const uint8_t* 
 // Dynamic shared memory that nobody touches caps the chains per SM at ceil(nblocks / SMs): the chains spread over the GPU whatever runs beside them.
 // The chains of an SM take all of its shared memory, so that no CTA of another kernel shares their schedulers either: with room left for one
 // (half an SM per chain), a chain beside the -l 3 round trip of another context took 256 ms instead of the 224 ms it takes alone.
-template <typename K>
-static size_t spread_chains(K kernel, int nblocks) {
+// The kernel's dynamic shared memory cap is one setting of the process for each device, and contexts launch from several host threads at
+// once: it is raised once per device to the most any launch asks for, so that no thread lowers it between another thread's size and launch.
+template <bool RANK_MODE>
+static size_t spread_chains(int nblocks) {
+    const auto kernel = sbrt_inverse_multi_kernel<RANK_MODE>;
     int dev = 0, sms = 0, sm_bytes = 0, block_max = 0, reserved = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0 ||
         cudaDeviceGetAttribute(&sm_bytes, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
@@ -519,14 +524,20 @@ static size_t spread_chains(K kernel, int nblocks) {
         cudaGetLastError();
         return 0;
     }
+    static std::mutex mu;
+    static std::vector<int8_t> capped;  // per device: 0 not set yet, 1 set to block_max - static, -1 setting it failed
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if ((int)capped.size() <= dev) capped.resize(dev + 1, 0);
+        if (capped[dev] == 0) {
+            capped[dev] = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, block_max - (int)fa.sharedSizeBytes) == cudaSuccess ? 1 : -1;
+            if (capped[dev] < 0) cudaGetLastError();
+        }
+        if (capped[dev] < 0) return 0;
+    }
     const size_t room = (size_t)sm_bytes / (size_t)per, fixed = (size_t)reserved + fa.sharedSizeBytes;
     if (room <= fixed) return 0;
-    const size_t dyn = std::min(room - fixed, (size_t)block_max - fa.sharedSizeBytes);
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess) {
-        cudaGetLastError();
-        return 0;
-    }
-    return dyn;
+    return std::min(room - fixed, (size_t)block_max - fa.sharedSizeBytes);
 }
 
 void sbrt_rank_launch(const uint8_t* data, const SbrtBlock* d_blocks, int mode, const uint32_t* seg_block, uint32_t nsegs, const int32_t* table,
@@ -539,8 +550,8 @@ void sbrt_rank_launch(const uint8_t* data, const SbrtBlock* d_blocks, int mode, 
 
 void sbrt_inverse_launch_len(const uint8_t* data, const SbrtBlock* d_blocks, int nblocks, int mode, uint8_t* out, uint32_t max_len, cudaStream_t stream) {
     if (max_len > (1u << 24)) sbrt_inverse_warp_kernel<uint64_t><<<nblocks, 32, 0, stream>>>(data, d_blocks, nblocks, mode, out);
-    else if (mode == 2) sbrt_inverse_multi_kernel<true><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<true>, nblocks), stream>>>(data, d_blocks, nblocks, out);
-    else sbrt_inverse_multi_kernel<false><<<nblocks, 128, spread_chains(sbrt_inverse_multi_kernel<false>, nblocks), stream>>>(data, d_blocks, nblocks, out);
+    else if (mode == 2) sbrt_inverse_multi_kernel<true><<<nblocks, 128, spread_chains<true>(nblocks), stream>>>(data, d_blocks, nblocks, out);
+    else sbrt_inverse_multi_kernel<false><<<nblocks, 128, spread_chains<false>(nblocks), stream>>>(data, d_blocks, nblocks, out);
 }
 
 }  // namespace kz

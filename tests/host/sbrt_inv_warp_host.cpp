@@ -1,8 +1,9 @@
-// NEXT ROUND — CPU model of the planned warp-resident RANK / MTFT inverse (tests/test_sbrt_inv_warp_host.py), written lane by lane the way
-// the kernel (kanzi-go_b200/csrc/next/kz_sbrt_warp.cu) moves data: 32 lanes x 8 consecutive ranks of 64-bit entries
-// (q << 35 | p << 8 | symbol), the decoded symbol fetched with one shuffle, the new rank from a popc over "entry above rank r with a larger q"
-// (valid because the list is always sorted by q), the move-up as a predicated register shift per lane plus one shuffle-up for the lane
-// boundaries. Reference: v2/transform/SBRT.go:177-226 (Inverse), modes :93-111.
+// CPU model of a warp-resident formulation of the RANK / MTFT inverse (tests/test_sbrt_inv_warp_host.py): 32 lanes x 8 consecutive ranks of
+// 64-bit entries (q << 35 | p << 8 | symbol), the decoded symbol fetched with one shuffle, the new rank from a popc over "entry above rank r
+// with a larger q" (valid because the list is always sorted by q), the move-up as a predicated register shift per lane plus one shuffle-up for
+// the lane boundaries. sbrt_inverse_warp_kernel (kanzi-go_b200/csrc/kz_sbrt.cu) keeps the same list layout but decides the move-up locally
+// per entry instead of counting the new rank, and takes a zero run in one step; this model checks the list rule they share.
+// Reference: v2/transform/SBRT.go:177-226 (Inverse), modes :93-111.
 #include <cstdint>
 
 namespace {

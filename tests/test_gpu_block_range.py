@@ -279,3 +279,30 @@ def test_range_session_memory_1gib(kz, synth):
     for i in range(npieces):
         h.update(piece(i))
     assert full_digest == h.digest()
+
+
+def test_device_variants_follow_the_callers_default_stream(kz, gpu, oracle, synth, torch):
+    """the device variants run after what the caller queued on its default stream: the input reaches its device buffer, and the output
+    buffer is cleared, only behind a kernel of some 50 ms, and every call still reads all of its input and keeps all of its output"""
+    x, s = stream_of(oracle, synth, CHAINS[6])
+    cap, ecap = len(x) + 64, int(gpu.lib.kz_max_stream_output(len(x), BS))
+    src_s, src_x = to_dev(torch, s), to_dev(torch, x)
+    d_src, d_x = torch.zeros_like(src_s), torch.zeros_like(src_x)
+    d_dst = torch.full((max(cap, ecap) + 64,), 7, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+
+    def behind_a_kernel(dst, src):
+        dst.zero_()
+        torch.cuda._sleep(100_000_000)
+        dst.copy_(src)
+        d_dst.fill_(0)
+
+    behind_a_kernel(d_src, src_s)
+    n = gpu.decompress_device(d_src.data_ptr(), len(s), d_dst.data_ptr(), cap)
+    assert n == len(x) and np.array_equal(d_dst[:n].cpu().numpy(), x)
+    behind_a_kernel(d_src, src_s)
+    out_len, st = gpu.decompress_streams_device(d_src, [0], [len(s)], d_dst, [0], [cap])
+    assert list(st) == [0] and int(out_len[0]) == len(x) and np.array_equal(d_dst[: len(x)].cpu().numpy(), x)
+    behind_a_kernel(d_x, src_x)
+    n = gpu.compress_device(d_x.data_ptr(), len(x), d_dst.data_ptr(), ecap, kz.transform_type("NONE"), kz.E_NONE, BS, 64, input_size=len(x))
+    assert n == len(s) and np.array_equal(d_dst[:n].cpu().numpy(), s)
