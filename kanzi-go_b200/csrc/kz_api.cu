@@ -265,6 +265,54 @@ int gather_heads(kz_ctx* ctx, const uint8_t* d_base, const uint64_t* off, const 
     return 0;
 }
 
+// The first INDEX_HEAD bytes of n streams (stream i: len[i] bytes at base + off[i]) to out, INDEX_HEAD bytes per stream and zero padded:
+// copied on the host, or gathered from device memory.
+int read_heads(kz_ctx* ctx, const uint8_t* base, bool device, const uint64_t* off, const uint64_t* len, size_t n, uint8_t* out) {
+    if (device) return gather_heads(ctx, base, off, len, n, INDEX_HEAD, out);
+    memset(out, 0, n * INDEX_HEAD);
+    for (size_t i = 0; i < n; i++) memcpy(out + i * INDEX_HEAD, base + off[i], std::min<uint64_t>(len[i], INDEX_HEAD));
+    return 0;
+}
+
+// Host bytes staged through ctx->h_io. An upload piece copies `copy` bytes from src into a slot of `slot` >= copy bytes; the slots lie at
+// 16-byte aligned offsets of ctx->d_in, and the bytes of a slot behind its copy are zero. A download piece copies len bytes at offset `at`
+// of a device staging area to dst.
+struct UploadPiece {
+    const uint8_t* src;
+    uint64_t copy, slot;
+};
+struct DownloadPiece {
+    uint8_t* dst;
+    uint64_t at, len;
+};
+
+// The pieces packed into ctx->h_io and moved to ctx->d_in in one transfer; at[i]: piece i's offset in d_in, *total: the bytes moved.
+int upload_pieces(kz_ctx* ctx, const std::vector<UploadPiece>& pieces, std::vector<uint64_t>& at, uint64_t* total) {
+    at.resize(pieces.size());
+    uint64_t t = 0;
+    for (size_t i = 0; i < pieces.size(); i++) at[i] = t, t += round16(pieces[i].slot);
+    CK(ctx->h_io.ensure(t + 64));
+    CK(ctx->d_in.ensure(t + 64));
+    uint8_t* h = (uint8_t*)ctx->h_io.p;
+    for (size_t i = 0; i < pieces.size(); i++) {
+        const UploadPiece& pc = pieces[i];
+        if (pc.copy) memcpy(h + at[i], pc.src, pc.copy);
+        memset(h + at[i] + pc.copy, 0, round16(pc.slot) - pc.copy);
+    }
+    if (t) CK(cudaMemcpyAsync(ctx->d_in.p, h, t, cudaMemcpyHostToDevice, ctx->stream));
+    *total = t;
+    return 0;
+}
+
+// Bytes [0, total) of d_stage moved into ctx->h_io in one transfer, then each piece copied out to the caller's memory.
+int download_pieces(kz_ctx* ctx, const uint8_t* d_stage, uint64_t total, const std::vector<DownloadPiece>& pieces) {
+    CK(ctx->h_io.ensure(total + 64));
+    if (total) CK(cudaMemcpyAsync(ctx->h_io.p, d_stage, total, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (const DownloadPiece& pc : pieces) memcpy(pc.dst, (const uint8_t*)ctx->h_io.p + pc.at, pc.len);
+    return 0;
+}
+
 // XXHash32/64 of a set of blocks (hash/XXHash32.go, XXHash64.go; seed "KANZ", io/CompressedStream.go:354-356). Synchronous.
 int hash_blocks(kz_ctx* ctx, const uint8_t* d_base, const std::vector<uint64_t>& off, const std::vector<uint32_t>& len, uint32_t bits,
                 std::vector<uint64_t>& out) {
@@ -312,8 +360,22 @@ int check_encode_args(kz_ctx* ctx, uint32_t block_size, uint32_t checksum_bits) 
     return check_checksum_bits(ctx, checksum_bits);
 }
 
+// The spans of a many-stream argument, span i being len[i] bytes at base + off[i]: no offset + length overflows, a buffer lies under
+// spans that reach past its first byte, and in device memory (device) the base and every offset are multiples of 16.
+int check_spans(kz_ctx* ctx, const void* base, const uint64_t* off, const uint64_t* len, size_t n, bool device) {
+    uint64_t end = 0;
+    for (size_t i = 0; i < n; i++) {
+        if (off[i] + len[i] < off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+        if (device && (off[i] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
+        end = std::max(end, off[i] + len[i]);
+    }
+    if (end && !base) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+    if (device && ((uintptr_t)base & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+    return 0;
+}
+
 // The gather of every bit-granular output (kz_concat.cu): segment i, seg_bits[i] bits at address seg_src[i], lands at bit seg_dst[i] of
-// d_out. The three tables are device arrays. encode_batch, the many-stream assembly and kz_concat_bits_device all write through it.
+// d_out. The three tables are device arrays. encode_batch and SegmentList write through it.
 int concat_segments(kz_ctx* ctx, const uint64_t* d_seg_src, const uint64_t* d_seg_bits, const uint64_t* d_seg_dst, int nsegs, uint8_t* d_out) {
     if (nsegs <= 0) return 0;
     {
@@ -327,6 +389,56 @@ int concat_segments(kz_ctx* ctx, const uint64_t* d_seg_src, const uint64_t* d_se
     CK(cudaGetLastError());
     return 0;
 }
+
+// The segments of one concat_segments call, laid out on the host: each lands behind the previous one, from the bit at() names. Device bit
+// strings (from any bit) are cut into RAW_PIECE pieces; short strings built on the host (a stream header, a record prefix, the end marker)
+// travel with the segment table.
+struct SegmentList {
+    std::vector<uint64_t> src, bits, dst;
+    std::vector<size_t> host_seg;  // segments whose src is an offset into `host` until write() knows where it lands
+    std::vector<uint8_t> host;
+    uint64_t next = 0;
+
+    void at(uint64_t bit) { next = bit; }
+    void add_device(const uint8_t* p, uint64_t bit, uint64_t nbits) {
+        for (uint64_t o = 0; o < nbits; o += 8 * RAW_PIECE) push(seg_source(p, bit + o), std::min<uint64_t>(8 * RAW_PIECE, nbits - o));
+    }
+    void add_host(const uint8_t* bytes, uint64_t nbits) {
+        if (!nbits) return;
+        const size_t o = host.size();
+        host.resize(o + (nbits + 63) / 64 * 8, 0);
+        memcpy(&host[o], bytes, (nbits + 7) / 8);
+        host_seg.push_back(src.size());
+        push(o, nbits);
+    }
+    void add_end_marker() {
+        const uint8_t zero[8] = {0};
+        add_host(zero, END_MARKER_BITS);
+    }
+    void push(uint64_t s, uint64_t n) {
+        src.push_back(s), bits.push_back(n), dst.push_back(next);
+        next += n;
+    }
+    // the host strings, then the three tables, in one upload; the concat; one synchronisation (the tables live in ctx->d_tables)
+    int write(kz_ctx* ctx, uint8_t* d_out) {
+        if (src.empty()) return 0;
+        Packer pk;
+        const size_t o_host = pk.add(host.data(), host.size());
+        const size_t o_src = pk.add(src.data(), src.size() * 8);
+        const size_t o_bits = pk.add(bits.data(), bits.size() * 8);
+        const size_t o_dst = pk.add(dst.data(), dst.size() * 8);
+        CK(ctx->d_tables.ensure(pk.bytes.size() + 256));  // what upload() ensures: the host strings' addresses are final from here
+        const uint64_t h = (uint64_t)(uintptr_t)(ctx->d_tables.as<uint8_t>() + o_host);
+        for (size_t i : host_seg) ((uint64_t*)(pk.bytes.data() + o_src))[i] += h;
+        int rc = upload(ctx, pk);
+        if (rc) return rc;
+        const uint8_t* T = ctx->d_tables.as<uint8_t>();
+        rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), (int)src.size(), d_out);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));
+        return 0;
+    }
+};
 
 // The per-chunk scratch encode_batch allocates for codec e (d_enc_tab, d_hdr, d_pay, d_hist), for the pass planner (kz_stream_plan.h)
 EntropyScratch entropy_scratch(uint32_t e) {
@@ -1813,6 +1925,43 @@ int encode_slots(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_
     return 0;
 }
 
+// The bit strings of blocks encoded pass by pass, kept for one assembly behind the last pass: record r is bits[r] bits at offset[r] of
+// ctx->d_bits, each record at a 16-byte aligned offset; `used` bytes are taken.
+struct RecordArena {
+    std::vector<uint64_t> bits, offset;
+    uint64_t used = 0;
+    explicit RecordArena(size_t n) : bits(n), offset(n) {}
+    const uint8_t* record(kz_ctx* ctx, size_t r) const { return ctx->d_bits.as<uint8_t>() + offset[r]; }
+
+    // encode_slots over the k blocks of one pass, then block j's bit string packed behind the arena's records as record rec[j]
+    int encode_pass(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_t checksum_bits, const uint8_t* d_slots, uint64_t stride,
+                    const std::vector<uint32_t>& len, const std::vector<uint64_t>& bs, const BlockPrep& prep, const uint32_t* rec) {
+        const uint32_t k = (uint32_t)len.size();
+        uint64_t ostride = 0;
+        std::vector<uint64_t> b;
+        int rc = encode_slots(ctx, plan, etype, checksum_bits, d_slots, stride, len, bs, prep, &ostride, b);
+        if (rc) return rc;
+        uint64_t need = used;
+        for (uint32_t j = 0; j < k; j++) need += round16((b[j] + 7) / 8);
+        if (need + 64 + 256 > ctx->d_bits.cap) {  // grow d_bits, keeping the records of the earlier passes (DevBuf::ensure drops them)
+            DevBuf nb;
+            CK(nb.ensure(std::max<size_t>(need + 64, 2 * ctx->d_bits.cap)));
+            if (used) CK(cudaMemcpyAsync(nb.p, ctx->d_bits.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            ctx->d_bits.release();
+            ctx->d_bits = nb;
+        }
+        CopyList pack;
+        for (uint32_t j = 0; j < k; j++) {
+            bits[rec[j]] = b[j];
+            offset[rec[j]] = used;
+            pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + used, (b[j] + 7) / 8);
+            used += round16((b[j] + 7) / 8);
+        }
+        return run_copies(ctx, pack);
+    }
+};
+
 // Inverse transform stage (ByteTransformSequence.Inverse, transform/Sequence.go:131-186) of every block of a batch. The entropy
 // stage left block b's pre_len bytes at d_pre + b*pstride, a scratch buffer of this context with room for pstride - 64 bytes per
 // block; the stages alternate between it and ctx->d_tmp2. out_len[b] = decoded length of block b. Once the lengths are known,
@@ -2289,37 +2438,14 @@ int kz_concat_bits_device(kz_ctx* ctx, uint32_t nseg, const void* const* d_seg, 
     if (int rc = after_caller_work(ctx)) return rc;
     if (!ctx || !total_bits || (nseg && (!d_seg || !seg_bits)) || !d_dst) return -KZ_ERR_INVALID_PARAM;
     CK(cudaSetDevice(ctx->device));
-    std::vector<uint64_t> src, bits;
-    uint64_t total = 0;
+    SegmentList sl;
     for (uint32_t i = 0; i < nseg; i++) {
         if (((uintptr_t)d_seg[i] & 3) != 0) return ctx->fail(KZ_ERR_INVALID_PARAM, "segments must be 4-byte aligned");
-        const uint64_t nbytes = (seg_bits[i] + 7) / 8;
-        for (uint64_t o = 0; o < nbytes; o += RAW_PIECE) {
-            src.push_back((uint64_t)(uintptr_t)((const uint8_t*)d_seg[i] + o));
-            bits.push_back(std::min<uint64_t>(8 * RAW_PIECE, seg_bits[i] - 8 * o));
-        }
-        total += seg_bits[i];
+        sl.add_device((const uint8_t*)d_seg[i], 0, seg_bits[i]);
     }
-    *total_bits = total;
-    if ((total + 7) / 8 + 8 > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-    const int nsegs = (int)src.size();
-    if (nsegs == 0) return 0;
-    Packer pk;
-    const size_t o_src = pk.add(src.data(), src.size() * 8);
-    const size_t o_bits = pk.add(bits.data(), bits.size() * 8);
-    const size_t o_dst = pk.reserve((size_t)(nsegs + 1) * 8);
-    const size_t o_total = pk.reserve(8);
-    int rc = upload(ctx, pk);
-    if (rc) return rc;
-    uint8_t* T = ctx->d_tables.as<uint8_t>();
-    {
-        LaunchScope ls(ctx, "scan");
-        scan_bits_kernel<<<1, 1024, 0, ctx->stream>>>((const uint64_t*)(T + o_bits), (uint64_t*)(T + o_dst), nsegs + 1, 0, (uint64_t*)(T + o_total));
-    }
-    rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), nsegs, (uint8_t*)d_dst);
-    if (rc) return rc;
-    CK(cudaStreamSynchronize(ctx->stream));
-    return 0;
+    *total_bits = sl.next;
+    if ((sl.next + 7) / 8 + 8 > cap) return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
+    return sl.write(ctx, (uint8_t*)d_dst);
 }
 
 // A stream's blocks decoded to d_dst (cap bytes). given: the header fields (as sharded decompression gets them from rank 0) and the first
@@ -2454,31 +2580,11 @@ int kz_decompress_stream(kz_ctx* ctx, const uint8_t* src, size_t n, uint8_t* dst
 // Every input file of BlockCompressor is a stream of its own (app/BlockCompressor.go:543-613); blocks are independent
 // (io/CompressedStream.go:896-898), so the blocks of all streams run through the stages together, pass by pass (kz_stream_plan.h).
 
-// Grows b to n bytes and keeps its first `used` bytes (DevBuf::ensure does not keep them).
-static int ensure_keep(kz_ctx* ctx, DevBuf& b, size_t used, size_t n) {
-    if (n + 256 <= b.cap) return 0;
-    DevBuf nb;
-    CK(nb.ensure(std::max(n, 2 * b.cap)));
-    if (used) CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    b.release();
-    b = nb;
-    return 0;
-}
-
 static int check_stream_args(kz_ctx* ctx, uint32_t nstreams, const void* src, const uint64_t* src_off, const uint64_t* src_len, const void* dst,
                              const uint64_t* dst_off, const uint64_t* dst_cap, const uint64_t* out_len, const int32_t* status, bool device) {
     if (nstreams && (!src_off || !src_len || !dst_off || !dst_cap || !out_len || !status)) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
-    uint64_t src_end = 0, dst_end = 0;
-    for (uint32_t s = 0; s < nstreams; s++) {
-        if (src_off[s] + src_len[s] < src_off[s] || dst_off[s] + dst_cap[s] < dst_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
-        src_end = std::max(src_end, src_off[s] + src_len[s]);
-        dst_end = std::max(dst_end, dst_off[s] + dst_cap[s]);
-        if (device && ((src_off[s] | dst_off[s]) & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
-    }
-    if ((src_end && !src) || (dst_end && !dst)) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
-    if (device && (((uintptr_t)src & 15) || ((uintptr_t)dst & 15))) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    return 0;
+    int rc = check_spans(ctx, src, src_off, src_len, nstreams, device);
+    return rc ? rc : check_spans(ctx, dst, dst_off, dst_cap, nstreams, device);
 }
 
 // The return value and statuses of a many-stream call: a call-level failure rc sets every status; otherwise the first failing stream's code.
@@ -2496,13 +2602,12 @@ static int finish_streams(uint32_t nstreams, int32_t* status, uint64_t* out_len,
 }
 
 // Compresses stream s = d_src[src_off[s] : + src_len[s]] with blocks of block_size[s] bytes. Stream s is assembled in ctx->d_asm at
-// 8 * stage_off[s] (16-byte aligned, behind the header / prefix table of `small_bytes`); its length is out_len[s], status[s] =
-// -KZ_ERR_WRITE_FILE when it exceeds dst_cap[s]. A stream whose block size kz_compress_stream refuses gets -KZ_ERR_INVALID_PARAM and no
-// blocks; the other streams' blocks share every pass, whatever their block sizes.
+// 8 * stage_off[s] (16-byte aligned); its length is out_len[s], status[s] = -KZ_ERR_WRITE_FILE when it exceeds dst_cap[s]. A stream whose
+// block size kz_compress_stream refuses gets -KZ_ERR_INVALID_PARAM and no blocks; the other streams' blocks share every pass, whatever
+// their block sizes.
 static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, const uint32_t* block_size, uint32_t checksum_bits, uint32_t nstreams,
                                  const uint8_t* d_src, const uint64_t* src_off, const uint64_t* src_len, const int64_t* input_size,
-                                 const uint64_t* dst_cap, uint64_t* out_len, int32_t* status, std::vector<uint64_t>& stage_off, uint64_t* stage_base,
-                                 uint64_t* stage_total) {
+                                 const uint64_t* dst_cap, uint64_t* out_len, int32_t* status, std::vector<uint64_t>& stage_off, uint64_t* stage_total) {
     int rc = check_checksum_bits(ctx, checksum_bits);
     if (rc) return rc;
     if (!etype_supported(etype)) return ctx->fail(KZ_ERR_CREATE_CODEC, "entropy codec not available on the GPU path");
@@ -2521,11 +2626,10 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, cons
     BlockPrep prep;
     rc = prepare_blocks(ctx, plan, ctx->skip_blocks, checksum_bits, d_src, bl, prep);
     if (rc) return rc;
-    // passes: transforms and entropy coding of the blocks of a pass, then their bit strings packed into ctx->d_bits
+    // passes: transforms and entropy coding of the blocks of a pass, then their bit strings packed into the arena as records b
     const EntropyScratch es = entropy_scratch(etype);
     const PassPlan P = plan_compress_passes(bl.len, [&](uint64_t s) { return compress_block_cost(s, es); });
-    std::vector<uint64_t> bbits(nb), barena(nb);
-    uint64_t arena = 0;
+    RecordArena arena(nb);
     for (uint32_t p = 0; p < P.npasses(); p++) {
         const uint32_t i0 = P.first[p], k = P.first[p + 1] - i0;
         const uint64_t s = P.stride[p];
@@ -2542,95 +2646,45 @@ static int compress_streams_impl(kz_ctx* ctx, uint64_t t48, uint32_t etype, cons
         }
         rc = run_copies(ctx, place);
         if (rc) return rc;
-        uint64_t ostride = 0;
-        std::vector<uint64_t> bits;
-        rc = encode_slots(ctx, plan, etype, checksum_bits, slots, s, lens, pbs, prep.pick(&P.order[i0], k), &ostride, bits);
-        if (rc) return rc;
-        uint64_t need = arena;
-        for (uint32_t j = 0; j < k; j++) need += round16((bits[j] + 7) / 8);
-        rc = ensure_keep(ctx, ctx->d_bits, arena, need + 64);
-        if (rc) return rc;
-        CopyList pack;
-        for (uint32_t j = 0; j < k; j++) {
-            const uint32_t b = P.order[i0 + j];
-            const uint64_t nbytes = (bits[j] + 7) / 8;
-            bbits[b] = bits[j];
-            barena[b] = arena;
-            pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + arena, nbytes);
-            arena += round16(nbytes);
-        }
-        rc = run_copies(ctx, pack);
+        rc = arena.encode_pass(ctx, plan, etype, checksum_bits, slots, s, lens, pbs, prep.pick(&P.order[i0], k), &P.order[i0]);
         if (rc) return rc;
     }
     // assembly (Writer.processBlock :951-976, Close :593-594): stream header, then 5 b | lw b prefix and bit string of every block, then the
-    // end marker. Lengths are known here, so the host lays out every segment; one concat_zero / concat_copy pair writes all streams.
-    const size_t o_zero = 64 * (size_t)nstreams + 8 * (size_t)nb;
-    const uint64_t small_bytes = (o_zero + 16 + 255) & ~255ull;
-    std::vector<uint8_t> small(small_bytes, 0);
-    std::vector<uint32_t> hdr_bits(nstreams), pre_bits(nb);
+    // end marker. Lengths are known here, so the host lays out every segment; one concat writes all streams.
     stage_off.assign(nstreams, 0);
-    uint64_t stage = 0, nsegs = 0;
+    uint64_t stage = 0;
+    SegmentList sl;
     for (uint32_t s = 0; s < nstreams; s++) {
-        hdr_bits[s] = 0;
         if (!block_size_ok(block_size[s])) {
             out_len[s] = 0;
             status[s] = -KZ_ERR_INVALID_PARAM;
             continue;
         }
-        if (!ctx->headerless_writer) {  // Writer.writeHeader :430
-            std::vector<uint8_t> hdr;
-            hdr_bits[s] = build_stream_header(hdr, t48, etype, block_size[s], checksum_bits, input_size ? input_size[s] : 0);
-            memcpy(&small[64 * (size_t)s], hdr.data(), 64);
-        }
-        uint64_t bits = hdr_bits[s] + END_MARKER_BITS;
+        std::vector<uint8_t> hdr, pre(8 * (size_t)(bl.first[s + 1] - bl.first[s]), 0);
+        const uint32_t hdr_bits =
+            ctx->headerless_writer ? 0 : build_stream_header(hdr, t48, etype, block_size[s], checksum_bits, input_size ? input_size[s] : 0);  // Writer.writeHeader :430
+        std::vector<uint32_t> pre_bits;
+        uint64_t bits = hdr_bits + END_MARKER_BITS;
         for (uint32_t b = bl.first[s]; b < bl.first[s + 1]; b++) {
-            pre_bits[b] = write_block_prefix(&small[64 * (size_t)nstreams + 8 * (size_t)b], bbits[b]);
-            bits += pre_bits[b] + bbits[b];
-            nsegs += 1 + (bbits[b] + 8 * RAW_PIECE - 1) / (8 * RAW_PIECE);
+            pre_bits.push_back(write_block_prefix(&pre[8 * pre_bits.size()], arena.bits[b]));
+            bits += pre_bits.back() + arena.bits[b];
         }
         out_len[s] = (bits + 7) / 8;
         status[s] = out_len[s] > dst_cap[s] ? -KZ_ERR_WRITE_FILE : 0;
-        stage_off[s] = stage;
-        if (!status[s]) stage += round16(out_len[s]);
-        nsegs += 2;
-    }
-    *stage_base = small_bytes;
-    *stage_total = stage;
-    CK(ctx->d_asm.ensure(small_bytes + stage + 64));
-    uint8_t* A = ctx->d_asm.as<uint8_t>();
-    CK(cudaMemcpyAsync(A, small.data(), small_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    std::vector<uint64_t> seg_src, seg_bits, seg_dst;
-    seg_src.reserve(nsegs), seg_bits.reserve(nsegs), seg_dst.reserve(nsegs);
-    for (uint32_t s = 0; s < nstreams; s++) {
         if (status[s]) continue;
-        uint64_t d = 8 * (small_bytes + stage_off[s]);
-        auto add = [&](const uint8_t* src, uint64_t nbits) {
-            seg_src.push_back((uint64_t)(uintptr_t)src);
-            seg_bits.push_back(nbits);
-            seg_dst.push_back(d);
-            d += nbits;
-        };
-        if (hdr_bits[s]) add(A + 64 * (size_t)s, hdr_bits[s]);
-        for (uint32_t b = bl.first[s]; b < bl.first[s + 1]; b++) {
-            add(A + 64 * (size_t)nstreams + 8 * (size_t)b, pre_bits[b]);
-            for (uint64_t o = 0; o < bbits[b]; o += 8 * RAW_PIECE) add(ctx->d_bits.as<uint8_t>() + barena[b] + o / 8, std::min<uint64_t>(8 * RAW_PIECE, bbits[b] - o));
+        stage_off[s] = stage;
+        sl.at(8 * stage);
+        sl.add_host(hdr.data(), hdr_bits);
+        for (uint32_t b = bl.first[s], j = 0; b < bl.first[s + 1]; b++, j++) {
+            sl.add_host(&pre[8 * j], pre_bits[j]);
+            sl.add_device(arena.record(ctx, b), 0, arena.bits[b]);
         }
-        add(A + o_zero, END_MARKER_BITS);
+        sl.add_end_marker();
+        stage += round16(out_len[s]);
     }
-    const int ns = (int)seg_src.size();
-    if (ns) {
-        Packer pk;
-        const size_t o_src = pk.add(seg_src.data(), seg_src.size() * 8);
-        const size_t o_bits = pk.add(seg_bits.data(), seg_bits.size() * 8);
-        const size_t o_dst = pk.add(seg_dst.data(), seg_dst.size() * 8);
-        rc = upload(ctx, pk);
-        if (rc) return rc;
-        uint8_t* T = ctx->d_tables.as<uint8_t>();
-        rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), ns, A);
-        if (rc) return rc;
-        CK(cudaStreamSynchronize(ctx->stream));  // the segment tables live in d_tables
-    }
-    return 0;
+    *stage_total = stage;
+    CK(ctx->d_asm.ensure(stage + 64));
+    return sl.write(ctx, ctx->d_asm.as<uint8_t>());
 }
 
 // One group of streams whose headers differ at most in block size (sh: the first one's; shs[s]: stream s's, which gives its first record's
@@ -2746,13 +2800,13 @@ static int compress_streams_device(kz_ctx* ctx, uint64_t t48, uint32_t etype, co
     if (cudaSetDevice(ctx->device) != cudaSuccess) return finish_streams(nstreams, status, out_len, -KZ_ERR_PROCESS_BLOCK);
     if (one_size && (rc = check_encode_args(ctx, *one_size, checksum_bits)) != 0) return finish_streams(nstreams, status, out_len, rc);
     std::vector<uint64_t> stage_off;
-    uint64_t stage_base = 0, stage_total = 0;
+    uint64_t stage_total = 0;
     rc = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, (const uint8_t*)d_src, src_off, src_len, input_size, dst_cap, out_len,
-                               status, stage_off, &stage_base, &stage_total);
+                               status, stage_off, &stage_total);
     if (!rc) {
         CopyList out;
         for (uint32_t s = 0; s < nstreams; s++)
-            if (!status[s]) out.add(ctx->d_asm.as<uint8_t>() + stage_base + stage_off[s], (uint8_t*)d_dst + dst_off[s], out_len[s]);
+            if (!status[s]) out.add(ctx->d_asm.as<uint8_t>() + stage_off[s], (uint8_t*)d_dst + dst_off[s], out_len[s]);
         rc = run_copies(ctx, out);
         if (!rc && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = ctx->cuda_fail(cudaGetLastError(), "compress_streams");
     }
@@ -2773,24 +2827,19 @@ static int compress_streams_host(kz_ctx* ctx, uint64_t t48, uint32_t etype, cons
             if (r) return r;
         }
         // the inputs packed at 16-byte aligned offsets and moved in one transfer
-        std::vector<uint64_t> in_off(nstreams);
-        uint64_t total = 0;
-        for (uint32_t s = 0; s < nstreams; s++) in_off[s] = total, total += round16(src_len[s]);
-        CK(ctx->h_io.ensure(total + 64));
-        CK(ctx->d_in.ensure(total + 64));
-        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
-        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
-        std::vector<uint64_t> stage_off;
-        uint64_t stage_base = 0, stage_total = 0;
-        int r = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, ctx->d_in.as<uint8_t>(), in_off.data(), src_len, input_size, dst_cap,
-                                      out_len, status, stage_off, &stage_base, &stage_total);
+        std::vector<UploadPiece> in(nstreams);
+        for (uint32_t s = 0; s < nstreams; s++) in[s] = UploadPiece{src + src_off[s], src_len[s], src_len[s]};
+        std::vector<uint64_t> in_off, stage_off;
+        uint64_t total = 0, stage_total = 0;
+        int r = upload_pieces(ctx, in, in_off, &total);
         if (r) return r;
-        CK(ctx->h_io.ensure(stage_total + 64));
-        if (stage_total) CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.as<uint8_t>() + stage_base, stage_total, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
+        r = compress_streams_impl(ctx, t48, etype, block_size, checksum_bits, nstreams, ctx->d_in.as<uint8_t>(), in_off.data(), src_len, input_size, dst_cap,
+                                  out_len, status, stage_off, &stage_total);
+        if (r) return r;
+        std::vector<DownloadPiece> out;
         for (uint32_t s = 0; s < nstreams; s++)
-            if (!status[s]) memcpy(dst + dst_off[s], (uint8_t*)ctx->h_io.p + stage_off[s], out_len[s]);
-        return 0;
+            if (!status[s]) out.push_back(DownloadPiece{dst + dst_off[s], stage_off[s], out_len[s]});
+        return download_pieces(ctx, ctx->d_asm.as<uint8_t>(), stage_total, out);
     }();
     return finish_streams(nstreams, status, out_len, rc);
 }
@@ -2851,19 +2900,17 @@ int kz_decompress_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, co
         CK(cudaSetDevice(ctx->device));
         // inputs packed at 16-byte aligned offsets with 64 zero bytes behind each (what kz_decompress_stream gives a single stream);
         // outputs staged at 16-byte aligned offsets of dst_cap[s] bytes each, packed by length and moved back in one transfer
-        std::vector<uint64_t> in_off(nstreams), st_off(nstreams), pk_off(nstreams);
+        std::vector<UploadPiece> in(nstreams);
+        std::vector<uint64_t> in_off, st_off(nstreams), pk_off(nstreams);
         uint64_t total = 0, st_total = 0;
         for (uint32_t s = 0; s < nstreams; s++) {
-            in_off[s] = total, total += round16(src_len[s]) + 64;
+            in[s] = UploadPiece{src + src_off[s], src_len[s], src_len[s] + 64};
             st_off[s] = st_total, st_total += round16(dst_cap[s]);
         }
-        CK(ctx->h_io.ensure(total + 64));
-        CK(ctx->d_in.ensure(total + 64));
+        int r = upload_pieces(ctx, in, in_off, &total);
+        if (r) return r;
         CK(ctx->d_out.ensure(st_total + 64));
-        memset(ctx->h_io.p, 0, total);
-        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
-        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
-        int r = decompress_streams_impl(ctx, nstreams, ctx->d_in.as<uint8_t>(), total, in_off.data(), src_len, ctx->d_out.as<uint8_t>(), st_off.data(), dst_cap,
+        r = decompress_streams_impl(ctx, nstreams, ctx->d_in.as<uint8_t>(), total, in_off.data(), src_len, ctx->d_out.as<uint8_t>(), st_off.data(), dst_cap,
                                         out_len, status);
         if (r) return r;
         uint64_t pk_total = 0;
@@ -2877,12 +2924,10 @@ int kz_decompress_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, co
             if (!status[s]) pack.add(ctx->d_out.as<uint8_t>() + st_off[s], ctx->d_asm.as<uint8_t>() + pk_off[s], out_len[s]);
         r = run_copies(ctx, pack);
         if (r) return r;
-        CK(ctx->h_io.ensure(pk_total + 64));
-        if (pk_total) CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.p, pk_total, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
+        std::vector<DownloadPiece> out;
         for (uint32_t s = 0; s < nstreams; s++)
-            if (!status[s]) memcpy(dst + dst_off[s], (uint8_t*)ctx->h_io.p + pk_off[s], out_len[s]);
-        return 0;
+            if (!status[s]) out.push_back(DownloadPiece{dst + dst_off[s], pk_off[s], out_len[s]});
+        return download_pieces(ctx, ctx->d_asm.as<uint8_t>(), pk_total, out);
     }();
     return finish_streams(nstreams, status, out_len, rc);
 }
@@ -2925,31 +2970,30 @@ int upload_windows(kz_ctx* ctx, const std::vector<ReadSource>& S, const ReadPlan
                    std::vector<uint64_t>& bit_off, PassInput& in) {
     struct Window {
         uint32_t s;
-        uint64_t lo, hi, at;  // bytes [lo, hi) of stream s at packed offset `at`
+        uint64_t lo, hi;  // bytes [lo, hi) of stream s
     };
     std::vector<Window> win;
     std::vector<uint32_t> win_of(ks.size());
-    uint64_t total = 0;
     for (size_t i = 0; i < ks.size(); i++) {
         const uint32_t s = P.stream[ks[i]];
         const kz_index& ix = *S[s].ix;
         const uint64_t b = P.blocks[ks[i]];
         const uint64_t lo = (ix.start[b] / 8) & ~15ull, hi = (ix.start[b] + ix.bits[b] + 7) / 8 + 64;
-        if (win.empty() || win.back().s != s || lo > win.back().hi) win.push_back(Window{s, lo, hi, 0});
+        if (win.empty() || win.back().s != s || lo > win.back().hi) win.push_back(Window{s, lo, hi});
         else win.back().hi = std::max(win.back().hi, hi);
         win_of[i] = (uint32_t)win.size() - 1;
     }
-    for (Window& w : win) w.at = total, total += round16(w.hi - w.lo);
-    CK(ctx->h_io.ensure(total + 64));
-    CK(ctx->d_in.ensure(total + 128));
-    memset(ctx->h_io.p, 0, total);
-    for (const Window& w : win) memcpy((uint8_t*)ctx->h_io.p + w.at, src + S[w.s].at + w.lo, std::min<uint64_t>(w.hi, S[w.s].n) - w.lo);
-    CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<UploadPiece> pieces;
+    for (const Window& w : win) pieces.push_back(UploadPiece{src + S[w.s].at + w.lo, std::min<uint64_t>(w.hi, S[w.s].n) - w.lo, w.hi - w.lo});
+    std::vector<uint64_t> at;
+    uint64_t total = 0;
+    int rc = upload_pieces(ctx, pieces, at, &total);
+    if (rc) return rc;
     in.d_words = ctx->d_in.as<uint32_t>();
     in.words_len = (total + 3) / 4 + 16;
     for (size_t i = 0; i < ks.size(); i++) {
         const Window& w = win[win_of[i]];
-        bit_off[ks[i]] = S[w.s].ix->start[P.blocks[ks[i]]] - 8 * w.lo + 8 * w.at;
+        bit_off[ks[i]] = S[w.s].ix->start[P.blocks[ks[i]]] - 8 * w.lo + 8 * at[win_of[i]];
     }
     if (ctx->profile) {
         auto& e = ctx->prof["read:h2d"];
@@ -3250,11 +3294,11 @@ int read_ranges_impl(kz_ctx* ctx, kz_cache* cache, const uint8_t* src, const uin
         if (status[i]) out_len[i] = 0;
     // delivery of the staged requests: one transfer to the host, or one copy launch on the device
     if (host && stage_total) {
-        CK(ctx->h_io.ensure(stage_total));
-        CK(cudaMemcpyAsync(ctx->h_io.p, ctx->d_asm.p, stage_total, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
+        std::vector<DownloadPiece> out;
         for (uint32_t i = 0; i < nreq; i++)
-            if (!status[i] && out_len[i]) memcpy(dst + dst_off[i], (uint8_t*)ctx->h_io.p + stage_at[i], out_len[i]);
+            if (!status[i] && out_len[i]) out.push_back(DownloadPiece{dst + dst_off[i], stage_at[i], out_len[i]});
+        rc = download_pieces(ctx, ctx->d_asm.as<uint8_t>(), stage_total, out);
+        if (rc) return rc;
     } else if (stage_total) {
         CopyList deliver;
         for (uint32_t i = 0; i < nreq; i++)
@@ -3308,10 +3352,9 @@ int read_ranges(kz_ctx* ctx, kz_index* ix, kz_cache* cache, const uint8_t* src, 
         if (r) return r;
         if (!src && ((uintptr_t)d_src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
         // the stream the index was built from: its length and its leading bytes
-        uint8_t head[INDEX_HEAD] = {0};
+        uint8_t head[INDEX_HEAD];
         const uint64_t at = 0, nh = n == ix->stream_bytes ? n : 0;
-        if (src) memcpy(head, src, std::min<uint64_t>(nh, INDEX_HEAD));
-        else if ((r = gather_heads(ctx, (const uint8_t*)d_src, &at, &nh, 1, INDEX_HEAD, head))) return r;
+        if ((r = read_heads(ctx, src ? src : (const uint8_t*)d_src, !src, &at, &nh, 1, head))) return r;
         r = read_stream_check(ctx, ix, n, head);
         if (r) return r;
         return read_ranges_impl(ctx, cache, src, (const uint8_t*)d_src, {ReadSource{ix, 0, n}}, nreq, nullptr, off, len, (uint8_t*)dst, dst_off, out_len,
@@ -3337,26 +3380,15 @@ int read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_inde
             if (req_stream[i] >= nstreams) return ctx->fail(KZ_ERR_INVALID_PARAM, "a request names a stream past nstreams");
             named[req_stream[i]] = 1;
         }
+        // the spans of the named streams, and their first 32 bytes (one device stream: copied straight back, as kz_read_ranges_device does)
         std::vector<uint32_t> names;
-        for (uint32_t s = 0; s < nstreams; s++) {
-            if (!named[s]) continue;
-            if (src_off[s] + src_len[s] < src_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
-            if (src_len[s] && !base) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
-            if (device && (src_off[s] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
-            names.push_back(s);
-        }
-        if (device && ((uintptr_t)base & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-        // the first 32 bytes of every named stream: copied on the host, or gathered on the device (one stream: copied straight back, as
-        // kz_read_ranges_device does)
+        std::vector<uint64_t> hoff, hlen;
+        for (uint32_t s = 0; s < nstreams; s++)
+            if (named[s]) names.push_back(s), hoff.push_back(src_off[s]), hlen.push_back(src_len[s]);
         const size_t nn = names.size();
-        std::vector<uint8_t> head(INDEX_HEAD * nn, 0);
-        std::vector<uint64_t> hoff(nn), hlen(nn);
-        for (size_t j = 0; j < nn; j++) hoff[j] = src_off[names[j]], hlen[j] = src_len[names[j]];
-        if (!device) {
-            for (size_t j = 0; j < nn; j++) memcpy(&head[INDEX_HEAD * j], base + hoff[j], std::min<uint64_t>(hlen[j], INDEX_HEAD));
-        } else if ((r = gather_heads(ctx, base, hoff.data(), hlen.data(), nn, INDEX_HEAD, head.data()))) {
-            return r;
-        }
+        if ((r = check_spans(ctx, base, hoff.data(), hlen.data(), nn, device))) return r;
+        std::vector<uint8_t> head(INDEX_HEAD * nn);
+        if ((r = read_heads(ctx, base, device, hoff.data(), hlen.data(), nn, head.data()))) return r;
         // per stream: a missing or stale index or a chain without a GPU path fails the stream's requests with kz_read_ranges's code
         std::vector<int32_t> code(nstreams, 0);
         std::vector<uint32_t> slot(nstreams, 0);
@@ -3462,15 +3494,7 @@ int check_index_streams_args(kz_ctx* ctx, uint32_t ns, const void* src, const ui
                              bool device) {
     for (uint32_t s = 0; out && s < ns; s++) out[s] = nullptr;
     if (ns && (!src_off || !src_len || !out || !status)) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument array");
-    uint64_t end = 0;
-    for (uint32_t s = 0; s < ns; s++) {
-        if (src_off[s] + src_len[s] < src_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
-        end = std::max(end, src_off[s] + src_len[s]);
-        if (device && (src_off[s] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
-    }
-    if (end && !src) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
-    if (device && ((uintptr_t)src & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
-    return 0;
+    return check_spans(ctx, src, src_off, src_len, ns, device);
 }
 
 // ---- writes into a compressed stream (kz_write_ranges[_device]; plan in kz_write_plan.h) -------------------------------------------
@@ -3496,12 +3520,10 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
     }
     if (!host && (((uintptr_t)d_src & 15) || ((uintptr_t)dst & 15))) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
     if (!host && dst && dst < d_src + n && d_src < dst + cap) return ctx->fail(KZ_ERR_INVALID_PARAM, "the output overlaps the stream");
-    uint8_t head[INDEX_HEAD] = {0};
+    uint8_t head[INDEX_HEAD];
     const uint64_t at0 = 0, nh = n == ix->stream_bytes ? n : 0;
-    int rc = 0;
-    if (host) memcpy(head, src, std::min<uint64_t>(nh, INDEX_HEAD));
-    else if ((rc = gather_heads(ctx, d_src, &at0, &nh, 1, INDEX_HEAD, head))) return rc;
-    if ((rc = read_stream_check(ctx, ix, n, head))) return rc;
+    int rc = read_heads(ctx, host ? src : d_src, !host, &at0, &nh, 1, head);
+    if (rc || (rc = read_stream_check(ctx, ix, n, head))) return rc;
     TransformPlan plan;
     if ((rc = plan_transforms(ctx, ix->t48, ix->etype, plan, KZ_ERR_CREATE_CODEC))) return rc;
     const StreamHeader sh = index_header(*ix);
@@ -3585,8 +3607,8 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
     // passes: decode, apply the writes, encode; each pass's records packed into ctx->d_bits
     const uint32_t ne = (uint32_t)P.enc.size();
     const uint64_t astride = decompress_slot(bs);
-    std::vector<uint64_t> rbits(ne), rarena(ne);
-    uint64_t arena = 0, enc_bytes = 0;
+    RecordArena arena(ne);
+    uint64_t enc_bytes = 0;
     for (uint32_t p = 0; p < P.npasses(); p++) {
         const uint32_t a = P.first[p], k = P.first[p + 1] - a;
         CK(ctx->d_slots.ensure(astride * k + 64));
@@ -3627,30 +3649,18 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
         bl.first = {0, k};
         BlockPrep prep;
         if ((rc = prepare_blocks(ctx, plan, ctx->skip_blocks, sh.checksum_bits, slots, bl, prep))) return rc;
-        uint64_t ostride = 0;
-        std::vector<uint64_t> bits;
-        rc = encode_slots(ctx, plan, ix->etype, sh.checksum_bits, slots, astride, lens, std::vector<uint64_t>(k, bs), prep, &ostride, bits);
+        std::vector<uint32_t> rec(k);
+        for (uint32_t j = 0; j < k; j++) rec[j] = a + j;
+        rc = arena.encode_pass(ctx, plan, ix->etype, sh.checksum_bits, slots, astride, lens, std::vector<uint64_t>(k, bs), prep, rec.data());
         if (rc) return rc;
-        uint64_t need = arena;
-        for (uint32_t j = 0; j < k; j++) need += round16((bits[j] + 7) / 8);
-        if ((rc = ensure_keep(ctx, ctx->d_bits, arena, need + 64))) return rc;
-        CopyList pack;
-        for (uint32_t j = 0; j < k; j++) {
-            rbits[a + j] = bits[j];
-            rarena[a + j] = arena;
-            pack.add(ctx->d_enc.as<uint8_t>() + j * ostride, ctx->d_bits.as<uint8_t>() + arena, (bits[j] + 7) / 8);
-            arena += round16((bits[j] + 7) / 8);
-        }
-        if ((rc = run_copies(ctx, pack))) return rc;
         CK(cudaStreamSynchronize(ctx->stream));  // the slots and the copy lists are reused by the next pass
     }
     // the new record table, then the tail: one concat of every segment behind byte floor(cut / 8)
-    const uint64_t zero_off = 8 * (uint64_t)ne;
-    std::vector<uint8_t> small(zero_off + 16, 0);
-    std::vector<uint32_t> pre(ne);
-    for (uint32_t j = 0; j < ne; j++) pre[j] = write_block_prefix(&small[8 * (size_t)j], rbits[j]);
+    std::vector<uint8_t> pre(8 * (size_t)ne, 0);
+    std::vector<uint32_t> pre_bits(ne);
+    for (uint32_t j = 0; j < ne; j++) pre_bits[j] = write_block_prefix(&pre[8 * (size_t)j], arena.bits[j]);
     StreamIndex y;
-    const uint64_t total_bits = splice_records(x, P, rbits, pre, END_MARKER_BITS, y);
+    const uint64_t total_bits = splice_records(x, P, arena.bits, pre_bits, END_MARKER_BITS, y);
     const uint64_t kp = P.cut / 8, tail_bits = total_bits - 8 * kp, tail_bytes = (tail_bits + 7) / 8;
     const uint64_t need_cap = (tail_bits + 31) / 32 * 4;  // the concat writes whole 32-bit words
     if (need_cap > cap) {
@@ -3658,29 +3668,21 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
         return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
     }
     if (!dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
-    CK(ctx->d_asm.ensure(small.size()));
-    uint8_t* A = ctx->d_asm.as<uint8_t>();
-    CK(cudaMemcpyAsync(A, small.data(), small.size(), cudaMemcpyHostToDevice, ctx->stream));
-    std::vector<uint64_t> seg_src, seg_bits, seg_dst;
-    uint64_t d = 0, moved_runs = 0, moved_bits = 0;
-    auto add = [&](uint64_t word, uint64_t nbits) {
-        seg_src.push_back(word), seg_bits.push_back(nbits), seg_dst.push_back(d);
-        d += nbits;
-    };
+    SegmentList sl;
+    uint64_t moved_runs = 0, moved_bits = 0;
     for (const WriteSeg& sg : P.segs) {
         if (sg.kind == SEG_CARRY) {
-            add(seg_source(d_base, sg.bit - base_bit), sg.bits);
+            sl.add_device(d_base, sg.bit - base_bit, sg.bits);
         } else if (sg.kind == SEG_NEW) {
             for (uint64_t j = sg.first; j < sg.first + sg.count; j++) {
-                add(seg_source(A + 8 * j, 0), pre[j]);
-                for (uint64_t o = 0; o < rbits[j]; o += 8 * RAW_PIECE)
-                    add(seg_source(ctx->d_bits.as<uint8_t>() + rarena[j], o), std::min<uint64_t>(8 * RAW_PIECE, rbits[j] - o));
+                sl.add_host(&pre[8 * j], pre_bits[j]);
+                sl.add_device(arena.record(ctx, j), 0, arena.bits[j]);
             }
         } else if (sg.kind == SEG_OLD) {
-            for (uint64_t o = 0; o < sg.bits; o += 8 * RAW_PIECE) add(seg_source(d_base, sg.bit - base_bit + o), std::min<uint64_t>(8 * RAW_PIECE, sg.bits - o));
+            sl.add_device(d_base, sg.bit - base_bit, sg.bits);
             moved_runs++, moved_bits += sg.bits;
         } else {
-            add(seg_source(A + zero_off, 0), END_MARKER_BITS);
+            sl.add_end_marker();
         }
     }
     uint8_t* d_out = dst;
@@ -3688,14 +3690,7 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
         CK(ctx->d_out.ensure(need_cap + 64));
         d_out = ctx->d_out.as<uint8_t>();
     }
-    Packer pk;
-    const size_t o_src = pk.add(seg_src.data(), seg_src.size() * 8);
-    const size_t o_bits = pk.add(seg_bits.data(), seg_bits.size() * 8);
-    const size_t o_dst = pk.add(seg_dst.data(), seg_dst.size() * 8);
-    if ((rc = upload(ctx, pk))) return rc;
-    uint8_t* T = ctx->d_tables.as<uint8_t>();
-    rc = concat_segments(ctx, (const uint64_t*)(T + o_src), (const uint64_t*)(T + o_bits), (const uint64_t*)(T + o_dst), (int)seg_src.size(), d_out);
-    if (rc) return rc;
+    if ((rc = sl.write(ctx, d_out))) return rc;
     // the new stream's first 32 bytes: the old ones before floor(cut / 8), the tail's behind it
     uint8_t lead[INDEX_HEAD] = {0};
     const uint64_t nlead = kp < INDEX_HEAD ? std::min<uint64_t>(INDEX_HEAD - kp, tail_bytes) : 0;
@@ -3821,14 +3816,12 @@ int kz_index_build_streams(kz_ctx* ctx, uint32_t nstreams, const uint8_t* src, c
     if (!rc) rc = [&]() -> int {
         CK(cudaSetDevice(ctx->device));
         // the streams packed at 16-byte aligned offsets with 64 zero bytes behind each, moved in one transfer
-        std::vector<uint64_t> in_off(nstreams);
+        std::vector<UploadPiece> in(nstreams);
+        for (uint32_t s = 0; s < nstreams; s++) in[s] = UploadPiece{src + src_off[s], src_len[s], src_len[s] + 64};
+        std::vector<uint64_t> in_off;
         uint64_t total = 0;
-        for (uint32_t s = 0; s < nstreams; s++) in_off[s] = total, total += round16(src_len[s]) + 64;
-        CK(ctx->h_io.ensure(total + 64));
-        CK(ctx->d_in.ensure(total + 64));
-        memset(ctx->h_io.p, 0, total);
-        for (uint32_t s = 0; s < nstreams; s++) memcpy((uint8_t*)ctx->h_io.p + in_off[s], src + src_off[s], src_len[s]);
-        if (total) CK(cudaMemcpyAsync(ctx->d_in.p, ctx->h_io.p, total, cudaMemcpyHostToDevice, ctx->stream));
+        int r = upload_pieces(ctx, in, in_off, &total);
+        if (r) return r;
         return index_build_streams(ctx, nstreams, ctx->d_in.as<uint8_t>(), in_off.data(), src_len, out, status);
     }();
     return finish_streams(nstreams, status, nullptr, rc);

@@ -7,7 +7,7 @@ exchange steps are the ones the reference's Writer / Reader do in memory:
               every rank: kz_compress_fragment_device (its block records `5 b | lw b | payload`, bit exact length)
               all_gather of the fragment bit lengths -> gather-v of the fragments to rank 0 (grouped send / recv)
               rank 0: ordered bit-granular commit (Writer.processBlock :951-976): header | fragments in rank order | end marker,
-                      one scan + funnel-shift copy on the GPU (kz_concat_bits_device)
+                      a segment table laid out on the host, one funnel-shift copy on the GPU (kz_concat_bits_device)
   decompress  rank 0 holds the stream -> header + walk over the block length prefixes (kz_stream_index_device, Reader :1816-1852)
               broadcast of the stream parameters and record boundaries -> scatter of the byte windows that hold each rank's records
               every rank: kz_decompress_fragment_device at its start bit -> gather of the decoded ranges to rank 0
