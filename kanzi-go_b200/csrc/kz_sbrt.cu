@@ -399,15 +399,24 @@ __global__ void __launch_bounds__(32) sbrt_inverse_warp_kernel(const uint8_t* __
 // look-up served by the mirror nothing but the lane boundary ties the lanes together, so the 256 entries are spread over 4 warps (2 entries
 // per lane) that sit on different schedulers: every warp takes the same decision about the next entry from the same shared-memory
 // candidates, moves its own part of the list, stores it, and one CTA barrier per rank publishes the stores.
-// The entry that crosses a warp boundary is read from the mirror instead of a shuffle. With one warp per scheduler nothing hides a step's
-// latency, and its time follows its instruction count (DESIGN.md §4.3): an entry is (q, x = p << 8 | symbol) in one 8-byte word of the
-// mirror, so that one load fetches a candidate or the boundary entry and one 16-byte store publishes a lane's two entries.
+// With one warp per scheduler nothing hides a step's latency, so a step spends as few instructions as it can (DESIGN.md §4.3):
+//   - an entry is (q, x = p << 8 | symbol) in one 8-byte word of the mirror: one load fetches a candidate or the entry above a warp's first
+//     one, and one 16-byte store publishes a thread's two entries;
+//   - both copies have a sentinel slot above position 0 (a q larger than any qc), so that the candidate r2 - 1 for r2 = 0 and the entry
+//     above thread 0 are plain loads, with no test for position 0;
+//   - warp 0 stages the ranks of a round in shared memory a round ahead and every thread holds them as 8 words: a step takes its rank r3
+//     out of a register with one byte extract, and its r / r2 are the r2 / r3 of the two steps before.
+// But what lies between one barrier and the next counts as well: the entry above a thread's first one is a shuffle inside a warp and a
+// mirror load on lane 0 only. Loading it from the mirror on every lane, and packing a round's symbols into words for one store, each took
+// instructions out of the step but made the chain slower (§4.3).
 template <bool RANK_MODE>
 __global__ void __launch_bounds__(128) sbrt_inverse_multi_kernel(const uint8_t* __restrict__ data, const SbrtBlock* __restrict__ blocks, int nblocks,
                                                                  uint8_t* __restrict__ out) {
     constexpr int S = 2;  // entries per lane
-    // two copies, written alternately: a warp that runs ahead stores step j + 1 while another still reads the state after step j - 1 / j
-    __shared__ __align__(16) uint2 s_e[2][256];
+    // two copies, written alternately: a warp that runs ahead stores step j + 1 while another still reads the state after step j - 1 / j.
+    // Position k of a copy is slot k + 2: slot 1 is the sentinel above position 0, slot 0 keeps the threads' 16-byte stores aligned.
+    __shared__ __align__(16) uint2 s_e[2][258];
+    __shared__ __align__(16) uint32_t s_rk[2][8];  // the 32 ranks of round k in s_rk[k & 1], 0 past the end of the block
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (b >= nblocks) return;
     const SbrtBlock blk = blocks[b];
@@ -416,86 +425,93 @@ __global__ void __launch_bounds__(128) sbrt_inverse_multi_kernel(const uint8_t* 
     uint8_t* dst = out + blk.dst_off;
     const uint32_t n = blk.len;
     if (n == 0) return;
+    uint8_t* const rk8 = reinterpret_cast<uint8_t*>(s_rk);
     uint32_t Q[S], X[S];
     const uint32_t base = (uint32_t)(S * tid);
 #pragma unroll
     for (int k = 0; k < S; k++) {
         Q[k] = 0;
         X[k] = base + k;
-        s_e[0][base + k] = s_e[1][base + k] = make_uint2(0u, base + k);
+        s_e[0][2 + base + k] = s_e[1][2 + base + k] = make_uint2(0u, base + k);
+    }
+    if (tid < 2) s_e[tid][1] = make_uint2(0xFFFFFFFFu, 0u);
+    if (warp == 0) {
+        rk8[lane] = (uint32_t)lane < n ? src[lane] : 0u;
+        rk8[32 + lane] = 32u + lane < n ? src[32 + lane] : 0u;
     }
     __syncthreads();
     uint2 ca, cb;  // candidates: entries r2 and r2 - 1 of the state before the current step
     auto load_candidates = [&](uint32_t r2, int par) {  // from the copy step `par` wrote
-        ca = s_e[par][r2];
-        cb = r2 ? s_e[par][r2 - 1] : make_uint2(0xFFFFFFFFu, 0u);  // above position 0: a q larger than any qc
+        ca = s_e[par][2 + r2];
+        cb = s_e[par][1 + r2];
     };
-    // par = parity of the step: it reads the copy of parity par ^ 1 (the state before it) and writes the copy of parity par
+    // par = parity of the step: it reads the copy of parity par ^ 1 (the state before it) and writes the copy of parity par.
+    // x: the entry at rank r (the same in every thread), replaced by the entry at rank r2 after the step. Returns the entry at rank r.
     auto step = [&](uint32_t r, uint32_t r2, uint32_t i, int par, uint32_t& x) -> uint32_t {
-        // the entry above this lane's first one (state before the step): a shuffle inside the warp, the mirror across a warp boundary
-        uint32_t up_q = __shfl_up_sync(0xFFFFFFFFu, Q[S - 1], 1), up_x = __shfl_up_sync(0xFFFFFFFFu, X[S - 1], 1);
-        if (lane == 0 && warp > 0) {
-            const uint2 e = s_e[par ^ 1][base - 1];
-            up_q = e.x, up_x = e.y;
-        }
-        const uint32_t sym = x & 0xFFu;
-        const uint32_t qc = RANK_MODE ? (i + (x >> 8)) >> 1 : i;  // i, p < 2^24
-        const uint32_t fresh = (i << 8) | sym;
+        // the entry above this thread's first one (state before the step): a shuffle inside the warp, the mirror on lane 0
+        uint2 up = make_uint2(__shfl_up_sync(0xFFFFFFFFu, Q[S - 1], 1), __shfl_up_sync(0xFFFFFFFFu, X[S - 1], 1));
+        if (lane == 0) up = s_e[par ^ 1][1 + base];
+        const uint32_t e = x;
+        const uint32_t qc = RANK_MODE ? (i + (e >> 8)) >> 1 : i;  // i, p < 2^24
+        const uint32_t fresh = __byte_perm(e, i, 0x6540u);  // i << 8 | symbol
         {  // the entry at rank r2 after this step (every warp computes the same)
             const bool mv = r2 <= r && !(ca.x > qc);
             x = mv ? (cb.x > qc ? fresh : cb.y) : ca.y;
         }
-        const int d = (int)r - (int)base;
         bool gk = Q[S - 1] > qc;
 #pragma unroll
         for (int k = S - 1; k >= 1; k--) {
             const bool gk1 = Q[k - 1] > qc;
-            const bool mv = k <= d && !gk;
+            const bool mv = r >= base + k && !gk;
             const uint32_t xin = gk1 ? fresh : X[k - 1];
             Q[k] = mv ? min(Q[k - 1], qc) : Q[k];
             X[k] = mv ? xin : X[k];
             gk = gk1;
         }
         {
-            const bool g_up = tid == 0 ? true : up_q > qc;
-            const bool mv = 0 <= d && !gk;
-            Q[0] = mv ? (g_up ? qc : up_q) : Q[0];
-            X[0] = mv ? (g_up ? fresh : up_x) : X[0];
+            const bool mv = r >= base && !gk;
+            Q[0] = mv ? min(up.x, qc) : Q[0];  // up.x > qc: the fresh entry lands here
+            X[0] = mv ? (up.x > qc ? fresh : up.y) : X[0];
         }
-        reinterpret_cast<uint4*>(s_e[par])[tid] = make_uint4(Q[0], X[0], Q[1], X[1]);
+        reinterpret_cast<uint4*>(&s_e[par][2])[tid] = make_uint4(Q[0], X[0], Q[1], X[1]);
         __syncthreads();
-        return sym;
+        return e;
     };
-    uint32_t mine = (uint32_t)lane < n ? src[lane] : 0u;
-    uint32_t nxt = 32u + lane < n ? src[32 + lane] : 0u;
-    uint32_t x = s_e[1][__shfl_sync(0xFFFFFFFFu, mine, 0)].y;
-    load_candidates(__shfl_sync(0xFFFFFFFFu, mine, 1), 1);
+    uint32_t r = rk8[0], r2 = rk8[1];
+    uint32_t x = s_e[1][2 + r].y;
+    load_candidates(r2, 1);
     uint32_t i0 = 0;
     for (; i0 + 32 <= n; i0 += 32) {
-        const uint32_t nn = i0 + 64 + lane < n ? src[i0 + 64 + lane] : 0u;
+        const int rb = (int)(i0 >> 5) & 1;
+        const uint4 m0 = reinterpret_cast<const uint4*>(s_rk[rb])[0], m1 = reinterpret_cast<const uint4*>(s_rk[rb])[1];
+        const uint32_t M[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+        const uint32_t M8 = s_rk[rb ^ 1][0];  // the first ranks of the next round
+        // the ranks of round k + 2, stored into s_rk[k & 1] at step 30: as late as the barrier of step 31 still publishes them to round k + 1,
+        // so that the global load has a round's steps to arrive in
+        const uint32_t nn = warp == 0 && i0 + 64 + lane < n ? src[i0 + 64 + lane] : 0u;
         uint32_t ob = 0;
 #pragma unroll
         for (int j = 0; j < 32; j++) {
-            const uint32_t r = __shfl_sync(0xFFFFFFFFu, mine, j);
-            const uint32_t r2 = j < 31 ? __shfl_sync(0xFFFFFFFFu, mine, (j + 1) & 31) : __shfl_sync(0xFFFFFFFFu, nxt, 0);
-            const uint32_t r3 = j < 30 ? __shfl_sync(0xFFFFFFFFu, mine, (j + 2) & 31) : __shfl_sync(0xFFFFFFFFu, nxt, (j + 2) & 31);
-            const uint32_t sym = step(r, r2, i0 + (uint32_t)j, j & 1, x);  // i0 is a multiple of 32
+            const uint32_t r3 = __byte_perm(j < 30 ? M[(j + 2) >> 2] : M8, 0u, 0x4440u | ((j + 2) & 3));
+            const uint32_t e = step(r, r2, i0 + (uint32_t)j, j & 1, x);  // i0 is a multiple of 32
             load_candidates(r3, j & 1);
-            ob = lane == j ? sym : ob;
+            ob = lane == j ? e : ob;
+            if (j == 30 && warp == 0) rk8[32 * rb + lane] = (uint8_t)nn;
+            r = r2;
+            r2 = r3;
         }
         if (warp == 0) dst[i0 + lane] = (uint8_t)ob;
-        mine = nxt;
-        nxt = nn;
     }
     if (i0 < n) {
+        const uint8_t* rt = rk8 + 32 * ((i0 >> 5) & 1);
         uint32_t ob = 0;
         for (uint32_t j = 0; i0 + j < n; j++) {
-            const uint32_t r = __shfl_sync(0xFFFFFFFFu, mine, (int)j);
-            const uint32_t r2 = j < 31 ? __shfl_sync(0xFFFFFFFFu, mine, (int)((j + 1) & 31)) : 0u;
-            const uint32_t r3 = j < 30 ? __shfl_sync(0xFFFFFFFFu, mine, (int)((j + 2) & 31)) : 0u;
-            const uint32_t sym = step(r, r2, i0 + j, (int)(j & 1), x);
+            const uint32_t r3 = j < 30 ? rt[j + 2] : 0u;
+            const uint32_t e = step(r, r2, i0 + j, (int)(j & 1), x);
             load_candidates(r3, (int)(j & 1));
-            ob = (uint32_t)lane == j ? sym : ob;
+            ob = (uint32_t)lane == j ? e : ob;
+            r = r2;
+            r2 = r3;
         }
         if (warp == 0 && i0 + lane < n) dst[i0 + lane] = (uint8_t)ob;
     }
