@@ -546,7 +546,7 @@ __global__ void __launch_bounds__(32) alias_inv_plan_kernel(const uint8_t* __res
             }
         } else {  // :388-415 digram aliases
             const uint32_t tail = src[1];
-            if (tail > len || 2 + 3 * n > len - tail) err = 1;
+            if (2 + 3 * n > len) err = 1;  // the map is read whole (:415-418); the trailing bytes may overlap it
             if (!err) {
                 for (uint32_t i = 0; i < 256; i++) I.map32[i] = 0x10000u | i;
                 uint32_t si = 2;
@@ -556,7 +556,7 @@ __global__ void __launch_bounds__(32) alias_inv_plan_kernel(const uint8_t* __res
                 }
                 I.mode = 4;
                 I.hdr_len = si;
-                I.src_end = len - tail;
+                I.src_end = tail < len && len - tail > si ? len - tail : si;  // where srcIdx stands after the loop of :420-426
                 I.adjust = tail;
             }
         }

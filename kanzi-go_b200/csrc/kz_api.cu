@@ -4092,6 +4092,7 @@ int kz_transform_inverse(kz_ctx* ctx, uint64_t type, const uint8_t* src, size_t 
         if (n > (1u << 30) + 33) return ctx->fail(KZ_ERR_BLOCK_SIZE, "The max BWT block size is 1 GiB");
         cap = std::min(cap, n);  // the block is shorter than its header + BWT bytes: more room changes nothing
     } else if (type == KZ_T_LZ || type == KZ_T_LZX) {  // LZXCodec.inverseV6
+        if (cap == 0) return 0;  // LZCodec.go:622-624
         if (n > (1u << 30) || cap > (1u << 30) + 64) return ctx->fail(KZ_ERR_BLOCK_SIZE, "block too large");
     } else {
         if (cap == 0) return 0;

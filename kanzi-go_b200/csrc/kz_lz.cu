@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(32) lz_inverse_kernel(const uint8_t* __restric
                     m_len = ml;
                     const long long m_end = dst_idx + lit_len + m_len;
                     const long long ref = dst_idx + lit_len - dist;
-                    if (st == 0 && (ref < 0 || dist > max_dist || dist <= 0 || m_end > dst_end)) st = 2;
+                    if (st == 0 && (ref < 0 || dist > max_dist || m_end > dst_end)) st = 2;  // dist 0 passes, as in the reference
                 }
             }
         }
@@ -431,7 +431,9 @@ __global__ void __launch_bounds__(32) lz_inverse_kernel(const uint8_t* __restric
         if (st == 1) break;
         __syncwarp();
         const long long ref = dst_idx - dist;
-        if (dist >= m_len || dist >= 32) {
+        if (dist == 0) {
+            // the reference copies every byte onto itself (LZCodec.go:762-764): the match keeps what the destination held
+        } else if (dist >= m_len || dist >= 32) {
             // rounds of 32 bytes; a round only reads bytes written by earlier rounds when dist >= 32
             for (long long k0 = 0; k0 < m_len; k0 += 32) {
                 const long long k = k0 + lane;

@@ -187,16 +187,26 @@ __global__ void __launch_bounds__(ZT) zrlt_forward_kernel(const uint8_t* __restr
     }
 }
 
+// The run length of a digit group as ZRLT.go:159-170 computes it: runLength = 1, then runLength = 2 * runLength + digit per digit, in
+// a 64-bit uint. head = the value of the group's digits before these nd (1: none), digits = the last nd digits, nd <= 64. Past 64
+// digits the leading ones have left the word, so the result is the group's value modulo 2^64, as in the reference.
+KZ_D uint64_t zrlt_group_value(uint64_t head, uint64_t digits, uint32_t nd) { return nd >= 64 ? digits : (head << nd) | digits; }
+
 // ---- inverse. The destination block [dst_off, dst_off + cap) must be zero filled by the caller.
-// status: 0 ok, -KZ_E_PROCESS_BLOCK when the output does not fit (the reference returns an error)
+// status: 0 ok, -KZ_E_PROCESS_BLOCK where the reference returns an error (ZRLT.go:172-173, :204-222): a run of zeros longer than the
+// room left, output past cap, or bytes left over once the output is full. The last one decides only when the block's last item writes
+// nothing (a trailing escape with no second byte, or a final group whose value is 0 or 1 modulo 2^64): the reference stops on the
+// full output before it reads that item, and every other last item needs room of its own.
 __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restrict__ data, const ZrltBlock* __restrict__ blocks, int nblocks,
                                                           uint8_t* __restrict__ out, uint32_t* __restrict__ out_len, int32_t* __restrict__ status) {
     __shared__ int64_t s_scan[32];
     __shared__ uint8_t s_cls[ZTILE + 16];  // per byte of the tile: 0 regular, 1 digit 0, 2 digit 1, 3 escape, 4 follower
     __shared__ uint8_t s_first[ZT + 1];
     __shared__ int64_t s_carry_ff;   // position of the last byte != 0xFF before the tile (-1: none)
-    __shared__ uint64_t s_carry_val; // value of the digit group that is open at the tile start (0: none)
+    __shared__ uint64_t s_carry_val; // value of the digit group that is open at the tile start (modulo 2^64)
+    __shared__ int s_carry_open;     // 1: a digit group is open at the tile start
     __shared__ uint64_t s_carry_off;
+    __shared__ int s_bad, s_last_empty;
     const ZrltBlock blk = blocks[blockIdx.x];
     if (!blk.active) return;
     const uint8_t* src = data + blk.src_off;
@@ -206,7 +216,10 @@ __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restr
     if (tid == 0) {
         s_carry_ff = -1;
         s_carry_val = 0;
+        s_carry_open = 0;
         s_carry_off = 0;
+        s_bad = 0;
+        s_last_empty = 0;
     }
     __syncthreads();
     for (uint64_t base = 0; base < n; base += ZTILE) {
@@ -268,6 +281,7 @@ __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restr
         __syncthreads();
         // ---- output bytes per input byte: followers and regular bytes 1; the last digit of a group: value - 1 zeros
         const uint64_t carry_val = s_carry_val;
+        const bool carry_open = s_carry_open != 0;
         uint64_t adv[ZB];
         uint64_t mine = 0;
         bool bad = false;
@@ -291,16 +305,17 @@ __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restr
                             nd++;
                             j--;
                         }
-                        uint64_t head = 1;
-                        if (j < 0) head = carry_val ? carry_val : 1;
-                        if (nd >= 40 || head >= (1ull << 22)) {
-                            bad = true;  // a run longer than any block: corrupt input
-                        } else {
-                            const uint64_t v = (head << nd) | digits;
-                            a = v - 1;
+                        const uint64_t head = j < 0 && carry_open ? carry_val : 1;
+                        const uint64_t v = zrlt_group_value(head, digits, nd);
+                        // value 0: inside the stream runLength-- wraps to 2^64 - 1 (:170-173); at its end the group is skipped (:205)
+                        a = v == 0 && p0 + k + 1 == n ? 0 : v - 1;
+                        if (a > cap) {
+                            bad = true;  // more zeros than the block holds
+                            a = 0;
                         }
                     }
                 }
+                if (p0 + k + 1 == n && (c == 3 || ((c == 1 || c == 2) && a == 0))) s_last_empty = 1;
             }
             adv[k] = a;
             mine += a;
@@ -320,13 +335,14 @@ __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restr
                 o += adv[k];
             }
         }
-        if (bad) status[blockIdx.x] = -KZ_E_PROCESS_BLOCK;
+        if (bad) s_bad = 1;
         __syncthreads();
         if (tid == ZT - 1) {
             s_carry_off = carry_off + incl_off;
             s_carry_ff = incl_ff < -1 ? carry_ff : incl_ff;
             // digit group still open at the end of the tile?
             uint64_t open = 0;
+            int is_open = 0;
             const uint8_t lc = s_cls[ZTILE - 1];
             if (base + ZTILE < n && (lc == 1 || lc == 2) && (s_cls[ZTILE] == 1 || s_cls[ZTILE] == 2)) {
                 uint64_t digits = 0;
@@ -337,17 +353,18 @@ __global__ void __launch_bounds__(ZT) zrlt_inverse_kernel(const uint8_t* __restr
                     nd++;
                     j--;
                 }
-                uint64_t head = 1;
-                if (j < 0) head = carry_val ? carry_val : 1;
-                open = (nd >= 40 || head >= (1ull << 22)) ? (1ull << 40) : ((head << nd) | digits);
+                open = zrlt_group_value(j < 0 && carry_open ? carry_val : 1, digits, nd);
+                is_open = 1;
             }
             s_carry_val = open;
+            s_carry_open = is_open;
         }
         __syncthreads();
     }
     if (tid == 0) {
         const uint64_t total = s_carry_off;
-        if (total > cap) status[blockIdx.x] = -KZ_E_PROCESS_BLOCK;
+        const bool fail = s_bad || total > cap || (s_last_empty && total >= cap);
+        status[blockIdx.x] = fail ? -KZ_E_PROCESS_BLOCK : 0;
         out_len[blockIdx.x] = (uint32_t)(total > cap ? cap : total);
     }
 }

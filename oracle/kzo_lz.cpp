@@ -249,7 +249,7 @@ bool lz_forward(Ctx& ctx, bool extra, const uint8_t* src, size_t n, uint8_t* dst
 }
 
 bool lz_inverse(Ctx&, bool, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_n) {
-    if (n == 0) {
+    if (n == 0 || cap == 0) {  // :622-624
         *out_n = 0;
         return true;
     }

@@ -140,7 +140,7 @@ bool alias_forward(Ctx& ctx, bool only_dna, const uint8_t* src, size_t count, ui
 
 bool alias_inverse(const uint8_t* src, size_t len, uint8_t* dst, size_t cap, size_t* out_n) {
     *out_n = 0;
-    if (len == 0) return true;
+    if (len == 0 || cap == 0) return true;  // :298-300
     if (len < 2) return false;
     int n = src[0];
     if (n < 16) return false;
@@ -193,8 +193,8 @@ bool alias_inverse(const uint8_t* src, size_t len, uint8_t* dst, size_t cap, siz
         }
     } else {
         int map16[256];
-        if (size_t(src[1]) > len || 2 + 3 * size_t(n) > len) return false;
-        const size_t src_end = len - src[1];
+        if (2 + 3 * size_t(n) > len) return false;  // the map is read whole (:415-418); src[1] may reach into it or past the start (:408)
+        const size_t src_end = size_t(src[1]) < len ? len - src[1] : 0;
         src_idx = 2;
         for (int i = 0; i < 256; i++) map16[i] = 0x10000 | i;
         for (int i = 0; i < n; i++) {
@@ -314,7 +314,7 @@ bool fsd_forward(Ctx& ctx, const uint8_t* src, size_t n, uint8_t* dst, size_t ca
 
 bool fsd_inverse(const uint8_t* src, size_t len, uint8_t* dst, size_t cap, size_t* out_n) {
     *out_n = 0;
-    if (len == 0) return true;
+    if (len == 0 || cap == 0) return true;  // :327-329
     if (len < 2) return false;
     const uint8_t mode = src[0];
     const int dist = src[1];

@@ -126,10 +126,12 @@ def transform_forward(ttype, data, data_type=0, block_size=0):
     return out[: n.value].copy(), dt.value
 
 
-def transform_inverse(ttype, data, cap, data_type=0, block_size=0):
+def transform_inverse(ttype, data, cap, data_type=0, block_size=0, fill=None):
+    """fill: the byte the destination holds before the call (None: whatever np.empty gives). A stream can make the reference copy
+    destination bytes it never wrote (an LZ match of distance 0), so its output depends on them."""
     a = _arr(data)
     lib().kzo_set_stream_block_size(block_size)
-    out = np.empty(max(cap, 1), np.uint8)
+    out = np.empty(max(cap, 1), np.uint8) if fill is None else np.full(max(cap, 1), fill, np.uint8)
     n = C.c_size_t(0)
     rc = lib().kzo_transform_inverse(ttype, data_type, _ptr(a), a.size, out.ctypes.data, cap, C.byref(n))
     if rc:
