@@ -200,7 +200,10 @@ uint32_t kz_stage_bytes(kz_ctx* ctx, const char* name, uint64_t* bytes_in, uint6
 size_t kz_profile_names(kz_ctx* ctx, char* buf, size_t cap);
 /* BWT forward doubling rounds of this context (a profiling aid; the default is 0 and the output bytes never depend on it):
  * bit 0: with kz_profile(ctx,1), time every round's parts under "bwt_round:<r>:<part>" (parts: small, sort, large, select, gap);
- * bit 1: run the 56-bit global sort in every round, also where the blocks would take the small-group / narrow-key rounds. */
+ * bit 1: run the 56-bit global sort in every round, also where the blocks would take the small-group / narrow-key rounds.
+ * The same bit 0 times the parts of every BWT inverse under "bwt_inverse:<part>" (parts: sort, walk, doubling, copy, sync), and bits 8-19
+ * set the shape of the inverse's walk (0 in a field = its default): bits 8-11 log2 of the sub-list stride (32), bits 12-19 the staging
+ * bytes per sub-list / 16 (128 bytes). */
 void kz_bwt_profile(kz_ctx* ctx, int flags);
 
 /* ctx["blockSize"] of the stream the following kz_encode_blocks / kz_transform_forward / kz_transform_inverse calls belong to

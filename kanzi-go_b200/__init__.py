@@ -702,9 +702,17 @@ class Context:
         self.lib.kz_profile_names(self.h, buf, n + 16)
         return [x for x in buf.value.decode().split("\n") if x]
 
-    def bwt_profile(self, time_rounds=False, wide_rounds=False):
-        """BWT forward rounds (kz_bwt_profile): time every round under "bwt_round:<r>:<part>" / run the 56-bit global sort in every round"""
-        self.lib.kz_bwt_profile(self.h, (1 if time_rounds else 0) | (2 if wide_rounds else 0))
+    def bwt_profile(self, time_rounds=False, wide_rounds=False, inverse_stride=0, inverse_stage=0):
+        """BWT forward rounds (kz_bwt_profile): time every round under "bwt_round:<r>:<part>" (and the inverse's parts under
+        "bwt_inverse:<part>") / run the 56-bit global sort in every round / the inverse's sub-list stride (a power of two) and staging
+        bytes per sub-list (a multiple of 16); 0 = the default of each"""
+        lg = inverse_stride.bit_length() - 1 if inverse_stride else 0
+        if inverse_stride and (1 << lg) != inverse_stride or not 0 <= lg < 16:
+            raise ValueError("inverse_stride must be a power of two below 65536")
+        if inverse_stage % 16 or not 0 <= inverse_stage // 16 < 256:
+            raise ValueError("inverse_stage must be a multiple of 16 below 4096")
+        flags = (1 if time_rounds else 0) | (2 if wide_rounds else 0) | (lg << 8) | ((inverse_stage // 16) << 12)
+        self.lib.kz_bwt_profile(self.h, flags)
 
     def launch_count(self, reset=False):
         return self.lib.kz_launch_count(self.h, 1 if reset else 0)

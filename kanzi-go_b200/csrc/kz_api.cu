@@ -1592,6 +1592,14 @@ int apply_forward(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint64_t istride
     return 0;
 }
 
+// kz_bwt_profile bits 8-19: the shape of the BWT inverse's walk (a profiling aid; 0 = the default of each field)
+IbwtShape ibwt_shape(const kz_ctx* ctx) {
+    IbwtShape sh;
+    const uint32_t f = (uint32_t)ctx->bwt_profile;
+    if (const uint32_t lg = (f >> 8) & 15) sh.stride = 1u << std::max(lg, 1u);
+    if (const uint32_t st = (f >> 12) & 255) sh.stage = st * 16;
+    return sh;
+}
 // One inverse stage, mirror of apply_forward. cap = capacity of a destination block; bs[b] = 0: TEXT takes cap as ctx["blockSize"].
 int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, uint64_t stride, uint32_t cap, std::vector<uint32_t>& len,
                   const std::vector<uint8_t>& active, const std::vector<uint64_t>& bs) {
@@ -1607,6 +1615,7 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
             std::vector<uint32_t> ll, num;
             std::vector<uint8_t> hh;
             uint64_t total = 0;
+            uint32_t max_len = 0;
             uint32_t b = b0;
             for (; b < nblocks; b++) {
                 if (!active[b]) continue;
@@ -1614,14 +1623,18 @@ int apply_inverse(kz_ctx* ctx, uint64_t t, const uint8_t* d_in, uint8_t* d_out, 
                 so.push_back(b * stride), dof.push_back(b * stride), ll.push_back(len[b]), num.push_back(b);
                 hh.insert(hh.end(), heads.begin() + (size_t)b * 64, heads.begin() + (size_t)(b + 1) * 64);
                 total += len[b];
+                max_len = std::max(max_len, len[b]);
             }
             b0 = b;
             if (ll.empty()) continue;
-            CK(ctx->d_ws.ensure(bwt_inverse_batch_workspace(total, (uint32_t)ll.size())));
+            const IbwtShape shape = ibwt_shape(ctx);
+            CK(ctx->d_ws.ensure(bwt_inverse_batch_workspace(total, (uint32_t)ll.size(), max_len, shape)));
             std::vector<uint32_t> produced(ll.size(), 0);
             LaunchScope ls(ctx, "bwt_inverse");
+            CtxLzHook parts(ctx);  // kz_bwt_profile bit 0: the parts timed under their own names
             cudaError_t e = bwt_inverse_batch(d_in, d_out, so.data(), dof.data(), ll.data(), hh.data(), (uint32_t)ll.size(), cap, produced.data(),
-                                              ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches);
+                                              ctx->d_ws.as<uint8_t>(), ctx->d_ws.cap, ctx->stream, &ctx->launches, shape,
+                                              (ctx->profile && (ctx->bwt_profile & 1)) ? &parts : nullptr);
             if (e == cudaErrorInvalidValue) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "BWT inverse transform failed: invalid header or data");
             if (e != cudaSuccess) return ctx->cuda_fail(e, "bwt_inverse");
             for (size_t k = 0; k < num.size(); k++) len[num[k]] = produced[k];

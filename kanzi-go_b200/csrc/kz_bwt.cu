@@ -10,9 +10,9 @@
 //     (cub::DeviceRadixSort for the sort itself; everything else is hand written).
 //   transform/BWT.go:178-358 Inverse (inverseMergeTPSI) / :361-628 (biPSIv2): both walk the permutation
 //     "rank of suffix i -> rank of suffix i+1" from primaryIndex(0)-1. The format only offers 8 independent walks,
-//     far too few for a GPU, so the permutation list is cut at every rank that is a multiple of 64 (plus the 8 primary
-//     ranks): all sub-lists are walked in parallel once to measure them, the few thousand sub-list heads are ranked with
-//     pointer doubling, and a second parallel walk writes the bytes at their final offsets.
+//     far too few for a GPU, so the permutation list is cut at every rank that is a multiple of 32 (plus the 8 primary
+//     ranks): all sub-lists are walked in parallel once, their bytes staged per sub-list, the sub-list heads are ranked
+//     with pointer doubling, and the staged bytes are copied to their final offsets.
 //   transform/BWTBlockCodec.go:78-136, :141-225: block header (mode byte + big-endian primaryIndex-1 per chunk).
 #include <cub/device/device_radix_sort.cuh>
 #include <thrust/iterator/reverse_iterator.h>
@@ -195,8 +195,6 @@ __global__ void bwt_header_kernel(const uint32_t* __restrict__ primary, uint32_t
 }
 
 // ---------------- inverse ----------------
-static const uint32_t IBWT_STRIDE = 64;  // a sub-list starts at every rank that is a multiple of this (1024 left < 1 warp per SM for a 4 MiB block)
-
 // Wyllie pointer doubling over the heads: after the rounds dist[j] = number of bytes from head j to the end of the list
 __global__ void ibwt_jump_kernel(const uint32_t* __restrict__ succ_in, const uint64_t* __restrict__ dist_in, uint32_t nheads, uint32_t* __restrict__ succ_out,
                                  uint64_t* __restrict__ dist_out) {
@@ -897,10 +895,16 @@ cudaError_t bwt_forward_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
 }
 
 // ---- inverse, all blocks of a batch together ---------------------------------------------------------------------------------------------------
-// The inverse of the file header (LF mapping by a stable sort, sub-lists cut every IBWT_STRIDE ranks, heads ranked by pointer doubling) in
+// The inverse of the file header (LF mapping by a stable sort, sub-lists cut every `stride` ranks, heads ranked by pointer doubling) in
 // one position space for the batch (block b = [base, base + n)), the block index above the byte in the key of the stable sort (so the LF
-// mapping of block b lands in its own range), one head list for all blocks, one set of launches: a 4 MiB block is 17 pointer-doubling
+// mapping of block b lands in its own range), one head list for all blocks, one set of launches: a 4 MiB block is 18 pointer-doubling
 // launches of a few hundred threads each, so blocks inverted one after another would be mostly launch latency.
+// The value that travels with the sort key is already the LF word the walk reads: (byte << 24) | local successor in 32 bits while every
+// block has fewer than 2^24 bytes, (byte << 32) | local successor in 64 bits above that, so one random load per position gives both the
+// successor and the output byte. Each head walks its sub-list once: the first `stage` bytes go to the head's staging slot in order, the
+// length, the successor head and (for a longer sub-list) the node after the slot are recorded; once pointer doubling has given every head
+// its output offset, the slots are copied to the output with coalesced stores and only the few sub-lists longer than their slot are walked
+// again, from the recorded node on.
 namespace {
 struct IbwtBatchBlock {
     uint64_t src_off, dst_off;  // BWT bytes (behind the header) / output
@@ -910,6 +914,27 @@ struct IbwtBatchBlock {
     uint32_t prim[8];           // primary ranks (local), 0xFFFFFFFF when absent
 };
 const int IBWT_BATCH_MAX = 1024;
+const uint32_t IBWT_NARROW_MAX_N = 0xFFFFFF;  // largest block of the 32-bit words: local ranks 0 .. n - 1 and the end mark in 24 bits
+template <typename W>
+struct IbwtWord;
+template <>
+struct IbwtWord<uint32_t> {
+    static constexpr int SHIFT = 24;
+    static constexpr uint32_t END = 0xFFFFFFu;  // successor of the last position of the block's list
+};
+template <>
+struct IbwtWord<uint64_t> {
+    static constexpr int SHIFT = 32;
+    static constexpr uint32_t END = 0xFFFFFFFFu;
+};
+template <typename W>
+__device__ __forceinline__ uint32_t ibwtb_next(W w) {
+    return (uint32_t)(w & ((W(1) << IbwtWord<W>::SHIFT) - 1));
+}
+template <typename W>
+__device__ __forceinline__ uint32_t ibwtb_byte(W w) {
+    return (uint32_t)(w >> IbwtWord<W>::SHIFT);
+}
 __device__ __forceinline__ uint32_t ibwtb_find(const uint32_t* __restrict__ s_base, uint32_t nb, uint32_t i) {
     uint32_t lo = 0, hi = nb;
     while (hi - lo > 1) {
@@ -919,8 +944,9 @@ __device__ __forceinline__ uint32_t ibwtb_find(const uint32_t* __restrict__ s_ba
     }
     return lo;
 }
+template <typename W>
 __global__ void __launch_bounds__(256) ibwtb_init_kernel(const uint8_t* __restrict__ in, const IbwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t total,
-                                                          uint16_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+                                                          uint16_t* __restrict__ keys, W* __restrict__ vals) {
     __shared__ uint32_t s_base[IBWT_BATCH_MAX];
     for (uint32_t k = threadIdx.x; k < nb; k += 256) s_base[k] = blocks[k].base;
     __syncthreads();
@@ -930,98 +956,224 @@ __global__ void __launch_bounds__(256) ibwtb_init_kernel(const uint8_t* __restri
     const IbwtBatchBlock& B = blocks[b];
     const uint32_t i = g - B.base;
     const uint32_t pidx = B.prim[0] + 1;
-    keys[g] = (uint16_t)((b << 8) | in[B.src_off + i]);
-    vals[g] = i == 0 ? 0xFFFFFFFFu : B.base + (i < pidx ? i - 1 : i);
+    const uint8_t c = in[B.src_off + i];
+    keys[g] = (uint16_t)((b << 8) | c);
+    vals[g] = ((W)c << IbwtWord<W>::SHIFT) | (i == 0 ? IbwtWord<W>::END : (i < pidx ? i - 1 : i));
 }
-__device__ __forceinline__ bool ibwtb_is_head(uint32_t t_local, const IbwtBatchBlock& B) {
-    if ((t_local & (IBWT_STRIDE - 1)) == 0) return true;
+__device__ __forceinline__ bool ibwtb_is_head(uint32_t t_local, const IbwtBatchBlock& B, uint32_t mask) {
+    if ((t_local & mask) == 0) return true;
     for (uint32_t k = 0; k < B.nprim; k++)
         if (t_local == B.prim[k]) return true;
     return false;
 }
-__device__ __forceinline__ uint32_t ibwtb_head_id(uint32_t t_local, const IbwtBatchBlock& B) {
-    if ((t_local & (IBWT_STRIDE - 1)) == 0) return B.hbase + t_local / IBWT_STRIDE;
+__device__ __forceinline__ uint32_t ibwtb_head_id(uint32_t t_local, const IbwtBatchBlock& B, uint32_t shift) {
+    if ((t_local & ((1u << shift) - 1)) == 0) return B.hbase + (t_local >> shift);
     for (uint32_t k = 0; k < B.nprim; k++)
         if (t_local == B.prim[k]) return B.hbase + B.nstride + k;
     return 0xFFFFFFFFu;
 }
-__global__ void __launch_bounds__(256) ibwtb_measure_kernel(const uint32_t* __restrict__ next, const IbwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t nheads,
-                                                             uint32_t* __restrict__ succ, uint32_t* __restrict__ len, uint64_t* __restrict__ dist0, uint32_t* __restrict__ bad) {
+// heads j0 .. j1 - 1, one thread per head: walk the sub-list once; the first `stage` bytes into the head's slot, resume[j] = the node after them.
+// CTAs are launched in head order, so the LF words of the resident threads come from a few consecutive blocks at a time.
+template <typename W>
+__global__ void __launch_bounds__(256) ibwtb_walk_kernel(const W* __restrict__ words, const IbwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t nheads,
+                                                          uint32_t shift, uint32_t stage, uint32_t* __restrict__ succ, uint32_t* __restrict__ len,
+                                                          uint64_t* __restrict__ dist0, uint32_t* __restrict__ resume, uint8_t* __restrict__ slots,
+                                                          uint32_t* __restrict__ bad) {
     __shared__ uint32_t s_hbase[IBWT_BATCH_MAX];
     for (uint32_t k = threadIdx.x; k < nb; k += 256) s_hbase[k] = blocks[k].hbase;
     __syncthreads();
     const uint32_t j = blockIdx.x * 256 + threadIdx.x;
     if (j >= nheads) return;
-    const uint32_t b = ibwtb_find(s_hbase, nb, j);
-    const IbwtBatchBlock B = blocks[b];
-    const uint32_t jl = j - B.hbase;
-    uint32_t t = jl < B.nstride ? jl * IBWT_STRIDE : B.prim[jl - B.nstride];
-    if (t >= B.n || (jl >= B.nstride && (t & (IBWT_STRIDE - 1)) == 0)) {  // duplicate head or out of range
+    const IbwtBatchBlock& B = blocks[ibwtb_find(s_hbase, nb, j)];
+    const uint32_t n = B.n, hbase = B.hbase, nstride = B.nstride, nprim = B.nprim, mask = (1u << shift) - 1;
+    uint32_t prim[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) prim[k] = B.prim[k];
+    const uint32_t jl = j - hbase;
+    uint32_t t = jl << shift;
+#pragma unroll
+    for (int k = 0; k < 8; k++)
+        if (jl == nstride + k) t = prim[k];
+    if (t >= n || (jl >= nstride && (t & mask) == 0)) {  // duplicate head or out of range
         succ[j] = 0xFFFFFFFEu;
         len[j] = 0;
         dist0[j] = 0;
         return;
     }
-    uint32_t l = 0;
-    uint32_t g = B.base + t;
+    const W* __restrict__ wb = words + B.base;
+    uint32_t* __restrict__ slot = (uint32_t*)(slots + (size_t)j * stage);
+    uint32_t l = 0, acc = 0, cur = t, s = 0xFFFFFFFFu;
     for (;;) {
-        g = next[g];
-        l++;
-        if (g == 0xFFFFFFFFu) {
-            succ[j] = 0xFFFFFFFFu;
-            break;
+        const W w = wb[cur];
+        const uint32_t nx = ibwtb_next(w);
+        if (l < stage) {
+            acc |= ibwtb_byte(w) << ((l & 3) * 8);
+            if ((l & 3) == 3) {
+                slot[l >> 2] = acc;
+                acc = 0;
+            }
         }
-        const uint32_t tl = g - B.base;
-        if (g < B.base || tl >= B.n || l > B.n) {  // corrupt permutation
-            succ[j] = 0xFFFFFFFDu;
+        l++;
+        if (l == stage) resume[j] = nx;
+        if (nx == IbwtWord<W>::END) break;
+        if (nx >= n || l > n) {  // corrupt permutation
+            s = 0xFFFFFFFDu;
             *bad = 1;
             break;
         }
-        if (ibwtb_is_head(tl, B)) {
-            succ[j] = ibwtb_head_id(tl, B);
+        if ((nx & mask) == 0) {
+            s = hbase + (nx >> shift);
             break;
         }
+#pragma unroll
+        for (int k = 7; k >= 0; k--)  // the first of equal primary ranks owns the head
+            if (k < (int)nprim && nx == prim[k]) s = hbase + nstride + k;
+        if (s != 0xFFFFFFFFu) break;
+        cur = nx;
     }
+    if ((l & 3) != 0 && l < stage) slot[l >> 2] = acc;
+    succ[j] = s;
     len[j] = l;
     dist0[j] = l;
 }
-__global__ void __launch_bounds__(256) ibwtb_write_kernel(const uint32_t* __restrict__ next, const uint16_t* __restrict__ first, const IbwtBatchBlock* __restrict__ blocks,
-                                                           uint32_t nb, uint32_t nheads, const uint32_t* __restrict__ succ0, const uint32_t* __restrict__ len,
-                                                           const uint64_t* __restrict__ dist, uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
+// thread per head: its offset (corrupt input reported); then the warp copies the slots of its 32 heads one after another with coalesced
+// loads and stores, and a head whose sub-list is longer than the slot walks on from the recorded node
+template <typename W>
+__global__ void __launch_bounds__(256) ibwtb_copy_kernel(const W* __restrict__ words, const IbwtBatchBlock* __restrict__ blocks, uint32_t nb, uint32_t nheads,
+                                                          uint32_t shift, uint32_t stage, const uint32_t* __restrict__ succ0, const uint32_t* __restrict__ len,
+                                                          const uint64_t* __restrict__ dist, const uint32_t* __restrict__ resume,
+                                                          const uint8_t* __restrict__ slots, uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
     __shared__ uint32_t s_hbase[IBWT_BATCH_MAX];
     for (uint32_t k = threadIdx.x; k < nb; k += 256) s_hbase[k] = blocks[k].hbase;
     __syncthreads();
-    const uint32_t j = blockIdx.x * 256 + threadIdx.x;
-    if (j >= nheads) return;
-    if (succ0[j] == 0xFFFFFFFEu) return;
-    const uint32_t b = ibwtb_find(s_hbase, nb, j);
-    const IbwtBatchBlock B = blocks[b];
-    const uint32_t jl = j - B.hbase;
-    const uint32_t t = jl < B.nstride ? jl * IBWT_STRIDE : B.prim[jl - B.nstride];
-    const uint64_t d = dist[j];
-    if (d > B.n) {  // head not on the main list (corrupt input: the permutation has more than one cycle)
-        *bad = 1;
-        return;
+    const uint32_t j = blockIdx.x * 256 + threadIdx.x, lane = threadIdx.x & 31;
+    uint32_t m = 0, l = 0, n = 0, base = 0;
+    uint64_t off = 0;
+    uint8_t* dst = out;
+    if (j < nheads && succ0[j] != 0xFFFFFFFEu) {
+        const IbwtBatchBlock& B = blocks[ibwtb_find(s_hbase, nb, j)];
+        n = B.n, base = B.base;
+        const uint32_t jl = j - B.hbase;
+        const uint32_t t = jl < B.nstride ? jl << shift : B.prim[jl - B.nstride];
+        const uint64_t d = dist[j];
+        // corrupt input: a head not on the list that ends the block (the permutation has more than one cycle), or the list that starts at
+        // the first primary rank (the one rank no position points to) does not run through all n ranks
+        if (d > n || (t == B.prim[0] && d != n)) {
+            *bad = 1;
+        } else {
+            dst = out + B.dst_off;
+            off = (uint64_t)n - d;
+            l = len[j];
+            m = min(l, stage);
+        }
     }
-    uint8_t* dst = out + B.dst_off;
-    const uint64_t off = (uint64_t)B.n - d;
-    const uint32_t l = len[j];
-    uint32_t g = B.base + t;
-    for (uint32_t i = 0; i < l; i++) {
-        if (off + i < B.n) dst[off + i] = (uint8_t)first[g];
-        g = next[g];
-        if (g - B.base >= B.n) break;
+    for (uint32_t q = 0; q < 32; q++) {
+        const uint32_t mq = __shfl_sync(0xFFFFFFFFu, m, q);
+        if (mq == 0) continue;
+        const uint32_t nq = __shfl_sync(0xFFFFFFFFu, n, q);
+        const uint64_t oq = ((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)(off >> 32), q) << 32) | __shfl_sync(0xFFFFFFFFu, (uint32_t)off, q);
+        uint8_t* const dq = (uint8_t*)(((uint64_t)__shfl_sync(0xFFFFFFFFu, (uint32_t)((uint64_t)dst >> 32), q) << 32) |
+                                       __shfl_sync(0xFFFFFFFFu, (uint32_t)(uint64_t)dst, q));
+        const uint32_t* __restrict__ slot = (const uint32_t*)(slots + (size_t)(j - lane + q) * stage);
+        for (uint32_t w = lane; w * 4 < mq; w += 32) {
+            const uint32_t v = slot[w];
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++) {
+                const uint32_t i = w * 4 + k;
+                if (i < mq && oq + i < nq) dq[oq + i] = (uint8_t)(v >> (8 * k));
+            }
+        }
     }
+    if (l <= stage) return;
+    const W* __restrict__ wb = words + base;
+    uint32_t cur = resume[j];
+    for (uint32_t i = stage; i < l && cur < n; i++) {
+        const W w = wb[cur];
+        if (off + i < n) dst[off + i] = (uint8_t)ibwtb_byte(w);
+        cur = ibwtb_next(w);
+    }
+}
+bool ibwtb_wide(uint32_t max_n) { return max_n > IBWT_NARROW_MAX_N; }
+size_t ibwtb_sort_temp(uint64_t total, bool wide) {
+    size_t temp = 0;
+    cub::DoubleBuffer<uint16_t> k(nullptr, nullptr);
+    if (wide) {
+        cub::DoubleBuffer<uint64_t> v(nullptr, nullptr);
+        cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int64_t)total, 0, 16);
+    } else {
+        cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
+        cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int64_t)total, 0, 16);
+    }
+    return temp;
+}
+struct IbwtBufs {
+    uint16_t *keys_a, *keys_b;
+    void *val_a, *val_b;
+    uint32_t *succ_a, *succ_b, *succ0, *lenv, *resume, *bad;
+    uint64_t *dist_a, *dist_b;
+    uint8_t* slots;
+    IbwtBatchBlock* blocks;
+    void* temp;
+    size_t temp_bytes;
+};
+template <typename W>
+cudaError_t ibwtb_run(const uint8_t* d_in, uint8_t* d_out, const std::vector<IbwtBatchBlock>& hb, uint32_t total, uint32_t nheads, const IbwtBufs& U,
+                      const IbwtShape& shape, cudaStream_t stream, uint64_t* launches, LzHook* hook) {
+    const uint32_t nbb = (uint32_t)hb.size(), T = 256, G = (total + T - 1) / T, GH = (nheads + T - 1) / T;
+    uint32_t shift = 0;
+    while ((1u << shift) < shape.stride) shift++;
+    cudaError_t e;
+    const W* words;
+    {
+        LzHookScope hs(hook, "bwt_inverse:sort");
+        ibwtb_init_kernel<W><<<G, T, 0, stream>>>(d_in, U.blocks, nbb, total, U.keys_a, (W*)U.val_a);
+        cub::DoubleBuffer<uint16_t> k(U.keys_a, U.keys_b);
+        cub::DoubleBuffer<W> v((W*)U.val_a, (W*)U.val_b);
+        size_t tb = U.temp_bytes;
+        int key_bits = 8;
+        while ((1u << (key_bits - 8)) < nbb) key_bits++;
+        if ((e = cub::DeviceRadixSort::SortPairs(U.temp, tb, k, v, (int64_t)total, 0, key_bits, stream)) != cudaSuccess) return e;  // stable: LF mapping per block
+        words = v.Current();
+        (*launches) += 5;
+    }
+    {
+        LzHookScope hs(hook, "bwt_inverse:walk");
+        ibwtb_walk_kernel<W><<<GH, T, 0, stream>>>(words, U.blocks, nbb, nheads, shift, shape.stage, U.succ0, U.lenv, U.dist_a, U.resume, U.slots, U.bad);
+        (*launches)++;
+    }
+    uint32_t* succ_a = U.succ_a;
+    uint32_t* succ_b = U.succ_b;
+    uint64_t* dist_a = U.dist_a;
+    uint64_t* dist_b = U.dist_b;
+    {
+        LzHookScope hs(hook, "bwt_inverse:doubling");
+        if ((e = cudaMemcpyAsync(succ_a, U.succ0, (size_t)nheads * 4, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess) return e;
+        uint32_t max_heads = 1;
+        for (const IbwtBatchBlock& B : hb) max_heads = std::max(max_heads, B.nstride + B.nprim);
+        uint32_t rounds = 1;
+        while ((1u << rounds) < max_heads) rounds++;
+        for (uint32_t r = 0; r < rounds + 1; r++) {
+            ibwt_jump_kernel<<<GH, T, 0, stream>>>(succ_a, dist_a, nheads, succ_b, dist_b);
+            std::swap(succ_a, succ_b);
+            std::swap(dist_a, dist_b);
+            (*launches)++;
+        }
+    }
+    {
+        LzHookScope hs(hook, "bwt_inverse:copy");
+        ibwtb_copy_kernel<W><<<GH, T, 0, stream>>>(words, U.blocks, nbb, nheads, shift, shape.stage, U.succ0, U.lenv, dist_a, U.resume, U.slots,
+                                                                 d_out, U.bad);
+        (*launches)++;
+    }
+    return cudaGetLastError();
 }
 }  // namespace
 
-size_t bwt_inverse_batch_workspace(uint64_t total, uint32_t nblocks) {
-    size_t temp = 0;
-    cub::DoubleBuffer<uint16_t> k(nullptr, nullptr);
-    cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
-    cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int64_t)total, 0, 16);
-    const size_t nheads = (size_t)total / IBWT_STRIDE + (size_t)nblocks * 10 + 16;
-    return (size_t)total * (2 * 2 + 4 * 2) + nheads * (4 * 4 + 8 * 2) + (size_t)nblocks * sizeof(IbwtBatchBlock) + 17 * 256 + temp + 4096;
+size_t bwt_inverse_batch_workspace(uint64_t total, uint32_t nblocks, uint32_t max_len, const IbwtShape& shape) {
+    const bool wide = ibwtb_wide(max_len);
+    const size_t nheads = (size_t)total / shape.stride + (size_t)nblocks * 10 + 16;
+    return (size_t)total * (2 * 2 + (wide ? 8 : 4) * 2) + nheads * (4 * 5 + 8 * 2 + shape.stage) + (size_t)nblocks * sizeof(IbwtBatchBlock) + 17 * 256 +
+           ibwtb_sort_temp(total, wide) + 4096;
 }
 uint64_t bwt_inverse_batch_max_total() { return (1ull << 31) - 1; }
 uint32_t bwt_inverse_batch_max_blocks() { return 256; }  // 8 bits of block index above the byte in a 16-bit key
@@ -1029,12 +1181,15 @@ uint32_t bwt_inverse_batch_max_blocks() { return 256; }  // 8 bits of block inde
 // BWTBlockCodec.Inverse of blocks k = 0..nb-1: stream at d_in + src_off[k] (len_of[k] bytes), h_headers + 64 k = its first 33 bytes on the host.
 // out_len[k] = decoded length. cudaErrorInvalidValue: a malformed header (checked before anything is launched).
 cudaError_t bwt_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_t* src_off, const uint64_t* dst_off, const uint32_t* len_of, const uint8_t* h_headers,
-                              uint32_t nb, uint32_t cap, uint32_t* out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches) {
+                              uint32_t nb, uint32_t cap, uint32_t* out_len, uint8_t* ws, size_t ws_bytes, cudaStream_t stream, uint64_t* launches,
+                              const IbwtShape& shape, LzHook* hook) {
     if (nb == 0) return cudaSuccess;
     if (nb > bwt_inverse_batch_max_blocks()) return cudaErrorInvalidValue;
+    if (shape.stride < 2 || (shape.stride & (shape.stride - 1)) || shape.stage < 4 || (shape.stage & 3)) return cudaErrorInvalidValue;
     std::vector<IbwtBatchBlock> hb;
     hb.reserve(nb);
     uint64_t total64 = 0, heads64 = 0;
+    uint32_t max_n = 0;
     struct Tiny {
         uint64_t src, dst;
     };
@@ -1068,9 +1223,10 @@ cudaError_t bwt_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
             continue;
         }
         B.src_off = src_off[k] + header, B.dst_off = dst_off[k], B.base = (uint32_t)total64, B.n = n;
-        B.hbase = (uint32_t)heads64, B.nstride = (n + IBWT_STRIDE - 1) / IBWT_STRIDE, B.nprim = chunks, B.pad = 0;
+        B.hbase = (uint32_t)heads64, B.nstride = (n + shape.stride - 1) / shape.stride, B.nprim = chunks, B.pad = 0;
         total64 += n;
         heads64 += B.nstride + B.nprim;
+        max_n = std::max(max_n, n);
         hb.push_back(B);
     }
     cudaError_t e;
@@ -1078,57 +1234,43 @@ cudaError_t bwt_inverse_batch(const uint8_t* d_in, uint8_t* d_out, const uint64_
         if ((e = cudaMemcpyAsync(d_out + t.dst, d_in + t.src, 1, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess) return e;
     if (hb.empty()) return cudaSuccess;
     if (total64 > bwt_inverse_batch_max_total()) return cudaErrorInvalidValue;
+    const bool wide = ibwtb_wide(max_n);
+    const size_t wb = wide ? 8 : 4;
     const uint32_t total = (uint32_t)total64, nheads = (uint32_t)heads64, nbb = (uint32_t)hb.size();
     auto align = [](size_t x) { return (x + 255) & ~size_t(255); };
     size_t off = 0;
-    uint16_t* keys_a = (uint16_t*)(ws + off); off = align(off + (size_t)total * 2);
-    uint16_t* keys_b = (uint16_t*)(ws + off); off = align(off + (size_t)total * 2);
-    uint32_t* val_a = (uint32_t*)(ws + off); off = align(off + (size_t)total * 4);
-    uint32_t* val_b = (uint32_t*)(ws + off); off = align(off + (size_t)total * 4);
-    uint32_t* succ_a = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* succ_b = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* succ0 = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint32_t* lenv = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
-    uint64_t* dist_a = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
-    uint64_t* dist_b = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
-    IbwtBatchBlock* d_blocks = (IbwtBatchBlock*)(ws + off); off = align(off + (size_t)nbb * sizeof(IbwtBatchBlock));
-    uint32_t* d_bad = (uint32_t*)(ws + off); off = align(off + 64);
-    void* temp = ws + off;
+    IbwtBufs U;
+    U.keys_a = (uint16_t*)(ws + off); off = align(off + (size_t)total * 2);
+    U.keys_b = (uint16_t*)(ws + off); off = align(off + (size_t)total * 2);
+    U.val_a = (void*)(ws + off); off = align(off + (size_t)total * wb);
+    U.val_b = (void*)(ws + off); off = align(off + (size_t)total * wb);
+    U.succ_a = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
+    U.succ_b = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
+    U.succ0 = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
+    U.lenv = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
+    U.resume = (uint32_t*)(ws + off); off = align(off + (size_t)nheads * 4);
+    U.dist_a = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
+    U.dist_b = (uint64_t*)(ws + off); off = align(off + (size_t)nheads * 8);
+    U.slots = ws + off; off = align(off + (size_t)nheads * shape.stage);
+    U.blocks = (IbwtBatchBlock*)(ws + off); off = align(off + (size_t)nbb * sizeof(IbwtBatchBlock));
+    U.bad = (uint32_t*)(ws + off); off = align(off + 64);
+    U.temp = ws + off;
     if (ws_bytes < off) return cudaErrorInvalidValue;
-    const size_t temp_bytes = ws_bytes - off;
-    if ((e = cudaMemcpyAsync(d_blocks, hb.data(), (size_t)nbb * sizeof(IbwtBatchBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(d_bad, 0, 4, stream)) != cudaSuccess) return e;
+    U.temp_bytes = ws_bytes - off;
+    if ((e = cudaMemcpyAsync(U.blocks, hb.data(), (size_t)nbb * sizeof(IbwtBatchBlock), cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(U.bad, 0, 4, stream)) != cudaSuccess) return e;
     // a corrupt payload (several cycles, a bad primary index) must not leave parts of the output unwritten: clear it first, report it afterwards
     for (const IbwtBatchBlock& B : hb)
         if ((e = cudaMemsetAsync(d_out + B.dst_off, 0, B.n, stream)) != cudaSuccess) return e;
-    const uint32_t T = 256, G = (total + T - 1) / T, GH = (nheads + T - 1) / T;
-    ibwtb_init_kernel<<<G, T, 0, stream>>>(d_in, d_blocks, nbb, total, keys_a, val_a);
-    cub::DoubleBuffer<uint16_t> k(keys_a, keys_b);
-    cub::DoubleBuffer<uint32_t> v(val_a, val_b);
-    size_t tb = temp_bytes;
-    int key_bits = 8;
-    while ((1u << (key_bits - 8)) < nbb) key_bits++;
-    if ((e = cub::DeviceRadixSort::SortPairs(temp, tb, k, v, (int64_t)total, 0, key_bits, stream)) != cudaSuccess) return e;  // stable: LF mapping per block
-    const uint16_t* first = k.Current();
-    const uint32_t* next = v.Current();
-    ibwtb_measure_kernel<<<GH, T, 0, stream>>>(next, d_blocks, nbb, nheads, succ0, lenv, dist_a, d_bad);
-    if ((e = cudaMemcpyAsync(succ_a, succ0, (size_t)nheads * 4, cudaMemcpyDeviceToDevice, stream)) != cudaSuccess) return e;
-    (*launches) += 8;
-    uint32_t max_heads = 1;
-    for (const IbwtBatchBlock& B : hb) max_heads = std::max(max_heads, B.nstride + B.nprim);
-    uint32_t rounds = 1;
-    while ((1u << rounds) < max_heads) rounds++;
-    for (uint32_t r = 0; r < rounds + 1; r++) {
-        ibwt_jump_kernel<<<GH, T, 0, stream>>>(succ_a, dist_a, nheads, succ_b, dist_b);
-        std::swap(succ_a, succ_b);
-        std::swap(dist_a, dist_b);
-        (*launches)++;
-    }
-    ibwtb_write_kernel<<<GH, T, 0, stream>>>(next, first, d_blocks, nbb, nheads, succ0, lenv, dist_a, d_out, d_bad);
-    (*launches)++;
+    e = wide ? ibwtb_run<uint64_t>(d_in, d_out, hb, total, nheads, U, shape, stream, launches, hook)
+             : ibwtb_run<uint32_t>(d_in, d_out, hb, total, nheads, U, shape, stream, launches, hook);
+    if (e != cudaSuccess) return e;
     uint32_t h_bad = 0;
-    if ((e = cudaMemcpyAsync(&h_bad, d_bad, 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
-    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    {
+        LzHookScope hs(hook, "bwt_inverse:sync");
+        if ((e = cudaMemcpyAsync(&h_bad, U.bad, 4, cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+        if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    }
     if (h_bad) return cudaErrorInvalidValue;  // the permutation of some block is not one list through its n ranks
     return cudaGetLastError();
 }

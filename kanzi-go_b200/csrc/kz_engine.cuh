@@ -134,7 +134,7 @@ struct kz_ctx {
     std::string err;
     uint64_t launches = 0;
     bool profile = false;
-    int bwt_profile = 0;  // kz_bwt_profile: bit 0 times the BWT forward rounds (with profile), bit 1 forces the 56-bit rounds
+    int bwt_profile = 0;  // kz_bwt_profile: bit 0 times the BWT forward rounds and inverse parts (with profile), bit 1 forces the 56-bit rounds, bits 8-19 shape the inverse walk
     kz::EncPlan enc_plan;
     uint64_t user_stream_bs = 0;  // kz_set_stream_block_size: ctx["blockSize"] for the block / single-transform entry points
     int64_t range_from = -1, range_to = -1;  // kz_set_block_range: ctx["from"] / ctx["to"] of the stream-level decodes (-1 = not given)
