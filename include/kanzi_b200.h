@@ -385,7 +385,8 @@ int kz_read_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, size_t n, uint
 int kz_read_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t n, uint32_t nreq, const uint64_t* off, const uint64_t* len, void* d_dst,
                           const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
 
-/* ---- writes: byte ranges written into a compressed stream, and appends, re-encoding only the blocks they touch ------------------------
+/* ---- writes: byte ranges written into a compressed stream, and appends, re-encoding only the blocks they touch (many streams in one call:
+ *      kz_write_ranges_streams) ------------------------------------------------------------------------------------------------------------
  * Blocks are independent, every block but the last decodes to exactly block_size bytes, and nothing in a record depends on its position,
  *   so a write that touches blocks k .. m re-encodes only those; everything before record k stays as it is and the records behind m are
  *   copied, moved by the change in bit length. The caller rewrites only the stream's tail: for an append, the last record and the end marker.
@@ -510,6 +511,40 @@ int kz_read_ranges_streams(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_i
 int kz_read_ranges_streams_device(kz_ctx* ctx, kz_cache* cache, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
                                   const uint64_t* src_len, uint32_t nreq, const uint32_t* req_stream, const uint64_t* off, const uint64_t* len, void* d_dst,
                                   const uint64_t* dst_off, uint64_t* out_len, int32_t* status);
+
+/* ---- many streams per call: writes and appends into many compressed objects in one call (a batch of partial PUTs or appends over
+ *      thousands of small objects: log segments, records, a mutable directory) ----------------------------------------------------------------
+ * Streams use the layout of kz_read_ranges_streams. Write i goes to slot w_stream[i]; off[i], len[i], data + data_off[i] and KZ_WRITE_APPEND
+ *   mean what they mean in kz_write_ranges. Slot s's new stream is src + src_off[s] up to keep[s], followed by the out_n[s] bytes at
+ *   dst + dst_off[s]; at most dst_cap[s] bytes are written there, and nothing outside [dst_off[s], dst_off[s] + dst_cap[s]).
+ * Equivalence: for every slot s, keep[s], the tail, out_n[s] (the capacity needed on -KZ_ERR_WRITE_FILE included), status[s] and ix[s]
+ *   afterwards (as a kz_index_save blob) are what kz_write_ranges[_device] returns when called with ix[s], stream s and only the writes on
+ *   s, in array order, under the same skip-blocks setting. An index changes only when its slot succeeds.
+ * Slots no write of length > 0 names are neither checked nor read; their index may be NULL. They return keep[s] = src_len[s], out_n[s] = 0
+ *   and status[s] = 0, so a caller can pass its whole object table.
+ * Slot-level failures (status[s], the others are served): a NULL or stale index, a chain or codec the GPU path lacks, a block that must be
+ *   decoded and fails (with the code of decoding it alone), a decoded block before the last that is not block_size bytes long, a data size
+ *   past what an index holds, dst_cap[s] too small.
+ * Call-level failures set every status, write nothing and change no index: a bad argument, w_stream[i] >= nstreams, one kz_index* in two
+ *   slots that writes name (a write mutates its index), an open session, CUDA and allocation failures, a transform or entropy failure on
+ *   the encode side; in the device variant also d_src, d_dst or an offset of a named slot that is not a multiple of 16, and output windows
+ *   that overlap each other or a named stream. Buffers are checked only when a slot is named: a call that names none reads and writes
+ *   nothing and returns 0. The return value is 0, the call-level code, or the first failing slot's code in slot order.
+ * Work: re-encoded blocks of slots with the same transform48, entropy, block_size and checksum_bits share passes (blocks of different ones
+ *   never do): per pass one decode of the partly covered blocks, one copy launch that applies every slot's writes and zero gaps, and one
+ *   encode. Slots whose size the result depends on get their old last block decoded once, in shared passes before the others, and that
+ *   decode is reused for its encode. All tails are laid out by one concat; the host variant uploads every named slot's window and the write
+ *   bytes in one transfer and brings the tails back in one; the device variant gathers the new first 32 bytes with one copy. Launches and
+ *   synchronisations follow the passes, not the number of slots. kz_write_ranges[_device] is the one-slot case of the same routine. With
+ *   kz_profile(ctx,1) the "write:*" counters count the call once, summed over the slots that succeeded. */
+int kz_write_ranges_streams(kz_ctx* ctx, uint32_t nstreams, kz_index* const* ix, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len,
+                            uint32_t nw, const uint32_t* w_stream, const uint64_t* off, const uint64_t* len, const uint8_t* data, const uint64_t* data_off,
+                            uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* keep, uint64_t* out_n, int32_t* status);
+/* d_src, d_data and d_dst device memory (at least 64 readable bytes behind each stream); every array is a host array. */
+int kz_write_ranges_streams_device(kz_ctx* ctx, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
+                                   const uint64_t* src_len, uint32_t nw, const uint32_t* w_stream, const uint64_t* off, const uint64_t* len,
+                                   const void* d_data, const uint64_t* data_off, void* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                   uint64_t* keep, uint64_t* out_n, int32_t* status);
 
 #ifdef __cplusplus
 }

@@ -379,3 +379,166 @@ func (c *Context) WriteRanges(x *Index, stream []byte, writes []Write) (keep int
 func (c *Context) Append(x *Index, stream []byte, p []byte) (keep int, tail []byte, err error) {
 	return c.WriteRanges(x, stream, []Write{{Append: true, Data: p}})
 }
+
+// StreamWrite is one write of WriteRangesStreams: a Write on stream Stream.
+type StreamWrite struct {
+	Stream int
+	Write
+}
+
+// StreamTail is what WriteRangesStreams gives one stream: the new stream is stream[:Keep] followed by Tail, as WriteRanges gives it, or
+// Err when that stream failed (its index and bytes are unchanged). A stream no write names keeps Keep = len(stream) and an empty Tail.
+type StreamTail struct {
+	Keep int
+	Tail []byte
+	Err  error
+}
+
+// WriteRangesStreams applies writes to many streams in one kz_write_ranges_streams call: each stream gets what WriteRanges gives it for
+// its own writes, in order, and idx[s] then describes its new stream. A nil or stale index, a chain the GPU path lacks, a block that
+// fails to decode or a data size past what an index holds fails only that stream; streams no write names are not read, so callers may
+// pass their whole object table. A stream whose tail did not fit is written again alone with the capacity the call named. The returned
+// error is a failure of the call as a whole (a write on a stream out of range, one index in two written slots, a session open on c, an
+// encode failure), in which case no index changed. The call carries one extra slot that no write names: the library sets its status only
+// when the whole call fails, which tells such a failure from every named stream failing with the same code.
+func (c *Context) WriteRangesStreams(idx []*Index, streams [][]byte, writes []StreamWrite) ([]StreamTail, error) {
+	ns, n := len(streams), len(writes)
+	if len(idx) != ns {
+		return nil, errors.New("gpu: one index per stream")
+	}
+	out := make([]StreamTail, ns)
+	for s, b := range streams {
+		out[s].Keep = len(b)
+	}
+	if ns == 0 || n == 0 {
+		return out, nil
+	}
+	named := make([]bool, ns)
+	blocks := make([]int, ns)
+	for _, w := range writes {
+		if w.Stream < 0 || w.Stream >= ns {
+			return nil, errors.New("gpu: write on a stream out of range")
+		}
+		if len(w.Data) > 0 {
+			named[w.Stream] = true
+		}
+	}
+	// one slot more than the streams, named by no write: only a failure of the whole call sets its status
+	srcOff := make([]C.uint64_t, ns+1)
+	srcLen := make([]C.uint64_t, ns+1)
+	dstCap := make([]C.uint64_t, ns+1)
+	hs := make([]*C.kz_index, ns+1)
+	total := 0
+	for s, b := range streams {
+		if idx[s] != nil {
+			hs[s] = idx[s].h
+		}
+		if named[s] { // only the named streams are copied: the others are neither checked nor read
+			srcOff[s], srcLen[s] = C.uint64_t(total), C.uint64_t(len(b))
+			total += len(b)
+		}
+	}
+	src := make([]byte, total+1)
+	for s, b := range streams {
+		if named[s] {
+			copy(src[int(srcOff[s]):], b)
+		}
+	}
+	ws := make([]C.uint32_t, n)
+	off := make([]C.uint64_t, n)
+	ln := make([]C.uint64_t, n)
+	dataOff := make([]C.uint64_t, n)
+	dtotal := 0
+	for i, w := range writes {
+		ws[i], off[i], ln[i], dataOff[i] = C.uint32_t(w.Stream), C.uint64_t(w.Off), C.uint64_t(len(w.Data)), C.uint64_t(dtotal)
+		if w.Append {
+			off[i] = C.KZ_WRITE_APPEND
+		}
+		dtotal += len(w.Data)
+	}
+	data := make([]byte, dtotal+1)
+	for i, w := range writes {
+		copy(data[int(dataOff[i]):], w.Data)
+	}
+	// WriteRanges's capacity per stream: len(stream) + k * kz_max_block_output(block_size) + 16, k bounded by the blocks the writes span
+	for _, w := range writes {
+		if len(w.Data) > 0 && idx[w.Stream] != nil {
+			var bs C.uint32_t
+			C.kz_index_info(idx[w.Stream].h, nil, nil, &bs, nil, nil, nil, nil, nil)
+			blocks[w.Stream] += len(w.Data)/int(bs) + 2
+			dstCap[w.Stream] = C.uint64_t(len(streams[w.Stream]) + blocks[w.Stream]*int(C.kz_max_block_output(C.size_t(bs))) + 16)
+		}
+	}
+	keep := make([]C.uint64_t, ns+1)
+	outN := make([]C.uint64_t, ns+1)
+	status := make([]C.int32_t, ns+1)
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	for {
+		dstOff := make([]C.uint64_t, ns+1)
+		dcap := uint64(0)
+		for s := range streams {
+			dstOff[s] = C.uint64_t(dcap)
+			dcap += uint64(dstCap[s])
+		}
+		dst := make([]byte, dcap+1)
+		rc := C.kz_write_ranges_streams(c.h, C.uint32_t(ns+1), &hs[0], (*C.uint8_t)(unsafe.Pointer(&src[0])), &srcOff[0], &srcLen[0], C.uint32_t(n),
+			&ws[0], &off[0], &ln[0], (*C.uint8_t)(unsafe.Pointer(&data[0])), &dataOff[0], (*C.uint8_t)(unsafe.Pointer(&dst[0])), &dstOff[0],
+			&dstCap[0], &keep[0], &outN[0], &status[0])
+		if status[ns] != 0 { // the call failed as a whole: no index changed
+			return nil, c.err(rc)
+		}
+		// a stream whose tail did not fit keeps its index unchanged: it alone is written again, with the capacity the call named
+		var again []int
+		for s := range streams {
+			if !named[s] {
+				continue
+			}
+			if status[s] == -C.KZ_ERR_WRITE_FILE && outN[s] > dstCap[s] {
+				dstCap[s] = outN[s]
+				again = append(again, s)
+				continue
+			}
+			out[s] = StreamTail{Keep: int(keep[s])}
+			if status[s] != 0 {
+				out[s].Keep, out[s].Err = len(streams[s]), &StreamError{Code: int(-status[s])}
+				continue
+			}
+			out[s].Tail = append([]byte(nil), dst[uint64(dstOff[s]):uint64(dstOff[s])+uint64(outN[s])]...)
+		}
+		if len(again) == 0 {
+			return out, nil
+		}
+		retry := make([]bool, ns)
+		for _, s := range again {
+			retry[s] = true
+		}
+		for s := range streams {
+			named[s] = retry[s]
+			if !retry[s] {
+				dstCap[s] = 0
+			}
+		}
+		ws, off, ln, dataOff = ws[:0], off[:0], ln[:0], dataOff[:0]
+		dtotal = 0
+		var left []StreamWrite
+		for _, w := range writes {
+			if !retry[w.Stream] {
+				continue
+			}
+			o := C.uint64_t(w.Off)
+			if w.Append {
+				o = C.KZ_WRITE_APPEND
+			}
+			ws, off, ln = append(ws, C.uint32_t(w.Stream)), append(off, o), append(ln, C.uint64_t(len(w.Data)))
+			dataOff = append(dataOff, C.uint64_t(dtotal))
+			dtotal += len(w.Data)
+			left = append(left, w)
+		}
+		writes, n = left, len(left)
+		data = make([]byte, dtotal+1)
+		for i, w := range writes {
+			copy(data[int(dataOff[i]):], w.Data)
+		}
+	}
+}

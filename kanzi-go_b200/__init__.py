@@ -45,6 +45,7 @@ ABI_SYMBOLS = [
     "kz_read_ranges_device", "kz_cache_create", "kz_cache_free", "kz_cache_clear", "kz_cache_stats", "kz_read_ranges_cached",
     "kz_read_ranges_cached_device", "kz_index_build_streams", "kz_index_build_streams_device", "kz_read_ranges_streams",
     "kz_read_ranges_streams_device", "kz_compress_streams_bs", "kz_compress_streams_bs_device", "kz_write_ranges", "kz_write_ranges_device",
+    "kz_write_ranges_streams", "kz_write_ranges_streams_device",
 ]
 
 WRITE_APPEND = (1 << 64) - 1  # KZ_WRITE_APPEND: a write's offset that means the end of the data as the call's earlier writes left it
@@ -193,6 +194,8 @@ def load_library(build_if_missing=True):
     L.kz_read_ranges_streams_device.argtypes = [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
     L.kz_write_ranges.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, sz, C.POINTER(u64), C.POINTER(sz)]
     L.kz_write_ranges_device.argtypes = [vp, vp, vp, sz, u32, vp, vp, vp, vp, vp, sz, C.POINTER(u64), C.POINTER(sz)]
+    L.kz_write_ranges_streams.argtypes = [vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.kz_write_ranges_streams_device.argtypes = [vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -642,6 +645,72 @@ class Context:
                                                _p(rs), _p(o), _p(ln), _dptr(d_dst), _p(do), _p(out_len), _p(status))
         return out_len, status
 
+    def write_streams(self, streams, indexes, writes):
+        """writes: [(slot, off, data), ...] in order on host streams with their indexes (None allowed for slots no write names) ->
+        (keeps, tails, status): slot s gets what indexes[s].write_many(streams[s], its writes) gives, as keeps[s] and tails[s], in one call
+        over all slots (kz_write_ranges_streams). Failures do not raise: status[s] = 0 or -(kanzi error code), and a failed slot's index
+        is unchanged. A slot whose tail did not fit is called again alone with the capacity it named."""
+        arrs = [_u8(x) for x in streams]
+        ns = len(arrs)
+        src_len = np.array([a.size for a in arrs], np.uint64)
+        src_off = _offsets(src_len)
+        src = np.concatenate(arrs) if arrs else np.zeros(0, np.uint8)
+        bufs = [_u8(w[2]) for w in writes]
+        ws = np.array([int(w[0]) for w in writes], np.uint32)
+        off = np.array([int(w[1]) for w in writes], np.uint64)
+        ln = np.array([b.size for b in bufs], np.uint64)
+        data = np.concatenate(bufs) if bufs else np.zeros(0, np.uint8)
+        data_off = _offsets(ln)
+        # write_many's capacity per slot: (n - keep) + k * kz_max_block_output(block_size) + 16, k bounded by the blocks the writes span
+        cap = np.zeros(ns, np.uint64)
+        for s in sorted(set(int(w) for w, n in zip(ws, ln) if n)):
+            bs = indexes[s].info["block_size"] if indexes[s] is not None else 1024
+            k = sum(int(n) // bs + 2 for w, n in zip(ws, ln) if n and w == s)
+            cap[s] = src_len[s] + k * self.lib.kz_max_block_output(bs) + 16
+        keeps, tails, status = [int(n) for n in src_len], [b""] * ns, [0] * ns
+        todo = np.arange(ns)
+        while True:
+            # the slots still to serve, and the writes on them, renumbered
+            slot = np.full(ns, -1, np.int64)
+            slot[todo] = np.arange(len(todo))
+            pick = np.array([i for i in range(len(writes)) if slot[ws[i]] >= 0], np.int64)
+            sub = [arrs[s] for s in todo]
+            t_len = src_len[todo]
+            t_so = _offsets(t_len)
+            t_src = np.concatenate(sub) if sub else np.zeros(0, np.uint8)
+            t_cap = cap[todo]
+            dst_off = _offsets(t_cap)
+            dst = np.empty(max(int(t_cap.sum()), 1), np.uint8)
+            keep, out_n, st = np.zeros(len(todo), np.uint64), np.zeros(len(todo), np.uint64), np.zeros(len(todo), np.int32)
+            ix = self._index_slots([indexes[s] for s in todo])
+            t_ws = slot[ws[pick]].astype(np.uint32) if len(pick) else np.zeros(0, np.uint32)
+            t_off, t_ln, t_do = (np.ascontiguousarray(a[pick] if len(pick) else a[:0]) for a in (off, ln, data_off))
+            self.lib.kz_write_ranges_streams(self.h, len(todo), C.addressof(ix), _p(t_src), _p(t_so), _p(t_len), len(pick), _p(t_ws),
+                                             _p(t_off), _p(t_ln), _p(data), _p(t_do), dst.ctypes.data, _p(dst_off), _p(t_cap), _p(keep), _p(out_n),
+                                             _p(st))
+            again = []
+            for j, s in enumerate(todo):
+                if st[j] == -12 and out_n[j] > t_cap[j]:  # KZ_ERR_WRITE_FILE: the index is unchanged, call again with the capacity named
+                    cap[s] = out_n[j]
+                    again.append(s)
+                    continue
+                keeps[s], status[s] = int(keep[j]), int(st[j])
+                tails[s] = dst[int(dst_off[j]): int(dst_off[j]) + int(out_n[j])].tobytes() if not st[j] else b""
+            if not again:
+                return keeps, tails, status
+            todo = np.array(again, np.int64)
+
+    def write_streams_device(self, d_src, src_off, src_len, indexes, w_stream, off, length, d_data, data_off, d_dst, dst_off, dst_cap):
+        """Device-resident write_streams (kz_write_ranges_streams_device): d_src / d_data / d_dst are CUDA tensors or addresses, the rest
+        host sequences -> (keep, out_n, status). On -KZ_ERR_WRITE_FILE (code 12) out_n[s] is the capacity slot s needs."""
+        so, sl, o, ln, doff, dso, dcap = (np.ascontiguousarray(a, np.uint64) for a in (src_off, src_len, off, length, data_off, dst_off, dst_cap))
+        ws = np.ascontiguousarray(w_stream, np.uint32)
+        ix = self._index_slots(indexes)
+        keep, out_n, status = np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.uint64), np.zeros(len(sl), np.int32)
+        self.lib.kz_write_ranges_streams_device(self.h, len(sl), C.addressof(ix), _dptr(d_src), _p(so), _p(sl), len(o), _p(ws), _p(o), _p(ln),
+                                                _dptr(d_data), _p(doff), _dptr(d_dst), _p(dso), _p(dcap), _p(keep), _p(out_n), _p(status))
+        return keep, out_n, status
+
     def block_cache(self, budget):
         """A BlockCache of decoded blocks in `budget` bytes of HBM (kz_cache_create), for StreamIndex.read / read_many /
         read_many_device(cache=...) on this context."""
@@ -820,9 +889,10 @@ class StreamIndex:
         k = sum(int(n) // bs + 2 for n in ln if n)
         cap = s.size + k * self.lib.kz_max_block_output(bs) + 16
         keep, out_n = C.c_uint64(0), C.c_size_t(0)
+        data_off = _offsets(ln)  # held for the call: a temporary's buffer could be freed before the library reads it
         while True:
             dst = np.empty(max(cap, 1), np.uint8)
-            rc = self.lib.kz_write_ranges(ctx.h, self.h, _p(s), s.size, len(writes), _p(off), _p(ln), _p(data), _p(_offsets(ln)), dst.ctypes.data, cap,
+            rc = self.lib.kz_write_ranges(ctx.h, self.h, _p(s), s.size, len(writes), _p(off), _p(ln), _p(data), _p(data_off), dst.ctypes.data, cap,
                                           C.byref(keep), C.byref(out_n))
             if rc == -12 and out_n.value > cap:  # KZ_ERR_WRITE_FILE
                 cap = out_n.value

@@ -1938,6 +1938,18 @@ int encode_slots(kz_ctx* ctx, const TransformPlan& plan, uint32_t etype, uint32_
     return 0;
 }
 
+// Grows b to hold `need` bytes, keeping its first `used` bytes (DevBuf::ensure drops them).
+int grow_keeping(kz_ctx* ctx, DevBuf& b, uint64_t used, uint64_t need) {
+    if (need + 64 + 256 <= b.cap) return 0;
+    DevBuf nb;
+    CK(nb.ensure(std::max<size_t>(need + 64, 2 * b.cap)));
+    if (used) CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    b.release();
+    b = nb;
+    return 0;
+}
+
 // The bit strings of blocks encoded pass by pass, kept for one assembly behind the last pass: record r is bits[r] bits at offset[r] of
 // ctx->d_bits, each record at a 16-byte aligned offset; `used` bytes are taken.
 struct RecordArena {
@@ -1956,14 +1968,8 @@ struct RecordArena {
         if (rc) return rc;
         uint64_t need = used;
         for (uint32_t j = 0; j < k; j++) need += round16((b[j] + 7) / 8);
-        if (need + 64 + 256 > ctx->d_bits.cap) {  // grow d_bits, keeping the records of the earlier passes (DevBuf::ensure drops them)
-            DevBuf nb;
-            CK(nb.ensure(std::max<size_t>(need + 64, 2 * ctx->d_bits.cap)));
-            if (used) CK(cudaMemcpyAsync(nb.p, ctx->d_bits.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            ctx->d_bits.release();
-            ctx->d_bits = nb;
-        }
+        rc = grow_keeping(ctx, ctx->d_bits, used, need);  // the records of the earlier passes stay
+        if (rc) return rc;
         CopyList pack;
         for (uint32_t j = 0; j < k; j++) {
             bits[rec[j]] = b[j];
@@ -3510,13 +3516,367 @@ int check_index_streams_args(kz_ctx* ctx, uint32_t ns, const void* src, const ui
     return check_spans(ctx, src, src_off, src_len, ns, device);
 }
 
-// ---- writes into a compressed stream (kz_write_ranges[_device]; plan in kz_write_plan.h) -------------------------------------------
-// The blocks plan_writes re-encodes go through the stages in passes: the ones whose old bytes survive are decoded into their slots, the
-// write slices are copied over them and the gaps zeroed, and the slots are encoded; every pass's records are packed into ctx->d_bits.
-// One concat then lays out the tail of the new stream: the carry, the new records behind their prefixes, the old records behind them
-// moved to their new bit (read where they lie, at any bit), and the end marker. The index is updated only when everything succeeded.
-// Host variant (src set): the old stream from the first byte a record the call may read or move lies in is uploaded once, the write bytes
-// once, and the tail comes back in one copy. Device variant: d_src, d_data and d_dst are device memory.
+// ---- writes into compressed streams (kz_write_ranges[_device], kz_write_ranges_streams[_device]; plan in kz_write_plan.h) ----------
+// The blocks plan_writes_streams re-encodes go through the stages in passes of one group: the ones whose old bytes survive are decoded into
+// their slots, the write slices and the zero gaps (copied from a zeroed area behind the slots) are copied over them by one launch, and the
+// slots are encoded; every pass's records are packed into ctx->d_bits. One concat then lays out the tail of every new stream: the carry,
+// the new records behind their prefixes, the old records behind them moved to their new bit (read where they lie, at any bit), and the
+// end marker. An index is updated only when its slot succeeded.
+// Host variant (src set): each slot's old stream from the first byte a record the call may read or move lies in, and the write bytes,
+// go up in one transfer, and the tails come back in one. Device variant: d_src, d_data and dst are device memory.
+
+// One slot of a write call: the stream ix was built from (n bytes at byte `at` of the source) and its output window.
+struct WriteSlot {
+    kz_index* ix;
+    uint64_t at, n, dst_off, cap;
+};
+
+// The writes i (write i to slot w_slot[i], null: every write to S[0]) on slots that passed their checks. keep, out_n and status are per
+// slot; each slot gets what a call on it alone gives. The return value is a call-level failure (CUDA, allocation, an encode failure).
+int write_ranges_impl(kz_ctx* ctx, const uint8_t* src, const uint8_t* d_src, const std::vector<WriteSlot>& S, uint32_t nw, const uint32_t* w_slot,
+                      const uint64_t* off, const uint64_t* len, const uint8_t* data, const uint64_t* data_off, uint8_t* dst, uint64_t* keep,
+                      uint64_t* out_n, int32_t* status) {
+    const bool host = src != nullptr;
+    const uint32_t ns = (uint32_t)S.size();
+    auto slot_of = [&](uint32_t i) { return w_slot ? w_slot[i] : 0u; };
+    for (uint32_t s = 0; s < ns; s++) keep[s] = S[s].n, out_n[s] = 0, status[s] = 0;
+    // groups, numbered in the order they first appear: the header, transform plan and encode cost of each
+    std::map<std::tuple<uint64_t, uint32_t, uint32_t, uint32_t>, uint32_t> group_of;
+    std::vector<StreamHeader> gsh;
+    std::vector<TransformPlan> gplan;
+    std::vector<uint64_t> gcost;
+    std::vector<StreamIndex> X(ns);  // what the plan knows; the indexes change only on success
+    std::vector<WriteStream> WS(ns);
+    for (uint32_t s = 0; s < ns; s++) {
+        const kz_index& ix = *S[s].ix;
+        const auto key = std::make_tuple(ix.t48, ix.etype, ix.block_size, ix.checksum_bits);
+        auto it = group_of.find(key);
+        if (it == group_of.end()) {
+            it = group_of.emplace(key, (uint32_t)gsh.size()).first;
+            gsh.push_back(index_header(ix));
+            gplan.emplace_back();
+            int rc = plan_transforms(ctx, ix.t48, ix.etype, gplan.back(), KZ_ERR_CREATE_CODEC);
+            if (rc) return rc;
+            gcost.push_back(compress_block_cost(round16(ix.block_size), entropy_scratch(ix.etype)));
+        }
+        X[s] = ix;
+        WS[s] = WriteStream{&X[s], it->second, gcost[it->second]};
+    }
+    // live[s]: the slot still makes a new tail; a failed slot, or one whose writes change nothing, takes no further part
+    std::vector<uint8_t> live(ns, 0), need(ns, 0);
+    auto fail = [&](uint32_t s, int code) {
+        status[s] = code;
+        live[s] = 0;
+        WS[s].x = nullptr;
+    };
+    WriteStreamsPlan W = plan_writes_streams(WS, nw, w_slot, off, len);
+    std::vector<uint64_t> low(ns, 0);  // with the size to learn: the first block a write names, or the last block
+    for (uint32_t s = 0; s < ns; s++) {
+        const WritePlan& P = W.plans[s];
+        low[s] = X[s].nblocks() ? X[s].nblocks() - 1 : 0;
+        if (P.status == WRITE_TOO_LARGE) fail(s, ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds"));
+        else if (P.status == WRITE_NEED_SIZE) live[s] = need[s] = 1;
+        else if (P.nothing()) WS[s].x = nullptr;
+        else live[s] = 1;
+    }
+    if (!std::count(live.begin(), live.end(), 1)) return 0;
+    for (uint32_t i = 0; i < nw; i++) {
+        const uint32_t s = slot_of(i);
+        if (need[s] && len[i] && off[i] != WRITE_APPEND) low[s] = std::min<uint64_t>(low[s], off[i] / X[s].block_size);
+    }
+    // the old streams and the write bytes on the device: slot s's stream bit b lies at bit b + org[s] of d_words, write i at d_wdata + w_at[i]
+    std::vector<uint64_t> org(ns, 0), w_at(nw, 0);
+    const uint8_t* d_words = d_src;
+    const uint8_t* d_wdata = data;
+    uint64_t words_bytes = 0;
+    if (host) {
+        std::vector<UploadPiece> up;
+        std::vector<uint32_t> up_slot;
+        uint64_t pieces = 0, bytes = 0;
+        for (uint32_t s = 0; s < ns; s++) {
+            if (!live[s]) continue;
+            const uint64_t ubase = ((need[s] ? record_prefix_bit(X[s], low[s]) : W.plans[s].cut) / 8) & ~15ull, tail = S[s].n - ubase;
+            org[s] = 0 - 8 * ubase;  // + 8 * (its offset in d_in), below
+            up.push_back(UploadPiece{src + S[s].at + ubase, tail, tail + 128}), up_slot.push_back(s);
+            pieces += tail ? 1 : 0, bytes += tail;
+        }
+        const size_t nslots = up.size();
+        uint64_t wtotal = 0;
+        for (uint32_t i = 0; i < nw; i++)
+            if (len[i] && live[slot_of(i)]) up.push_back(UploadPiece{data + data_off[i], len[i], len[i]}), wtotal += len[i];
+        std::vector<uint64_t> at;
+        int rc = upload_pieces(ctx, up, at, &words_bytes);
+        if (rc) return rc;
+        for (size_t k = 0; k < nslots; k++) org[up_slot[k]] += 8 * at[k];
+        for (uint32_t i = 0, k = (uint32_t)nslots; i < nw; i++)
+            if (len[i] && live[slot_of(i)]) w_at[i] = at[k++];
+        d_words = d_wdata = ctx->d_in.as<uint8_t>();
+        if (ctx->profile) {
+            auto& e = ctx->prof["write:h2d"];
+            e.bytes_in += pieces + (wtotal ? 1 : 0), e.bytes_out += bytes + wtotal, e.launches++;
+        }
+    } else {
+        for (uint32_t s = 0; s < ns; s++) org[s] = 8 * S[s].at, words_bytes = std::max(words_bytes, S[s].at + S[s].n);
+        for (uint32_t i = 0; i < nw; i++) w_at[i] = len[i] ? data_off[i] : 0;
+    }
+    const uint32_t* d_w32 = (const uint32_t*)d_words;
+    const uint64_t words_len = (words_bytes + 3) / 4 + 16;
+    auto job_of = [&](uint32_t s, uint64_t b) {
+        DecJob j = DecJob();
+        j.bit_off = X[s].start[b] + org[s];
+        j.bits = X[s].bits[b];
+        j.block_size = X[s].block_size;
+        return j;
+    };
+    // the failure of decoded block b of slot s: its own code, or a length that breaks the block arithmetic
+    auto check_decoded = [&](uint32_t s, uint64_t b, const DecodeFailure& f, uint32_t m) {
+        const uint64_t nb = X[s].nblocks(), bs = X[s].block_size;
+        if (m > bs || (!f.failed() && (b + 1 == nb ? m == 0 || (X[s].size >= 0 && m != (uint64_t)X[s].size - (nb - 1) * bs) : m != bs)))
+            return ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: a block before the last is not block_size bytes long");
+        if (f.failed()) return ctx->fail(-f.code, f.msg);
+        return 0;
+    };
+    std::vector<uint64_t> dec_blocks(ns, 0), dec_bytes(ns, 0);
+    // slots whose size the result depends on: their old last blocks decoded, group by group in passes, packed into ctx->d_out at
+    // learned[s], where the encode passes copy them from
+    std::vector<uint64_t> learned(ns, NO_ROOM);
+    if (std::count(need.begin(), need.end(), 1)) {
+        uint64_t used = 0;
+        for (uint32_t g = 0; g < (uint32_t)gsh.size(); g++) {
+            std::vector<uint32_t> ss;
+            for (uint32_t s = 0; s < ns; s++)
+                if (need[s] && live[s] && WS[s].group == g) ss.push_back(s);
+            if (ss.empty()) continue;
+            const uint32_t bs = gsh[g].block_size;
+            const PassPlan pp = plan_decompress_passes((uint32_t)ss.size(), decompress_slot(bs), read_block_cost(bs));
+            for (uint32_t p = 0; p < pp.npasses(); p++) {
+                const uint32_t a = pp.first[p], k = pp.first[p + 1] - a;
+                int rc = grow_keeping(ctx, ctx->d_out, used, used + k * decompress_slot(bs));
+                if (rc) return rc;
+                std::vector<DecJob> jobs;
+                for (uint32_t i = a; i < a + k; i++) jobs.push_back(job_of(ss[i], X[ss[i]].nblocks() - 1));
+                std::vector<uint64_t> at(k, NO_ROOM);  // a block decoded again alone keeps the place it was first given
+                std::vector<DecodeFailure> fl;
+                std::vector<uint32_t> olen;
+                rc = decode_isolated(ctx, gsh[g], gplan[g], d_w32, words_len, jobs, std::vector<uint8_t>(k, 1),
+                                     [&](uint32_t i, uint32_t m) {
+                                         if (m > bs) return NO_ROOM;
+                                         if (at[i] == NO_ROOM) at[i] = used, used += round16(m);
+                                         return at[i];
+                                     },
+                                     ctx->d_out.as<uint8_t>(), fl, olen);
+                if (rc) return rc;
+                for (uint32_t i = 0; i < k; i++) {
+                    const uint32_t s = ss[a + i];
+                    const uint64_t nb = X[s].nblocks();
+                    if ((rc = check_decoded(s, nb - 1, fl[i], olen[i]))) {
+                        fail(s, rc);
+                        continue;
+                    }
+                    X[s].size = (int64_t)((nb - 1) * bs + olen[i]);
+                    learned[s] = at[i];
+                    dec_blocks[s]++, dec_bytes[s] += olen[i];
+                }
+            }
+        }
+        W = plan_writes_streams(WS, nw, w_slot, off, len);
+        for (uint32_t s = 0; s < ns; s++) {
+            if (!need[s] || !live[s]) continue;
+            if (W.plans[s].status != WRITE_OK) fail(s, ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds"));
+            else if (W.plans[s].nothing()) live[s] = 0;
+        }
+    }
+    // passes: decode, apply the writes, encode; each pass's records packed into ctx->d_bits as records of their pairs
+    const uint32_t npairs = (uint32_t)W.stream.size();
+    RecordArena arena(npairs);
+    std::vector<uint64_t> enc_bytes(ns, 0);
+    for (uint32_t p = 0; p < W.npasses(); p++) {
+        const uint32_t a = W.first[p], k = W.first[p + 1] - a;
+        const uint32_t g = WS[W.stream[a]].group, bs = gsh[g].block_size;
+        const uint64_t astride = decompress_slot(bs);
+        uint32_t zmax = 0;  // the longest zero gap of the pass: the zeroed area behind the slots
+        bool any = false;
+        for (uint32_t i = a; i < a + k; i++) {
+            const uint32_t s = W.stream[i];
+            if (!live[s]) continue;
+            any = true;
+            const WritePlan& P = W.plans[s];
+            for (uint64_t q = P.piece_of[W.enc[i]]; q < P.piece_of[W.enc[i] + 1]; q++)
+                if (P.pieces[q].kind == PIECE_ZERO) zmax = std::max(zmax, P.pieces[q].len);
+        }
+        if (!any) continue;
+        CK(ctx->d_slots.ensure(astride * k + zmax + 64));
+        uint8_t* slots = ctx->d_slots.as<uint8_t>();
+        uint8_t* zero = slots + astride * k;
+        if (zmax) CK(cudaMemsetAsync(zero, 0, zmax, ctx->stream));
+        std::vector<uint32_t> who;
+        std::vector<DecJob> jobs;
+        std::vector<uint8_t> last;
+        CopyList fill;
+        for (uint32_t i = a; i < a + k; i++) {
+            const uint32_t s = W.stream[i], j = W.enc[i];
+            const WritePlan& P = W.plans[s];
+            if (!live[s] || !P.decode[j]) continue;
+            const uint64_t b = P.enc[j], nb = X[s].nblocks();
+            if (learned[s] != NO_ROOM && b + 1 == nb) {
+                // only the old bytes that survive: the write and zero copies of the same launch cover the rest, and copies of one launch
+                // run in no particular order
+                for (uint64_t q = P.piece_of[j]; q < P.piece_of[j + 1]; q++)
+                    if (P.pieces[q].kind == PIECE_OLD)
+                        fill.add(ctx->d_out.as<uint8_t>() + learned[s] + P.pieces[q].at, slots + (uint64_t)(i - a) * astride + P.pieces[q].at,
+                                 P.pieces[q].len);
+                continue;
+            }
+            who.push_back(i), jobs.push_back(job_of(s, b)), last.push_back(b + 1 == nb);
+        }
+        if (!jobs.empty()) {
+            std::vector<DecodeFailure> fl;
+            std::vector<uint32_t> olen;
+            int rc = decode_isolated(ctx, gsh[g], gplan[g], d_w32, words_len, jobs, last,
+                                     [&](uint32_t q, uint32_t m) { return m > bs ? NO_ROOM : (uint64_t)(who[q] - a) * astride; }, slots, fl, olen);
+            if (rc) return rc;
+            // a slot's first failing block in block order decides its code, as in a call on it alone
+            for (size_t q = 0; q < who.size(); q++) {
+                const uint32_t s = W.stream[who[q]];
+                if (!live[s]) continue;
+                if ((rc = check_decoded(s, W.plans[s].enc[W.enc[who[q]]], fl[q], olen[q]))) fail(s, rc);
+                else dec_blocks[s]++, dec_bytes[s] += olen[q];
+            }
+        }
+        any = false;
+        for (uint32_t i = a; i < a + k; i++) {
+            const uint32_t s = W.stream[i];
+            if (!live[s]) continue;
+            any = true;
+            const WritePlan& P = W.plans[s];
+            for (uint64_t q = P.piece_of[W.enc[i]]; q < P.piece_of[W.enc[i] + 1]; q++) {
+                const WritePiece& pc = P.pieces[q];
+                uint8_t* to = slots + (uint64_t)(i - a) * astride + pc.at;
+                if (pc.kind == PIECE_WRITE) fill.add(d_wdata + w_at[pc.write] + pc.from, to, pc.len);
+                else if (pc.kind == PIECE_ZERO) fill.add(zero, to, pc.len);
+            }
+        }
+        if (!any) {  // every slot of the pass failed: nothing to encode
+            CK(cudaStreamSynchronize(ctx->stream));
+            continue;
+        }
+        int rc = run_copies(ctx, fill);
+        if (rc) return rc;
+        BlockList bl;
+        std::vector<uint32_t> lens(k), rec(k);
+        for (uint32_t i = 0; i < k; i++) {
+            const uint32_t s = W.stream[a + i];
+            lens[i] = W.plans[s].enc_len[W.enc[a + i]];
+            bl.off.push_back((uint64_t)i * astride), bl.len.push_back(lens[i]);
+            rec[i] = a + i;
+            enc_bytes[s] += lens[i];
+        }
+        bl.first = {0, k};
+        BlockPrep prep;
+        if ((rc = prepare_blocks(ctx, gplan[g], ctx->skip_blocks, gsh[g].checksum_bits, slots, bl, prep))) return rc;
+        rc = arena.encode_pass(ctx, gplan[g], gsh[g].etype, gsh[g].checksum_bits, slots, astride, lens, std::vector<uint64_t>(k, bs), prep, rec.data());
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));  // the slots and the copy lists are reused by the next pass
+    }
+    // the new record tables, then every tail: one concat of the segments behind byte floor(cut / 8) of each slot, the tail of slot s at
+    // dst + dst_off[s] (host variant: at stage_at[s] of ctx->d_out)
+    std::vector<uint8_t> pre(8 * (size_t)npairs, 0);
+    std::vector<uint32_t> pre_bits(npairs, 0);
+    std::vector<StreamIndex> Y(ns);
+    std::vector<uint64_t> kp(ns, 0), tail_bytes(ns, 0), stage_at(ns, 0), moved_runs(ns, 0), moved_bits(ns, 0);
+    uint64_t stage_total = 0;
+    SegmentList sl;
+    for (uint32_t s = 0; s < ns; s++) {
+        if (!live[s]) continue;
+        const WritePlan& P = W.plans[s];
+        const uint64_t base = W.pair_of[s], ne = P.enc.size();
+        std::vector<uint64_t> bits(ne);
+        std::vector<uint32_t> pb(ne);
+        for (uint64_t j = 0; j < ne; j++) bits[j] = arena.bits[base + j], pb[j] = pre_bits[base + j] = write_block_prefix(&pre[8 * (base + j)], bits[j]);
+        const uint64_t total_bits = splice_records(X[s], P, bits, pb, END_MARKER_BITS, Y[s]);
+        kp[s] = P.cut / 8;
+        const uint64_t tail_bits = total_bits - 8 * kp[s];
+        tail_bytes[s] = (tail_bits + 7) / 8;
+        const uint64_t need_cap = (tail_bits + 31) / 32 * 4;  // the concat writes whole 32-bit words
+        if (need_cap > S[s].cap) {
+            out_n[s] = need_cap;
+            fail(s, ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small"));
+            continue;
+        }
+        if (!dst) {
+            fail(s, ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer"));
+            continue;
+        }
+        stage_at[s] = stage_total, stage_total += round16(need_cap);
+        sl.at(8 * (host ? stage_at[s] : S[s].dst_off));
+        for (const WriteSeg& sg : P.segs) {
+            if (sg.kind == SEG_CARRY) {
+                sl.add_device(d_words, sg.bit + org[s], sg.bits);
+            } else if (sg.kind == SEG_NEW) {
+                for (uint64_t j = base + sg.first; j < base + sg.first + sg.count; j++) {
+                    sl.add_host(&pre[8 * j], pre_bits[j]);
+                    sl.add_device(arena.record(ctx, j), 0, arena.bits[j]);
+                }
+            } else if (sg.kind == SEG_OLD) {
+                sl.add_device(d_words, sg.bit + org[s], sg.bits);
+                moved_runs[s]++, moved_bits[s] += sg.bits;
+            } else {
+                sl.add_end_marker();
+            }
+        }
+    }
+    if (!std::count(live.begin(), live.end(), 1)) return 0;
+    uint8_t* d_out = dst;
+    if (host) {
+        CK(ctx->d_out.ensure(stage_total + 64));
+        d_out = ctx->d_out.as<uint8_t>();
+    }
+    int rc = sl.write(ctx, d_out);
+    if (rc) return rc;
+    // each new stream's first 32 bytes: the old ones before floor(cut / 8), the tail's behind it
+    auto nlead = [&](uint32_t s) { return kp[s] < INDEX_HEAD ? std::min<uint64_t>(INDEX_HEAD - kp[s], tail_bytes[s]) : 0; };
+    std::vector<uint8_t> lead(INDEX_HEAD * (size_t)ns, 0);
+    if (host) {
+        std::vector<DownloadPiece> down;
+        for (uint32_t s = 0; s < ns; s++)
+            if (live[s]) down.push_back(DownloadPiece{dst + S[s].dst_off, stage_at[s], tail_bytes[s]});
+        if ((rc = download_pieces(ctx, d_out, stage_total, down))) return rc;
+        for (uint32_t s = 0; s < ns; s++)
+            if (live[s]) memcpy(&lead[INDEX_HEAD * (size_t)s], dst + S[s].dst_off, nlead(s));
+    } else {
+        std::vector<uint32_t> ls;
+        std::vector<uint64_t> loff, llen;
+        for (uint32_t s = 0; s < ns; s++)
+            if (live[s] && nlead(s)) ls.push_back(s), loff.push_back(S[s].dst_off), llen.push_back(nlead(s));
+        std::vector<uint8_t> got(INDEX_HEAD * ls.size());
+        if ((rc = gather_heads(ctx, d_out, loff.data(), llen.data(), ls.size(), (uint32_t)INDEX_HEAD, got.data()))) return rc;
+        for (size_t q = 0; q < ls.size(); q++) memcpy(&lead[INDEX_HEAD * (size_t)ls[q]], &got[INDEX_HEAD * q], INDEX_HEAD);
+    }
+    uint64_t dec_b = 0, dec_n = 0, enc_b = 0, enc_n = 0, mv_r = 0, mv_b = 0;
+    for (uint32_t s = 0; s < ns; s++) {
+        if (!live[s]) continue;
+        StreamIndex& y = Y[s];
+        const uint64_t h = std::min<uint64_t>(kp[s], INDEX_HEAD);
+        memset(y.head + h, 0, INDEX_HEAD - h);
+        memcpy(y.head + h, &lead[INDEX_HEAD * (size_t)s], nlead(s));
+        static_cast<StreamIndex&>(*S[s].ix) = y;
+        keep[s] = kp[s];
+        out_n[s] = tail_bytes[s];
+        dec_b += dec_blocks[s], dec_n += dec_bytes[s], enc_b += W.plans[s].enc.size(), enc_n += enc_bytes[s], mv_r += moved_runs[s], mv_b += moved_bits[s];
+    }
+    if (ctx->profile) {
+        auto note = [&](const char* name, uint64_t a, uint64_t b) {
+            auto& e = ctx->prof[name];
+            e.bytes_in += a, e.bytes_out += b, e.launches++;
+        };
+        note("write:decoded", dec_b, dec_n);
+        note("write:encoded", enc_b, enc_n);
+        note("write:moved", mv_r, mv_b);
+    }
+    return 0;
+}
+
+// kz_write_ranges[_device]: the one-slot case of write_ranges_impl, behind its own checks.
 int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d_src, size_t n, uint32_t nw, const uint64_t* off, const uint64_t* len,
                  const uint8_t* data, const uint64_t* data_off, uint8_t* dst, size_t cap, uint64_t* keep, size_t* out_n) {
     if (!ctx) return -KZ_ERR_INVALID_PARAM;
@@ -3537,195 +3897,96 @@ int write_ranges(kz_ctx* ctx, kz_index* ix, const uint8_t* src, const uint8_t* d
     const uint64_t at0 = 0, nh = n == ix->stream_bytes ? n : 0;
     int rc = read_heads(ctx, host ? src : d_src, !host, &at0, &nh, 1, head);
     if (rc || (rc = read_stream_check(ctx, ix, n, head))) return rc;
-    TransformPlan plan;
-    if ((rc = plan_transforms(ctx, ix->t48, ix->etype, plan, KZ_ERR_CREATE_CODEC))) return rc;
-    const StreamHeader sh = index_header(*ix);
-    const uint32_t bs = ix->block_size;
-    const uint64_t nb = ix->nblocks();
-    const uint64_t enc_cost = compress_block_cost(round16(bs), entropy_scratch(ix->etype));
-    StreamIndex x = *ix;  // what the plan knows; ix changes only on success
-    WritePlan P = plan_writes(x, nw, off, len, enc_cost);
-    if (P.status == WRITE_TOO_LARGE) return ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds");
-    // the lowest record the call reads or moves: the cut, or with the size to learn the first block a write names or the last block
-    uint64_t low = nb ? nb - 1 : 0;
-    if (P.status == WRITE_NEED_SIZE) {
+    uint64_t k = n, o = 0;
+    int32_t st = 0;
+    rc = write_ranges_impl(ctx, src, d_src, {WriteSlot{ix, 0, n, 0, cap}}, nw, nullptr, off, len, data, data_off, dst, &k, &o, &st);
+    if (rc) return rc;
+    *keep = k;
+    *out_n = (size_t)o;
+    return st;
+}
+
+// kz_write_ranges_streams[_device]: the call-level checks, then each slot a write names checked against its own bytes (a failure fails
+// that slot only), then the writes on the slots that pass served by one write_ranges_impl call.
+int write_ranges_streams(kz_ctx* ctx, uint32_t nstreams, kz_index* const* ix, const uint8_t* base, bool device, const uint64_t* src_off,
+                         const uint64_t* src_len, uint32_t nw, const uint32_t* w_stream, const uint64_t* off, const uint64_t* len, const uint8_t* data,
+                         const uint64_t* data_off, uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* keep, uint64_t* out_n,
+                         int32_t* status) {
+    if (!ctx) return -KZ_ERR_INVALID_PARAM;
+    const int rc = [&]() -> int {
+        if (nstreams && (!keep || !out_n || !status)) return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+        for (uint32_t s = 0; s < nstreams; s++) keep[s] = src_len ? src_len[s] : 0, out_n[s] = 0, status[s] = 0;
+        if (nw && (!ix || !src_off || !src_len || !w_stream || !off || !len || !dst_off || !dst_cap))
+            return ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument");
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return ctx->fail(KZ_ERR_PROCESS_BLOCK, "cudaSetDevice failed");
+        if (ctx->session) return ctx->fail(KZ_ERR_INVALID_PARAM, "a session is open on this context");
+        std::vector<uint8_t> named(nstreams, 0);
+        for (uint32_t i = 0; i < nw; i++) {
+            if (w_stream[i] >= nstreams) return ctx->fail(KZ_ERR_INVALID_PARAM, "a write names a stream past nstreams");
+            if (!len[i]) continue;
+            if (!data || !data_off) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+            if (data_off[i] + len[i] < data_off[i]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+            named[w_stream[i]] = 1;
+        }
+        std::vector<uint32_t> names;
+        std::vector<uint64_t> hoff, hlen;
+        std::set<const kz_index*> seen;
+        for (uint32_t s = 0; s < nstreams; s++) {
+            if (!named[s]) continue;
+            if (ix[s] && !seen.insert(ix[s]).second) return ctx->fail(KZ_ERR_INVALID_PARAM, "one index in two slots that writes name");
+            if (dst_off[s] + dst_cap[s] < dst_off[s]) return ctx->fail(KZ_ERR_INVALID_PARAM, "offset + length overflows");
+            if (dst_cap[s] && !dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
+            if (device && (dst_off[s] & 15)) return ctx->fail(KZ_ERR_INVALID_PARAM, "device offsets must be multiples of 16");
+            names.push_back(s), hoff.push_back(src_off[s]), hlen.push_back(src_len[s]);
+        }
+        const size_t nn = names.size();
+        if (!nn) return 0;  // no slot is named: no buffer is read or written, so none is checked
+        int r = check_spans(ctx, base, hoff.data(), hlen.data(), nn, device);
+        if (r) return r;
+        if (device) {
+            if ((uintptr_t)dst & 15) return ctx->fail(KZ_ERR_INVALID_PARAM, "device buffers must be 16-byte aligned");
+            // the output windows may overlap neither each other nor a named stream: a sweep over both, ordered by first address
+            struct Span {
+                uintptr_t a, e;
+                bool window;
+            };
+            std::vector<Span> sp;
+            for (uint32_t s : names) {
+                if (dst_cap[s]) sp.push_back(Span{(uintptr_t)dst + dst_off[s], (uintptr_t)dst + dst_off[s] + dst_cap[s], true});
+                if (src_len[s]) sp.push_back(Span{(uintptr_t)base + src_off[s], (uintptr_t)base + src_off[s] + src_len[s], false});
+            }
+            std::sort(sp.begin(), sp.end(), [](const Span& x, const Span& y) { return x.a < y.a; });
+            uintptr_t wend = 0, send = 0;
+            for (const Span& x : sp) {
+                if (x.a < wend || (x.window && x.a < send)) return ctx->fail(KZ_ERR_INVALID_PARAM, "an output window overlaps another or a stream");
+                if (x.window) wend = std::max(wend, x.e);
+                else send = std::max(send, x.e);
+            }
+        }
+        std::vector<uint8_t> head(INDEX_HEAD * nn);
+        if ((r = read_heads(ctx, base, device, hoff.data(), hlen.data(), nn, head.data()))) return r;
+        // per slot: a missing or stale index or a chain without a GPU path fails the slot with kz_write_ranges's code
+        std::vector<uint32_t> slot(nstreams, 0);
+        std::vector<WriteSlot> S;
+        std::vector<uint32_t> who;
+        for (size_t j = 0; j < nn; j++) {
+            const uint32_t s = names[j];
+            status[s] = ix[s] ? read_stream_check(ctx, ix[s], src_len[s], &head[INDEX_HEAD * j]) : ctx->fail(KZ_ERR_INVALID_PARAM, "missing index");
+            if (!status[s]) slot[s] = (uint32_t)S.size(), S.push_back(WriteSlot{ix[s], src_off[s], src_len[s], dst_off[s], dst_cap[s]}), who.push_back(s);
+        }
+        std::vector<uint32_t> ws;
+        std::vector<uint64_t> o, l, d;
         for (uint32_t i = 0; i < nw; i++)
-            if (len[i] && off[i] != WRITE_APPEND) low = std::min<uint64_t>(low, off[i] / bs);
-    } else if (P.nothing()) {
+            if (len[i] && !status[w_stream[i]]) ws.push_back(slot[w_stream[i]]), o.push_back(off[i]), l.push_back(len[i]), d.push_back(data_off[i]);
+        std::vector<uint64_t> k(S.size()), on(S.size());
+        std::vector<int32_t> st(S.size());
+        r = write_ranges_impl(ctx, device ? nullptr : base, device ? base : nullptr, S, (uint32_t)ws.size(), ws.data(), o.data(), l.data(), data,
+                              d.data(), dst, k.data(), on.data(), st.data());
+        if (r) return r;
+        for (size_t j = 0; j < S.size(); j++) keep[who[j]] = k[j], out_n[who[j]] = on[j], status[who[j]] = st[j];
         return 0;
-    }
-    const uint64_t ubase = host ? ((P.status == WRITE_NEED_SIZE ? record_prefix_bit(x, low) : P.cut) / 8) & ~15ull : 0;  // first stream byte on the device
-    const uint64_t base_bit = 8 * ubase;
-    const uint8_t* d_base = d_src;
-    const uint8_t* d_wdata = data;  // device bytes of write i at d_wdata + w_at[i]
-    std::vector<uint64_t> w_at(nw, 0);
-    if (host) {
-        uint64_t wtotal = 0;
-        for (uint32_t i = 0; i < nw; i++) w_at[i] = wtotal, wtotal += len[i];
-        const uint64_t tail = n - ubase, wpos = round16(tail) + 128;
-        CK(ctx->d_in.ensure(wpos + wtotal + 64));
-        uint8_t* din = ctx->d_in.as<uint8_t>();
-        CK(cudaMemsetAsync(din + (tail & ~3ull), 0, 128, ctx->stream));
-        if (tail) CK(cudaMemcpyAsync(din, src + ubase, tail, cudaMemcpyHostToDevice, ctx->stream));
-        if (wtotal) {
-            std::vector<uint8_t> wbytes(wtotal);
-            for (uint32_t i = 0; i < nw; i++)
-                if (len[i]) memcpy(&wbytes[w_at[i]], data + data_off[i], len[i]);
-            CK(cudaMemcpyAsync(din + wpos, wbytes.data(), wtotal, cudaMemcpyHostToDevice, ctx->stream));
-        }
-        d_base = din;
-        d_wdata = din + wpos;
-        if (ctx->profile) {
-            auto& e = ctx->prof["write:h2d"];
-            e.bytes_in += (tail ? 1 : 0) + (wtotal ? 1 : 0), e.bytes_out += tail + wtotal, e.launches++;
-        }
-    } else {
-        for (uint32_t i = 0; i < nw; i++) w_at[i] = len[i] ? data_off[i] : 0;
-    }
-    const uint32_t* d_words = (const uint32_t*)d_base;
-    const uint64_t words_len = (n - ubase + 3) / 4 + 16;
-    auto job_of = [&](uint64_t b) {
-        DecJob j = DecJob();
-        j.bit_off = x.start[b] - base_bit;
-        j.bits = x.bits[b];
-        j.block_size = bs;
-        return j;
-    };
-    // the first failure among decoded blocks, in block order: the block's own code, or a length that breaks the block arithmetic
-    auto check_decoded = [&](const std::vector<uint64_t>& blocks, const std::vector<DecodeFailure>& fail, const std::vector<uint32_t>& olen) {
-        for (size_t i = 0; i < blocks.size(); i++) {
-            const bool last = blocks[i] + 1 == nb;
-            if (olen[i] > bs || (!fail[i].failed() && (last ? olen[i] == 0 || (x.size >= 0 && olen[i] != (uint64_t)x.size - (nb - 1) * bs) : olen[i] != bs)))
-                return ctx->fail(KZ_ERR_INVALID_FILE, "Invalid bitstream: a block before the last is not block_size bytes long");
-            if (fail[i].failed()) return ctx->fail(-fail[i].code, fail[i].msg);
-        }
-        return 0;
-    };
-    uint64_t dec_blocks = 0, dec_bytes = 0;
-    bool have_last = false;  // the old last block sits decoded in ctx->d_out
-    if (P.status == WRITE_NEED_SIZE) {
-        CK(ctx->d_out.ensure(decompress_slot(bs) + 64));
-        std::vector<DecodeFailure> fail;
-        std::vector<uint32_t> olen;
-        rc = decode_isolated(ctx, sh, plan, d_words, words_len, {job_of(nb - 1)}, {1}, [&](uint32_t, uint32_t m) { return m > bs ? NO_ROOM : 0; },
-                             ctx->d_out.as<uint8_t>(), fail, olen);
-        if (rc || (rc = check_decoded({nb - 1}, fail, olen))) return rc;
-        x.size = (int64_t)((nb - 1) * bs + olen[0]);
-        have_last = true;
-        dec_blocks++, dec_bytes += olen[0];
-        P = plan_writes(x, nw, off, len, enc_cost);
-        if (P.status != WRITE_OK) return ctx->fail(KZ_ERR_INVALID_PARAM, "the data would grow past what an index holds");
-        if (P.nothing()) return 0;
-    }
-    // passes: decode, apply the writes, encode; each pass's records packed into ctx->d_bits
-    const uint32_t ne = (uint32_t)P.enc.size();
-    const uint64_t astride = decompress_slot(bs);
-    RecordArena arena(ne);
-    uint64_t enc_bytes = 0;
-    for (uint32_t p = 0; p < P.npasses(); p++) {
-        const uint32_t a = P.first[p], k = P.first[p + 1] - a;
-        CK(ctx->d_slots.ensure(astride * k + 64));
-        uint8_t* slots = ctx->d_slots.as<uint8_t>();
-        std::vector<uint64_t> blocks;
-        std::vector<DecJob> jobs;
-        std::vector<uint8_t> last;
-        std::vector<uint32_t> slot;
-        CopyList fill;
-        for (uint32_t j = a; j < a + k; j++) {
-            const uint64_t b = P.enc[j];
-            if (!P.decode[j]) continue;
-            if (have_last && b + 1 == nb) {
-                fill.add(ctx->d_out.p, slots + (j - a) * astride, (uint64_t)x.size - (nb - 1) * bs);
-                continue;
-            }
-            blocks.push_back(b), jobs.push_back(job_of(b)), last.push_back(b + 1 == nb), slot.push_back(j - a);
-        }
-        if (!jobs.empty()) {
-            std::vector<DecodeFailure> fail;
-            std::vector<uint32_t> olen;
-            rc = decode_isolated(ctx, sh, plan, d_words, words_len, jobs, last,
-                                 [&](uint32_t i, uint32_t m) { return m > bs ? NO_ROOM : (uint64_t)slot[i] * astride; }, slots, fail, olen);
-            if (rc || (rc = check_decoded(blocks, fail, olen))) return rc;
-            for (uint32_t m : olen) dec_blocks++, dec_bytes += m;
-        }
-        for (uint32_t j = a; j < a + k; j++)
-            for (uint64_t q = P.piece_of[j]; q < P.piece_of[j + 1]; q++) {
-                const WritePiece& pc = P.pieces[q];
-                uint8_t* to = slots + (uint64_t)(j - a) * astride + pc.at;
-                if (pc.kind == PIECE_WRITE) fill.add(d_wdata + w_at[pc.write] + pc.from, to, pc.len);
-                else if (pc.kind == PIECE_ZERO) CK(cudaMemsetAsync(to, 0, pc.len, ctx->stream));
-            }
-        if ((rc = run_copies(ctx, fill))) return rc;
-        BlockList bl;
-        std::vector<uint32_t> lens(P.enc_len.begin() + a, P.enc_len.begin() + a + k);
-        for (uint32_t j = 0; j < k; j++) bl.off.push_back((uint64_t)j * astride), bl.len.push_back(lens[j]), enc_bytes += lens[j];
-        bl.first = {0, k};
-        BlockPrep prep;
-        if ((rc = prepare_blocks(ctx, plan, ctx->skip_blocks, sh.checksum_bits, slots, bl, prep))) return rc;
-        std::vector<uint32_t> rec(k);
-        for (uint32_t j = 0; j < k; j++) rec[j] = a + j;
-        rc = arena.encode_pass(ctx, plan, ix->etype, sh.checksum_bits, slots, astride, lens, std::vector<uint64_t>(k, bs), prep, rec.data());
-        if (rc) return rc;
-        CK(cudaStreamSynchronize(ctx->stream));  // the slots and the copy lists are reused by the next pass
-    }
-    // the new record table, then the tail: one concat of every segment behind byte floor(cut / 8)
-    std::vector<uint8_t> pre(8 * (size_t)ne, 0);
-    std::vector<uint32_t> pre_bits(ne);
-    for (uint32_t j = 0; j < ne; j++) pre_bits[j] = write_block_prefix(&pre[8 * (size_t)j], arena.bits[j]);
-    StreamIndex y;
-    const uint64_t total_bits = splice_records(x, P, arena.bits, pre_bits, END_MARKER_BITS, y);
-    const uint64_t kp = P.cut / 8, tail_bits = total_bits - 8 * kp, tail_bytes = (tail_bits + 7) / 8;
-    const uint64_t need_cap = (tail_bits + 31) / 32 * 4;  // the concat writes whole 32-bit words
-    if (need_cap > cap) {
-        *out_n = (size_t)need_cap;
-        return ctx->fail(KZ_ERR_WRITE_FILE, "output buffer too small");
-    }
-    if (!dst) return ctx->fail(KZ_ERR_INVALID_PARAM, "null buffer");
-    SegmentList sl;
-    uint64_t moved_runs = 0, moved_bits = 0;
-    for (const WriteSeg& sg : P.segs) {
-        if (sg.kind == SEG_CARRY) {
-            sl.add_device(d_base, sg.bit - base_bit, sg.bits);
-        } else if (sg.kind == SEG_NEW) {
-            for (uint64_t j = sg.first; j < sg.first + sg.count; j++) {
-                sl.add_host(&pre[8 * j], pre_bits[j]);
-                sl.add_device(arena.record(ctx, j), 0, arena.bits[j]);
-            }
-        } else if (sg.kind == SEG_OLD) {
-            sl.add_device(d_base, sg.bit - base_bit, sg.bits);
-            moved_runs++, moved_bits += sg.bits;
-        } else {
-            sl.add_end_marker();
-        }
-    }
-    uint8_t* d_out = dst;
-    if (host) {
-        CK(ctx->d_out.ensure(need_cap + 64));
-        d_out = ctx->d_out.as<uint8_t>();
-    }
-    if ((rc = sl.write(ctx, d_out))) return rc;
-    // the new stream's first 32 bytes: the old ones before floor(cut / 8), the tail's behind it
-    uint8_t lead[INDEX_HEAD] = {0};
-    const uint64_t nlead = kp < INDEX_HEAD ? std::min<uint64_t>(INDEX_HEAD - kp, tail_bytes) : 0;
-    if (host) CK(cudaMemcpyAsync(dst, d_out, tail_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    else if (nlead) CK(cudaMemcpyAsync(lead, d_out, nlead, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (host && nlead) memcpy(lead, dst, nlead);
-    memset(y.head + std::min<uint64_t>(kp, INDEX_HEAD), 0, INDEX_HEAD - std::min<uint64_t>(kp, INDEX_HEAD));
-    memcpy(y.head + std::min<uint64_t>(kp, INDEX_HEAD), lead, nlead);
-    static_cast<StreamIndex&>(*ix) = y;
-    *keep = kp;
-    *out_n = (size_t)tail_bytes;
-    if (ctx->profile) {
-        auto note = [&](const char* name, uint64_t a, uint64_t b) {
-            auto& e = ctx->prof[name];
-            e.bytes_in += a, e.bytes_out += b, e.launches++;
-        };
-        note("write:decoded", dec_blocks, dec_bytes);
-        note("write:encoded", ne, enc_bytes);
-        note("write:moved", moved_runs, moved_bits);
-    }
-    return 0;
+    }();
+    return finish_streams(nstreams, status, out_n, rc);
 }
 
 }  // namespace
@@ -3809,6 +4070,22 @@ int kz_write_ranges_device(kz_ctx* ctx, kz_index* ix, const void* d_src, size_t 
     if (int rc = after_caller_work(ctx)) return rc;
     if (!d_src) return ctx ? ctx->fail(KZ_ERR_INVALID_PARAM, "missing argument") : -KZ_ERR_INVALID_PARAM;
     return write_ranges(ctx, ix, nullptr, (const uint8_t*)d_src, n, nw, off, len, (const uint8_t*)d_data, data_off, (uint8_t*)d_dst, cap, keep, out_n);
+}
+
+int kz_write_ranges_streams(kz_ctx* ctx, uint32_t nstreams, kz_index* const* ix, const uint8_t* src, const uint64_t* src_off, const uint64_t* src_len,
+                            uint32_t nw, const uint32_t* w_stream, const uint64_t* off, const uint64_t* len, const uint8_t* data, const uint64_t* data_off,
+                            uint8_t* dst, const uint64_t* dst_off, const uint64_t* dst_cap, uint64_t* keep, uint64_t* out_n, int32_t* status) {
+    return write_ranges_streams(ctx, nstreams, ix, src, false, src_off, src_len, nw, w_stream, off, len, data, data_off, dst, dst_off, dst_cap, keep, out_n,
+                                status);
+}
+
+int kz_write_ranges_streams_device(kz_ctx* ctx, uint32_t nstreams, kz_index* const* ix, const void* d_src, const uint64_t* src_off,
+                                   const uint64_t* src_len, uint32_t nw, const uint32_t* w_stream, const uint64_t* off, const uint64_t* len,
+                                   const void* d_data, const uint64_t* data_off, void* d_dst, const uint64_t* dst_off, const uint64_t* dst_cap,
+                                   uint64_t* keep, uint64_t* out_n, int32_t* status) {
+    if (int rc = after_caller_work(ctx)) return finish_streams(nstreams, status, out_n, rc);
+    return write_ranges_streams(ctx, nstreams, ix, (const uint8_t*)d_src, true, src_off, src_len, nw, w_stream, off, len, (const uint8_t*)d_data, data_off,
+                                (uint8_t*)d_dst, dst_off, dst_cap, keep, out_n, status);
 }
 
 // ---- many streams per call (kz_index_build_streams[_device], kz_read_ranges_streams[_device]) ----------------------------------------

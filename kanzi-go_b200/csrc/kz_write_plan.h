@@ -61,13 +61,8 @@ inline uint64_t record_prefix_bit(const StreamIndex& x, uint64_t b) { return b =
 // compress_block_cost of the stream's block size and codec).
 inline uint64_t write_block_cost(uint32_t block_size, uint64_t enc_cost) { return read_block_cost(block_size) + enc_cost; }
 
-// The plan of writes i = 0 .. nw - 1 (len[i] bytes to decoded offset off[i], or to the current end when off[i] == WRITE_APPEND) on the
-// stream x, whose decoded size is x.size (-1: unknown). With the size unknown the old last block's length decides the result when a
-// KZ_WRITE_APPEND comes before the writes reach past the last block's range, or a write reaches into that range or beyond without the
-// writes covering all of it: then status is WRITE_NEED_SIZE and the caller plans again with the size. WRITE_TOO_LARGE: an offset plus its
-// length overflows, the blocks after the writes times the block size pass 2^62, or more than 2^32 - 2 blocks would be re-encoded.
-inline WritePlan plan_writes(const StreamIndex& x, uint32_t nw, const uint64_t* off, const uint64_t* len, uint64_t enc_cost,
-                             uint64_t budget = STREAM_PASS_BUDGET) {
+// Everything of the plan but its passes: plan_writes_streams cuts those.
+inline WritePlan plan_write_blocks(const StreamIndex& x, uint32_t nw, const uint64_t* off, const uint64_t* len) {
     WritePlan P;
     const uint64_t bs = x.block_size, nb = x.nblocks();
     const bool known = x.size >= 0;
@@ -193,8 +188,84 @@ inline WritePlan plan_writes(const StreamIndex& x, uint32_t nw, const uint64_t* 
         }
     }
     P.segs.push_back(WriteSeg{SEG_END, 0, 0, 0, 0});
-    P.first = plan_decompress_passes((uint32_t)count, decompress_slot(x.block_size), write_block_cost(x.block_size, enc_cost), budget).first;
     return P;
+}
+
+// ---- the plan of writes into many streams (kz_write_ranges_streams) ----------------------------------------------------------------
+// Each stream has a group, as in plan_reads_streams: streams of one group share transform48, entropy, block_size and checksum_bits, so
+// their re-encoded blocks may share a pass (one decode, one copy launch, one encode); blocks of different groups never do.
+struct WriteStream {
+    const StreamIndex* x;  // null: the stream takes no part (no write names it, or it failed a check): its plan is empty
+    uint32_t group;        // equal groups have equal block sizes and encode costs
+    uint64_t enc_cost;     // compress_block_cost of the stream's block size and codec
+};
+
+struct WriteStreamsPlan {
+    std::vector<WritePlan> plans;   // per stream: what plan_writes gives for its writes alone (passes included), its pieces naming
+                                    // writes by their index in the call's arrays
+    std::vector<uint32_t> stream;   // per re-encoded pair: its stream ...
+    std::vector<uint32_t> enc;      // ... and its index into plans[stream].enc; pairs in plan order (group, then stream, then block)
+    std::vector<uint64_t> pair_of;  // per stream: its first pair (a stream's pairs are contiguous)
+    std::vector<uint32_t> first;    // pass p re-encodes pairs first[p] .. first[p + 1] - 1, all of one group
+    uint32_t npasses() const { return first.empty() ? 0 : (uint32_t)first.size() - 1; }
+};
+
+// Write i goes to stream w_stream[i] (null: every write to stream 0); a stream's writes keep their array order. Groups are ordered by
+// their first appearance among the streams, each group's run of pairs is cut into passes by plan_decompress_passes under
+// write_block_cost. Only streams whose plan is WRITE_OK have pairs.
+inline WriteStreamsPlan plan_writes_streams(const std::vector<WriteStream>& S, uint32_t nw, const uint32_t* w_stream, const uint64_t* off,
+                                            const uint64_t* len, uint64_t budget = STREAM_PASS_BUDGET) {
+    WriteStreamsPlan W;
+    const uint32_t ns = (uint32_t)S.size();
+    std::vector<std::vector<uint64_t>> o(ns), l(ns);
+    std::vector<std::vector<uint32_t>> idx(ns);  // the writes of each stream, by their index in the call's arrays
+    for (uint32_t i = 0; i < nw; i++) {
+        const uint32_t s = w_stream ? w_stream[i] : 0u;
+        if (len[i] && s < ns && S[s].x) o[s].push_back(off[i]), l[s].push_back(len[i]), idx[s].push_back(i);
+    }
+    W.plans.resize(ns);
+    W.pair_of.assign(ns, 0);
+    std::vector<uint32_t> groups;  // in order of first appearance
+    for (uint32_t s = 0; s < ns; s++) {
+        if (!S[s].x) continue;
+        const StreamIndex& x = *S[s].x;
+        WritePlan& P = W.plans[s];
+        P = plan_write_blocks(x, (uint32_t)o[s].size(), o[s].data(), l[s].data());
+        for (WritePiece& pc : P.pieces)
+            if (pc.kind == PIECE_WRITE) pc.write = idx[s][pc.write];
+        if (P.status == WRITE_OK && !P.nothing())
+            P.first = plan_decompress_passes((uint32_t)P.enc.size(), decompress_slot(x.block_size), write_block_cost(x.block_size, S[s].enc_cost), budget).first;
+        if (std::find(groups.begin(), groups.end(), S[s].group) == groups.end()) groups.push_back(S[s].group);
+    }
+    for (uint32_t g : groups) {
+        const size_t a = W.stream.size();
+        uint32_t bs = 0;
+        uint64_t cost = 0;
+        for (uint32_t s = 0; s < ns; s++) {
+            if (!S[s].x || S[s].group != g) continue;
+            W.pair_of[s] = W.stream.size();
+            const WritePlan& P = W.plans[s];
+            if (P.status != WRITE_OK) continue;
+            for (uint32_t j = 0; j < (uint32_t)P.enc.size(); j++) W.stream.push_back(s), W.enc.push_back(j);
+            bs = S[s].x->block_size, cost = S[s].enc_cost;
+        }
+        const uint32_t n = (uint32_t)(W.stream.size() - a);
+        if (!n) continue;
+        const PassPlan pp = plan_decompress_passes(n, decompress_slot(bs), write_block_cost(bs, cost), budget);
+        for (uint32_t p = 0; p < pp.npasses(); p++) W.first.push_back((uint32_t)a + pp.first[p]);
+    }
+    W.first.push_back((uint32_t)W.stream.size());
+    return W;
+}
+
+// The one-stream plan: writes i = 0 .. nw - 1 (len[i] bytes to decoded offset off[i], or to the current end when off[i] == WRITE_APPEND)
+// on the stream x, whose decoded size is x.size (-1: unknown). With the size unknown the old last block's length decides the result when
+// a KZ_WRITE_APPEND comes before the writes reach past the last block's range, or a write reaches into that range or beyond without the
+// writes covering all of it: then status is WRITE_NEED_SIZE and the caller plans again with the size. WRITE_TOO_LARGE: an offset plus its
+// length overflows, the blocks after the writes times the block size pass 2^62, or more than 2^32 - 2 blocks would be re-encoded.
+inline WritePlan plan_writes(const StreamIndex& x, uint32_t nw, const uint64_t* off, const uint64_t* len, uint64_t enc_cost,
+                             uint64_t budget = STREAM_PASS_BUDGET) {
+    return plan_writes_streams({WriteStream{&x, 0, enc_cost}}, nw, nullptr, off, len, budget).plans[0];
 }
 
 // The index of the new stream: x with the records from the cut on laid out again. new_bits[j] / prefix_bits[j]: the payload and prefix
